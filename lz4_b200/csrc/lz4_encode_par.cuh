@@ -162,13 +162,8 @@ __global__ void __launch_bounds__(kEpThreads, 2) lz4_encode_par_kernel(lz4k_enco
             if (tid == 0) { int r = 0; if (n == 0 && cap >= 1) { dst[0] = 0; r = 1; } a.outSize[b] = r; }
             continue;
         }
-        const int head = (int)(reinterpret_cast<uintptr_t>(gsrc) & 15);
-        const uint32_t loadBytes = (uint32_t)((head + n + 15) & ~15);
-        if (tid == 0) {
-            mbar_expect_tx(&S.mbar, loadBytes);
-            for (uint32_t o = 0; o < loadBytes; o += 16384u) tma_load_1d(S.src + o, gsrc - head + o, min(16384u, loadBytes - o), &S.mbar);
-            S.E = 0; S.O = 0; S.fail = 0; S.carry[2] = 0;
-        }
+        const int head = tma_stage(S.src, gsrc, n, &S.mbar, tid == 0);
+        if (tid == 0) { S.E = 0; S.O = 0; S.fail = 0; S.carry[2] = 0; }
         for (int k = tid; k < (1 << kEpHashLog) / 4; k += kEpThreads) reinterpret_cast<uint4*>(S.TT)[k] = make_uint4(0, 0, 0, 0);
         __syncthreads();
         mbar_wait(&S.mbar, parity);

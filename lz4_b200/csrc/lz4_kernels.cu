@@ -75,17 +75,15 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes)
 {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-/* wait for the phase with the given parity; the hardware may suspend the warp for up to `hintNs` per attempt, so that
+/* wait for the phase with the given parity; the hardware may suspend the warp for up to kWaitHintNs per attempt, so that
  * waiting warps do not take issue slots from the warps they are waiting for */
-#ifndef LZ4K_WAIT_HINT_NS
-#define LZ4K_WAIT_HINT_NS 2000
-#endif
+constexpr uint32_t kWaitHintNs = 2000;
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity)
 {
     uint32_t ok;
     do {
         asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n selp.u32 %0, 1, 0, p;\n}\n"
-                     : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity), "r"((uint32_t)LZ4K_WAIT_HINT_NS) : "memory");
+                     : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity), "r"(kWaitHintNs) : "memory");
     } while (!ok);
 }
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity)
@@ -111,6 +109,19 @@ __device__ __forceinline__ void tma_wait_all0() { asm volatile("cp.async.bulk.wa
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_acq_rel_cta() { asm volatile("fence.acq_rel.cta;" ::: "memory"); }
 
+/* TMA bulk load of the n bytes at src into shared memory at dst, completing on `bar`.  The load starts at the 16-byte
+ * boundary below src and is rounded up to 16 bytes, so dst needs room for head + n + 15 bytes; byte i of the block lands
+ * at dst[head + i].  Only `issuer` issues the load; every caller gets the head. */
+__device__ __forceinline__ int tma_stage(uint8_t* dst, const uint8_t* src, int n, uint64_t* bar, bool issuer = true)
+{
+    const int head = (int)(reinterpret_cast<uintptr_t>(src) & 15);
+    if (issuer) {
+        const uint32_t loadBytes = (uint32_t)((head + n + 15) & ~15);
+        mbar_expect_tx(bar, loadBytes);
+        for (uint32_t o = 0; o < loadBytes; o += 16384u) tma_load_1d(dst + o, src - head + o, min(16384u, loadBytes - o), bar);
+    }
+    return head;
+}
 
 
 /* workspace layout (lz4k_decode_workspace_bytes): header | nSeq[N] | slowList[N] | marks[N][markStride] */
@@ -179,6 +190,24 @@ __device__ __forceinline__ bool rows_eligible(int n, int cap, uint32_t nseq, uin
     return n > 0 && n <= 65535 && cap > 0 && cap <= 65536 && nseq <= (uint32_t)kMaxSeqFast && nseq <= markStride;
 }
 
+/* where a scan kernel leaves block b's marks: blocks the rows kernel may take have them, and so does every block of a
+ * wide batch (two words per sequence, for the tiles kernel); nullptr: no marks */
+__device__ __forceinline__ uint32_t* scan_marks(const WsView& w, int64_t b, int n, int cap, bool wide = false)
+{
+    const bool want = wide ? n > 0 : (n > 0 && n <= 65535 && cap > 0 && cap <= 65536 && w.markStride > 0);
+    return want ? w.marks + (size_t)b * w.markStride : nullptr;
+}
+
+/* a scan kernel's result for block b: the decoder's return value and the sequence count; an accepted block that neither
+ * the rows kernel nor (`tiled`) the tiles kernel takes goes on the generic kernel's list */
+__device__ __forceinline__ void scan_result(const lz4k_decode_args& a, const WsView& w, int64_t b, int n, int cap, int r,
+                                            uint32_t ns, bool tiled = false)
+{
+    a.outSize[b] = r;
+    w.nSeq[b] = ns;
+    if (r > 0 && !tiled && !rows_eligible(n, cap, ns, w.markStride)) w.slowList[atomicAdd(&w.hdr->slowCount, 1u)] = (uint32_t)b;
+}
+
 /* ---- scan, one THREAD per block: reads through the read-only data cache with L1 prefetch hints ---- */
 
 __global__ void __launch_bounds__(128) lz4_scan_kernel(lz4k_decode_args a)
@@ -190,13 +219,9 @@ __global__ void __launch_bounds__(128) lz4_scan_kernel(lz4k_decode_args a)
     const int n = a.srcSize[b];
     int cap = a.dstCapArr ? a.dstCapArr[b] : a.dstCap;
     uint32_t ns = 0;
-    const bool wantMarks = (n > 0 && n <= 65535 && cap > 0 && cap <= 65536 && w.markStride > 0);
-    uint32_t* marks = wantMarks ? (w.marks + b * w.markStride) : nullptr;
     MemPtr<true> mem{src};
-    const int r = scan_block(mem, n, cap, &ns, marks, w.markStride);
-    a.outSize[b] = r;
-    w.nSeq[b] = ns;
-    if (r > 0 && !rows_eligible(n, cap, ns, w.markStride)) w.slowList[atomicAdd(&w.hdr->slowCount, 1u)] = (uint32_t)b;
+    const int r = scan_block(mem, n, cap, &ns, scan_marks(w, b, n, cap), w.markStride);
+    scan_result(a, w, b, n, cap, r, ns);
 }
 
 /* ---- scan, kSsLanes lanes per block that merge (lz4_scan_split.h): the chain of dependent steps is kSsLanes times shorter ----
@@ -217,13 +242,12 @@ __global__ void __launch_bounds__(kSplitThreads, 10) lz4_scan_split_kernel(lz4k_
     const uint8_t* src = a.src + a.srcOff[b];
     const int n = a.srcSize[b];
     const int cap = a.dstCapArr ? a.dstCapArr[b] : a.dstCap;
-    const bool wantMarks = (n > 0 && n <= 65535 && cap > 0 && cap <= 65536 && w.markStride > 0);
-    uint32_t* marks = wantMarks ? (w.marks + b * w.markStride) : nullptr;
+    uint32_t* marks = scan_marks(w, b, n, cap);
     SsBlock& S = sh[slot];
     MemPtr<true> mem{src};
     int r = 0;
     uint32_t ns = 0;
-    bool serial = !(wantMarks && cap >= 64 && n >= kSsMinBytes);
+    bool serial = !(marks && cap >= 64 && n >= kSsMinBytes);
     if (!serial) {
         const uint32_t R = w.markStride / kSsLanes;
         uint32_t* sc = w.scratch + b * 2 * (int64_t)w.markStride;
@@ -251,21 +275,14 @@ __global__ void __launch_bounds__(kSplitThreads, 10) lz4_scan_split_kernel(lz4k_
         }
     }
     if (serial && lane == 0) r = scan_block(mem, n, cap, &ns, marks, w.markStride);
-    if (lane == 0) {
-        a.outSize[b] = r;
-        w.nSeq[b] = ns;
-        if (r > 0 && !rows_eligible(n, cap, ns, w.markStride)) w.slowList[atomicAdd(&w.hdr->slowCount, 1u)] = (uint32_t)b;
-    }
+    if (lane == 0) scan_result(a, w, b, n, cap, r, ns);
 }
 
 /* ---- scan, one CTA of NL lanes per block (lz4_scan_par.h): same outputs as lz4_scan_kernel ----
  * Blocks of up to 65 535 bytes are staged in shared memory by one TMA bulk load (the walks are chains of
  * dependent 4-byte reads: ~30 cycles each from shared memory instead of an L2 / HBM round trip); larger
  * blocks (lz4frame's 4 MB blocks) are walked in global memory by the same lanes. */
-#ifndef LZ4K_SCAN_LANES
-#define LZ4K_SCAN_LANES 128
-#endif
-constexpr int kScanLanes = LZ4K_SCAN_LANES;
+constexpr int kScanLanes = 128;
 static_assert(kScanLanes % 32 == 0 && kScanLanes <= kSpMaxLanes, "scan lanes");
 
 struct ScanParSmem {
@@ -335,53 +352,28 @@ __global__ void __launch_bounds__(kScanLanes) lz4_scan_par_kernel(lz4k_decode_ar
         const int n = a.srcSize[b];
         const int cap = a.dstCapArr ? a.dstCapArr[b] : a.dstCap;
         const bool wide = w.tilesMax != 0;                            /* a batch of blocks above 64 KB: two-word marks for the tiles kernel */
-        const bool wantMarks = wide ? n > 0 : (n > 0 && n <= 65535 && cap > 0 && cap <= 65536 && w.markStride > 0);
-        uint32_t* marks = wantMarks ? (w.marks + (size_t)b * w.markStride) : nullptr;
+        uint32_t* marks = scan_marks(w, b, n, cap, wide);
         const uint32_t markCap = wide ? w.markStride / 2u : w.markStride;
         int r = -1;
         uint32_t ns = 0;
-        if (wide && n > 0 && n <= 65535) {
-            const int head = (int)(reinterpret_cast<uintptr_t>(src) & 15);
-            const uint32_t loadBytes = (uint32_t)((head + n + 15) & ~15);
-            if (tid == 0) {
-                mbar_expect_tx(&S.mbar, loadBytes);
-                for (uint32_t o = 0; o < loadBytes; o += 16384u)
-                    tma_load_1d(S.in + o, src - head + o, min(16384u, loadBytes - o), &S.mbar);
-            }
+        /* the lanes' walk over `mem`; in a wide batch the marks are two words per sequence (MemPtr<G, true>) */
+        auto lanes = [&](auto mem) { scan_par_block(S, mem, n, cap, marks, markCap, r, ns); };
+        if (n > 0 && n <= 65535 && cap > 0) {                     /* staged in shared memory */
+            const int head = tma_stage(S.in, src, n, &S.mbar, tid == 0);
             while (!mbar_try_wait(&S.mbar, parity)) { }
             parity ^= 1;
-            MemPtr<false, true> mem{S.in + head};
-            scan_par_block(S, mem, n, cap, marks, markCap, r, ns);
-        } else if (wide && n > 65535) {
-            MemPtr<true, true> mem{src};
-            scan_par_block(S, mem, n, cap, marks, markCap, r, ns);
-        } else if (n > 0 && n <= 65535 && cap > 0) {
-            const int head = (int)(reinterpret_cast<uintptr_t>(src) & 15);
-            const uint32_t loadBytes = (uint32_t)((head + n + 15) & ~15);
-            if (tid == 0) {
-                mbar_expect_tx(&S.mbar, loadBytes);
-                for (uint32_t o = 0; o < loadBytes; o += 16384u)
-                    tma_load_1d(S.in + o, src - head + o, min(16384u, loadBytes - o), &S.mbar);
-            }
-            while (!mbar_try_wait(&S.mbar, parity)) { }
-            parity ^= 1;
-            MemPtr<false> mem{S.in + head};
-            scan_par_block(S, mem, n, cap, marks, w.markStride, r, ns);
-        } else if (n > 65535 && cap >= 64) {
-            MemPtr<true> mem{src};
-            scan_par_block(S, mem, n, cap, marks, w.markStride, r, ns);
-        } else {                                               /* degenerate arguments: the one-thread code decides (lz4.c:2036, :2064-2069) */
+            if (wide) lanes(MemPtr<false, true>{S.in + head});
+            else lanes(MemPtr<false>{S.in + head});
+        } else if (n > 65535 && cap >= 64) {                      /* walked in global memory */
+            if (wide) lanes(MemPtr<true, true>{src});
+            else lanes(MemPtr<true>{src});
+        } else {                                                   /* degenerate arguments: the one-thread code decides (lz4.c:2036, :2064-2069) */
             if (tid == 0) { uint32_t q = 0; MemPtr<true> mem{src}; S.sp.ret = scan_block(mem, n, cap, &q, nullptr, 0u); S.sp.nseq = q; }
             __syncthreads();
             r = S.sp.ret; ns = S.sp.nseq;
             __syncthreads();
         }
-        if (tid == 0) {
-            a.outSize[b] = r;
-            w.nSeq[b] = ns;
-            const bool tiled = wide && ns <= markCap;                 /* lz4_expand_tiles_kernel takes it */
-            if (r > 0 && !tiled && !rows_eligible(n, cap, ns, w.markStride)) w.slowList[atomicAdd(&w.hdr->slowCount, 1u)] = (uint32_t)b;
-        }
+        if (tid == 0) scan_result(a, w, b, n, cap, r, ns, wide && ns <= markCap);   /* tiled: lz4_expand_tiles_kernel takes it */
     }
 }
 
@@ -468,11 +460,8 @@ __global__ void __launch_bounds__(128) lz4_expand_generic_kernel(lz4k_decode_arg
  *                    rank -> delta -> (follow sources inside the wave) -> LDS.U8 -> STS.U8
  *   TMA bulk store : decoded block smem -> HBM
  * ============================================================================================= */
-#ifndef LZ4K_ROWS_RPT
-#define LZ4K_ROWS_RPT 4                      /* rows per thread per wave: wave = 1024 * RPT bytes */
-#endif
 constexpr int kRowsThreads = 1024;
-constexpr int kRowsRpt = LZ4K_ROWS_RPT;
+constexpr int kRowsRpt = 4;                  /* rows per thread per wave: wave = 1024 * kRowsRpt bytes */
 constexpr int kWave = kRowsThreads * kRowsRpt;
 constexpr int kRowsCache = 3;                /* sequences per thread whose parse is kept in registers between the passes */
 
@@ -532,51 +521,150 @@ __device__ __forceinline__ uint32_t lanemask_le()
     return m;
 }
 
-/* Source addresses of one thread's bytes of a wave: bytes p0 + r*1024 (r < kRowsRpt) of the wave that starts at shared
- * address waveS.  FULL: the whole wave lies inside the block (no bounds checks).  All addresses are 32-bit
- * shared-window addresses.  Nothing here reads the output window: the run table alone decides where a byte comes
- * from, so a warp resolves wave w+1 while other warps still copy wave w. */
-template <bool FULL>
-__device__ __forceinline__ void rows_resolve(uint32_t (&sa)[LZ4K_ROWS_RPT], const uint32_t p0, const uint32_t waveS,
-                                             const uint32_t lim, const uint32_t outS, const uint32_t rowsS,
-                                             const uint32_t tabS, const uint32_t zeroS, const uint32_t le)
+/* ---- the phases of a window shared by lz4_expand_rows_kernel and lz4_expand_tiles_kernel ---- */
+
+/* rank: rows[r].y = (number of run starts in rows [0, r)) - 1.  Returns the number of runs. */
+__device__ __forceinline__ uint32_t rows_rank(RowsSmem& S)
 {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    constexpr int WPT = 2048 / kRowsThreads;
+    uint32_t cnt[WPT], x = 0;
+    #pragma unroll
+    for (int j = 0; j < WPT; j++) { cnt[j] = __popc(S.rows[tid * WPT + j].x); x += cnt[j]; }
+    uint32_t incl = x;
+    #pragma unroll
+    for (int dd = 1; dd < 32; dd <<= 1) { uint32_t y = __shfl_up_sync(kFull, incl, dd); if (lane >= dd) incl += y; }
+    if (lane == 31) S.warpSum[warp] = incl;
+    __syncthreads();
+    if (warp == 0) {
+        uint32_t v = S.warpSum[lane];
+        #pragma unroll
+        for (int dd = 1; dd < 32; dd <<= 1) { uint32_t y = __shfl_up_sync(kFull, v, dd); if (lane >= dd) v += y; }
+        S.warpSum[lane] = v;
+        if (lane == 31) S.nRuns = v;
+    }
+    __syncthreads();
+    uint32_t ex = incl - x + (warp ? S.warpSum[warp - 1] : 0);
+    #pragma unroll
+    for (int j = 0; j < WPT; j++) { S.rows[tid * WPT + j].y = ex - 1u; ex += cnt[j]; }
+    return S.nRuns;
+}
+
+/* Source addresses of one thread's bytes of a wave: bytes p0 + r*1024 (r < kRowsRpt) of the window at shared address outS.
+ * FULL: the whole wave lies inside the window (no bounds checks); otherwise bytes at or past `lim` get `pastEnd`, an
+ * address the wave's fetch may read and that never tests as inside the wave.  A source x lies inside the wave being
+ * resolved when key(x) >= keyFloor; those are followed through the run table again.  The test is written this way so
+ * that "any row inside" is one maximum and one compare.  All addresses are 32-bit shared-window addresses.  Nothing here
+ * reads the output window: the run table alone decides where a byte comes from, so a warp resolves wave w+1 while other
+ * warps still copy wave w. */
+template <bool FULL, class Key>
+__device__ __forceinline__ void rows_resolve(uint32_t (&sa)[kRowsRpt], const uint32_t p0, const uint32_t lim,
+                                             const uint32_t outS, const uint32_t rowsS, const uint32_t tabS,
+                                             const uint32_t pastEnd, const uint32_t le, Key&& key, const uint32_t keyFloor)
+{
+    static_assert(kRowsThreads == 1024, "rows_resolve assumes 1024 threads (32 rows per wave slice)");
     const uint32_t rowAddr = rowsS + ((p0 >> 5) << 3);
     #pragma unroll
-    for (int r = 0; r < LZ4K_ROWS_RPT; r++) {
-        sa[r] = zeroS;
+    for (int r = 0; r < kRowsRpt; r++) {
+        sa[r] = pastEnd;
         if (FULL || p0 + (uint32_t)(r * 1024) < lim) {
             const uint2 row = lds_u64(rowAddr + (uint32_t)(r * 32 * 8));
             const uint32_t j = row.y + (uint32_t)__popc(row.x & le);
             sa[r] = outS + p0 + (uint32_t)(r * 1024) + lds_u32(tabS + (j << 2));
         }
     }
-    uint32_t hi = sa[0];
+    uint32_t hi = key(sa[0]);
     #pragma unroll
-    for (int r = 1; r < LZ4K_ROWS_RPT; r++) hi = max(hi, sa[r]);
-    while (hi >= waveS) {                                      /* sources inside this wave: follow them, all rows of the thread at once */
+    for (int r = 1; r < kRowsRpt; r++) hi = max(hi, key(sa[r]));
+    while (hi >= keyFloor) {                                   /* sources inside this wave: follow them, all rows of the thread at once */
         hi = 0;
         #pragma unroll
-        for (int r = 0; r < LZ4K_ROWS_RPT; r++) {
+        for (int r = 0; r < kRowsRpt; r++) {
             uint32_t x = sa[r];
-            if (x >= waveS) {
+            if (key(x) >= keyFloor) {
                 const uint32_t q = x - outS;
                 const uint2 row = lds_u64(rowsS + ((q >> 5) << 3));
                 const uint32_t j = row.y + (uint32_t)__popc(row.x & (0xFFFFFFFFu >> (31u - (q & 31u))));
                 x += lds_u32(tabS + (j << 2));
                 sa[r] = x;
             }
-            hi = max(hi, x);
+            hi = max(hi, key(x));
         }
+    }
+}
+
+/* The waves over the window's bytes [0, len) at shared address outS: thread t writes bytes t, t + 1024, ... of every
+ * kWave-byte wave.  resolve(sa, wv) sets the source addresses of the thread's bytes of wave wv (rows_resolve); fetch(x)
+ * reads the byte at source address x, also for bytes past the end (they are not stored).  A warp arrives on the wave
+ * barrier once its bytes of a wave are written and then resolves the next wave while other warps still copy; `wpar` is
+ * the wave barrier's phase parity, carried from window to window.  On return the window is written and visible to the
+ * bulk store. */
+template <class Resolve, class Fetch>
+__device__ __forceinline__ void rows_waves(RowsSmem& S, const uint32_t outS, const int len, uint32_t& wpar,
+                                           Resolve&& resolve, Fetch&& fetch)
+{
+    const int tid = threadIdx.x;
+    const int nWaves = (len + kWave - 1) / kWave;
+    uint32_t sa[kRowsRpt];
+    auto copy = [&](int wv) {
+        const uint32_t p0 = (uint32_t)(wv * kWave + tid);
+        const uint32_t lim = ((wv + 1) * kWave <= len) ? 0xFFFFFFFFu : (uint32_t)len;
+        uint32_t v[kRowsRpt];
+        #pragma unroll
+        for (int r = 0; r < kRowsRpt; r++) v[r] = fetch(sa[r]);
+        #pragma unroll
+        for (int r = 0; r < kRowsRpt; r++)
+            if (p0 + (uint32_t)(r * kRowsThreads) < lim) sts_u8(outS + p0 + (uint32_t)(r * kRowsThreads), v[r]);
+        if (wv == nWaves - 1) fence_proxy_async();         /* generic-proxy writes of `out` before the bulk store reads them */
+    };
+#ifdef LZ4K_WAVE_BARSYNC
+    /* debug build: the same waves with a plain CTA barrier instead of the split mbarrier (no overlap of the resolve with
+     * the wait).  compute-sanitizer's racecheck does not model mbarrier arrive / wait as synchronisation; this variant
+     * shows that the wave structure itself is hazard free. */
+    for (int wv = 0; wv < nWaves; wv++) {
+        resolve(sa, wv);
+        copy(wv);
+        __syncthreads();
+    }
+#else
+    resolve(sa, 0);
+    for (int wv = 0; wv < nWaves; wv++) {
+        if (wv > 0) { mbar_wait(&S.wbar, wpar); wpar ^= 1; }   /* every warp has copied wave wv-1 */
+        copy(wv);
+        __syncwarp();
+        if ((tid & 31) == 0) mbar_arrive(&S.wbar);         /* release: this warp's bytes of wave wv are written */
+        if (wv + 1 < nWaves) resolve(sa, wv + 1);
+    }
+    mbar_wait(&S.wbar, wpar);
+    wpar ^= 1;
+#endif
+}
+
+/* the window's bytes [0, len) -> dst: if dst is 16-byte aligned, TMA bulk stores of the 16-byte multiple (thread 0, one
+ * commit group) and plain stores of the tail; plain stores throughout otherwise.  FENCE: every thread's plain stores are
+ * followed by __threadfence(). */
+template <bool FENCE>
+__device__ __forceinline__ void rows_store(uint8_t* dst, const uint8_t* out, const int len)
+{
+    const int tid = threadIdx.x;
+    if ((reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+        const uint32_t bulk = (uint32_t)len & ~15u;
+        if (tid == 0 && bulk) {
+            for (uint32_t o = 0; o < bulk; o += 16384u) tma_store_1d(dst + o, out + o, min(16384u, bulk - o));
+            tma_commit();
+        }
+        if (tid < (len & 15)) { dst[bulk + tid] = out[bulk + tid]; if (FENCE) __threadfence(); }
+    } else {
+        for (int k = tid; k < len; k += kRowsThreads) dst[k] = out[k];
+        if (FENCE) __threadfence();
     }
 }
 
 __global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_rows_kernel(lz4k_decode_args a)
 {
-    static_assert(kRowsThreads == 1024, "rows_resolve assumes 1024 threads (32 rows per wave slice)");
     extern __shared__ __align__(16) uint8_t smemRaw[];
     RowsSmem& S = *reinterpret_cast<RowsSmem*>(smemRaw);
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const WsView w = ws_view(a);
     const uint32_t le = lanemask_le();
     const uint32_t outA = (uint32_t)offsetof(RowsSmem, out);
@@ -609,13 +697,7 @@ __global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_rows_kernel(lz4k_d
         }
         return d;
     };
-    auto issueLoad = [&](const RowsDesc& d) {                     /* thread 0: TMA bulk load of the compressed block */
-        const int head = (int)(reinterpret_cast<uintptr_t>(d.src) & 15);
-        const uint32_t loadBytes = (uint32_t)((head + d.n + 15) & ~15);
-        mbar_expect_tx(&S.mbar, loadBytes);
-        for (uint32_t o = 0; o < loadBytes; o += 16384u)
-            tma_load_1d(S.in + o, d.src - head + o, min(16384u, loadBytes - o), &S.mbar);
-    };
+    auto issueLoad = [&](const RowsDesc& d) { tma_stage(S.in, d.src, d.n, &S.mbar); };   /* thread 0 */
 
     if (tid == 0) { mbar_init(&S.mbar, 1); mbar_init(&S.wbar, kRowsThreads / 32); }
     if (tid < 4) reinterpret_cast<uint32_t*>(S.zero)[tid] = 0;
@@ -681,30 +763,7 @@ __global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_rows_kernel(lz4k_d
         __syncthreads();
         PHASE_MARK(2);                                     // pass 1
 
-        /* ---- rank: rows[r].y = (number of run starts in rows [0, r)) - 1 ---- */
-        {
-            constexpr int WPT = 2048 / kRowsThreads;
-            uint32_t cnt[WPT], x = 0;
-            #pragma unroll
-            for (int j = 0; j < WPT; j++) { cnt[j] = __popc(S.rows[tid * WPT + j].x); x += cnt[j]; }
-            uint32_t incl = x;
-            #pragma unroll
-            for (int dd = 1; dd < 32; dd <<= 1) { uint32_t y = __shfl_up_sync(kFull, incl, dd); if (lane >= dd) incl += y; }
-            if (lane == 31) S.warpSum[warp] = incl;
-            __syncthreads();
-            if (warp == 0) {
-                uint32_t v = S.warpSum[lane];
-                #pragma unroll
-                for (int dd = 1; dd < 32; dd <<= 1) { uint32_t y = __shfl_up_sync(kFull, v, dd); if (lane >= dd) v += y; }
-                S.warpSum[lane] = v;
-                if (lane == 31) S.nRuns = v;
-            }
-            __syncthreads();
-            uint32_t ex = incl - x + (warp ? S.warpSum[warp - 1] : 0);
-            #pragma unroll
-            for (int j = 0; j < WPT; j++) { S.rows[tid * WPT + j].y = ex - 1u; ex += cnt[j]; }
-        }
-        const uint32_t nRuns = S.nRuns;
+        const uint32_t nRuns = rows_rank(S);
         if (tid == 0) tma_wait_read0();                    /* the previous block's bulk store has finished reading S.out */
         __syncthreads();
         PHASE_MARK(3);                                     // rank
@@ -732,50 +791,13 @@ __global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_rows_kernel(lz4k_d
             PHASE_MARK(4);                                     // pass 2
 
             /* ---- waves: resolve (run table only) | wait for the previous wave | copy | arrive ---- */
-            const int nWaves = (total + kWave - 1) / kWave;
-            uint32_t sa[kRowsRpt];
-            auto resolve = [&](int wv) {
-                const uint32_t p0 = (uint32_t)(wv * kWave + tid);
-                if ((wv + 1) * kWave <= total) rows_resolve<true>(sa, p0, outS + (uint32_t)(wv * kWave), 0xFFFFFFFFu, outS, rowsS, tabS, zeroS, le);
-                else rows_resolve<false>(sa, p0, outS + (uint32_t)(wv * kWave), (uint32_t)total, outS, rowsS, tabS, zeroS, le);
+            auto resolve = [&](uint32_t (&sa)[kRowsRpt], int wv) {
+                const uint32_t p0 = (uint32_t)(wv * kWave + tid), waveS = outS + (uint32_t)(wv * kWave);
+                auto key = [](uint32_t x) { return x; };           /* inside the wave: x >= waveS */
+                if ((wv + 1) * kWave <= total) rows_resolve<true>(sa, p0, 0xFFFFFFFFu, outS, rowsS, tabS, zeroS, le, key, waveS);
+                else rows_resolve<false>(sa, p0, (uint32_t)total, outS, rowsS, tabS, zeroS, le, key, waveS);
             };
-#ifdef LZ4K_WAVE_BARSYNC
-            /* debug build: the same waves with a plain CTA barrier instead of the split mbarrier (no overlap of the
-             * resolve with the wait).  compute-sanitizer's racecheck does not model mbarrier arrive / wait as
-             * synchronisation; this variant shows that the wave structure itself is hazard free. */
-            for (int wv = 0; wv < nWaves; wv++) {
-                resolve(wv);
-                const uint32_t p0 = (uint32_t)(wv * kWave + tid);
-                const uint32_t lim = ((wv + 1) * kWave <= total) ? 0xFFFFFFFFu : (uint32_t)total;
-                uint32_t v[kRowsRpt];
-                #pragma unroll
-                for (int r = 0; r < kRowsRpt; r++) v[r] = lds_u8(sa[r]);
-                #pragma unroll
-                for (int r = 0; r < kRowsRpt; r++)
-                    if (p0 + (uint32_t)(r * kRowsThreads) < lim) sts_u8(outS + p0 + (uint32_t)(r * kRowsThreads), v[r]);
-                if (wv == nWaves - 1) fence_proxy_async();
-                __syncthreads();
-            }
-#else
-            resolve(0);
-            for (int wv = 0; wv < nWaves; wv++) {
-                if (wv > 0) { mbar_wait(&S.wbar, wpar); wpar ^= 1; }   /* every warp has copied wave wv-1 */
-                const uint32_t p0 = (uint32_t)(wv * kWave + tid);
-                const uint32_t lim = ((wv + 1) * kWave <= total) ? 0xFFFFFFFFu : (uint32_t)total;
-                uint32_t v[kRowsRpt];
-                #pragma unroll
-                for (int r = 0; r < kRowsRpt; r++) v[r] = lds_u8(sa[r]);
-                #pragma unroll
-                for (int r = 0; r < kRowsRpt; r++)
-                    if (p0 + (uint32_t)(r * kRowsThreads) < lim) sts_u8(outS + p0 + (uint32_t)(r * kRowsThreads), v[r]);
-                if (wv == nWaves - 1) fence_proxy_async();     /* generic-proxy writes of `out` before the bulk store reads them */
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&S.wbar);           /* release: this warp's bytes of wave wv are written */
-                if (wv + 1 < nWaves) resolve(wv + 1);
-            }
-            mbar_wait(&S.wbar, wpar);
-            wpar ^= 1;
-#endif
+            rows_waves(S, outS, total, wpar, resolve, [](uint32_t x) { return lds_u8(x); });
             PHASE_MARK(5);                                     // waves
         }
 
@@ -786,19 +808,7 @@ __global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_rows_kernel(lz4k_d
             if (dn.n > 0) issueLoad(dn);
         }
         /* ---- store: smem -> HBM ---- */
-        if (!tooMany) {
-            uint8_t* dst = d.dst;
-            if ((reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
-                const uint32_t bulk = (uint32_t)total & ~15u;
-                if (tid == 0 && bulk) {
-                    for (uint32_t o = 0; o < bulk; o += 16384u) tma_store_1d(dst + o, S.out + o, min(16384u, bulk - o));
-                    tma_commit();
-                }
-                if (tid < (total & 15)) dst[bulk + tid] = S.out[bulk + tid];
-            } else {
-                for (int k = tid; k < total; k += kRowsThreads) dst[k] = S.out[k];
-            }
-        }
+        if (!tooMany) rows_store<false>(d.dst, S.out, total);
         __syncthreads();                                   /* desc[(it+1)&1] is visible; `out` tail reads are done */
         PHASE_MARK(6);                                     // store issue
     }
@@ -836,45 +846,11 @@ __device__ __forceinline__ void st_release_gpu(uint32_t* p, uint32_t v)
     asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
-template <bool FULL>
-__device__ __forceinline__ void tiles_resolve(uint32_t (&sa)[LZ4K_ROWS_RPT], const uint32_t p0, const uint32_t waveS,
-                                              const uint32_t lim, const uint32_t outS, const uint32_t rowsS,
-                                              const uint32_t tabS, const uint32_t le)
-{
-    const uint32_t rowAddr = rowsS + ((p0 >> 5) << 3);
-    bool any = false;
-    #pragma unroll
-    for (int r = 0; r < LZ4K_ROWS_RPT; r++) {
-        sa[r] = outS + 65536u;                                  /* (a byte past the tile: never read, never "inside the wave") */
-        if (FULL || p0 + (uint32_t)(r * 1024) < lim) {
-            const uint2 row = lds_u64(rowAddr + (uint32_t)(r * 32 * 8));
-            const uint32_t j = row.y + (uint32_t)__popc(row.x & le);
-            sa[r] = outS + p0 + (uint32_t)(r * 1024) + lds_u32(tabS + (j << 2));
-        }
-        any |= (sa[r] - waveS) < (uint32_t)kWave;
-    }
-    while (any) {                                               /* sources inside this wave: follow them */
-        any = false;
-        #pragma unroll
-        for (int r = 0; r < LZ4K_ROWS_RPT; r++) {
-            uint32_t x = sa[r];
-            if ((x - waveS) < (uint32_t)kWave) {
-                const uint32_t q = x - outS;
-                const uint2 row = lds_u64(rowsS + ((q >> 5) << 3));
-                const uint32_t j = row.y + (uint32_t)__popc(row.x & (0xFFFFFFFFu >> (31u - (q & 31u))));
-                x += lds_u32(tabS + (j << 2));
-                sa[r] = x;
-            }
-            any |= (x - waveS) < (uint32_t)kWave;
-        }
-    }
-}
-
 __global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_tiles_kernel(lz4k_decode_args a)
 {
     extern __shared__ __align__(16) uint8_t smemRaw[];
     RowsSmem& S = *reinterpret_cast<RowsSmem*>(smemRaw);
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const WsView w = ws_view(a);
     const uint32_t le = lanemask_le();
     const uint32_t sBase = smem_u32(smemRaw);
@@ -929,31 +905,8 @@ __global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_tiles_kernel(lz4k_
             rw_tile_runs(s, os, oe, litBase, zeroDelta0, [&](int st, int) { atomicOr(&S.rows[st >> 5].x, 1u << (st & 31)); });
         }
         __syncthreads();
-        /* ---- rank ---- */
-        {
-            constexpr int WPT = 2048 / kRowsThreads;
-            uint32_t cnt[WPT], x = 0;
-            #pragma unroll
-            for (int j = 0; j < WPT; j++) { cnt[j] = __popc(S.rows[tid * WPT + j].x); x += cnt[j]; }
-            uint32_t incl = x;
-            #pragma unroll
-            for (int dd = 1; dd < 32; dd <<= 1) { uint32_t y = __shfl_up_sync(kFull, incl, dd); if (lane >= dd) incl += y; }
-            if (lane == 31) S.warpSum[warp] = incl;
-            __syncthreads();
-            if (warp == 0) {
-                uint32_t v = S.warpSum[lane];
-                #pragma unroll
-                for (int dd = 1; dd < 32; dd <<= 1) { uint32_t y = __shfl_up_sync(kFull, v, dd); if (lane >= dd) v += y; }
-                S.warpSum[lane] = v;
-                if (lane == 31) S.nRuns = v;
-            }
-            __syncthreads();
-            uint32_t ex = incl - x + (warp ? S.warpSum[warp - 1] : 0);
-            #pragma unroll
-            for (int j = 0; j < WPT; j++) { S.rows[tid * WPT + j].y = ex - 1u; ex += cnt[j]; }
-        }
-        const uint32_t nRuns = S.nRuns;
-        if (tid == 0) publishPending();                        /* the previous unit's store is complete: its flag goes up, `out` is free */
+        const uint32_t nRuns = rows_rank(S);
+        if (tid == 0) publishPending();                       /* the previous unit's store is complete: its flag goes up, `out` is free */
         __syncthreads();
         if (nRuns > (uint32_t)kRowsMaxRuns) {                  /* (pathological) the generic kernel redoes the whole block */
             if (tid == 0) {
@@ -980,84 +933,24 @@ __global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_tiles_kernel(lz4k_
             if (tid == 0) { while (ld_acquire_gpu(&flags[t - 1]) == 0u) __nanosleep(200); }
             __syncthreads();
         }
-        /* ---- waves ---- */
-        {
-            const int nWaves = (len + kWave - 1) / kWave;
-            uint32_t sa[kRowsRpt];
-            auto resolve = [&](int wv) {
-                const uint32_t p0 = (uint32_t)(wv * kWave + tid);
-                if ((wv + 1) * kWave <= len) tiles_resolve<true>(sa, p0, outS + (uint32_t)(wv * kWave), 0xFFFFFFFFu, outS, rowsS, tabS, le);
-                else tiles_resolve<false>(sa, p0, outS + (uint32_t)(wv * kWave), (uint32_t)len, outS, rowsS, tabS, le);
-            };
-#ifdef LZ4K_WAVE_BARSYNC
-            /* debug build (see lz4_expand_rows_kernel): a plain CTA barrier between the waves, for compute-sanitizer's racecheck */
-            for (int wv = 0; wv < nWaves; wv++) {
-                resolve(wv);
-                const uint32_t p0 = (uint32_t)(wv * kWave + tid);
-                const uint32_t lim = ((wv + 1) * kWave <= len) ? 0xFFFFFFFFu : (uint32_t)len;
-                uint32_t v[kRowsRpt];
-                #pragma unroll
-                for (int r = 0; r < kRowsRpt; r++) {
-                    const uint32_t x = sa[r];
-                    v[r] = 0u;
-                    if (p0 + (uint32_t)(r * kRowsThreads) < lim) {
-                        if (x >= kLitBase) v[r] = (x == kZeroV) ? 0u : (uint32_t)__ldg(src + (x - kLitBase));
-                        else if (x >= outS) v[r] = lds_u8(x);
-                        else v[r] = (uint32_t)__ldcg(dstB + (os - (int)(outS - x)));
-                    }
-                }
-                #pragma unroll
-                for (int r = 0; r < kRowsRpt; r++)
-                    if (p0 + (uint32_t)(r * kRowsThreads) < lim) sts_u8(outS + p0 + (uint32_t)(r * kRowsThreads), v[r]);
-                if (wv == nWaves - 1) fence_proxy_async();
-                __syncthreads();
-            }
-#else
-            resolve(0);
-            for (int wv = 0; wv < nWaves; wv++) {
-                if (wv > 0) { mbar_wait(&S.wbar, wpar); wpar ^= 1; }   /* every warp has copied wave wv-1 */
-                const uint32_t p0 = (uint32_t)(wv * kWave + tid);
-                const uint32_t lim = ((wv + 1) * kWave <= len) ? 0xFFFFFFFFu : (uint32_t)len;
-                uint32_t v[kRowsRpt];
-                #pragma unroll
-                for (int r = 0; r < kRowsRpt; r++) {
-                    const uint32_t x = sa[r];
-                    v[r] = 0u;
-                    if (p0 + (uint32_t)(r * kRowsThreads) < lim) {
-                        if (x >= kLitBase) v[r] = (x == kZeroV) ? 0u : (uint32_t)__ldg(src + (x - kLitBase));
-                        else if (x >= outS) v[r] = lds_u8(x);
-                        else v[r] = (uint32_t)__ldcg(dstB + (os - (int)(outS - x)));
-                    }
-                }
-                #pragma unroll
-                for (int r = 0; r < kRowsRpt; r++)
-                    if (p0 + (uint32_t)(r * kRowsThreads) < lim) sts_u8(outS + p0 + (uint32_t)(r * kRowsThreads), v[r]);
-                if (wv == nWaves - 1) fence_proxy_async();     /* generic-proxy writes of `out` before the bulk store reads them */
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&S.wbar);
-                if (wv + 1 < nWaves) resolve(wv + 1);
-            }
-            mbar_wait(&S.wbar, wpar);
-            wpar ^= 1;
-#endif
-        }
-        /* ---- store: smem -> HBM ---- */
-        {
-            uint8_t* dst = dstB + os;
-            if ((reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
-                const uint32_t bulk = (uint32_t)len & ~15u;
-                if (tid == 0 && bulk) {
-                    for (uint32_t o = 0; o < bulk; o += 16384u) tma_store_1d(dst + o, S.out + o, min(16384u, bulk - o));
-                    tma_commit();
-                }
-                if (tid < (len & 15)) { dst[bulk + tid] = S.out[bulk + tid]; __threadfence(); }
-            } else {
-                for (int k = tid; k < len; k += kRowsThreads) dst[k] = S.out[k];
-                __threadfence();
-            }
-            if (tid == 0) pendFlag = &flags[t];
-        }
-        __syncthreads();                                       /* `out` tail reads are done; direct stores are fenced */
+        /* ---- waves: a source x is a compressed byte (x >= kLitBase), a byte of this tile, or one of an earlier tile ---- */
+        auto resolve = [&](uint32_t (&sa)[kRowsRpt], int wv) {
+            const uint32_t p0 = (uint32_t)(wv * kWave + tid), waveE = outS + (uint32_t)((wv + 1) * kWave);
+            /* inside the wave: (x - waveS) < kWave, i.e. x - waveE >= -kWave; not x >= waveS, since the literal sources
+             * lie above the window.  Bytes past the tile get outS + 65536: never inside a wave, and readable by the fetch. */
+            auto key = [waveE](uint32_t x) { return x - waveE; };
+            if ((wv + 1) * kWave <= len) rows_resolve<true>(sa, p0, 0xFFFFFFFFu, outS, rowsS, tabS, outS + 65536u, le, key, 0u - (uint32_t)kWave);
+            else rows_resolve<false>(sa, p0, (uint32_t)len, outS, rowsS, tabS, outS + 65536u, le, key, 0u - (uint32_t)kWave);
+        };
+        rows_waves(S, outS, len, wpar, resolve, [&](uint32_t x) {
+            if (x >= kLitBase) return (x == kZeroV) ? 0u : (uint32_t)__ldg(src + (x - kLitBase));
+            if (x >= outS) return lds_u8(x);
+            return (uint32_t)__ldcg(dstB + (os - (int)(outS - x)));
+        });
+        /* ---- store: smem -> HBM; the plain stores are fenced before the flag goes up ---- */
+        rows_store<true>(dstB + os, S.out, len);
+        if (tid == 0) pendFlag = &flags[t];
+        __syncthreads();                                      /* `out` tail reads are done; direct stores are fenced */
     }
     if (tid == 0) publishPending();
 }
@@ -1077,14 +970,7 @@ __global__ void __launch_bounds__(kRowsThreads, 1) lz4_ceiling_kernel(lz4k_decod
     const uint32_t sBase = smem_u32(smemRaw);
     const uint32_t outS = sBase + (uint32_t)offsetof(RowsSmem, out), inS = sBase + (uint32_t)offsetof(RowsSmem, in);
     uint32_t parity = 0;
-    auto issueLoad = [&](int64_t b) {
-        const uint8_t* src = a.src + a.srcOff[b];
-        const int n = a.srcSize[b];
-        const int head = (int)(reinterpret_cast<uintptr_t>(src) & 15);
-        const uint32_t loadBytes = (uint32_t)((head + n + 15) & ~15);
-        mbar_expect_tx(&S.mbar, loadBytes);
-        for (uint32_t o = 0; o < loadBytes; o += 16384u) tma_load_1d(S.in + o, src - head + o, min(16384u, loadBytes - o), &S.mbar);
-    };
+    auto issueLoad = [&](int64_t b) { tma_stage(S.in, a.src + a.srcOff[b], a.srcSize[b], &S.mbar); };
     if (tid == 0) { mbar_init(&S.mbar, 1); }
     __syncthreads();
     if (tid == 0 && blockIdx.x < a.nBlocks) issueLoad(blockIdx.x);
@@ -1432,6 +1318,28 @@ __global__ void __launch_bounds__(256) lz4_pack_gather_kernel(const uint8_t* __r
 /* =============================================================================================
  * extern "C" launchers
  * ============================================================================================= */
+static int device_sms()
+{
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    return sms;
+}
+
+static int launch_pack(const uint8_t* slots, int64_t slotStride, const int32_t* sizes, int64_t nBlocks, uint8_t* packed,
+                       int64_t* outOff, int headerBytes, FrameRule fr, cudaStream_t s)
+{
+    lz4_pack_scan_kernel<<<1, 1024, 0, s>>>(sizes, nBlocks, outOff, headerBytes, fr);
+    g_launches++;
+    if (nBlocks > 0) {
+        const int64_t cap = (int64_t)device_sms() * 16;
+        int64_t grid = nBlocks < cap ? nBlocks : cap;
+        lz4_pack_gather_kernel<<<(unsigned)grid, 256, 0, s>>>(slots, slotStride, sizes, nBlocks, packed, outOff, headerBytes, fr);
+        g_launches++;
+    }
+    return (int)cudaGetLastError();
+}
+
 extern "C" {
 
 uint64_t lz4k_launch_count(void) { return g_launches; }
@@ -1478,9 +1386,7 @@ int lz4k_launch_decode(const lz4k_decode_args* a, int phases, void* stream)
     const bool wide = use_wide(a->dstCapArr, a->dstCap, a->nBlocks, a->workspaceBytes);
     static int sms = 0, scanImpl = -1;
     if (sms == 0) {
-        int dev = 0, v = 132;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
+        const int v = device_sms();
         /* opt in to the large dynamic shared memory (once; every device of a process runs the same kernels) */
         cudaError_t e = cudaFuncSetAttribute(lz4_expand_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RowsSmem));
         if (e == cudaSuccess) e = cudaFuncSetAttribute(lz4_scan_par_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ScanParSmem));
@@ -1554,9 +1460,7 @@ int lz4k_launch_encode(const lz4k_encode_args* a, void* stream)
 {
     cudaStream_t s = (cudaStream_t)stream;
     if (a->nBlocks == 0) return 0;
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int sms = device_sms();
     const int perSm = 13;    // 16 KB table per warp: 13 x 16 KB + reserved fits the 228 KB SM
     int64_t grid = (int64_t)sms * perSm;
     if (grid > a->nBlocks) grid = a->nBlocks;
@@ -1576,9 +1480,7 @@ __global__ void __launch_bounds__(kEpThreads, 2) lz4_poison_smem_kernel(uint32_t
 }
 int lz4k_debug_poison_smem(uint32_t pattern, int lo, int hi, void* stream)
 {
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int sms = device_sms();
     cudaError_t e = cudaFuncSetAttribute(lz4_poison_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(EncParSmem));
     if (e != cudaSuccess) return (int)e;
     if (hi > (int)sizeof(EncParSmem)) hi = (int)sizeof(EncParSmem);
@@ -1590,9 +1492,7 @@ int lz4k_launch_ceiling(const lz4k_decode_args* a, int mode, void* stream)
 {
     cudaStream_t s = (cudaStream_t)stream;
     if (a->nBlocks == 0) return 0;
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int sms = device_sms();
     cudaError_t e = cudaFuncSetAttribute(lz4_ceiling_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RowsSmem));
     if (e != cudaSuccess) return (int)e;
     const int64_t grid = a->nBlocks < sms ? a->nBlocks : sms;
@@ -1606,12 +1506,9 @@ int lz4k_launch_encode_par(const lz4k_encode_args* a, void* stream)
     if (a->nBlocks == 0) return 0;
     static int sms = 0;
     if (sms == 0) {
-        int dev = 0, v = 132;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
         cudaError_t e = cudaFuncSetAttribute(lz4_encode_par_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(EncParSmem));
         if (e != cudaSuccess) return (int)e;
-        sms = v;
+        sms = device_sms();
     }
     const int64_t grid = a->nBlocks < 2 * sms ? a->nBlocks : 2 * sms;        // persistent: two CTAs per SM, blocks c, c + grid, ...
     lz4_encode_par_kernel<<<(unsigned)grid, kEpThreads, sizeof(EncParSmem), s>>>(*a);
@@ -1619,45 +1516,19 @@ int lz4k_launch_encode_par(const lz4k_encode_args* a, void* stream)
     return (int)cudaGetLastError();
 }
 
-static int device_sms()
-{
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    return sms;
-}
-
 int lz4k_launch_pack(const uint8_t* slots, int64_t slotStride, const int32_t* sizes, int64_t nBlocks,
                      uint8_t* packed, int64_t* outOff, int headerBytes, void* stream)
 {
-    cudaStream_t s = (cudaStream_t)stream;
     FrameRule fr; fr.raw = nullptr; fr.rawStride = 0; fr.blockSize = 0; fr.lastSize = 0;
-    lz4_pack_scan_kernel<<<1, 1024, 0, s>>>(sizes, nBlocks, outOff, headerBytes, fr);
-    g_launches++;
-    if (nBlocks > 0) {
-        const int64_t cap = (int64_t)device_sms() * 16;
-        int64_t grid = nBlocks < cap ? nBlocks : cap;
-        lz4_pack_gather_kernel<<<(unsigned)grid, 256, 0, s>>>(slots, slotStride, sizes, nBlocks, packed, outOff, headerBytes, fr);
-        g_launches++;
-    }
-    return (int)cudaGetLastError();
+    return launch_pack(slots, slotStride, sizes, nBlocks, packed, outOff, headerBytes, fr, (cudaStream_t)stream);
 }
 
 /* frame body: [LE32 header][payload] per block, stored-raw rule applied on the device (src = the blocks' source bytes) */
 int lz4k_launch_pack_frame(const uint8_t* slots, int64_t slotStride, const int32_t* sizes, const uint8_t* src, int64_t srcStride,
                            int32_t blockSize, int32_t lastSize, int64_t nBlocks, uint8_t* packed, int64_t* outOff, void* stream)
 {
-    cudaStream_t s = (cudaStream_t)stream;
     FrameRule fr; fr.raw = src; fr.rawStride = srcStride; fr.blockSize = blockSize; fr.lastSize = lastSize;
-    lz4_pack_scan_kernel<<<1, 1024, 0, s>>>(sizes, nBlocks, outOff, 4, fr);
-    g_launches++;
-    if (nBlocks > 0) {
-        const int64_t cap = (int64_t)device_sms() * 16;
-        int64_t grid = nBlocks < cap ? nBlocks : cap;
-        lz4_pack_gather_kernel<<<(unsigned)grid, 256, 0, s>>>(slots, slotStride, sizes, nBlocks, packed, outOff, 4, fr);
-        g_launches++;
-    }
-    return (int)cudaGetLastError();
+    return launch_pack(slots, slotStride, sizes, nBlocks, packed, outOff, 4, fr, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -40,15 +40,11 @@ def main():
     t1.record()
     torch.cuda.synchronize()
     raw.LZ4B200_debug_phase_cycles(buf)
-    names = (["fetch+zero", "tma load wait", "runs pass 1", "rank + prev store", "runs pass 2", "waves", "store issue", "-"]
-             if os.environ.get("LZ4K_EXPAND_IMPL", "")[:1] != "p" else
-             ["fetch+zero", "tma load wait", "phase A", "rank", "prev store wait", "phase B", "store issue", "-"])
+    names = ["fetch+zero", "tma load wait", "runs pass 1", "rank + prev store", "runs pass 2", "waves", "store issue", "-"]
     tot = sum(buf[:8])
     print("expand ms per launch %.3f, blocks %d" % (t0.elapsed_time(t1) / reps, n_blocks))
     for n, v in zip(names, buf[:8]):
         print("%-16s %8.0f cycles/block  %5.1f%%" % (n, v / (reps * n_blocks), 100.0 * v / max(tot, 1)))
-    it, la, bl = buf[8] / (reps * n_blocks), buf[9] / (reps * n_blocks), buf[10] / (reps * n_blocks)
-    print("phase B per block: %.0f warp-iterations, %.0f lane-iterations with a piece (%.1f per warp-iteration), %.0f blocked" % (it, la, la / max(it, 1), bl))
     assert torch.equal(out, src)
 
 
