@@ -47,12 +47,8 @@ constexpr int kMfLimit = 12;
  * How the scan reads the compressed block.  Every read goes through a "memory" object:
  *   MemPtr<true>   the block lies in GLOBAL memory (read-only data cache loads, L1 prefetch hints)
  *   MemPtr<false>  the block is staged in SHARED memory (plain loads through the generic address space)
- * b(i) / u16(i) / u32(i) read bytes [i, i+1/2/4) of the block.  ensure(i) / tick(i) announce where the walk is about to
- * read; they are no-ops for both kinds (they served a per-thread shared-memory ring fed by cp.async, which was slower
- * than the plain loads and was dropped).
+ * b(i) / u16(i) / u32(i) read bytes [i, i+1/2/4) of the block.
  * ------------------------------------------------------------------------------------------- */
-constexpr int kMemAhead = 32;
-
 template <bool G> SC_FN uint32_t ldb(const uint8_t* p) { return G ? (uint32_t)SC_LDG(p) : (uint32_t)*p; }
 template <bool G> SC_FN uint32_t ldw(const uint32_t* p) { return G ? SC_LDG(p) : *p; }
 template <bool G> SC_FN uint32_t ld16(const uint8_t* p) { return ldb<G>(p) | (ldb<G>(p + 1) << 8); }
@@ -74,11 +70,9 @@ template <bool G, bool W = false> struct MemPtr {
     SC_MFN uint32_t b(int64_t i) const { return ldb<G>(p + i); }
     SC_MFN uint32_t u16(int64_t i) const { return ld16<G>(p + i); }
     SC_MFN uint32_t u32(int64_t i) const { return ld32u<G>(p + i); }
-    SC_MFN void ensure(int64_t) const { }
-    SC_MFN void tick(int64_t) const { }
     SC_MFN void prefetch(int64_t i) const { if (G) SC_PREFETCH_L1(p + i); }
     static constexpr bool kPrefetch = G;
-    static constexpr bool kWide = W;            /* marks are two words per sequence (blocks above 64 KB): see MARK_COMMIT */
+    static constexpr bool kWide = W;            /* marks are two words per sequence (blocks above 64 KB): see mark_commit */
 };
 
 /* =============================================================================================
@@ -93,7 +87,6 @@ template <class M> SC_FN bool read_runlength(M& mem, int64_t& ip, int64_t ilimit
     if (initialCheck && ip >= ilimit) return false;
     uint32_t b;
     do {
-        mem.ensure(ip);
         b = mem.b(ip);
         ip++;
         total += b;
@@ -113,11 +106,12 @@ constexpr int kMaxSeqFast = 8192;              // most sequences a block of the 
  * expanded from shared memory has at most capacity/4 + 1 sequences (every sequence but the last makes >= 4 bytes) */
 /* Blocks above 64 KB (decoded in 60 KB output tiles by lz4_expand_tiles_kernel) get WIDE marks: two words per sequence,
  * {token position, match start}; the memory class of the walk says which (M::kWide). */
-#define MARK_COMMIT(tokpos, matchpos)                                                           \
-    do { if (marks && nseq < markCap) {                                                         \
-        if (M::kWide) { marks[2 * (size_t)nseq] = (uint32_t)(tokpos); marks[2 * (size_t)nseq + 1] = (uint32_t)(matchpos); } \
-        else marks[nseq] = (uint32_t)(tokpos) | ((uint32_t)(matchpos) << 16);                   \
-    } } while (0)
+template <class M> SC_FN void mark_commit(uint32_t* marks, uint32_t markCap, uint32_t nseq, uint32_t tok, uint32_t matchStart)
+{
+    if (!marks || nseq >= markCap) return;
+    if (M::kWide) { marks[2 * (size_t)nseq] = tok; marks[2 * (size_t)nseq + 1] = matchStart; }
+    else marks[nseq] = tok | (matchStart << 16);
+}
 
 /* where the walk of one block stands between its two loops */
 struct ScanState {
@@ -133,58 +127,81 @@ struct ScanState {
  * dependent 4-byte reads per sequence (token + first length byte; offset + first match-length
  * byte).  Anything that would leave the fast loop (either end of the block getting close, an
  * error, absurd lengths) exits WITHOUT committing; the exact byte-wise code replays it.
- * Returns false for the one error it decides itself (offset before the start of the output,
- * lz4.c:2161), with st.ip at the reference's error position. */
+ *
+ * front_step parses the sequence whose token is at fip and applies the rules that depend on input positions only;
+ * the three scans (scan_front here, the split and the parallel scan) add the rules that depend on the output position.
+ * The lanes of a warp walk unrelated positions, so every data-dependent branch splits the warp and a walk's time is
+ * (instructions issued per step, all paths of all lanes) x (latency of a dependent instruction).  The step is therefore
+ * straight-line code for every sequence whose lengths need at most two extension bytes (literal runs < 525 bytes,
+ * matches < 529); longer ones go round the reference's loops, which are skipped (condition false for every lane)
+ * otherwise. */
+struct FrontSeq {
+    int ipn;                                    /* the next token's position */
+    int lit, mlen;                              /* literal length, match length (kMinMatch included) */
+    uint32_t off16;                             /* match offset */
+    bool stop;                                  /* the front loop ends at fip (the other fields are then meaningless) */
+};
+
+/* `stop` is set for a reason that depends on input positions only, unless the caller passes `litCap`: then also when
+ * the literal run ends past it (fop + lit > litCap: the output half of lz4.c:2104).  The capacity rule lz4.c:2137/2142,
+ * which every scan applies, implies that rule, so only scan_front passes it: there the early exit skips the offset read
+ * and the match-length loop, which keeps the one-thread scan kernel at fewer registers. */
+template <class M> SC_FN FrontSeq front_step(M& mem, int nI, int fip, uint32_t fop = 0u, uint32_t litCap = 0xFFFFFFFFu)
+{
+    FrontSeq s = {fip, 0, 0, 0u, true};
+    if (fip > nI - 26) return s;                               // lz4.c:2083 (the reads below stay inside the block)
+    const uint32_t v = mem.u32(fip);                           // token, then the 3 bytes that follow it
+    const int mcode = (int)(v & 15u), lit4 = (int)((v >> 4) & 15u);
+    /* read_variable_length (lz4.c:2093), limit n-15: the first two extension bytes come with the token */
+    const bool e1 = (lit4 == 15);
+    const uint32_t l1 = (v >> 8) & 0xFFu, l2 = (v >> 16) & 0xFFu;
+    const bool e2 = e1 && l1 == 255u;                          // (fip + 2 <= nI - 15 holds: fip <= nI - 26)
+    int lit = lit4 + (e1 ? (int)l1 : 0) + (e2 ? (int)l2 : 0);
+    int q = 1 + (e1 ? 1 : 0) + (e2 ? 1 : 0);
+    uint32_t b = e2 ? l2 : l1;
+    while (e1 && b == 255u && fip + q <= nI - 15 && lit < (1 << 28)) { b = mem.b(fip + q); q++; lit += (int)b; }
+    /* read limit / absurd run, or literals ending within 32 bytes of the input end (lz4.c:2104 -> safe_literal_copy) */
+    const bool stopL = e1 && (b == 255u || fip + q > nI - 15 || fop + (uint32_t)lit > litCap ||
+                              (uint32_t)(fip + q) + (uint32_t)lit + 32u > (uint32_t)nI);   // (unsigned: sums may pass 2^31)
+    const int offPos = fip + q + lit;
+    const uint32_t v3 = mem.u32(stopL ? fip : offPos);         // offset (LE16), then the first two match-length bytes;
+                                                               // a stopping step must not read at a wild position
+    /* read_variable_length (lz4.c:2128), limit n-4 */
+    const bool m1 = (mcode == 15);
+    const uint32_t x1 = (v3 >> 16) & 0xFFu, x2 = v3 >> 24;
+    const bool m2 = m1 && x1 == 255u && offPos + 3 <= nI - 4;
+    int mlen = mcode + kMinMatch + (m1 ? (int)x1 : 0) + (m2 ? (int)x2 : 0);
+    int ipn = offPos + 2 + (m1 ? 1 : 0) + (m2 ? 1 : 0);
+    b = m2 ? x2 : x1;
+    while (!stopL && m1 && b == 255u && ipn <= nI - 4 && mlen < (1 << 28)) { b = mem.b(ipn); ipn++; mlen += (int)b; }
+    s.ipn = ipn; s.lit = lit; s.mlen = mlen; s.off16 = v3 & 0xFFFFu;
+    s.stop = stopL || (m1 && (b == 255u || ipn > nI - 4));
+    return s;
+}
+
+/* L1 prefetch hint, once per 128 input bytes of a walk over global memory */
+template <class M> SC_FN void front_prefetch(M& mem, int nI, int fip, int& nextEvt)
+{
+    if (M::kPrefetch && fip >= nextEvt) {
+        if (fip + 128 < nI) mem.prefetch(fip + 128);
+        nextEvt = ((fip >> 7) + 1) << 7;
+    }
+}
+
+/* Returns false for the one error it decides itself (offset before the start of the output, lz4.c:2161), with st.ip at
+ * the reference's error position.  The exits are collected and taken once, in the reference's order. */
 template <class M> SC_FN bool scan_front(M& mem, int nIn, int capIn, ScanState& st, uint32_t* marks, uint32_t markCap)
 {
     uint32_t nseq = st.nseq;
     int fip = 0, fop = 0, nextEvt = 0;
-    const int nI = nIn, capI = capIn;
-    /* The 32 lanes of a warp walk 32 unrelated blocks, so every data-dependent branch splits the warp and the
-     * walk's time is (instructions issued per step, all paths of all lanes) x (latency of a dependent instruction).
-     * The body is therefore straight-line code for every sequence whose lengths need at most two extension bytes
-     * (literal runs < 525 bytes, matches < 529); longer ones go round the reference's loops, which are skipped
-     * (condition false for every lane) otherwise.  The exits are collected and taken once, in the reference's order. */
-    while (fip <= nI - 26) {
-        if (M::kPrefetch && fip >= nextEvt) {                      // L1 prefetch hint, once per 128 input bytes
-            if (fip + 128 < nI) mem.prefetch(fip + 128);
-            nextEvt = ((fip >> 7) + 1) << 7;
-        }
-        mem.tick(fip);
-        mem.ensure(fip);                                           // [fip, fip + kMemAhead) is readable: token, short literals, offset
-        const uint32_t v = mem.u32(fip);                           // token, then the 3 bytes that follow it
-        const int mcode = (int)(v & 15u), lit4 = (int)((v >> 4) & 15u);
-        /* read_variable_length (lz4.c:2093), limit n-15: the first two extension bytes come with the token */
-        const bool e1 = (lit4 == 15);
-        const uint32_t l1 = (v >> 8) & 0xFFu, l2 = (v >> 16) & 0xFFu;
-        const bool e2 = e1 && l1 == 255u;                          // (fip + 2 <= nI - 15 holds: fip <= nI - 26)
-        int lit = lit4 + (e1 ? (int)l1 : 0) + (e2 ? (int)l2 : 0);
-        int q = 1 + (e1 ? 1 : 0) + (e2 ? 1 : 0);
-        uint32_t b = e2 ? l2 : l1;
-        while (e1 && b == 255u && fip + q <= nI - 15 && lit < (1 << 28)) { mem.ensure(fip + q); b = mem.b(fip + q); q++; lit += (int)b; }
-        const bool exitL = e1 && (b == 255u || fip + q > nI - 15 ||                      // read limit / absurd run: replay byte-wise
-                                  (uint32_t)fop + (uint32_t)lit > (uint32_t)(capI - 32) ||              // lz4.c:2104 -> safe_literal_copy
-                                  (uint32_t)(fip + q) + (uint32_t)lit + 32u > (uint32_t)nI);           // (unsigned: sums may pass 2^31)
-        const int offPos = fip + q + lit;
-        const int offRead = exitL ? fip : offPos;                  // an exiting lane must not read at a wild position
-        if (e1) mem.ensure(offRead);                               // a long literal run: the offset lies beyond the window
-        const uint32_t v3 = mem.u32(offRead);                      // offset (LE16), then the first two match-length bytes
-        const int off16 = (int)(v3 & 0xFFFFu);
-        /* read_variable_length (lz4.c:2128), limit n-4 */
-        const bool m1 = (mcode == 15);
-        const uint32_t x1 = (v3 >> 16) & 0xFFu, x2 = v3 >> 24;
-        const bool m2 = m1 && x1 == 255u && offPos + 3 <= nI - 4;
-        int mlen = mcode + kMinMatch + (m1 ? (int)x1 : 0) + (m2 ? (int)x2 : 0);
-        int ipn = offPos + 2 + (m1 ? 1 : 0) + (m2 ? 1 : 0);
-        b = m2 ? x2 : x1;
-        while (!exitL && m1 && b == 255u && ipn <= nI - 4 && mlen < (1 << 28)) { mem.ensure(ipn); b = mem.b(ipn); ipn++; mlen += (int)b; }
-        const bool exitM = m1 && (b == 255u || ipn > nI - 4);
-        const int opn = fop + lit;
-        const bool exitC = (uint32_t)opn + (uint32_t)mlen >= (uint32_t)(capI - 64);   // lz4.c:2137/2142 -> safe_match_copy
-        if (exitL || exitM || exitC) break;
-        if (off16 > opn) { st.ip = ipn; st.nseq = nseq; return false; }       // lz4.c:2161
-        MARK_COMMIT(fip, opn);
-        fip = ipn; fop = opn + mlen; nseq++;
+    while (fip <= nIn - 26) {                                  // front_step tests it too; testing it first here, before
+        front_prefetch(mem, nIn, fip, nextEvt);                // the prefetch, compiles to fewer registers
+        const FrontSeq s = front_step(mem, nIn, fip, (uint32_t)fop, (uint32_t)(capIn - 32));
+        const int opn = fop + s.lit;
+        if (s.stop || (uint32_t)opn + (uint32_t)s.mlen >= (uint32_t)(capIn - 64)) break;   // lz4.c:2137/2142 -> safe_match_copy
+        if ((int)s.off16 > opn) { st.ip = s.ipn; st.nseq = nseq; return false; }            // lz4.c:2161
+        mark_commit<M>(marks, markCap, nseq, (uint32_t)fip, (uint32_t)opn);
+        fip = s.ipn; fop = opn + s.mlen; nseq++;
     }
     st.ip = fip; st.op = fop; st.nseq = nseq;
     if (nextEvt > 0) st.nextPrefetch = (int64_t)nextEvt + 128;
@@ -205,7 +222,6 @@ template <class M> SC_FN int scan_tail(M& mem, int nIn, int capIn, const ScanSta
             if (ip + 128 < n) mem.prefetch(ip + 128);
             nextPrefetch = ip + 256;
         }
-        mem.ensure(ip);
         token = mem.b(ip); ip++;
         ll = token >> 4;
         ml = token & 15;
@@ -219,7 +235,6 @@ template <class M> SC_FN int scan_tail(M& mem, int nIn, int capIn, const ScanSta
                 fast = false; goto safe_literals;
             }
             ip += ll; op += ll; mop = op;
-            mem.ensure(ip);
             offset = mem.u16(ip); ip += 2;
             if (ml == 15) {
                 if (!read_runlength(mem, ip, n - 4, false, add)) goto bad;
@@ -228,7 +243,7 @@ template <class M> SC_FN int scan_tail(M& mem, int nIn, int capIn, const ScanSta
             ml += kMinMatch;
             if (op + ml >= cap - 64) { fast = false; goto safe_match; }
             if ((int64_t)offset > op) goto bad;                        // lz4.c:2161
-            MARK_COMMIT(tokPos, mop);
+            mark_commit<M>(marks, markCap, nseq, (uint32_t)tokPos, (uint32_t)mop);
             op += ml; nseq++;
             continue;
         }
@@ -236,9 +251,12 @@ template <class M> SC_FN int scan_tail(M& mem, int nIn, int capIn, const ScanSta
         /* safe loop, lz4.c:2215-2435 */
         if (ll != 15 && ip < n - 16 && op <= cap - 32) {               // two-stage shortcut :2230-2261
             op += ll; ip += ll; mop = op;
-            mem.ensure(ip);
             offset = mem.u16(ip); ip += 2;
-            if (ml != 15 && offset >= 8 && (int64_t)offset <= op) { MARK_COMMIT(tokPos, mop); op += ml + kMinMatch; nseq++; continue; }
+            if (ml != 15 && offset >= 8 && (int64_t)offset <= op) {
+                mark_commit<M>(marks, markCap, nseq, (uint32_t)tokPos, (uint32_t)mop);
+                op += ml + kMinMatch; nseq++;
+                continue;
+            }
             goto match_length;
         }
         if (ll == 15) {
@@ -249,13 +267,12 @@ safe_literals:
         if (op + ll > cap - kMfLimit || ip + ll > n - (2 + 1 + kLastLiterals)) {   // lz4.c:2279
             if (ip + ll != n || op + ll > cap) goto bad;               // lz4.c:2312
             op += ll;
-            MARK_COMMIT(tokPos, op);                                   /* last sequence: the end of its literals */
+            mark_commit<M>(marks, markCap, nseq, (uint32_t)tokPos, (uint32_t)op);   /* last sequence: the end of its literals */
             nseq++;
             *nSeqOut = nseq;
             return (int)op;                                            // lz4.c:2439
         }
         ip += ll; op += ll; mop = op;
-        mem.ensure(ip);
         offset = mem.u16(ip); ip += 2;
 match_length:
         if (ml == 15) {
@@ -266,7 +283,7 @@ match_length:
 safe_match:
         if ((int64_t)offset > op) goto bad;                            // lz4.c:2356
         if (op + ml > cap - kLastLiterals) goto bad;                   // lz4.c:2421-2423
-        MARK_COMMIT(tokPos, mop);
+        mark_commit<M>(marks, markCap, nseq, (uint32_t)tokPos, (uint32_t)mop);
         op += ml; nseq++;
     }
 bad:
@@ -280,7 +297,7 @@ template <class M> SC_DEV int scan_block(M& mem, int nIn, int capIn, uint32_t* n
     st.ip = 0; st.op = 0; st.nextPrefetch = 128; st.nseq = 0;
 
     if (capIn < 0) return -1;                                          // lz4.c:2036
-    if (capIn == 0) { if (nIn != 1) return -1; mem.ensure(0); return mem.b(0) == 0 ? 0 : -1; }   // lz4.c:2064-2068
+    if (capIn == 0) { if (nIn != 1) return -1; return mem.b(0) == 0 ? 0 : -1; }   // lz4.c:2064-2068
     if (nIn <= 0) return -1;                                           // lz4.c:2069
     st.fast = (capIn >= 64);                                           // lz4.c:2076
 

@@ -63,7 +63,7 @@ struct SpLane {                            /* registers of one lane */
     int newFrom, newVoid, need;
 };
 
-/* One walk over [from, segEnd): scan_front's loop body with the output position relative (COUNT) or
+/* One walk over [from, segEnd) with front_step (lz4_scan_core.h), the output position relative (COUNT) or
  * absolute (WRITE).  Position-only rules apply in both passes, output-dependent rules in WRITE only. */
 template <class M, bool WRITE>
 SC_FN void sp_walk(M& mem, int nI, int capI, int from, int segEnd,
@@ -72,39 +72,16 @@ SC_FN void sp_walk(M& mem, int nI, int capI, int from, int segEnd,
     int fip = from, nextEvt = 0, stop = 0, kind = SP_RAN, errIp = 0;
     uint32_t fop = opBase, cnt = 0;
     while (fip < segEnd) {
-        if (fip > nI - 26) { stop = 1; kind = SP_END; break; }
-        if (M::kPrefetch && fip >= nextEvt) {                      // L1 prefetch, once per 128 input bytes
-            if (fip + 128 < nI) mem.prefetch(fip + 128);
-            nextEvt = ((fip >> 7) + 1) << 7;
-        }
-        const uint32_t v = mem.u32(fip);
-        const int mcode = (int)(v & 15u);
-        int lit = (int)((v >> 4) & 15u), q = 1;
-        if (lit == 15) {
-            uint32_t b = (v >> 8) & 0xFFu;
-            lit += (int)b; q = 2;
-            while (b == 255u && fip + q <= nI - 15 && lit < (1 << 28)) { b = mem.b(fip + q); q++; lit += (int)b; }
-            if (b == 255u || fip + q > nI - 15) { stop = 1; kind = SP_END; break; }
-            if ((uint32_t)(fip + q) + (uint32_t)lit + 32u > (uint32_t)nI) { stop = 1; kind = SP_END; break; }
-            if (WRITE && fop + (uint32_t)lit > (uint32_t)(capI - 32)) { kind = SP_END; break; }
-        }
-        const int offPos = fip + q + lit;
-        const uint32_t v3 = mem.u32(offPos);
-        const uint32_t off16 = v3 & 0xFFFFu;
-        int mlen = mcode + kMinMatch, ipn = offPos + 2;
-        if (mcode == 15) {
-            uint32_t b = (v3 >> 16) & 0xFFu;
-            ipn++; mlen += (int)b;
-            while (b == 255u && ipn <= nI - 4 && mlen < (1 << 28)) { b = mem.b(ipn); ipn++; mlen += (int)b; }
-            if (b == 255u || ipn > nI - 4) { stop = 1; kind = SP_END; break; }
-        }
-        const uint32_t opn = fop + (uint32_t)lit;
+        front_prefetch(mem, nI, fip, nextEvt);
+        const FrontSeq s = front_step(mem, nI, fip);
+        if (s.stop) { stop = 1; kind = SP_END; break; }
+        const uint32_t opn = fop + (uint32_t)s.lit;
         if (WRITE) {
-            if (opn + (uint32_t)mlen >= (uint32_t)(capI - 64)) { kind = SP_END; break; }
-            if (off16 > opn) { kind = SP_ERR; errIp = ipn; break; }
-            { const uint32_t nseq = seqBase + cnt; MARK_COMMIT(fip, opn); }
+            if (opn + (uint32_t)s.mlen >= (uint32_t)(capI - 64)) { kind = SP_END; break; }   // lz4.c:2137/2142
+            if (s.off16 > opn) { kind = SP_ERR; errIp = s.ipn; break; }                        // lz4.c:2161
+            mark_commit<M>(marks, markCap, seqBase + cnt, (uint32_t)fip, opn);
         }
-        fip = ipn; fop = opn + (uint32_t)mlen; cnt++;
+        fip = s.ipn; fop = opn + (uint32_t)s.mlen; cnt++;
     }
     if (WRITE) {
         E.kind = kind; E.ip = (kind == SP_ERR) ? errIp : fip; E.op = fop; E.nseq = seqBase + cnt; E.nextEvt = nextEvt;

@@ -10,8 +10,9 @@
  * their segment as if it were a token.  Such a speculative chain falls onto the true chain after a few dozen bytes
  * (tests/perf/sync_study.py), so instead of re-walking:
  *
- *   P1  every lane walks its segment and LISTS what it commits: (token position, offset, match start relative to
- *       an output position 0 at its own start) -- only the rules that depend on input positions apply;
+ *   P1  every lane walks its segment with front_step (lz4_scan_core.h) and LISTS what it commits: (token position,
+ *       offset, match start relative to an output position 0 at its own start) -- only the rules that depend on input
+ *       positions apply;
  *   P2  a lane that reaches the end of its segment keeps walking until it stands on a token of the next lane's
  *       list: from there on the two chains are the same chain, so the rest of the next lane's list is TRUE, up to a
  *       constant shift of its output positions (a next lane that never meets the chain is void and skipped);
@@ -66,37 +67,6 @@ struct SsBlock {
     uint32_t capOpn;                        /* ... and that match start in full (it may not fit the 16 bits of a mark) */
 };
 
-/* One step of the front loop at token position fip (lz4.c:2083-2209; scan_front's body without the rules that need the
- * absolute output position).  Returns false when the front loop cannot continue here for a reason that depends on
- * input positions only; else the sequence's numbers. */
-template <class M>
-SC_FN bool ss_step(M& mem, int nI, int fip, int& ipn, int& lit, int& mlen, uint32_t& off16)
-{
-    if (fip > nI - 26) return false;
-    const uint32_t v = mem.u32(fip);
-    const int mcode = (int)(v & 15u), lit4 = (int)((v >> 4) & 15u);
-    const bool e1 = (lit4 == 15);
-    const uint32_t l1 = (v >> 8) & 0xFFu, l2 = (v >> 16) & 0xFFu;
-    const bool e2 = e1 && l1 == 255u;
-    lit = lit4 + (e1 ? (int)l1 : 0) + (e2 ? (int)l2 : 0);
-    int q = 1 + (e1 ? 1 : 0) + (e2 ? 1 : 0);
-    uint32_t b = e2 ? l2 : l1;
-    while (e1 && b == 255u && fip + q <= nI - 15 && lit < (1 << 28)) { b = mem.b(fip + q); q++; lit += (int)b; }
-    if (e1 && (b == 255u || fip + q > nI - 15 || (uint32_t)(fip + q) + (uint32_t)lit + 32u > (uint32_t)nI)) return false;
-    const int offPos = fip + q + lit;
-    const uint32_t v3 = mem.u32(offPos);
-    off16 = v3 & 0xFFFFu;
-    const bool m1 = (mcode == 15);
-    const uint32_t x1 = (v3 >> 16) & 0xFFu, x2 = v3 >> 24;
-    const bool m2 = m1 && x1 == 255u && offPos + 3 <= nI - 4;
-    mlen = mcode + kMinMatch + (m1 ? (int)x1 : 0) + (m2 ? (int)x2 : 0);
-    ipn = offPos + 2 + (m1 ? 1 : 0) + (m2 ? 1 : 0);
-    b = m2 ? x2 : x1;
-    while (m1 && b == 255u && ipn <= nI - 4 && mlen < (1 << 28)) { b = mem.b(ipn); ipn++; mlen += (int)b; }
-    if (m1 && (b == 255u || ipn > nI - 4)) return false;
-    return true;
-}
-
 /* literal length of the sequence whose token sits at `tok` (a committed sequence: the reads are in range) */
 template <class M>
 SC_FN int ss_lit_at(M& mem, int tok)
@@ -134,14 +104,11 @@ SC_FN void ss_p1(int lane, SsBlock& S, M& mem, int nI, uint32_t* A, uint32_t* B,
     me.cnt = 0; me.state = SS_RUN; me.inChain = 0; me.target = -1;
     int nextEvt = 0;
     while (fip < segEnd) {
-        if (M::kPrefetch && fip >= nextEvt) {
-            if (fip + 128 < nI) mem.prefetch(fip + 128);
-            nextEvt = ((fip >> 7) + 1) << 7;
-        }
-        int ipn, lit, mlen; uint32_t off16;
-        if (!ss_step(mem, nI, fip, ipn, lit, mlen, off16)) { me.state = SS_STOP; break; }
-        if (!ss_push(me, A, B, R, fip, off16, fop + (uint32_t)lit)) break;
-        fip = ipn; fop += (uint32_t)lit + (uint32_t)mlen;
+        front_prefetch(mem, nI, fip, nextEvt);
+        const FrontSeq s = front_step(mem, nI, fip);
+        if (s.stop) { me.state = SS_STOP; break; }
+        if (!ss_push(me, A, B, R, fip, s.off16, fop + (uint32_t)s.lit)) break;
+        fip = s.ipn; fop += (uint32_t)s.lit + (uint32_t)s.mlen;
     }
     me.fip = fip; me.fop = fop; me.cntP1 = me.cnt; me.fipP1 = fip; me.stateP1 = me.state;
     if (lane == 0) { S.fallback = 0; S.errIdx = 0xFFFFFFFFu; S.capIdx = 0xFFFFFFFFu; }
@@ -169,15 +136,15 @@ SC_FN void ss_p2(int lane, SsBlock& S, M& mem, int nI, uint32_t* A, uint32_t* B,
         } else if (fip == tk) {
             if (cur == T.cntP1 && T.stateP1 == SS_STOP) { me.state = SS_STOP; break; }   /* the front loop ends here for everybody */
             if (cur == T.cntP1 && T.stateP1 == SS_FULL) { me.state = SS_FULL; break; }
-            int ipn, lit, mlen; uint32_t off16;
-            if (!ss_step(mem, nI, fip, ipn, lit, mlen, off16)) { me.state = SS_STOP; break; }   /* (cannot happen for a committed entry) */
-            me.state = SS_MERGED; me.target = t; me.mergeIdx = cur; me.mergeOpn = fop + (uint32_t)lit;
+            const FrontSeq s = front_step(mem, nI, fip);
+            if (s.stop) { me.state = SS_STOP; break; }                   /* (cannot happen for a committed entry) */
+            me.state = SS_MERGED; me.target = t; me.mergeIdx = cur; me.mergeOpn = fop + (uint32_t)s.lit;
             break;
         }
-        int ipn, lit, mlen; uint32_t off16;
-        if (!ss_step(mem, nI, fip, ipn, lit, mlen, off16)) { me.state = SS_STOP; break; }
-        if (!ss_push(me, A, B, R, fip, off16, fop + (uint32_t)lit)) break;
-        fip = ipn; fop += (uint32_t)lit + (uint32_t)mlen;
+        const FrontSeq s = front_step(mem, nI, fip);
+        if (s.stop) { me.state = SS_STOP; break; }
+        if (!ss_push(me, A, B, R, fip, s.off16, fop + (uint32_t)s.lit)) break;
+        fip = s.ipn; fop += (uint32_t)s.lit + (uint32_t)s.mlen;
     }
     me.fip = fip; me.fop = fop;
 }

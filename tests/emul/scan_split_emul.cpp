@@ -2,8 +2,6 @@
 // Runs the lanes of a block phase by phase (the device puts a __syncwarp between phases) on the host build of the same
 // header and returns what the kernel would store for the block.
 #include <stdint.h>
-#include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
 #include <vector>
 #include "../../lz4_b200/csrc/lz4_scan_split.h"
@@ -37,36 +35,6 @@ extern "C" int scan_split_host(const uint8_t* src, int n, int cap, uint32_t* nSe
         stats[2] += S.lane[l].inChain;
     }
     return ss_p5(S, mem, n, cap, nSeqOut, marks, markCap);
-}
-
-extern "C" void scan_split_debug(const uint8_t* src, int n, int cap)
-{
-    MemPtr<true> mem{src};
-    std::vector<uint32_t> m(kMaxSeqFast);
-    ScanState st; st.ip = 0; st.op = 0; st.nextPrefetch = 128; st.nseq = 0; st.fast = true;
-    const bool ok = scan_front(mem, n, cap, st, m.data(), (uint32_t)kMaxSeqFast);
-    fprintf(stderr, "serial front: ok %d ip %lld op %lld nseq %u\n", (int)ok, (long long)st.ip, (long long)st.op, st.nseq);
-    const uint32_t R = (uint32_t)kMaxSeqFast / kSsLanes;
-    std::vector<uint32_t> A((size_t)kSsLanes * R + 1), B((size_t)kSsLanes * R + 1), marks(kMaxSeqFast);
-    static SsBlock S; memset(&S, 0, sizeof(S));
-    for (int l = 0; l < kSsLanes; l++) ss_p1(l, S, mem, n, A.data() + (size_t)l * R, B.data() + (size_t)l * R, R);
-    for (int l = 0; l < kSsLanes; l++) ss_p2(l, S, mem, n, A.data() + (size_t)l * R, B.data() + (size_t)l * R, R, [&](int t) { return B.data() + (size_t)t * R; });
-    ss_p3(S, [&](int t) { return A.data() + (size_t)t * R; });
-    for (int l = 0; l < kSsLanes; l++) {
-        const SsPub& L = S.lane[l];
-        fprintf(stderr, "lane %d: state %d cnt %u cntP1 %u fip %d fop %u target %d mergeIdx %u inChain %d first %u base %d place %u\n",
-                l, L.state, L.cnt, L.cntP1, L.fip, L.fop, L.target, L.mergeIdx, L.inChain, L.first, (int)L.base, L.place);
-        uint32_t e, c, co; ss_p4(l, S, cap, A.data() + (size_t)l * R, B.data() + (size_t)l * R, marks.data(), (uint32_t)kMaxSeqFast, e, c, co);
-        if (e < S.errIdx) S.errIdx = e;
-        if (c < S.capIdx) { S.capIdx = c; S.capOpn = co; }
-    }
-    fprintf(stderr, "fallback %d endLane %d nFront %u errIdx %u capIdx %u\n", S.fallback, S.endLane, S.nFront, S.errIdx, S.capIdx);
-    for (uint32_t g = 2308; g < 2318 && g < S.nFront; g++) fprintf(stderr, "  mark[%u] tok %u opn %u | serial mark tok %u opn %u\n", g, marks[g] & 0xFFFF, marks[g] >> 16, m[g] & 0xFFFF, m[g] >> 16);
-    uint32_t ns = 0;
-    int r = ss_p5(S, mem, n, cap, &ns, marks.data(), (uint32_t)kMaxSeqFast);
-    uint32_t ns1 = 0; std::vector<uint32_t> m1(kMaxSeqFast);
-    int r1 = scan_tail(mem, n, cap, st, &ns1, m1.data(), (uint32_t)kMaxSeqFast);
-    fprintf(stderr, "split p5 ret %d nseq %u | serial tail ret %d nseq %u\n", r, ns, r1, ns1);
 }
 
 // In-process differential fuzz: mutate a (valid) compressed block `iters` times, pick a capacity, and compare the split
@@ -109,15 +77,7 @@ extern "C" long long scan_split_fuzz(const uint8_t* base, int n, int rawSize, in
         const int r1 = scan_block(memP, (int)len, cap, &ns1, m1, markCap);
         const int r2 = scan_split_host(p, (int)len, cap, &ns2, m2, markCap, st);
         const uint32_t k = ns1 < markCap ? ns1 : markCap;
-        if (r1 != r2 || (r1 > 0 && ns1 != ns2) || (r1 > 0 && memcmp(m1, m2, sizeof(uint32_t) * k) != 0)) {
-            bad = -(1 + (long long)it);
-            if (getenv("SS_DEBUG")) {
-                uint32_t d = 0; while (d < k && m1[d] == m2[d]) d++;
-                FILE* f = fopen("/tmp/w/case.bin", "wb"); if (f) { fwrite(p, 1, len, f); fclose(f); }
-                fprintf(stderr, "case %d: len %zu cap %d markCap %u  serial ret %d nseq %u | split ret %d nseq %u fallback %d p2 %d chain %d | first differing mark %u: %08x vs %08x\n",
-                        it, len, cap, markCap, r1, ns1, r2, ns2, st[0], st[1], st[2], d, d < k ? m1[d] : 0, d < k ? m2[d] : 0);
-            }
-        }
+        if (r1 != r2 || (r1 > 0 && ns1 != ns2) || (r1 > 0 && memcmp(m1, m2, sizeof(uint32_t) * k) != 0)) bad = -(1 + (long long)it);
         cases++;
         errors += r1 < 0;
         fb += st[0];
