@@ -1406,7 +1406,8 @@ int lz4k_launch_decode(const lz4k_decode_args* a, int phases, void* stream)
         /* the lanes of the parallel scan re-walk their segments several times (fix-up rounds), many times the instructions of
          * the one-thread scan, so it only pays for blocks far beyond 64 KB (lz4frame's 4 MB blocks: 150 000 dependent steps for
          * one thread) */
-        const bool par = scanImpl >= 0 ? scanImpl == 1 : (a->dstCapArr == nullptr && a->dstCap > 65536);
+        /* the switch does not apply to a wide batch: only the parallel scan writes the wide marks the tiles kernel reads */
+        const bool par = wide || (scanImpl >= 0 ? scanImpl == 1 : (a->dstCapArr == nullptr && a->dstCap > 65536));
         /* blocks of 16..64 KB: kSsLanes merging lanes per block (smaller blocks have too few sequences to split).  Measured
          * on an H100 SXM at a 700 W power limit (tests/perf/scan_crossover.py, 64 KB P50 blocks, split against one thread per
          * block): faster while the batch is small (1.20 against 2.01 ms for 4096 blocks, 1.71 against 2.03 ms for 8192), slower beyond (2.49

@@ -1,4 +1,5 @@
-"""Helpers shared by the GPU parity tests."""
+"""Helpers shared by the GPU parity tests: device-API decode calls that check what they may not touch, the decode
+route a call takes, and the hostile block corpus of the route tests."""
 import hashlib
 
 import numpy as np
@@ -27,64 +28,282 @@ def pack_host_blocks(blocks):
     return buf, offs, sizes
 
 
-def decode_batch(blocks, caps):
-    """Run blocks through LZ4B200_decompress_blocks with per-block capacities (device API).
-    Returns list of (ret, bytes)."""
-    from lz4_b200 import _lib
-    lib = _lib.load()
-    buf, offs, sizes = pack_host_blocks(blocks)
-    caps = np.asarray(caps, dtype=np.int32)
-    dst_off = np.zeros(len(blocks), dtype=np.int64)
-    slot = (np.maximum(caps, 0).astype(np.int64) + 64)
-    dst_off[1:] = np.cumsum(slot[:-1])
-    total = int(slot.sum())
-    d_buf, d_offs, d_sizes = to_dev(buf), to_dev(offs), to_dev(sizes)
-    d_caps, d_dst_off = to_dev(caps), to_dev(dst_off)
-    d_out = torch.full((total,), 0xA5, dtype=torch.uint8, device=dev())
-    d_ret = torch.zeros(len(blocks), dtype=torch.int32, device=dev())
-    ws = torch.empty(int(lib.LZ4B200_decompress_workspace_bytes(len(blocks))), dtype=torch.uint8, device=dev())
-    rc = lib.LZ4B200_decompress_blocks(d_buf.data_ptr(), d_offs.data_ptr(), d_sizes.data_ptr(), d_out.data_ptr(),
-                                       d_dst_off.data_ptr(), 0, d_caps.data_ptr(), 0, d_ret.data_ptr(), len(blocks),
-                                       ws.data_ptr(), ws.numel(), torch.cuda.current_stream().cuda_stream)
-    _lib.check(rc, "decompress_blocks")
-    torch.cuda.synchronize()
-    out = d_out.cpu().numpy()
-    ret = d_ret.cpu().numpy()
-    res = []
-    for i in range(len(blocks)):
-        o, c = int(dst_off[i]), max(int(caps[i]), 0)
-        guard = out[o + c:o + c + 64]
-        assert (guard == 0xA5).all(), "block %d wrote past its capacity" % i
-        r = int(ret[i])
-        res.append((r, out[o:o + max(r, 0)].tobytes()))
-    return res
+# ------------------------------------------------------------------------------------------
+# decode calls
+# ------------------------------------------------------------------------------------------
+def ws_lists(ws, n):
+    """(nSeq[n], slow list) left in a decode workspace.  Layout (lz4_kernels.cu:149-164, ws_view): a 256-byte header
+    whose first word is the slow-list count, then nSeq[n] and slowList[n], each rounded up to 256 bytes."""
+    lst = (n * 4 + 255) // 256 * 256
+    w = ws[:256 + 2 * lst].cpu().numpy().view(np.uint32)
+    count = int(w[0])
+    assert count <= n, "slow list count %d > %d blocks" % (count, n)
+    return w[64:64 + n].copy(), w[(256 + lst) // 4:(256 + lst) // 4 + count].copy()
 
 
-def decode_batch_uniform(blocks, cap, wide=True):
-    """Run blocks through LZ4B200_decompress_blocks with ONE capacity for all of them (device API); wide=True gives the
-    workspace LZ4B200_decompress_workspace_bytes_for asks for (blocks above 64 KB: the tiles kernel), wide=False the
-    small one (blocks above 64 KB: the generic kernel).  Returns list of (ret, bytes)."""
+def route(n_blocks, cap=None, per_block_caps=False, ws_bytes=0):
+    """The decode route lz4k_launch_decode (lz4_kernels.cu:1381-1458) takes with LZ4K_SCAN_IMPL unset:
+      R1 per-block capacities: one-thread scan -> rows / generic
+      R2 one capacity in [16 KB, 64 KB], <= 8 192 blocks: split scan -> rows / generic
+      R3 one capacity in [16 KB, 64 KB], > 8 192 blocks: one-thread scan -> rows / generic
+      R4 one capacity below 16 KB: one-thread scan -> rows / generic
+      R5 one capacity in (64 KB, 64 MB] and the workspace of LZ4B200_decompress_workspace_bytes_for (use_wide,
+         lz4_kernels.cu:177): parallel scan -> tile index -> tiles / generic
+      R6 one capacity above 64 KB otherwise: parallel scan -> generic"""
+    if per_block_caps:
+        return "R1"
+    if cap > 65536:
+        from lz4_b200 import _lib
+        wide = cap <= (64 << 20) and ws_bytes >= int(_lib.load().LZ4B200_decompress_workspace_bytes_for(n_blocks, 0, cap))
+        return "R5" if wide else "R6"
+    if cap >= 16384:
+        return "R2" if n_blocks <= 8192 else "R3"
+    return "R4"
+
+
+class Decoded(list):
+    """(return value, decoded bytes) per block.  .slow: the slow list (blocks the generic kernel decoded), .nseq: the
+    scan's sequence count per block, .route: route(...) of the call."""
+
+
+def _decode(blocks, slot_off, slot_len, total, dst_off, stride, caps, cap, ws_bytes, phases, rt):
     from lz4_b200 import _lib
     lib = _lib.load()
-    buf, offs, sizes = pack_host_blocks(blocks)
+    assert phases in ("one", "split")
     n = len(blocks)
-    stride = (cap + 64 + 15) // 16 * 16
+    buf, offs, sizes = pack_host_blocks(blocks)
     d_buf, d_offs, d_sizes = to_dev(buf), to_dev(offs), to_dev(sizes)
-    d_out = torch.full((n * stride,), 0xA5, dtype=torch.uint8, device=dev())
+    d_caps = to_dev(np.asarray(caps, dtype=np.int32)) if caps is not None else None
+    d_dst_off = to_dev(dst_off) if dst_off is not None else None
+    d_out = torch.full((total,), 0xA5, dtype=torch.uint8, device=dev())
     d_ret = torch.zeros(n, dtype=torch.int32, device=dev())
-    nbytes = int(lib.LZ4B200_decompress_workspace_bytes_for(n, 0, cap)) if wide else int(lib.LZ4B200_decompress_workspace_bytes(n))
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev())
-    rc = lib.LZ4B200_decompress_blocks(d_buf.data_ptr(), d_offs.data_ptr(), d_sizes.data_ptr(), d_out.data_ptr(),
-                                       None, stride, None, cap, d_ret.data_ptr(), n,
-                                       ws.data_ptr(), ws.numel(), torch.cuda.current_stream().cuda_stream)
-    _lib.check(rc, "decompress_blocks")
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev())
+    args = (d_buf.data_ptr(), d_offs.data_ptr(), d_sizes.data_ptr(), d_out.data_ptr(),
+            d_dst_off.data_ptr() if d_dst_off is not None else None, stride,
+            d_caps.data_ptr() if d_caps is not None else None, cap, d_ret.data_ptr(), n, ws.data_ptr(), ws.numel())
+    stream = torch.cuda.current_stream().cuda_stream
+    scanned = None
+    if phases == "split":                       # scan, read the sizes, then expand with the same workspace
+        _lib.check(lib.LZ4B200_decompress_blocks_phased(*args, 1, stream), "decompress_blocks_phased(scan)")
+        scanned = d_ret.cpu().numpy().copy()
+        _lib.check(lib.LZ4B200_decompress_blocks_phased(*args, 2, stream), "decompress_blocks_phased(expand)")
+    else:
+        _lib.check(lib.LZ4B200_decompress_blocks(*args, stream), "decompress_blocks")
     torch.cuda.synchronize()
     out = d_out.cpu().numpy()
     ret = d_ret.cpu().numpy()
-    res = []
+    if scanned is not None:
+        assert (scanned == ret).all(), "the expand phase changed the sizes the scan left"
+    res = Decoded()
+    res.nseq, res.slow = ws_lists(ws, n)
+    res.route = rt
+    assert len(set(res.slow.tolist())) == len(res.slow), "a block is on the slow list twice"
+    assert all(ret[b] > 0 for b in res.slow), "a rejected or empty block is on the slow list"
     for i in range(n):
-        o = i * stride
-        assert (out[o + cap:o + stride] == 0xA5).all(), "block %d wrote past its capacity" % i
-        r = int(ret[i])
-        res.append((r, out[o:o + max(r, 0)].tobytes()))
+        o, r = int(slot_off[i]), int(ret[i])
+        keep = max(r, 0)
+        # every expand kernel writes exactly [0, ret): a rejected block's slot, and the rest of an accepted one, stay as they were
+        untouched = out[o + keep:o + int(slot_len[i])]
+        assert (untouched == 0xA5).all(), "block %d (return value %d) wrote outside [0, %d) of its %d-byte slot" % (
+            i, r, keep, int(slot_len[i]))
+        res.append((r, out[o:o + keep].tobytes()))
     return res
+
+
+def decode_batch(blocks, caps, phases="one"):
+    """Run blocks through LZ4B200_decompress_blocks with per-block capacities (device API; route R1), each in a slot of
+    its capacity + 64 bytes.  phases="split": the scan and the expand as two calls.  Returns a Decoded."""
+    from lz4_b200 import _lib
+    n = len(blocks)
+    caps = np.asarray(caps, dtype=np.int32)
+    slot = np.maximum(caps, 0).astype(np.int64) + 64
+    dst_off = np.zeros(n, dtype=np.int64)
+    dst_off[1:] = np.cumsum(slot[:-1])
+    ws_bytes = int(_lib.load().LZ4B200_decompress_workspace_bytes(n))
+    return _decode(blocks, dst_off, slot, int(slot.sum()), dst_off, 0, caps, 0, ws_bytes, phases,
+                   route(n, per_block_caps=True))
+
+
+def decode_batch_uniform(blocks, cap, wide=True, stride=None, phases="one"):
+    """Run blocks through LZ4B200_decompress_blocks with ONE capacity for all of them (device API).  wide=True gives the
+    workspace LZ4B200_decompress_workspace_bytes_for asks for (blocks above 64 KB: the tiles kernel), wide=False the
+    one for any capacities (blocks above 64 KB: the generic kernel).  stride: destination stride (default: capacity + 64
+    rounded up to 16 bytes; an odd one leaves the destinations unaligned).  Returns a Decoded."""
+    from lz4_b200 import _lib
+    lib = _lib.load()
+    n = len(blocks)
+    stride = (cap + 64 + 15) // 16 * 16 if stride is None else stride
+    assert stride >= cap
+    ws_bytes = int(lib.LZ4B200_decompress_workspace_bytes_for(n, 0, cap)) if wide else int(lib.LZ4B200_decompress_workspace_bytes(n))
+    slot_off = np.arange(n, dtype=np.int64) * stride
+    return _decode(blocks, slot_off, np.full(n, stride, dtype=np.int64), n * stride, None, stride, None, cap, ws_bytes,
+                   phases, route(n, cap, ws_bytes=ws_bytes))
+
+
+# ------------------------------------------------------------------------------------------
+# hostile corpus
+# ------------------------------------------------------------------------------------------
+def lz4_seq(lits, off, mlen=0):
+    """one LZ4 sequence: literals, then a match of offset `off` and length mlen >= 4; off=None: the last sequence"""
+    def ext(v):
+        if v < 15:
+            return b""
+        r = v - 15
+        return b"\xff" * (r // 255) + bytes([r % 255])
+    ll, ml = len(lits), (0 if off is None else mlen - 4)
+    out = bytes([(min(ll, 15) << 4) | min(ml, 15)]) + ext(ll) + lits
+    return out if off is None else out + bytes([off & 255, off >> 8]) + ext(ml)
+
+
+def seq_count_block(nseq):
+    """a valid block of exactly nseq sequences (the last one literals only): 1 literal + an offset-1 match of 4, then
+    empty-literal offset-1 matches of 4, then 16 literals; decodes to 4 * nseq + 13 bytes"""
+    return lz4_seq(b"\x07", 1, 4) + lz4_seq(b"", 1, 4) * (nseq - 2) + lz4_seq(bytes(range(1, 17)), None)
+
+
+# the rows kernel's run table holds kRowsMaxRuns = 20 480 runs (lz4_rows_core.h).  One literal + an offset-1 match of
+# 5 bytes is 4 runs (the literal, and match pieces of 1, 2 and 2 bytes: rw_match_runs), so k such sequences and a
+# literal tail make 4k + 1 runs: 20 477 for k = 5 119 and 20 481 for k = 5 120, in about 30 KB of output.
+RUNS_BELOW, RUNS_ABOVE = 5119, 5120
+
+
+def run_block(k, mlen=5, tail=29):
+    """a valid block of k sequences of 1 literal + an offset-1 match of mlen bytes, then `tail` literals"""
+    return b"".join(lz4_seq(bytes([1 + i % 251]), 1, mlen) for i in range(k)) + lz4_seq(bytes(range(1, tail + 1)), None)
+
+
+def _filler(rng, out, op, until):
+    """valid sequences (8..24 literals + a short match 8..200 back) appended to `out` until it holds `until` bytes"""
+    while len(out) < until:
+        lits = bytes(rng.integers(1, 256, int(rng.integers(8, 25)), dtype=np.uint8))
+        ml = int(rng.integers(4, 13))
+        off = min(op + len(lits), int(rng.integers(8, 201)))
+        out += lz4_seq(lits, off, ml)
+        op += len(lits) + ml
+    return op
+
+
+def event_block(rng, cap, quarter, kind):
+    """A block of about 0.7 * cap input bytes (split scan: >= 4 096) whose first event lies in the middle of input
+    quarter `quarter`: kind="offset", an offset that reaches before the output start (lz4.c:2161); kind="capacity", a
+    match that ends at or beyond capacity - 64 (lz4.c:2137/2142), after which the output runs past the capacity."""
+    n_in = min(int(cap * 0.7), 60000)
+    out = bytearray()
+    op = _filler(rng, out, 0, n_in * (2 * quarter + 1) // 8)
+    if kind == "offset":
+        out += lz4_seq(b"abc", min(op + 3 + int(rng.integers(1, 100)), 65535), 4)
+    else:
+        ml = cap - 64 - (op + 3) + int(rng.integers(0, 40))
+        out += lz4_seq(b"abc", 1, ml)
+        op += 3 + ml
+    _filler(rng, out, op, n_in - 40)
+    return bytes(out) + lz4_seq(bytes(rng.integers(1, 256, 29, dtype=np.uint8)), None)
+
+
+def corrupt(rng, c):
+    """1..5 random edits of the kinds of tests/fuzzer.c:588-622: set a byte, set a special value, flip a bit, delete,
+    insert"""
+    b = bytearray(c)
+    for _ in range(int(rng.integers(1, 6))):
+        if not b:
+            break
+        mode, pos = int(rng.integers(0, 5)), int(rng.integers(0, len(b)))
+        if mode == 0:
+            b[pos] = int(rng.integers(0, 256))
+        elif mode == 1:
+            b[pos] = int(rng.choice([0, 0xFF, 0xF0, 0x0F, 0x10, 0x1F]))
+        elif mode == 2:
+            b[pos] ^= 1 << int(rng.integers(0, 8))
+        elif mode == 3:
+            del b[pos:pos + int(rng.integers(1, 4))]
+        else:
+            b[pos:pos] = bytes(rng.integers(0, 256, int(rng.integers(1, 4)), dtype=np.uint8))
+    return bytes(b) if b else b"\x00"
+
+
+def hostile_corpus(oracle, cap, seed=0, n_corrupt=4):
+    """[(kind, block)] for a batch of one capacity `cap`:
+      datagen  P0 / P0.2 / P0.5 / P0.9 / P1 blocks of cap, cap -/+ 1, cap -/+ 64 and 2 * cap bytes (the capacity is
+               exact, +1, +64, -1, -64 and half of what the block needs)
+      broken   each of those truncated by one byte, cut in half, with one byte appended, and n_corrupt corrupted copies
+      seqs-fit, seqs-over   exactly 8 191, 8 192 / 8 193 sequences (kMaxSeqFast: the mark table is full / one slot short)
+      runs-fit, runs-over   4k + 1 runs just below (k = RUNS_BELOW) and just above (RUNS_ABOVE) the rows kernel's run table, and the
+               denser blocks of offset-1 matches of 8 and 9 bytes (29 109 and 32 746 runs)
+      offset   offset-0 and offset-1 runs of 4 .. 60 000 bytes
+      event    (capacities >= 16 KB: the split scan) an offset error and a capacity event in each input quarter"""
+    rng = np.random.default_rng(seed)
+    out = []
+    for p in (0.0, 0.2, 0.5, 0.9, 1.0):
+        for n in (cap, cap - 1, cap - 64, cap + 1, cap + 64, 2 * cap):
+            raw = oracle.datagen(max(n, 1), p, 1000 * seed + int(100 * p) + n % 97)
+            _, c = oracle.compress(raw, 1)
+            out.append(("datagen", c))
+            out += [("broken", c[:-1]), ("broken", c[:len(c) // 2] or b"\x00"), ("broken", c + b"\x00")]
+            out += [("broken", corrupt(rng, c)) for _ in range(n_corrupt)]
+    out += [("seqs-fit", seq_count_block(8191)), ("seqs-fit", seq_count_block(8192)), ("seqs-over", seq_count_block(8193))]
+    out += [("runs-fit", run_block(RUNS_BELOW)), ("runs-over", run_block(RUNS_ABOVE)),
+            ("runs-over", run_block(7277, 8)), ("runs-over", run_block(6549, 9))]
+    lit = lambda k: bytes(rng.integers(1, 256, k, dtype=np.uint8))
+    for off in (0, 1):
+        for ml in (4, 5, 19, 300, 5000, 60000):
+            out.append(("offset", lz4_seq(lit(20), off, ml) + lz4_seq(lit(3), 7, 9) + lz4_seq(lit(12), None)))
+        blk = b"".join(lz4_seq(lit(5 + k), off, 4 + 7 * k) for k in range(60))
+        out.append(("offset", blk + lz4_seq(lit(12), None)))
+    if cap >= 16384:
+        for q in range(4):
+            out += [("event", event_block(rng, cap, q, "offset")), ("event", event_block(rng, cap, q, "capacity"))]
+    return out
+
+
+def arrange(kinds, rets, n, ncta, seed=0):
+    """Indices into a corpus for a batch of n blocks: the corpus in a shuffled cycle, and hostile blocks (rejected or run
+    overflow) where the kernels' own structure puts blocks side by side:
+      - in all 8 slots of a warp of the split scan (blocks 8 .. 15: the second warp of its first CTA) and as the last
+        block (the last, partial group of lanes);
+      - on CTA columns 0, 1 and ncta - 1 of the persistent expand kernels, which take blocks b, b + ncta, ...: run
+        overflow, rejected and accepted blocks in turn, so that the block-ahead descriptor follows a skipped block."""
+    rng = np.random.default_rng(seed)
+    idx = np.resize(rng.permutation(len(kinds)), n)
+    over = [i for i, k in enumerate(kinds) if k == "runs-over" and rets[i] > 0] or [i for i, r in enumerate(rets) if r < 0]
+    rejected = [i for i, r in enumerate(rets) if r < 0]
+    accepted = [i for i, r in enumerate(rets) if r > 0 and kinds[i] != "runs-over"]
+    hostile = over + rejected
+    pools = (over, rejected, accepted)
+    for col in sorted({0, 1, ncta - 1}):
+        for k, b in enumerate(range(col, n, ncta)):
+            pool = pools[k % 3]
+            idx[b] = pool[(b // 3) % len(pool)]
+    for s in range(8, min(16, n)):
+        idx[s] = hostile[(7 * s) % len(hostile)]
+    if n < 8:
+        idx[:] = [hostile[(5 * s) % len(hostile)] for s in range(n)]
+    idx[n - 1] = rejected[len(rejected) // 2]
+    return idx
+
+
+def check_vs_oracle(oracle, blocks, caps, kinds, res, want_route):
+    """Every block against oracle.decompress: return value (incl. the negative error position) and bytes.  Accepted
+    run-overflow blocks and blocks of more sequences than the mark table must be on the slow list; accepted blocks the
+    rows kernel must take (run and sequence counts just within its tables) must not.  Returns the counts of rejected and
+    accepted blocks, of the slow list, and of the run-overflow blocks on it."""
+    assert res.route == want_route, (res.route, want_route)
+    slow = set(res.slow.tolist())
+    memo = {}
+    cnt = {"rejected": 0, "accepted": 0, "slow": len(slow), "overflow handed off": 0}
+    for i, (blk, cap, kind, (ret, out)) in enumerate(zip(blocks, caps, kinds, res)):
+        key = (blk, cap)
+        if key not in memo:
+            memo[key] = oracle.decompress(blk, cap)
+        eret, eout = memo[key]
+        assert ret == eret, (i, kind, len(blk), cap, ret, eret)
+        if ret < 0:
+            cnt["rejected"] += 1
+            continue
+        assert out == eout, (i, kind, len(blk), cap)
+        cnt["accepted"] += 1
+        if kind == "runs-over" or (kind == "seqs-over" and want_route != "R5"):   # (the tiles kernel has wide marks)
+            assert i in slow, (i, kind, cap, "not handed to the generic kernel")
+            cnt["overflow handed off"] += kind == "runs-over"
+        elif kind in ("runs-fit", "seqs-fit") and cap <= 65536:
+            assert i not in slow, (i, kind, cap, "the rows kernel must take it")
+    return cnt

@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from conftest import GOLDEN
-from gpu_util import decode_batch, decode_batch_uniform, dev, sha, to_dev
+from gpu_util import check_vs_oracle, decode_batch, decode_batch_uniform, dev, hostile_corpus, run_block, sha, to_dev
 
 pytestmark = pytest.mark.gpu
 
@@ -52,39 +52,23 @@ def test_decode_fixture_block(lib, oracle):
 
 
 def test_decode_noisy_source_vs_oracle(lib, oracle):
-    """tests/fuzzer.c:588-622: corrupted blocks -> same verdict / value / bytes as the oracle."""
+    """Per-block capacities (route R1): the hostile corpus of gpu_util -- datagen blocks against exact, slack and short
+    capacities, truncated, extended and corrupted blocks (tests/fuzzer.c:588-622), 8 191 .. 8 193 sequences, run-table
+    overflow, offset-0 / offset-1 runs, split-scan events -- at capacities from 20 bytes to 70 000, each block at its
+    corpus capacity and at one up to 80 bytes above and below -> the oracle's verdict / value / bytes; the run-overflow
+    blocks go to the generic kernel."""
     rng = np.random.default_rng(77)
-    blocks, caps = [], []
-    for trial in range(1500):
-        n = int(rng.choice([20, 64, 100, 300, 1000, 5000, 70000]))
-        d = oracle.datagen(n, float(rng.choice([0.1, 0.5, 0.9])), 5000 + trial)
-        _, c = oracle.compress(d, int(rng.choice([1, 4])))
-        b = bytearray(c)
-        for _ in range(int(rng.integers(0, 6))):
-            mode = rng.integers(0, 4)
-            pos = int(rng.integers(0, len(b)))
-            if mode == 0:
-                b[pos] = int(rng.integers(0, 256))
-            elif mode == 1:
-                b[pos] = int(rng.choice([0, 0xFF, 0xF0, 0x0F, 0x10, 0x1F]))
-            elif mode == 2:
-                del b[pos:pos + int(rng.integers(1, 4))]
-            else:
-                b[pos:pos] = bytes(rng.integers(0, 256, int(rng.integers(1, 4)), dtype=np.uint8))
-        if not b:
-            continue
-        for cap in [n, n + int(rng.integers(0, 80)), max(n - int(rng.integers(0, 80)), 0)]:
-            blocks.append(bytes(b))
-            caps.append(cap)
+    blocks, caps, kinds = [], [], []
+    for cap in (20, 64, 100, 300, 1000, 5000, 65536, 70000):
+        for kind, b in hostile_corpus(oracle, cap, seed=cap, n_corrupt=6):
+            for c in (cap, cap + int(rng.integers(0, 80)), max(cap - int(rng.integers(0, 80)), 0)):
+                blocks.append(b)
+                caps.append(c)
+                kinds.append(kind)
     res = decode_batch(blocks, caps)
-    accepted = 0
-    for blk, cap, (ret, out) in zip(blocks, caps, res):
-        eret, eout = oracle.decompress(blk, cap)
-        assert ret == eret, (len(blk), cap, ret, eret)
-        if ret >= 0:
-            accepted += 1
-            assert out == eout
-    assert accepted > 300
+    cnt = check_vs_oracle(oracle, blocks, caps, kinds, res, "R1")
+    print("R1 %d blocks: %s" % (len(blocks), cnt))
+    assert cnt["accepted"] > 300 and cnt["rejected"] > 2000 and cnt["overflow handed off"] >= 6, cnt
 
 
 def test_decode_overlap_and_long_runs(lib, oracle):
@@ -328,12 +312,24 @@ def test_big_blocks_in_tiles_vs_oracle(lib, oracle):
                 blocks.append(bytes(b))
             res = decode_batch_uniform(blocks, cap, wide=True)
             res_small = decode_batch_uniform(blocks, cap, wide=False)
+            assert (res.route, res_small.route) == ("R5", "R6")
             for blk, (ret, out), (ret2, out2) in zip(blocks, res, res_small):
                 eret, eout = oracle.decompress(blk, cap)
                 assert ret == eret and ret2 == eret, (n, cap, len(blk), ret, ret2, eret)
                 if ret >= 0:
                     assert out == eout and out2 == eout, (n, cap, len(blk))
             assert res[0][0] == n
+    # 200 KB of run-dense sequences (1 literal + an offset-1 match of 5 bytes: 4 runs per 6 bytes): every tile has more
+    # runs than the table holds, and the block goes to the generic kernel once, however many tiles give up
+    big = run_block(33333)
+    n = 6 * 33333 + 29
+    blocks = [big, big[:-1], big + b"\0", big]
+    kinds = ["runs-over", "broken", "broken", "runs-over"]
+    for cap, phases in ((n, "one"), (n + 64, "split")):
+        res = decode_batch_uniform(blocks, cap, wide=True, phases=phases)
+        cnt = check_vs_oracle(oracle, blocks, [cap] * 4, kinds, res, "R5")
+        assert cnt["accepted"] == 2 and sorted(res.slow.tolist()) == [0, 3], (cap, cnt, res.slow)
+        check_vs_oracle(oracle, blocks, [cap] * 4, kinds, decode_batch_uniform(blocks, cap, wide=False, phases=phases), "R6")
     # many big blocks at once: tile-major units across blocks, ragged sizes under one capacity
     raws = [oracle.datagen(int(rng.integers(70000, 600000)), float(rng.choice([0.2, 0.5, 0.9])), 100 + i).tobytes() for i in range(40)]
     blocks = [oracle.compress(r, 1)[1] for r in raws]
@@ -364,6 +360,28 @@ def test_host_buffer_batch_calls(lib, oracle):
     assert rc == 0
     assert (rets[:-1] == bs).all() and rets[-1] == bs - 777
     assert (out[:total] == d).all()
+    # broken blocks in the first and the last pipeline chunk (and one between): each gets the oracle's value, the other
+    # blocks stay intact
+    bad = [3, 1000, 2500, n_blocks - 10]
+    csz[3] -= 1                                         # truncated
+    csz[1000] += 1                                      # one byte appended (the slot's padding is zero)
+    slots[2500 * stride] = 0xFF                         # first token
+    slots[(n_blocks - 10) * stride + int(csz[n_blocks - 10]) // 2] ^= 0x40
+    out[:] = 0
+    rc = lib.LZ4B200_decompress_blocks_host(slots.ctypes.data, offs.ctypes.data, csz.ctypes.data, out.ctypes.data,
+                                            bs, bs, rets.ctypes.data, n_blocks)
+    assert rc == 0
+    for k in bad:
+        eret, eout = oracle.decompress(slots[k * stride:k * stride + int(csz[k])].tobytes(), bs)
+        assert rets[k] == eret, (k, int(rets[k]), eret)
+        if eret >= 0:
+            assert out[k * bs:k * bs + eret].tobytes() == eout, k
+    assert (rets[[3, 1000]] < 0).all()
+    good = np.ones(n_blocks, dtype=bool)
+    good[bad] = False
+    assert (rets[good][:-1] == bs).all() and rets[-1] == bs - 777
+    mask = np.repeat(good, bs)[:total]
+    assert (out[:total][mask] == d[mask]).all()
 
 
 def test_full_size_round_trip_property(lib, oracle):
