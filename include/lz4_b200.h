@@ -157,7 +157,12 @@ LZ4B200_API int LZ4B200_compress_blocks(const void* d_src, int64_t srcStride, co
  * rule, and the compression ratio is within 2 % of the reference's at acceleration 1 (usually above it).
  * acceleration 1..4 probe every position, 5..12 every 2nd, 13..20 every 3rd, ... (faster, lower ratio -- monotone
  * like the reference's parameter, not the same curve).  Blocks above 65 536 bytes are compressed by the
- * byte-identical encoder.  d_outSize[i] == 0: block i did not fit dstCap (as LZ4_compress_fast).
+ * byte-identical encoder; with d_srcSize every block is routed by its own size and srcSize is not used.
+ * d_outSize[i] == 0: block i did not fit dstCap (as LZ4_compress_fast); when it is 0, the first dstCap bytes of
+ * block i's slot may have been written, the bytes past them never are.
+ * Readable padding: a block of up to 65 536 bytes is staged by 16-byte-granular bulk loads, as in
+ * LZ4B200_decompress_blocks, so up to 15 bytes before d_src + i*srcStride and after the block's end must be readable
+ * device memory.
  */
 LZ4B200_API int LZ4B200_compress_blocks_parallel(const void* d_src, int64_t srcStride, const int32_t* d_srcSize, int32_t srcSize,
                                         void* d_dst, int64_t dstStride, int32_t dstCap, int acceleration,

@@ -209,7 +209,7 @@ int LZ4B200_compress_blocks(const void* d_src, int64_t srcStride, const int32_t*
     if (!d_dst || !d_outSize) return LZ4B200_ERR_ARG;
     a.src = (const uint8_t*)d_src; a.srcStride = srcStride; a.srcSizeArr = d_srcSize; a.srcSize = srcSize;
     a.dst = (uint8_t*)d_dst; a.dstStride = dstStride; a.dstCap = dstCap; a.acceleration = acceleration;
-    a.outSize = d_outSize; a.nBlocks = nBlocks;
+    a.outSize = d_outSize; a.nBlocks = nBlocks; a.minSize = INT32_MIN; a.maxSize = INT32_MAX;
     e = (cudaError_t)lz4k_launch_encode(&a, stream);
     return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_encode");
 }
@@ -225,10 +225,19 @@ int LZ4B200_compress_blocks_parallel(const void* d_src, int64_t srcStride, const
     if (!d_dst || !d_outSize) return LZ4B200_ERR_ARG;
     a.src = (const uint8_t*)d_src; a.srcStride = srcStride; a.srcSizeArr = d_srcSize; a.srcSize = srcSize;
     a.dst = (uint8_t*)d_dst; a.dstStride = dstStride; a.dstCap = dstCap; a.acceleration = acceleration;
-    a.outSize = d_outSize; a.nBlocks = nBlocks;
-    /* the parallel parse stages a whole block in shared memory: blocks above 64 KB take the byte-identical encoder */
-    e = (cudaError_t)(srcSize <= 65536 ? lz4k_launch_encode_par(&a, stream) : lz4k_launch_encode(&a, stream));
-    return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_encode_par");
+    a.outSize = d_outSize; a.nBlocks = nBlocks; a.minSize = INT32_MIN; a.maxSize = INT32_MAX;
+    /* the parallel parse stages a whole block in shared memory: blocks above 64 KB take the byte-identical encoder.  With
+     * per-block sizes each block goes by its own size (srcSize is not used): both kernels run, each on its blocks. */
+    if (!d_srcSize) {
+        e = (cudaError_t)(srcSize <= 65536 ? lz4k_launch_encode_par(&a, stream) : lz4k_launch_encode(&a, stream));
+        return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_encode_par");
+    }
+    a.maxSize = 65536;
+    e = (cudaError_t)lz4k_launch_encode_par(&a, stream);
+    if (e != cudaSuccess) return cuda_fail(e, "lz4k_launch_encode_par");
+    a.minSize = 65537; a.maxSize = INT32_MAX;
+    e = (cudaError_t)lz4k_launch_encode(&a, stream);
+    return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_encode");
 }
 
 int LZ4B200_pack_blocks(const void* d_slots, int64_t slotStride, const int32_t* d_sizes, int64_t nBlocks,

@@ -158,6 +158,7 @@ __global__ void __launch_bounds__(kEpThreads, 2) lz4_encode_par_kernel(lz4k_enco
         uint8_t* dst = a.dst + b * a.dstStride;
         const int n = a.srcSizeArr ? a.srcSizeArr[b] : a.srcSize;
         const int64_t cap = a.dstCap;
+        if (n < a.minSize || n > a.maxSize) continue;                 /* another launch's block */
         if (n <= 0 || n > 65536) {                                    /* n == 0: one token byte (lz4.c:1361-1371); larger blocks are not this kernel's */
             if (tid == 0) { int r = 0; if (n == 0 && cap >= 1) { dst[0] = 0; r = 1; } a.outSize[b] = r; }
             continue;

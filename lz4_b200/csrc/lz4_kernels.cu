@@ -1208,6 +1208,7 @@ __global__ void __launch_bounds__(32) lz4_encode_kernel(lz4k_encode_args a)
         const uint8_t* src = a.src + b * a.srcStride;
         uint8_t* dst = a.dst + b * a.dstStride;
         const int n = a.srcSizeArr ? a.srcSizeArr[b] : a.srcSize;
+        if (n < a.minSize || n > a.maxSize) continue;                   // another launch's block
         int r;
         if ((uint32_t)n > kMaxInput) {                                  // lz4.c:1360
             r = 0;

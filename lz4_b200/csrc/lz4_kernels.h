@@ -39,6 +39,8 @@ typedef struct {
     int32_t acceleration;
     int32_t* outSize;
     int64_t nBlocks;
+    int32_t minSize, maxSize;  /* only blocks of minSize .. maxSize bytes are compressed; the others (slot and outSize)
+                                  are left to another launch */
 } lz4k_encode_args;
 
 size_t lz4k_decode_workspace_bytes(int64_t nBlocks);   /* any capacities */

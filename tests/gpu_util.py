@@ -141,6 +141,121 @@ def decode_batch_uniform(blocks, cap, wide=True, stride=None, phases="one"):
 
 
 # ------------------------------------------------------------------------------------------
+# compress and pack calls
+# ------------------------------------------------------------------------------------------
+GUARD = 0xA5
+
+
+def odd_stride(nbytes):
+    """an odd slot stride with at least 16 guard bytes past nbytes"""
+    return nbytes + 17 if nbytes % 2 == 0 else nbytes + 16
+
+
+def compress_call(parallel, blocks, cap, accel, src_stride=None, src_phase=0, dst_stride=None, dst_mis=0,
+                  scalar=None, per_block_sizes=True, seed=0):
+    """One LZ4B200_compress_blocks(_parallel) call.  Block i is at d_src + src_phase + i * src_stride, between random
+    bytes (16 readable bytes around every block: the header's readable padding); its slot is at
+    d_dst + dst_mis + i * dst_stride (default: an odd stride), filled with GUARD bytes.  per_block_sizes=False passes no
+    d_srcSize (all blocks then have the size `scalar`, default len(blocks[0])); scalar defaults to 0 otherwise.
+    Checks that no byte outside the slots changed, nor any byte of a slot past `cap` -- or past the block's size when it
+    fitted.  Returns (return values, [slot i's bytes [0, ret)])."""
+    from lz4_b200 import _lib
+    lib = _lib.load()
+    n = len(blocks)
+    sizes = np.array([len(b) for b in blocks], dtype=np.int32)
+    src_stride = src_stride or int(sizes.max())
+    dst_stride = dst_stride or odd_stride(cap)
+    assert src_stride >= sizes.max() and dst_stride >= cap
+    if scalar is None:
+        scalar = 0 if per_block_sizes else int(sizes[0])
+    if not per_block_sizes:
+        assert (sizes == scalar).all()
+    rng = np.random.default_rng(seed)
+    src = rng.integers(0, 256, 16 + src_phase + n * src_stride + 16, dtype=np.uint8)
+    for i, b in enumerate(blocks):
+        o = 16 + src_phase + i * src_stride
+        src[o:o + len(b)] = np.frombuffer(b, dtype=np.uint8)
+    d_src = to_dev(src)
+    d_sizes = to_dev(sizes)
+    total = dst_mis + n * dst_stride + 64
+    d_dst = torch.full((total,), GUARD, dtype=torch.uint8, device=dev())
+    d_ret = torch.full((n,), -7, dtype=torch.int32, device=dev())
+    fn = lib.LZ4B200_compress_blocks_parallel if parallel else lib.LZ4B200_compress_blocks
+    rc = fn(d_src.data_ptr() + 16 + src_phase, src_stride, d_sizes.data_ptr() if per_block_sizes else None, scalar,
+            d_dst.data_ptr() + dst_mis, dst_stride, cap, accel, d_ret.data_ptr(), n, torch.cuda.current_stream().cuda_stream)
+    _lib.check(rc, "compress_blocks")
+    torch.cuda.synchronize()
+    out, ret = d_dst.cpu().numpy(), d_ret.cpu().numpy()
+    assert (out[:dst_mis] == GUARD).all() and (out[dst_mis + n * dst_stride:] == GUARD).all(), "wrote outside the slots"
+    res = []
+    for i in range(n):
+        r, o = int(ret[i]), dst_mis + i * dst_stride
+        assert 0 <= r <= max(cap, 0), (i, r, cap)
+        keep = r if r > 0 else max(cap, 0)
+        assert (out[o + keep:o + dst_stride] == GUARD).all(), \
+            "block %d (%d bytes, return value %d) wrote past %d bytes of its slot (capacity %d)" % (i, sizes[i], r, keep, cap)
+        res.append(out[o:o + r].tobytes())
+    return ret.copy(), res
+
+
+def pack_model(slots, slot_stride, sizes, header_bytes, frame=None):
+    """LZ4B200_pack_blocks / LZ4B200_pack_frame_blocks restated: (outOff[n + 1], packed bytes).  slots: host bytes of
+    the slots (slot i at i * slot_stride); frame = (source bytes, source stride, blockSize, lastSize)."""
+    n = len(sizes)
+    offs, out = [0], bytearray()
+    for i in range(n):
+        c = int(sizes[i])
+        raw = False
+        if frame is None:
+            pay = max(c, 0)
+            body = slots[i * slot_stride:i * slot_stride + pay]
+        else:
+            fsrc, fstride, bsz, last = frame
+            sz = last if (i == n - 1 and last > 0) else bsz
+            raw = c <= 0 or c >= sz                                      # lz4frame.c:896-899
+            pay = sz if raw else c
+            body = fsrc[i * fstride:i * fstride + pay] if raw else slots[i * slot_stride:i * slot_stride + pay]
+        if header_bytes:
+            out += (pay | (0x80000000 if raw else 0)).to_bytes(4, "little")
+        out += bytes(body)
+        offs.append(len(out))
+    return np.array(offs, dtype=np.int64), bytes(out)
+
+
+def pack_call(slots, slot_stride, sizes, header_bytes, packed_mis=0, slot_phase=0, frame=None):
+    """One LZ4B200_pack_blocks (frame=None) or LZ4B200_pack_frame_blocks call on host slots laid out at
+    d_slots + slot_phase; the packed stream at d_packed + packed_mis in a buffer of GUARD bytes.  Checks outOff and the
+    bytes against pack_model, and that nothing outside [0, outOff[n]) of the stream changed."""
+    from lz4_b200 import _lib
+    lib = _lib.load()
+    n = len(sizes)
+    want_off, want = pack_model(slots, slot_stride, sizes, header_bytes, frame)
+    d_slots = to_dev(np.concatenate([np.zeros(slot_phase, np.uint8), np.frombuffer(bytes(slots), np.uint8),
+                                     np.zeros(64, np.uint8)]))
+    d_sizes = to_dev(np.asarray(sizes, dtype=np.int32))
+    d_off = torch.full((n + 1,), -1, dtype=torch.int64, device=dev())
+    cap = packed_mis + len(want) + 64
+    d_packed = torch.full((cap,), GUARD, dtype=torch.uint8, device=dev())
+    st = torch.cuda.current_stream().cuda_stream
+    if frame is None:
+        rc = lib.LZ4B200_pack_blocks(d_slots.data_ptr() + slot_phase, slot_stride, d_sizes.data_ptr(), n,
+                                     d_packed.data_ptr() + packed_mis, d_off.data_ptr(), header_bytes, st)
+    else:
+        fsrc, fstride, bsz, last = frame
+        d_fsrc = to_dev(np.concatenate([np.frombuffer(bytes(fsrc), np.uint8), np.zeros(64, np.uint8)]))
+        rc = lib.LZ4B200_pack_frame_blocks(d_slots.data_ptr() + slot_phase, slot_stride, d_sizes.data_ptr(),
+                                           d_fsrc.data_ptr(), fstride, bsz, last, n, d_packed.data_ptr() + packed_mis,
+                                           d_off.data_ptr(), st)
+    _lib.check(rc, "pack")
+    torch.cuda.synchronize()
+    off, out = d_off.cpu().numpy(), d_packed.cpu().numpy()
+    assert (off == want_off).all(), "outOff differs at %d" % int(np.flatnonzero(off != want_off)[0])
+    assert out[packed_mis:packed_mis + len(want)].tobytes() == want, "packed bytes differ"
+    assert (out[:packed_mis] == GUARD).all() and (out[packed_mis + len(want):] == GUARD).all(), "wrote outside the stream"
+    return off
+
+
+# ------------------------------------------------------------------------------------------
 # hostile corpus
 # ------------------------------------------------------------------------------------------
 def lz4_seq(lits, off, mlen=0):
