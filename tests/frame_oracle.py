@@ -60,6 +60,24 @@ def compress_frame(oracle, data, block_size_id=4, level=0, content_size=False):
     return bytes(out)
 
 
+def frame_of_blocks(oracle, pieces, bsid, content_size=None, raw=()):
+    """a frame of independent blocks without checksums, one block per piece (at most the block size of bsid): piece i
+    stored raw when i is in `raw`, compressed otherwise; content_size: the header's content-size field (None: absent)"""
+    desc = bytes([(1 << 6) | (1 << 5) | ((content_size is not None) << 3), bsid << 4])
+    if content_size is not None:
+        desc += struct.pack("<Q", content_size)
+    out = bytearray(struct.pack("<I", 0x184D2204) + desc + bytes([(xxh32_short(desc) >> 8) & 0xFF]))
+    for i, p in enumerate(pieces):
+        p = bytes(p)
+        assert 0 < len(p) <= 1 << (8 + 2 * bsid)
+        if i in raw:
+            out += struct.pack("<I", len(p) | 0x80000000) + p
+        else:
+            r, c = oracle.compress(p, 1)
+            out += struct.pack("<I", r) + c
+    return bytes(out + struct.pack("<I", 0))
+
+
 def decompress_frame(oracle, frame):
     assert struct.unpack_from("<I", frame, 0)[0] == 0x184D2204
     flg, bd = frame[4], frame[5]

@@ -63,7 +63,7 @@ def route(n_blocks, cap=None, per_block_caps=False, ws_bytes=0):
 
 class Decoded(list):
     """(return value, decoded bytes) per block.  .slow: the slow list (blocks the generic kernel decoded), .nseq: the
-    scan's sequence count per block, .route: route(...) of the call."""
+    scan's sequence count per block, .route: route(...) of the call, .ws: the workspace (device tensor)."""
 
 
 def _decode(blocks, slot_off, slot_len, total, dst_off, stride, caps, cap, ws_bytes, phases, rt):
@@ -97,6 +97,7 @@ def _decode(blocks, slot_off, slot_len, total, dst_off, stride, caps, cap, ws_by
     res = Decoded()
     res.nseq, res.slow = ws_lists(ws, n)
     res.route = rt
+    res.ws = ws
     assert len(set(res.slow.tolist())) == len(res.slow), "a block is on the slow list twice"
     assert all(ret[b] > 0 for b in res.slow), "a rejected or empty block is on the slow list"
     for i in range(n):
@@ -124,20 +125,52 @@ def decode_batch(blocks, caps, phases="one"):
                    route(n, per_block_caps=True))
 
 
-def decode_batch_uniform(blocks, cap, wide=True, stride=None, phases="one"):
+def decode_batch_uniform(blocks, cap, wide=True, stride=None, phases="one", dst_off=None, ws_bytes=None):
     """Run blocks through LZ4B200_decompress_blocks with ONE capacity for all of them (device API).  wide=True gives the
     workspace LZ4B200_decompress_workspace_bytes_for asks for (blocks above 64 KB: the tiles kernel), wide=False the
-    one for any capacities (blocks above 64 KB: the generic kernel).  stride: destination stride (default: capacity + 64
-    rounded up to 16 bytes; an odd one leaves the destinations unaligned).  Returns a Decoded."""
+    one for any capacities (blocks above 64 KB: the generic kernel); ws_bytes: this many bytes instead.  stride:
+    destination stride (default: capacity + 64 rounded up to 16 bytes; an odd one leaves the destinations unaligned).
+    dst_off: per-block destination offsets instead of the stride (slots of capacity bytes that must not overlap).
+    Returns a Decoded."""
     from lz4_b200 import _lib
     lib = _lib.load()
     n = len(blocks)
     stride = (cap + 64 + 15) // 16 * 16 if stride is None else stride
     assert stride >= cap
-    ws_bytes = int(lib.LZ4B200_decompress_workspace_bytes_for(n, 0, cap)) if wide else int(lib.LZ4B200_decompress_workspace_bytes(n))
-    slot_off = np.arange(n, dtype=np.int64) * stride
-    return _decode(blocks, slot_off, np.full(n, stride, dtype=np.int64), n * stride, None, stride, None, cap, ws_bytes,
+    if ws_bytes is None:
+        ws_bytes = int(lib.LZ4B200_decompress_workspace_bytes_for(n, 0, cap)) if wide else int(lib.LZ4B200_decompress_workspace_bytes(n))
+    if dst_off is None:
+        slot_off, slot_len, total = np.arange(n, dtype=np.int64) * stride, np.full(n, stride, dtype=np.int64), n * stride
+    else:
+        slot_off = np.asarray(dst_off, dtype=np.int64)
+        order = np.argsort(slot_off)
+        assert (np.diff(slot_off[order]) >= cap).all(), "destination slots overlap"
+        slot_len = np.full(n, cap, dtype=np.int64)
+        total, stride = int(slot_off.max()) + cap + 64, 0
+    return _decode(blocks, slot_off, slot_len, total, None if dst_off is None else slot_off, stride, None, cap, ws_bytes,
                    phases, route(n, cap, ws_bytes=ws_bytes))
+
+
+def wide_workspace(res, n, cap):
+    """Readers of what the scan and the tile index left in an R5 call's workspace (ws_view, lz4_kernels.cu): header |
+    nSeq | slowList | marks (2 * (cap / 4 + 2) words per block) | tileFirst (tiles_of(cap) + 1 words per block) |
+    tileFlag.  Returns (marks(b, nseq): the first nseq wide marks of block b, flattened; tile_first(b, nt): its first
+    nt + 1 tileFirst entries)."""
+    r256 = lambda x: (x + 255) // 256 * 256
+    stride = 2 * (cap // 4 + 2)
+    tiles_max = (cap + 61439) // 61440
+    marks0 = 256 + 2 * r256(n * 4)
+    first0 = marks0 + r256(n * stride * 4)
+
+    def words(at, k):
+        return res.ws[at:at + 4 * k].cpu().numpy().view(np.uint32).copy()
+
+    def marks(b, nseq):
+        return words(marks0 + b * stride * 4, 2 * nseq)
+
+    def tile_first(b, nt):
+        return words(first0 + b * (tiles_max + 1) * 4, nt + 1)
+    return marks, tile_first
 
 
 # ------------------------------------------------------------------------------------------

@@ -4,8 +4,8 @@ every destination slot the decoder may not touch (gpu_util.decode_batch*).
 
 The route a call takes depends on the shape of the call alone (gpu_util.route); each test asserts the route it claims,
 so that a change of the dispatch fails here instead of silently moving the coverage.  R1 (per-block capacities) is
-covered here with the split phases and in test_gpu_parity.py::test_decode_noisy_source_vs_oracle; R5 / R6 in
-test_gpu_parity.py::test_big_blocks_in_tiles_vs_oracle.  The last test runs the same saved corpus under every value of
+covered here with the split phases and in test_gpu_parity.py::test_decode_noisy_source_vs_oracle; R5 / R6 (one capacity
+above 64 KB) in test_gpu_big_routes.py, on a corpus of their own.  The last test runs the same saved corpus under every value of
 the developer switch LZ4K_SCAN_IMPL, one process per value.
 """
 import os
