@@ -67,6 +67,25 @@ LZ4B200_API int LZ4_compress_fast_extState(void* state, const char* src, char* d
  * from a clean table, i.e. behaves like LZ4_compress_fast_extState. */
 LZ4B200_API int LZ4_compress_fast_extState_fastReset(void* state, const char* src, char* dst, int srcSize, int dstCapacity, int acceleration);
 
+/* lz4.h:248-272 / lz4.c:1506-1522.  Compresses as much of src as fits into targetDstSize bytes: returns the bytes written
+ * (<= targetDstSize) and sets *srcSizePtr to the input bytes they hold; the output decodes with a capacity of exactly
+ * that count.  Output, return value and *srcSizePtr are identical to the reference's:
+ *   targetDstSize >= LZ4_compressBound(*srcSizePtr): LZ4_compress_fast's result, *srcSizePtr left as it is (lz4.c:1486);
+ *   *srcSizePtr outside 0 .. LZ4_MAX_INPUT_SIZE: 0;  *srcSizePtr == 0: 0 if targetDstSize <= 0, else 1 (one 0x00 byte);
+ *   targetDstSize < 1: 0;  otherwise the fill parse (lz4.c:1118-1122, 1147-1152, 1187-1211, 1304-1333).
+ * Only the returned bytes are written to dst, never a byte at or past dst + targetDstSize.
+ * Deviations: a NULL srcSizePtr or dst returns 0 (the reference dereferences them), and so does a NULL src with
+ * *srcSizePtr > 0.  Without a CUDA device the call returns 0 and leaves *srcSizePtr untouched (no CPU fallback). */
+LZ4B200_API int LZ4_compress_destSize(const char* src, char* dst, int* srcSizePtr, int targetDstSize);
+/* lz4.h:613-617 / lz4.c:1497-1503.  LZ4_compress_destSize with an acceleration: on the compress_fast route it is clamped
+ * to 1 .. 65537 (lz4.c:1386-1387); the fill parse takes it unclamped (lz4.c:1490-1493) and gives the reference's result
+ * for every value from 1 to 2^25 - 1.  Deviations: acceleration <= 0 is treated as 1 there (the reference asserts, and its
+ * release build can emit offset-0 matches) and values of 2^25 and above as 2^25 - 1 (beyond it the reference's
+ * `acceleration << 6` overflows int).  `state` is validated as for LZ4_compress_fast_extState: an invalid state returns
+ * 0 and leaves *srcSizePtr untouched. */
+LZ4B200_API int LZ4_compress_destSize_extState(void* state, const char* src, char* dst, int* srcSizePtr, int targetDstSize,
+                                               int acceleration);
+
 /* lz4.h:208 / lz4.c:2451.  Returns the number of bytes decoded into dst (<= dstCapacity), or a
  * negative value for malformed input / too small dst -- the same value -(position)-1 as the
  * reference's x86-64 build (lz4.c:2443).  Never reads outside src[0,compressedSize) nor writes
@@ -149,6 +168,22 @@ LZ4B200_API int LZ4B200_decompress_blocks_phased(const void* d_src, const int64_
 LZ4B200_API int LZ4B200_compress_blocks(const void* d_src, int64_t srcStride, const int32_t* d_srcSize, int32_t srcSize,
                                         void* d_dst, int64_t dstStride, int32_t dstCap, int acceleration,
                                         int32_t* d_outSize, int64_t nBlocks, void* stream);
+
+/*
+ * Compress every block into a fixed-size destination (the batched LZ4_compress_destSize_extState, lz4.c:1497):
+ *   block i input : d_src + i*srcStride, size n_i = (d_srcSize ? d_srcSize[i] : srcSize)
+ *   block i output: d_dst + i*dstStride; at most min(targetDstSize, LZ4_compressBound(n_i)) bytes are written, never a
+ *                   byte at or past targetDstSize
+ *   d_outSize[i]    : LZ4_compress_destSize_extState(state, src_i, dst_i, &n_i, targetDstSize, acceleration)
+ *   d_srcConsumed[i]: what that call leaves in n_i -- the input bytes block i's output holds, or n_i itself where the
+ *                     reference leaves it alone (the compress_fast route, bad sizes, failures)
+ * The bytes and both values are identical to the reference's, with the acceleration rules of
+ * LZ4_compress_destSize_extState above.  One kernel launch; nBlocks == 0 returns LZ4B200_OK without one.  LZ4B200_ERR_ARG:
+ * nBlocks < 0, a NULL d_dst, d_outSize or d_srcConsumed, or a NULL d_src with blocks present.
+ */
+LZ4B200_API int LZ4B200_compress_blocks_destSize(const void* d_src, int64_t srcStride, const int32_t* d_srcSize, int32_t srcSize,
+                                                 void* d_dst, int64_t dstStride, int32_t targetDstSize, int acceleration,
+                                                 int32_t* d_outSize, int32_t* d_srcConsumed, int64_t nBlocks, void* stream);
 
 /*
  * The same call with the PARALLEL PARSE (throughput mode): every block is a valid LZ4 block that

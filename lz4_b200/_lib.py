@@ -22,6 +22,8 @@ PROTOTYPES = [
     ("LZ4_compress_fast", C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int]),
     ("LZ4_compress_fast_extState", C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int, C.c_int]),
     ("LZ4_compress_fast_extState_fastReset", C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int, C.c_int]),
+    ("LZ4_compress_destSize", C.c_int, [_vp, _vp, C.POINTER(C.c_int), C.c_int]),
+    ("LZ4_compress_destSize_extState", C.c_int, [_vp, _vp, _vp, C.POINTER(C.c_int), C.c_int, C.c_int]),
     ("LZ4_decompress_safe", C.c_int, [_vp, _vp, C.c_int, C.c_int]),
     ("LZ4_decompress_safe_usingDict", C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, C.c_int]),
     ("LZ4B200_device_count", C.c_int, []),
@@ -32,7 +34,8 @@ PROTOTYPES = [
     ("LZ4B200_decompress_blocks", C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i32, _vp, _i64, _vp, _sz, _vp]),
     ("LZ4B200_decompress_blocks_phased", C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i32, _vp, _i64, _vp, _sz, C.c_int, _vp]),
     ("LZ4B200_compress_blocks", C.c_int, [_vp, _i64, _vp, _i32, _vp, _i64, _i32, C.c_int, _vp, _i64, _vp]),
-    ("LZ4B200_compress_blocks_parallel", C.c_int, [_vp, _i64, _vp, _i32, _vp, _i64, _i32, C.c_int, _vp, _i64, _vp]),
+    ("LZ4B200_compress_blocks_destSize", C.c_int, [_vp, _i64, _vp, _i32, _vp, _i64, _i32, C.c_int, _vp, _vp, _i64, _vp]),
+    ("LZ4B200_compress_blocks_parallel",C.c_int, [_vp, _i64, _vp, _i32, _vp, _i64, _i32, C.c_int, _vp, _i64, _vp]),
     ("LZ4B200_pack_blocks", C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, C.c_int, _vp]),
     ("LZ4B200_pack_frame_blocks", C.c_int, [_vp, _i64, _vp, _vp, _i64, _i32, _i32, _i64, _vp, _vp, _vp]),
     ("LZ4B200_peer_copy_async", C.c_int, [_vp, C.c_int, _vp, C.c_size_t, _vp]),

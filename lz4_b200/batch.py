@@ -99,6 +99,39 @@ def compress_blocks(src, block_size, acceleration=1, slots=None, slot_stride=Non
     return slots, out_sizes[:n], stride
 
 
+def compress_blocks_dest_size(src, block_size, target, acceleration=1, slots=None, slot_stride=None, out_sizes=None,
+                              consumed=None, src_sizes=None, stream=None):
+    """Compress as much of each block of src as fits into `target` bytes (LZ4B200_compress_blocks_destSize: block i is
+    LZ4_compress_destSize_extState(state, block_i, slot_i, &n_i, target, acceleration)).
+
+    Returns (slots, out_sizes, consumed, slot_stride): block i's bytes are slots[i*slot_stride : i*slot_stride+out_sizes[i]]
+    and hold its first consumed[i] input bytes.
+    """
+    lib = _lib.load()
+    _need_cuda(src, slots, src_sizes)
+    total = int(src.numel())
+    n = (total + block_size - 1) // block_size if total else 0
+    room = max(min(int(target), compress_bound(block_size)), 1)
+    stride = int(slot_stride if slot_stride is not None else ((room + 15) // 16) * 16)
+    st = _stream(stream)
+    with torch.cuda.stream(st):
+        if slots is None:
+            slots = torch.empty(max(n, 1) * stride, dtype=torch.uint8, device=src.device)
+        if out_sizes is None:
+            out_sizes = torch.empty(max(n, 1), dtype=torch.int32, device=src.device)
+        if consumed is None:
+            consumed = torch.empty(max(n, 1), dtype=torch.int32, device=src.device)
+        if src_sizes is None and n and total != n * block_size:
+            src_sizes = torch.full((n,), block_size, dtype=torch.int32, device=src.device)
+            src_sizes[-1] = total - (n - 1) * block_size
+    rc = lib.LZ4B200_compress_blocks_destSize(src.data_ptr(), int(block_size),
+                                              src_sizes.data_ptr() if src_sizes is not None else None, int(block_size),
+                                              slots.data_ptr(), stride, int(target), int(acceleration),
+                                              out_sizes.data_ptr(), consumed.data_ptr(), n, st.cuda_stream)
+    _lib.check(rc, "LZ4B200_compress_blocks_destSize")
+    return slots, out_sizes[:n], consumed[:n], stride
+
+
 def pack_blocks(slots, slot_stride, sizes, header_bytes=0, packed=None, stream=None):
     """Gather variable-size blocks into one contiguous stream.  Returns (packed, offsets[n+1])."""
     lib = _lib.load()

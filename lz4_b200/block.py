@@ -41,6 +41,23 @@ def LZ4_compress_default(src, dst_capacity=None):
     return r, dst[:max(r, 0)].tobytes()
 
 
+def LZ4_compress_destSize(src, target, acceleration=None):
+    """Returns (ret, consumed, bytes): ret bytes written (<= target), consumed = what the call leaves in *srcSizePtr --
+    lz4.h:272.  acceleration None calls LZ4_compress_destSize, an integer LZ4_compress_destSize_extState (lz4.h:617)."""
+    lib = _lib.load()
+    s = _u8(src)
+    dst = np.empty(max(int(target), 1), dtype=np.uint8)
+    n = C.c_int(len(s))
+    sp = s.ctypes.data if len(s) else None
+    if acceleration is None:
+        r = int(lib.LZ4_compress_destSize(sp, dst.ctypes.data, C.byref(n), int(target)))
+    else:
+        state = np.empty(16416 // 8, dtype=np.uint64)          # LZ4_sizeofState(), 8-byte aligned
+        r = int(lib.LZ4_compress_destSize_extState(state.ctypes.data, sp, dst.ctypes.data, C.byref(n), int(target),
+                                                   int(acceleration)))
+    return r, int(n.value), dst[:max(r, 0)].tobytes()
+
+
 def LZ4_decompress_safe(src, dst_capacity):
     """Returns (ret, bytes): ret decoded size or negative error -- lz4.h:208."""
     lib = _lib.load()

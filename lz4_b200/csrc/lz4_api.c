@@ -214,6 +214,22 @@ int LZ4B200_compress_blocks(const void* d_src, int64_t srcStride, const int32_t*
     return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_encode");
 }
 
+int LZ4B200_compress_blocks_destSize(const void* d_src, int64_t srcStride, const int32_t* d_srcSize, int32_t srcSize,
+                                     void* d_dst, int64_t dstStride, int32_t targetDstSize, int acceleration,
+                                     int32_t* d_outSize, int32_t* d_srcConsumed, int64_t nBlocks, void* stream)
+{
+    lz4k_encode_args a;
+    cudaError_t e;
+    if (nBlocks < 0 || !d_dst || !d_outSize || !d_srcConsumed) return LZ4B200_ERR_ARG;
+    if (nBlocks == 0) return LZ4B200_OK;
+    if (!d_src) return LZ4B200_ERR_ARG;
+    a.src = (const uint8_t*)d_src; a.srcStride = srcStride; a.srcSizeArr = d_srcSize; a.srcSize = srcSize;
+    a.dst = (uint8_t*)d_dst; a.dstStride = dstStride; a.dstCap = targetDstSize; a.acceleration = acceleration;
+    a.outSize = d_outSize; a.nBlocks = nBlocks; a.minSize = INT32_MIN; a.maxSize = INT32_MAX;
+    e = (cudaError_t)lz4k_launch_encode_dest(&a, d_srcConsumed, stream);
+    return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_encode_dest");
+}
+
 int LZ4B200_compress_blocks_parallel(const void* d_src, int64_t srcStride, const int32_t* d_srcSize, int32_t srcSize,
                                      void* d_dst, int64_t dstStride, int32_t dstCap, int acceleration,
                                      int32_t* d_outSize, int64_t nBlocks, void* stream)
@@ -410,16 +426,20 @@ unlock:
 /* ------------------------------------------------------------------------------------------ */
 /* drop-in layer: one block, host pointers, synchronous                                        */
 /* ------------------------------------------------------------------------------------------ */
-static int one_block_compress(const char* src, char* dst, int srcSize, int dstCapacity, int acceleration)
+/* srcSizePtr == NULL: LZ4_compress_fast_extState (lz4.c:1382).  Otherwise LZ4_compress_destSize_extState (lz4.c:1481-1503)
+ * with srcSize = *srcSizePtr and targetDstSize = dstCapacity: *srcSizePtr receives the consumed input where the reference
+ * writes it (the fill route, lz4.c:1332 and :1369), and is left alone on the compress_fast route (lz4.c:1486-1487). */
+static int one_block_compress(const char* src, char* dst, int srcSize, int dstCapacity, int acceleration, int* srcSizePtr)
 {
     int rc = LZ4B200_OK, ret = 0;
+    int32_t res[2] = {0, 0};                 /* return value, consumed input */
     int32_t* d_ret;
     cudaStream_t st;
     size_t capBytes;
     /* argument rules of LZ4_compress_generic, lz4.c:1360-1372, decided on the host so that a bad
      * size never reaches the device */
     if ((unsigned)srcSize > (unsigned)LZ4B200_MAX_INPUT_SIZE) return 0;
-    if (dstCapacity <= 0) return 0;          /* nothing can be written (lz4.c:1362 and the limited checks) */
+    if (dstCapacity <= 0) return 0;          /* nothing can be written (lz4.c:1362, :985 and the limited checks) */
     if (dst == NULL) return 0;
     if (srcSize > 0 && src == NULL) return 0;
     pthread_mutex_lock(&g_lock);
@@ -435,13 +455,19 @@ static int one_block_compress(const char* src, char* dst, int srcSize, int dstCa
     d_ret = (int32_t*)g_ctx.d_meta[0];
     /* copy-in completes before any output is produced: in-place calls (lz4.h:619-678) are safe */
     if (srcSize) CU(cudaMemcpyAsync(g_ctx.d_in[0], src, (size_t)srcSize, cudaMemcpyHostToDevice, st));
-    rc = LZ4B200_compress_blocks(g_ctx.d_in[0], 0, NULL, srcSize, g_ctx.d_out[0], 0, dstCapacity, acceleration, d_ret, 1, st);
+    if (srcSizePtr)
+        rc = LZ4B200_compress_blocks_destSize(g_ctx.d_in[0], 0, NULL, srcSize, g_ctx.d_out[0], 0, dstCapacity, acceleration,
+                                              d_ret, d_ret + 1, 1, st);
+    else
+        rc = LZ4B200_compress_blocks(g_ctx.d_in[0], 0, NULL, srcSize, g_ctx.d_out[0], 0, dstCapacity, acceleration, d_ret, 1, st);
     if (rc != LZ4B200_OK) goto done;
-    CU(cudaMemcpyAsync(&ret, d_ret, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(res, d_ret, (srcSizePtr ? 2 : 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
+    ret = res[0];
     if (ret > 0) {
         CU(cudaMemcpyAsync(dst, g_ctx.d_out[0], (size_t)ret, cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
+        if (srcSizePtr && dstCapacity < LZ4_compressBound(srcSize)) *srcSizePtr = res[1];
     }
 done:
     pthread_mutex_unlock(&g_lock);
@@ -450,12 +476,12 @@ done:
 
 int LZ4_compress_fast(const char* src, char* dst, int srcSize, int dstCapacity, int acceleration)
 {
-    return one_block_compress(src, dst, srcSize, dstCapacity, acceleration);
+    return one_block_compress(src, dst, srcSize, dstCapacity, acceleration, NULL);
 }
 
 int LZ4_compress_default(const char* src, char* dst, int srcSize, int dstCapacity)
 {
-    return one_block_compress(src, dst, srcSize, dstCapacity, 1);
+    return one_block_compress(src, dst, srcSize, dstCapacity, 1, NULL);
 }
 
 static int state_is_valid(const void* state)
@@ -467,13 +493,25 @@ static int state_is_valid(const void* state)
 int LZ4_compress_fast_extState(void* state, const char* src, char* dst, int srcSize, int dstCapacity, int acceleration)
 {
     if (!state_is_valid(state)) return 0;
-    return one_block_compress(src, dst, srcSize, dstCapacity, acceleration);
+    return one_block_compress(src, dst, srcSize, dstCapacity, acceleration, NULL);
 }
 
 int LZ4_compress_fast_extState_fastReset(void* state, const char* src, char* dst, int srcSize, int dstCapacity, int acceleration)
 {
     if (!state_is_valid(state)) return 0;
-    return one_block_compress(src, dst, srcSize, dstCapacity, acceleration);
+    return one_block_compress(src, dst, srcSize, dstCapacity, acceleration, NULL);
+}
+
+int LZ4_compress_destSize(const char* src, char* dst, int* srcSizePtr, int targetDstSize)
+{
+    if (srcSizePtr == NULL) return 0;
+    return one_block_compress(src, dst, *srcSizePtr, targetDstSize, 1, srcSizePtr);
+}
+
+int LZ4_compress_destSize_extState(void* state, const char* src, char* dst, int* srcSizePtr, int targetDstSize, int acceleration)
+{
+    if (!state_is_valid(state) || srcSizePtr == NULL) return 0;
+    return one_block_compress(src, dst, *srcSizePtr, targetDstSize, acceleration, srcSizePtr);
 }
 
 int LZ4_decompress_safe(const char* src, char* dst, int compressedSize, int dstCapacity)

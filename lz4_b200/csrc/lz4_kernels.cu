@@ -1040,14 +1040,19 @@ __device__ __forceinline__ uint32_t emit_runlength(uint8_t* dst, uint32_t op, ui
     return op + full + 1;
 }
 
-template <bool SMALL>
+/* The reference's output directive (lz4.c:930-1338) is FILL or not: without FILL, dstCap decides between notLimited and
+ * limitedOutput at run time (LZ4_compress_fast_extState, lz4.c:1388); with FILL (fillOutput, LZ4_compress_destSize,
+ * lz4.c:1489-1494) the parse stops where dstCap is reached and *consumed receives the input bytes the output holds. */
+template <bool SMALL, bool FILL = false>
 __device__ int encode_block(const uint8_t* __restrict__ src, const int n, uint8_t* __restrict__ dst,
-                            const int dstCap, const uint32_t accel, void* tableMem, const int lane)
+                            const int dstCap, const uint32_t accel, void* tableMem, const int lane,
+                            uint32_t* consumed = nullptr)
 {
     Table<SMALL> T;
     T.t = reinterpret_cast<decltype(T.t)>(tableMem);
+    if (FILL && dstCap < 1) return 0;                         // lz4.c:985
     const int bound = n + n / 255 + 16;
-    const bool limited = !(dstCap >= bound);
+    const bool limited = !FILL && !(dstCap >= bound);
     const int64_t olimit = dstCap;
     const uint32_t mflimit1 = (uint32_t)n - kMfLimit + 1;     // lz4.c:963
     const uint32_t matchlimit = (uint32_t)n - kLastLiterals;  // lz4.c:964
@@ -1144,16 +1149,26 @@ __device__ int encode_block(const uint8_t* __restrict__ src, const int n, uint8_
                 if (haveLiterals) {
                     /* lz4.c:1114-1117 */
                     if (limited && (int64_t)o + lit + (2 + 1 + kLastLiterals) + lit / 255 > olimit) return 0;
+                    /* lz4.c:1118-1122: the token is dropped (op stays at tokenPos) */
+                    if (FILL && (int64_t)o + (lit + 240) / 255 + lit + 2 + 1 + kMfLimit - kMinMatch > olimit) goto tail;
                     if (lit >= 15) o = emit_runlength(dst, o, lit - 15, lane);
                     for (uint32_t k = lane; k < lit; k += 32) dst[o + k] = (uint8_t)ldb<true>(src + anchor + k);
                     o += lit;
                 }
+                /* lz4.c:1147-1152: rewind to the token */
+                if (FILL && (int64_t)o + 2 + 1 + kMfLimit - kMinMatch > olimit) goto tail;
                 /* offset, lz4.c:1162 */
                 const uint32_t off = ip - cand;
                 if (lane == 0) { dst[o] = (uint8_t)off; dst[o + 1] = (uint8_t)(off >> 8); }
                 o += 2;
                 /* lz4.c:1187-1211 */
                 if (limited && (int64_t)o + (1 + kLastLiterals) + (mcode + 240) / 255 > olimit) return 0;
+                bool reduced = false;
+                if (FILL && (int64_t)o + (1 + kLastLiterals) + (mcode + 240) / 255 > olimit) {
+                    /* lz4.c:1190-1194: the match is cut to what fits before the last 1 + LASTLITERALS bytes */
+                    mcode = 14u + ((uint32_t)(olimit - o) - 1u - kLastLiterals) * 255u;
+                    reduced = true;
+                }
                 if (lane == 0) {
                     const uint32_t lt = haveLiterals ? min(lit, 15u) : 0u;
                     dst[tokenPos] = (uint8_t)((lt << 4) | min(mcode, 15u));
@@ -1163,6 +1178,13 @@ __device__ int encode_block(const uint8_t* __restrict__ src, const int n, uint8_
 
                 ip += mcode + kMinMatch;
                 anchor = ip;
+                /* After a reduced match exactly 1 + LASTLITERALS bytes of room are left (op == olimit - 6), so every way on
+                 * from here reaches _last_literals with this anchor and this op, writing nothing before it: the end test
+                 * (lz4.c:1233) goes there directly, a re-test hit fails the _next_match check (op + 11 > olimit), and a
+                 * match found by the search fails the literal check (op + 1 + 11 > olimit).  Which positions the table
+                 * holds cannot change that, so the clearing of lz4.c:1195-1207 (it only matters to a later block that
+                 * reuses the table; every block here starts from a zeroed one) is skipped and the parse ends now. */
+                if (FILL && reduced) goto tail;
                 if (ip >= mflimit1) goto tail;                         // lz4.c:1233
 
                 if (lane == 0) T.put(T.hash(src + ip - 2), ip - 2);    // lz4.c:1236-1242
@@ -1187,12 +1209,17 @@ __device__ int encode_block(const uint8_t* __restrict__ src, const int n, uint8_
 
 tail:   /* lz4.c:1302-1329 */
     {
-        const uint32_t last = (uint32_t)n - anchor;
+        uint32_t last = (uint32_t)n - anchor;
         if (limited && (int64_t)op + last + 1 + (last + 255 - 15) / 255 > olimit) return 0;
+        if (FILL && (int64_t)op + last + 1 + (last + 255 - 15) / 255 > olimit) {
+            last = (uint32_t)(olimit - op) - 1u;              // lz4.c:1307-1311: as many literals as fit
+            last -= (last + 256 - 15) / 256;
+        }
         uint32_t o = op + 1;
         if (lane == 0) dst[op] = (uint8_t)(min(last, 15u) << 4);
         if (last >= 15) o = emit_runlength(dst, o, last - 15, lane);
         for (uint32_t k = lane; k < last; k += 32) dst[o + k] = (uint8_t)ldb<true>(src + anchor + k);
+        if (FILL) *consumed = anchor + last;                   // lz4.c:1327, 1332
         return (int)(o + last);
     }
 }
@@ -1222,6 +1249,47 @@ __global__ void __launch_bounds__(32) lz4_encode_kernel(lz4k_encode_args a)
             r = encode_block<false>(src, n, dst, a.dstCap, accel, tableMem, lane);
         }
         if (lane == 0) a.outSize[b] = r;
+        __syncwarp();
+    }
+}
+
+/* the fill parse takes the acceleration unclamped (lz4.c:1490-1493); above this value `acceleration << 6` overflows int
+ * (lz4.c:1044), and below 1 the reference asserts: both are brought into 1 .. kFillAccelMax */
+constexpr int kFillAccelMax = (1 << 25) - 1;
+
+/* LZ4_compress_destSize_extState per block (lz4.c:1481-1503), same warp, table and grid as lz4_encode_kernel: a target of
+ * at least LZ4_compressBound(n) is LZ4_compress_fast_extState (clamped acceleration, notLimited); below it the fill parse.
+ * srcConsumed[b] is what the reference leaves in *srcSizePtr: the consumed input, or n where it does not write it. */
+__global__ void __launch_bounds__(32) lz4_encode_dest_kernel(lz4k_encode_args a, int32_t* srcConsumed)
+{
+    extern __shared__ uint4 tableMem[];
+    const int lane = threadIdx.x;
+    const int target = a.dstCap;
+    const uint32_t accel = a.acceleration < 1 ? 1u : (a.acceleration > kAccelMax ? (uint32_t)kAccelMax : (uint32_t)a.acceleration);  // lz4.c:1386-1387
+    const uint32_t accelFill = a.acceleration < 1 ? 1u : (a.acceleration > kFillAccelMax ? (uint32_t)kFillAccelMax : (uint32_t)a.acceleration);
+    for (int64_t b = blockIdx.x; b < a.nBlocks; b += gridDim.x) {
+        const uint8_t* src = a.src + b * a.srcStride;
+        uint8_t* dst = a.dst + b * a.dstStride;
+        const int n = a.srcSizeArr ? a.srcSizeArr[b] : a.srcSize;
+        if (n < a.minSize || n > a.maxSize) continue;                   // another launch's block
+        const int bound = (uint32_t)n > kMaxInput ? 0 : n + n / 255 + 16;   // LZ4_compressBound
+        uint32_t consumed = (uint32_t)n;
+        int r;
+        if ((uint32_t)n > kMaxInput) {                                  // lz4.c:1360, on both routes
+            r = 0;
+        } else if (target >= bound) {                                   // lz4.c:1486-1487: notLimited, n > 0 (bound >= 16)
+            if (n == 0) { if (lane == 0) dst[0] = 0; r = 1; }             // lz4.c:1361-1371
+            else if (n < kSmallLimit) r = encode_block<true>(src, n, dst, target, accel, tableMem, lane);
+            else r = encode_block<false>(src, n, dst, target, accel, tableMem, lane);
+        } else if (n == 0) {                                            // lz4.c:1361-1371 with fillOutput
+            if (target <= 0) r = 0;
+            else { if (lane == 0) dst[0] = 0; r = 1; consumed = 0; }
+        } else if (n < kSmallLimit) {                                   // lz4.c:1489-1490
+            r = encode_block<true, true>(src, n, dst, target, accelFill, tableMem, lane, &consumed);
+        } else {                                                        // lz4.c:1492-1493
+            r = encode_block<false, true>(src, n, dst, target, accelFill, tableMem, lane, &consumed);
+        }
+        if (lane == 0) { a.outSize[b] = r; srcConsumed[b] = (int32_t)consumed; }
         __syncwarp();
     }
 }
@@ -1458,15 +1526,29 @@ int lz4k_launch_decode(const lz4k_decode_args* a, int phases, void* stream)
     return (int)cudaGetLastError();
 }
 
+/* grid of the one-warp encoders (lz4_encode_kernel, lz4_encode_dest_kernel) */
+static int64_t encode_grid(int64_t nBlocks)
+{
+    const int sms = device_sms();
+    const int perSm = 13;    // 16 KB table per warp: 13 x 16 KB + reserved fits the 228 KB SM
+    int64_t grid = (int64_t)sms * perSm;
+    return grid > nBlocks ? nBlocks : grid;
+}
+
 int lz4k_launch_encode(const lz4k_encode_args* a, void* stream)
 {
     cudaStream_t s = (cudaStream_t)stream;
     if (a->nBlocks == 0) return 0;
-    const int sms = device_sms();
-    const int perSm = 13;    // 16 KB table per warp: 13 x 16 KB + reserved fits the 228 KB SM
-    int64_t grid = (int64_t)sms * perSm;
-    if (grid > a->nBlocks) grid = a->nBlocks;
-    lz4_encode_kernel<<<(unsigned)grid, 32, kEncodeTableBytes, s>>>(*a);
+    lz4_encode_kernel<<<(unsigned)encode_grid(a->nBlocks), 32, kEncodeTableBytes, s>>>(*a);
+    g_launches++;
+    return (int)cudaGetLastError();
+}
+
+int lz4k_launch_encode_dest(const lz4k_encode_args* a, int32_t* srcConsumed, void* stream)
+{
+    cudaStream_t s = (cudaStream_t)stream;
+    if (a->nBlocks == 0) return 0;
+    lz4_encode_dest_kernel<<<(unsigned)encode_grid(a->nBlocks), 32, kEncodeTableBytes, s>>>(*a, srcConsumed);
     g_launches++;
     return (int)cudaGetLastError();
 }

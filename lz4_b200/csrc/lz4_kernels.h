@@ -51,6 +51,9 @@ size_t lz4k_decode_workspace_bytes_min(int64_t nBlocks, int perBlockCaps, int32_
 int lz4k_launch_decode(const lz4k_decode_args* a, int phases, void* stream);
 int lz4k_launch_encode(const lz4k_encode_args* a, void* stream);       /* byte-identical to LZ4_compress_fast */
 int lz4k_launch_encode_par(const lz4k_encode_args* a, void* stream);   /* parallel parse; blocks of <= 65 536 bytes */
+/* byte-identical to LZ4_compress_destSize_extState with targetDstSize = dstCap: outSize[i] its return value,
+ * srcConsumed[i] what it leaves in *srcSizePtr (block i's own size where it leaves it alone) */
+int lz4k_launch_encode_dest(const lz4k_encode_args* a, int32_t* srcConsumed, void* stream);
 int lz4k_launch_pack(const uint8_t* slots, int64_t slotStride, const int32_t* sizes, int64_t nBlocks,
                      uint8_t* packed, int64_t* outOff, int headerBytes, void* stream);
 /* the body of an LZ4 frame: [LE32 block header][payload] per block; blocks whose compression did not gain are stored raw */
