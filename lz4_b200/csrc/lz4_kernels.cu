@@ -208,7 +208,7 @@ __device__ __forceinline__ void scan_result(const lz4k_decode_args& a, const WsV
     if (r > 0 && !tiled && !rows_eligible(n, cap, ns, w.markStride)) w.slowList[atomicAdd(&w.hdr->slowCount, 1u)] = (uint32_t)b;
 }
 
-/* ---- scan, one THREAD per block: reads through the read-only data cache with L1 prefetch hints ---- */
+/* ---- scan, one THREAD per block: reads through the read-only data cache with L1 prefetch hints, marks in 32-byte chunks ---- */
 
 __global__ void __launch_bounds__(128) lz4_scan_kernel(lz4k_decode_args a)
 {
@@ -1478,10 +1478,10 @@ int lz4k_launch_decode(const lz4k_decode_args* a, int phases, void* stream)
         /* the switch does not apply to a wide batch: only the parallel scan writes the wide marks the tiles kernel reads */
         const bool par = wide || (scanImpl >= 0 ? scanImpl == 1 : (a->dstCapArr == nullptr && a->dstCap > 65536));
         /* blocks of 16..64 KB: kSsLanes merging lanes per block (smaller blocks have too few sequences to split).  Measured
-         * on an H100 SXM at a 700 W power limit (tests/perf/scan_crossover.py, 64 KB P50 blocks, split against one thread per
-         * block): faster while the batch is small (1.20 against 2.01 ms for 4096 blocks, 1.71 against 2.03 ms for 8192), slower beyond (2.49
-         * against 2.06 ms for 12288, 3.45 against 2.10 ms for 16384, 30.7 against 4.9 ms for 65536: the one-thread scan's
-         * time hardly grows with the batch, the split scan's does) */
+         * on an H100 SXM at a 700 W power limit (scan kernel alone, CUDA events, 64 KB P50 blocks, split against one thread
+         * per block, marks in 32-byte chunks): faster while the batch is small (1.20 against 2.13 ms for 4096 blocks, 1.72
+         * against 2.12 ms for 8192), slower beyond (2.51 against 2.10 ms for 12288, 3.47 against 2.14 ms for 16384, 30.6
+         * against 2.6 ms for 65536: the one-thread scan's time grows little with the batch, the split scan's does) */
         const bool split = scanImpl >= 0 ? scanImpl == 2
                                          : (a->dstCapArr == nullptr && a->dstCap >= 16384 && a->dstCap <= 65536 && a->nBlocks <= kSplitMaxBlocks);
         if (split && !par) {

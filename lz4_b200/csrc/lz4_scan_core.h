@@ -22,7 +22,11 @@
 #define SC_LDG(p) __ldg(p)
 #define SC_FUNNEL_R(lo, hi, s) __funnelshift_r((lo), (hi), (s))
 #define SC_PREFETCH_L1(p) asm volatile("prefetch.global.L1 [%0];" ::"l"(p))
+#define SC_ST16(p, a, b, c, d) (*reinterpret_cast<uint4*>(p) = make_uint4((a), (b), (c), (d)))
 #else
+#include <assert.h>
+#define SC_ST16(p, a, b, c, d) \
+    do { assert((reinterpret_cast<uintptr_t>(p) & 15u) == 0); (p)[0] = (a); (p)[1] = (b); (p)[2] = (c); (p)[3] = (d); } while (0)
 #define SC_FN static inline
 #define SC_MFN inline
 #define SC_MFN_COLD inline
@@ -72,7 +76,7 @@ template <bool G, bool W = false> struct MemPtr {
     SC_MFN uint32_t u32(int64_t i) const { return ld32u<G>(p + i); }
     SC_MFN void prefetch(int64_t i) const { if (G) SC_PREFETCH_L1(p + i); }
     static constexpr bool kPrefetch = G;
-    static constexpr bool kWide = W;            /* marks are two words per sequence (blocks above 64 KB): see mark_commit */
+    static constexpr bool kWide = W;            /* marks are two words per sequence (blocks above 64 KB): see MarkSink */
 };
 
 /* =============================================================================================
@@ -106,12 +110,57 @@ constexpr int kMaxSeqFast = 8192;              // most sequences a block of the 
  * expanded from shared memory has at most capacity/4 + 1 sequences (every sequence but the last makes >= 4 bytes) */
 /* Blocks above 64 KB (decoded in 60 KB output tiles by lz4_expand_tiles_kernel) get WIDE marks: two words per sequence,
  * {token position, match start}; the memory class of the walk says which (M::kWide). */
-template <class M> SC_FN void mark_commit(uint32_t* marks, uint32_t markCap, uint32_t nseq, uint32_t tok, uint32_t matchStart)
-{
-    if (!marks || nseq >= markCap) return;
-    if (M::kWide) { marks[2 * (size_t)nseq] = tok; marks[2 * (size_t)nseq + 1] = matchStart; }
-    else marks[nseq] = tok | (matchStart << 16);
-}
+/* A walk's marks leave it in whole 32-byte sectors.  The 32 lanes of a warp write 32 different blocks' marks, so a 4-byte
+ * store per sequence is 32 separate partial-sector writes per step: at 65 536 blocks of 64 KB on the H100 those writes, not
+ * the walk, were most of the scan's time above its floor (DESIGN §5.1: 5.0 ms with them, 2.1 ms without).  The sink
+ * collects the words of one aligned 32-byte chunk in registers and writes the chunk at once, as two 16-byte stores, when
+ * its last word is committed (2.6 ms; 16-byte chunks: 3.1 ms, 64-byte: 2.7 ms).  Words of a chunk that the walk does not
+ * own are never written: those before its first mark (a block's marks start at b x markStride words, rarely a multiple
+ * of 8) and another lane's part in the split / parallel scans.  Such a partial chunk goes out word by word, and so does
+ * the last one, by flush(), which every walk calls when it ends, whatever the exit; the workspace thus holds the same
+ * words as with 4-byte stores.  The words of a walk are consecutive: `first` is the index of its first mark (a mark =
+ * 1 word, or 2 when M::kWide). */
+constexpr int kMarkChunk = 8;                   // words per chunk: one 32-byte sector
+template <class M> struct MarkSink {
+    static constexpr uint32_t kWpm = M::kWide ? 2u : 1u;
+    uint32_t* marks;                            /* nullptr: the walk writes no marks */
+    uint32_t capWords;                          /* mark slots reserved for the block, in words */
+    uint32_t lo, hi;                            /* pending words [lo, hi): all in one aligned chunk */
+    uint32_t q[kMarkChunk];                     /* (indexed by constants only: registers) */
+    SC_MFN MarkSink(uint32_t* m, uint32_t markCap, uint32_t first)
+        : marks(m), capWords(markCap * kWpm), lo(first * kWpm), hi(first * kWpm), q{} {}
+    static SC_MFN uint32_t slot(const uint32_t* p) { return (uint32_t)(reinterpret_cast<uintptr_t>(p) >> 2) & (kMarkChunk - 1); }
+    SC_MFN void push(uint32_t v)
+    {
+        const uint32_t s = slot(marks + hi);
+        #pragma unroll
+        for (int j = 0; j < kMarkChunk; j++) q[j] = (s == (uint32_t)j) ? v : q[j];
+        hi++;
+        if (s == kMarkChunk - 1) flush();
+    }
+    /* the mark of the walk's next sequence (its index = first + marks committed so far) */
+    SC_MFN void commit(uint32_t tok, uint32_t matchStart)
+    {
+        if (!marks || hi >= capWords) return;
+        if (M::kWide) { push(tok); push(matchStart); }
+        else push(tok | (matchStart << 16));
+    }
+    SC_MFN void flush()
+    {
+        if (hi == lo) return;
+        if (hi - lo == kMarkChunk) {
+            #pragma unroll
+            for (int j = 0; j < kMarkChunk; j += 4) SC_ST16(marks + lo + j, q[j], q[j + 1], q[j + 2], q[j + 3]);
+        } else {                                  /* a chunk the walk owns only part of */
+            const uint32_t s0 = slot(marks + lo);
+            uint32_t* c = marks + lo - s0;
+            #pragma unroll
+            for (int j = 0; j < kMarkChunk; j++)
+                if ((uint32_t)j >= s0 && (uint32_t)j < s0 + (hi - lo)) c[j] = q[j];
+        }
+        lo = hi;
+    }
+};
 
 /* where the walk of one block stands between its two loops */
 struct ScanState {
@@ -190,7 +239,7 @@ template <class M> SC_FN void front_prefetch(M& mem, int nI, int fip, int& nextE
 
 /* Returns false for the one error it decides itself (offset before the start of the output, lz4.c:2161), with st.ip at
  * the reference's error position.  The exits are collected and taken once, in the reference's order. */
-template <class M> SC_FN bool scan_front(M& mem, int nIn, int capIn, ScanState& st, uint32_t* marks, uint32_t markCap)
+template <class M> SC_FN bool scan_front(M& mem, int nIn, int capIn, ScanState& st, MarkSink<M>& ms)
 {
     uint32_t nseq = st.nseq;
     int fip = 0, fop = 0, nextEvt = 0;
@@ -200,7 +249,7 @@ template <class M> SC_FN bool scan_front(M& mem, int nIn, int capIn, ScanState& 
         const int opn = fop + s.lit;
         if (s.stop || (uint32_t)opn + (uint32_t)s.mlen >= (uint32_t)(capIn - 64)) break;   // lz4.c:2137/2142 -> safe_match_copy
         if ((int)s.off16 > opn) { st.ip = s.ipn; st.nseq = nseq; return false; }            // lz4.c:2161
-        mark_commit<M>(marks, markCap, nseq, (uint32_t)fip, (uint32_t)opn);
+        ms.commit((uint32_t)fip, (uint32_t)opn);
         fip = s.ipn; fop = opn + s.mlen; nseq++;
     }
     st.ip = fip; st.op = fop; st.nseq = nseq;
@@ -209,7 +258,8 @@ template <class M> SC_FN bool scan_front(M& mem, int nIn, int capIn, ScanState& 
 }
 
 /* ---- the exact byte-wise walk (lz4.c:2083-2435) from the state `st` to the end of the block ---- */
-template <class M> SC_FN int scan_tail(M& mem, int nIn, int capIn, const ScanState& st, uint32_t* nSeqOut, uint32_t* marks, uint32_t markCap)
+/* The marks go to `ms`; the caller flushes it. */
+template <class M> SC_FN int scan_tail(M& mem, int nIn, int capIn, const ScanState& st, uint32_t* nSeqOut, MarkSink<M>& ms)
 {
     int64_t nextPrefetch = st.nextPrefetch;
     int64_t n = nIn, cap = capIn, ip = st.ip, op = st.op, ll = 0, ml = 0, add = 0, tokPos = 0, mop = 0;
@@ -243,7 +293,7 @@ template <class M> SC_FN int scan_tail(M& mem, int nIn, int capIn, const ScanSta
             ml += kMinMatch;
             if (op + ml >= cap - 64) { fast = false; goto safe_match; }
             if ((int64_t)offset > op) goto bad;                        // lz4.c:2161
-            mark_commit<M>(marks, markCap, nseq, (uint32_t)tokPos, (uint32_t)mop);
+            ms.commit((uint32_t)tokPos, (uint32_t)mop);
             op += ml; nseq++;
             continue;
         }
@@ -253,7 +303,7 @@ template <class M> SC_FN int scan_tail(M& mem, int nIn, int capIn, const ScanSta
             op += ll; ip += ll; mop = op;
             offset = mem.u16(ip); ip += 2;
             if (ml != 15 && offset >= 8 && (int64_t)offset <= op) {
-                mark_commit<M>(marks, markCap, nseq, (uint32_t)tokPos, (uint32_t)mop);
+                ms.commit((uint32_t)tokPos, (uint32_t)mop);
                 op += ml + kMinMatch; nseq++;
                 continue;
             }
@@ -267,7 +317,7 @@ safe_literals:
         if (op + ll > cap - kMfLimit || ip + ll > n - (2 + 1 + kLastLiterals)) {   // lz4.c:2279
             if (ip + ll != n || op + ll > cap) goto bad;               // lz4.c:2312
             op += ll;
-            mark_commit<M>(marks, markCap, nseq, (uint32_t)tokPos, (uint32_t)op);   /* last sequence: the end of its literals */
+            ms.commit((uint32_t)tokPos, (uint32_t)op);   /* last sequence: the end of its literals */
             nseq++;
             *nSeqOut = nseq;
             return (int)op;                                            // lz4.c:2439
@@ -283,7 +333,7 @@ match_length:
 safe_match:
         if ((int64_t)offset > op) goto bad;                            // lz4.c:2356
         if (op + ml > cap - kLastLiterals) goto bad;                   // lz4.c:2421-2423
-        mark_commit<M>(marks, markCap, nseq, (uint32_t)tokPos, (uint32_t)mop);
+        ms.commit((uint32_t)tokPos, (uint32_t)mop);
         op += ml; nseq++;
     }
 bad:
@@ -301,11 +351,16 @@ template <class M> SC_DEV int scan_block(M& mem, int nIn, int capIn, uint32_t* n
     if (nIn <= 0) return -1;                                           // lz4.c:2069
     st.fast = (capIn >= 64);                                           // lz4.c:2076
 
-    if (st.fast && !scan_front(mem, nIn, capIn, st, marks, markCap)) {
+    MarkSink<M> ms(marks, markCap, 0u);
+    int r;
+    if (st.fast && !scan_front(mem, nIn, capIn, st, ms)) {
         *nSeqOut = 0;
-        return (int)(-st.ip) - 1;                                      // lz4.c:2443
+        r = (int)(-st.ip) - 1;                                         // lz4.c:2443
+    } else {
+        r = scan_tail(mem, nIn, capIn, st, nSeqOut, ms);
     }
-    return scan_tail(mem, nIn, capIn, st, nSeqOut, marks, markCap);
+    ms.flush();
+    return r;
 }
 
 #endif /* LZ4_SCAN_CORE_H */

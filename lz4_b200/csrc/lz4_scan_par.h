@@ -71,6 +71,7 @@ SC_FN void sp_walk(M& mem, int nI, int capI, int from, int segEnd,
 {
     int fip = from, nextEvt = 0, stop = 0, kind = SP_RAN, errIp = 0;
     uint32_t fop = opBase, cnt = 0;
+    MarkSink<M> ms(marks, markCap, seqBase);
     while (fip < segEnd) {
         front_prefetch(mem, nI, fip, nextEvt);
         const FrontSeq s = front_step(mem, nI, fip);
@@ -79,11 +80,12 @@ SC_FN void sp_walk(M& mem, int nI, int capI, int from, int segEnd,
         if (WRITE) {
             if (opn + (uint32_t)s.mlen >= (uint32_t)(capI - 64)) { kind = SP_END; break; }   // lz4.c:2137/2142
             if (s.off16 > opn) { kind = SP_ERR; errIp = s.ipn; break; }                        // lz4.c:2161
-            mark_commit<M>(marks, markCap, seqBase + cnt, (uint32_t)fip, opn);
+            ms.commit((uint32_t)fip, opn);
         }
         fip = s.ipn; fop = opn + (uint32_t)s.mlen; cnt++;
     }
     if (WRITE) {
+        ms.flush();
         E.kind = kind; E.ip = (kind == SP_ERR) ? errIp : fip; E.op = fop; E.nseq = seqBase + cnt; E.nextEvt = nextEvt;
     } else {
         R.exitPos = fip; R.stop = stop; R.count = cnt; R.olen = fop - opBase;
@@ -154,7 +156,9 @@ SC_FN void sp_finish(int lane, int first, SpShared& S, M& mem, int nI, int capI,
     st.ip = e.ip; st.op = (int64_t)e.op; st.nseq = e.nseq; st.fast = true;
     st.nextPrefetch = (e.nextEvt > 0) ? (int64_t)e.nextEvt + 128 : 128;
     uint32_t ns = 0;
-    S.ret = scan_tail(mem, nI, capI, st, &ns, marks, markCap);
+    MarkSink<M> ms(marks, markCap, e.nseq);
+    S.ret = scan_tail(mem, nI, capI, st, &ns, ms);
+    ms.flush();
     S.nseq = ns;
 }
 

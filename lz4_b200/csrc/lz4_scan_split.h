@@ -218,7 +218,10 @@ SC_FN int ss_p5(SsBlock& S, M& mem, int nIn, int capIn, uint32_t* nSeqOut, uint3
     ScanState st;
     st.ip = tokOf(kx); st.op = (int64_t)startOf(kx); st.nseq = kx; st.fast = true;
     st.nextPrefetch = st.ip + 128;
-    return scan_tail(mem, nIn, capIn, st, nSeqOut, marks, markCap);
+    MarkSink<M> ms(marks, markCap, kx);
+    const int r = scan_tail(mem, nIn, capIn, st, nSeqOut, ms);
+    ms.flush();
+    return r;
 }
 
 #endif /* LZ4_SCAN_SPLIT_H */
