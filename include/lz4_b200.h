@@ -91,6 +91,16 @@ LZ4B200_API int LZ4_compress_destSize_extState(void* state, const char* src, cha
  * reference's x86-64 build (lz4.c:2443).  Never reads outside src[0,compressedSize) nor writes
  * outside dst[0,dstCapacity). */
 LZ4B200_API int LZ4_decompress_safe(const char* src, char* dst, int compressedSize, int dstCapacity);
+/* lz4.h:274-308 / lz4.c:2459-2465.  Decodes the first min(targetOutputSize, dstCapacity) bytes (outputSize) of the block
+ * and returns how many it wrote (<= outputSize), or the same negative value -(position)-1 as the reference (lz4.c:2443).
+ * The return value and the bytes are the reference's: outputSize < 0 or a NULL src -> -1, outputSize == 0 -> 0 whatever
+ * the input, srcSize == 0 -> -1 (lz4.c:2036, :2066, :2069); a valid block given at its exact size -> min(targetOutputSize,
+ * decoded size); bytes past the block's end inside srcSize are parsed as further sequences (lz4.h:299-306).  Only
+ * dst[0, return value) is written, nothing for a rejected block.
+ * Deviations: a NULL dst with outputSize > 0 and a negative srcSize return -1 (undefined in the reference); an offset-0
+ * match that reaches the last 12 bytes of outputSize writes zeros, as LZ4_decompress_safe does (lz4.c:2407), where the
+ * reference copies whatever dst held at those bytes (lz4.c:2392-2404). */
+LZ4B200_API int LZ4_decompress_safe_partial(const char* src, char* dst, int srcSize, int targetOutputSize, int dstCapacity);
 /* lz4.h:546 / lz4.c:2717.  The call lz4frame makes per block (lz4frame.c:1901,1946).  dictSize == 0
  * routes to LZ4_decompress_safe exactly as lz4.c:2721-2722 does; a non-empty dictionary is out
  * of scope for the GPU path (SURVEY.md section 8 f-4) and returns -1. */
@@ -155,6 +165,23 @@ LZ4B200_API int LZ4B200_decompress_blocks_phased(const void* d_src, const int64_
                                                  const int32_t* d_dstCap, int32_t dstCap,
                                                  int32_t* d_outSize, int64_t nBlocks,
                                                  void* d_workspace, size_t workspaceBytes, int phases, void* stream);
+
+/*
+ * Decode a prefix of every block (the batched LZ4_decompress_safe_partial): block i is
+ *   LZ4_decompress_safe_partial(src_i, dst_i, d_srcSize[i], t_i, t_i),  t_i = d_target ? d_target[i] : targetOutputSize
+ * with src_i / dst_i as in LZ4B200_decompress_blocks (the target is the capacity too, lz4.h:289-296).  d_outSize[i] is its
+ * return value; only dst_i[0, d_outSize[i]) is written.  Same readable padding as LZ4B200_decompress_blocks.  The workspace
+ * is sized by LZ4B200_decompress_workspace_bytes_for(nBlocks, d_target != NULL, targetOutputSize).  Three kernel launches
+ * (scan, shared-memory expand, one-warp expand); nBlocks == 0 returns LZ4B200_OK without one.  LZ4B200_ERR_ARG: nBlocks < 0,
+ * a NULL d_src, d_srcOff, d_srcSize, d_dst, d_outSize or d_workspace, or a workspace smaller than the call needs (for a
+ * uniform target above 64 KB that is less than LZ4B200_decompress_workspace_bytes_for asks: those blocks never use the
+ * wide marks).  Targets of at most 64 KB are decoded in shared memory; larger ones by one warp per block.
+ */
+LZ4B200_API int LZ4B200_decompress_blocks_partial(const void* d_src, const int64_t* d_srcOff, const int32_t* d_srcSize,
+                                                  void* d_dst, const int64_t* d_dstOff, int64_t dstStride,
+                                                  const int32_t* d_target, int32_t targetOutputSize,
+                                                  int32_t* d_outSize, int64_t nBlocks,
+                                                  void* d_workspace, size_t workspaceBytes, void* stream);
 
 /*
  * Compress nBlocks independent blocks (the batched LZ4_compress_fast; replaces bench.c:464-493 and

@@ -25,6 +25,7 @@ PROTOTYPES = [
     ("LZ4_compress_destSize", C.c_int, [_vp, _vp, C.POINTER(C.c_int), C.c_int]),
     ("LZ4_compress_destSize_extState", C.c_int, [_vp, _vp, _vp, C.POINTER(C.c_int), C.c_int, C.c_int]),
     ("LZ4_decompress_safe", C.c_int, [_vp, _vp, C.c_int, C.c_int]),
+    ("LZ4_decompress_safe_partial", C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int]),
     ("LZ4_decompress_safe_usingDict", C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, C.c_int]),
     ("LZ4B200_device_count", C.c_int, []),
     ("LZ4B200_last_cuda_error", C.c_char_p, []),
@@ -33,6 +34,7 @@ PROTOTYPES = [
     ("LZ4B200_decompress_workspace_bytes_for", _sz, [_i64, C.c_int, _i32]),
     ("LZ4B200_decompress_blocks", C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i32, _vp, _i64, _vp, _sz, _vp]),
     ("LZ4B200_decompress_blocks_phased", C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i32, _vp, _i64, _vp, _sz, C.c_int, _vp]),
+    ("LZ4B200_decompress_blocks_partial", C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i32, _vp, _i64, _vp, _sz, _vp]),
     ("LZ4B200_compress_blocks", C.c_int, [_vp, _i64, _vp, _i32, _vp, _i64, _i32, C.c_int, _vp, _i64, _vp]),
     ("LZ4B200_compress_blocks_destSize", C.c_int, [_vp, _i64, _vp, _i32, _vp, _i64, _i32, C.c_int, _vp, _vp, _i64, _vp]),
     ("LZ4B200_compress_blocks_parallel",C.c_int, [_vp, _i64, _vp, _i32, _vp, _i64, _i32, C.c_int, _vp, _i64, _vp]),

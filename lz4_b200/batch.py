@@ -66,6 +66,44 @@ def decompress_blocks(comp, offsets, sizes, block_capacity, out=None, out_stride
     return out, out_sizes
 
 
+def decompress_blocks_partial(comp, offsets, sizes, target, out=None, out_stride=None, out_sizes=None,
+                              workspace=None, stream=None):
+    """Decode a prefix of len(sizes) independent blocks (LZ4B200_decompress_blocks_partial: block i is
+    LZ4_decompress_safe_partial(block_i, slot_i, sizes[i], t_i, t_i)).
+
+    target: one int for every block, or an int32 device tensor of per-block targets.  Block i is written to
+    out[i*out_stride : i*out_stride + out_sizes[i]] (out_stride defaults to the largest target).
+    Returns (out, out_sizes) -- out_sizes[i] is LZ4_decompress_safe_partial's return value.
+    """
+    lib = _lib.load()
+    per_block = isinstance(target, torch.Tensor)
+    _need_cuda(comp, offsets, sizes, out, target if per_block else None)
+    n = int(sizes.numel())
+    if per_block:
+        assert target.dtype == torch.int32 and target.numel() == n
+        uniform = 0
+        biggest = int(target.max()) if n else 0
+    else:
+        uniform = biggest = int(target)
+    stride = int(out_stride if out_stride is not None else max(biggest, 0))
+    st = _stream(stream)
+    with torch.cuda.stream(st):
+        if out is None:
+            out = torch.empty(max(n * stride, 1), dtype=torch.uint8, device=comp.device)
+        if out_sizes is None:
+            out_sizes = torch.empty(n, dtype=torch.int32, device=comp.device)
+    ws_bytes = int(lib.LZ4B200_decompress_workspace_bytes_for(n, int(per_block), uniform))
+    if workspace is None or workspace.numel() < ws_bytes:
+        workspace = _workspace(comp.device, ws_bytes, st)
+    assert offsets.dtype == torch.int64 and sizes.dtype == torch.int32 and comp.dtype == torch.uint8
+    rc = lib.LZ4B200_decompress_blocks_partial(comp.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), out.data_ptr(),
+                                               None, stride, target.data_ptr() if per_block else None, uniform,
+                                               out_sizes.data_ptr(), n, workspace.data_ptr(), workspace.numel(),
+                                               st.cuda_stream)
+    _lib.check(rc, "LZ4B200_decompress_blocks_partial")
+    return out, out_sizes
+
+
 def compress_blocks(src, block_size, acceleration=1, slots=None, slot_stride=None, slot_capacity=None,
                     out_sizes=None, src_sizes=None, stream=None, mode="exact"):
     """Compress src (u8 device tensor) as ceil(len/block_size) independent blocks.

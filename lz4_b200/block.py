@@ -58,6 +58,19 @@ def LZ4_compress_destSize(src, target, acceleration=None):
     return r, int(n.value), dst[:max(r, 0)].tobytes()
 
 
+def LZ4_decompress_safe_partial(src, target, dst_capacity=None):
+    """Returns (ret, bytes): the first min(target, dst_capacity) decoded bytes at most, ret their count or a negative
+    error -- lz4.h:308.  dst_capacity None means target."""
+    lib = _lib.load()
+    s = _u8(src)
+    target = int(target)
+    cap = target if dst_capacity is None else int(dst_capacity)
+    dst = np.empty(max(min(target, cap), 1), dtype=np.uint8)
+    sp = s.ctypes.data if len(s) else np.zeros(1, dtype=np.uint8).ctypes.data
+    r = int(lib.LZ4_decompress_safe_partial(sp, dst.ctypes.data, len(s), target, cap))
+    return r, dst[:max(r, 0)].tobytes()
+
+
 def LZ4_decompress_safe(src, dst_capacity):
     """Returns (ret, bytes): ret decoded size or negative error -- lz4.h:208."""
     lib = _lib.load()

@@ -198,6 +198,26 @@ int LZ4B200_decompress_blocks(const void* d_src, const int64_t* d_srcOff, const 
                                             d_outSize, nBlocks, d_workspace, workspaceBytes, 3, stream);
 }
 
+int LZ4B200_decompress_blocks_partial(const void* d_src, const int64_t* d_srcOff, const int32_t* d_srcSize,
+                                      void* d_dst, const int64_t* d_dstOff, int64_t dstStride,
+                                      const int32_t* d_target, int32_t targetOutputSize,
+                                      int32_t* d_outSize, int64_t nBlocks,
+                                      void* d_workspace, size_t workspaceBytes, void* stream)
+{
+    lz4k_decode_args a;
+    cudaError_t e;
+    if (nBlocks < 0) return LZ4B200_ERR_ARG;
+    if (nBlocks == 0) return LZ4B200_OK;
+    if (!d_src || !d_srcOff || !d_srcSize || !d_dst || !d_outSize || !d_workspace) return LZ4B200_ERR_ARG;
+    if (workspaceBytes < lz4k_decode_workspace_bytes_min(nBlocks, d_target != NULL, targetOutputSize)) return LZ4B200_ERR_ARG;
+    a.src = (const uint8_t*)d_src; a.srcOff = d_srcOff; a.srcSize = d_srcSize;
+    a.dst = (uint8_t*)d_dst; a.dstOff = d_dstOff; a.dstStride = dstStride;
+    a.dstCapArr = d_target; a.dstCap = targetOutputSize; a.outSize = d_outSize; a.nBlocks = nBlocks;   /* capacity = target */
+    a.workspace = d_workspace; a.workspaceBytes = workspaceBytes;
+    e = (cudaError_t)lz4k_launch_decode_partial(&a, stream);
+    return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_decode_partial");
+}
+
 int LZ4B200_compress_blocks(const void* d_src, int64_t srcStride, const int32_t* d_srcSize, int32_t srcSize,
                             void* d_dst, int64_t dstStride, int32_t dstCap, int acceleration,
                             int32_t* d_outSize, int64_t nBlocks, void* stream)
@@ -514,17 +534,15 @@ int LZ4_compress_destSize_extState(void* state, const char* src, char* dst, int*
     return one_block_compress(src, dst, *srcSizePtr, targetDstSize, acceleration, srcSizePtr);
 }
 
-int LZ4_decompress_safe(const char* src, char* dst, int compressedSize, int dstCapacity)
+/* One block through the batch layer: LZ4_decompress_safe (partial == 0) or LZ4_decompress_safe_partial with outputSize =
+ * dstCapacity.  The caller has decided the argument rules (compressedSize > 0, dstCapacity > 0, src and dst non-NULL).
+ * Only the returned bytes are copied back: dst is untouched for a rejected block. */
+static int one_block_decompress(const char* src, char* dst, int compressedSize, int dstCapacity, int partial)
 {
     int rc = LZ4B200_OK, ret = -1;
     cudaStream_t st;
     int64_t* d_off; int32_t* d_size; int32_t* d_ret;
     int64_t zero = 0;
-    /* lz4.c:2036, :2064-2069 decided on the host */
-    if (src == NULL || dstCapacity < 0) return -1;
-    if (dstCapacity == 0) return (compressedSize == 1 && src[0] == 0) ? 0 : -1;
-    if (compressedSize <= 0) return -1;
-    if (dst == NULL) return -1;
     pthread_mutex_lock(&g_lock);
     if ((rc = ctx_init()) != LZ4B200_OK) goto done;
     st = g_ctx.stream[0];
@@ -540,8 +558,12 @@ int LZ4_decompress_safe(const char* src, char* dst, int compressedSize, int dstC
     /* the whole input is on the device before the first output byte is written back: in-place
      * decompression (lz4.h:619-678, tests/fuzzer.c:1177-1187) needs no special handling */
     CU(cudaMemcpyAsync(g_ctx.d_in[0], src, (size_t)compressedSize, cudaMemcpyHostToDevice, st));
-    rc = LZ4B200_decompress_blocks(g_ctx.d_in[0], d_off, d_size, g_ctx.d_out[0], NULL, 0, NULL, dstCapacity,
-                                   d_ret, 1, g_ctx.d_ws[0], g_ctx.ws_cap[0], st);
+    if (partial)
+        rc = LZ4B200_decompress_blocks_partial(g_ctx.d_in[0], d_off, d_size, g_ctx.d_out[0], NULL, 0, NULL, dstCapacity,
+                                               d_ret, 1, g_ctx.d_ws[0], g_ctx.ws_cap[0], st);
+    else
+        rc = LZ4B200_decompress_blocks(g_ctx.d_in[0], d_off, d_size, g_ctx.d_out[0], NULL, 0, NULL, dstCapacity,
+                                       d_ret, 1, g_ctx.d_ws[0], g_ctx.ws_cap[0], st);
     if (rc != LZ4B200_OK) goto done;
     CU(cudaMemcpyAsync(&ret, d_ret, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
@@ -552,6 +574,28 @@ int LZ4_decompress_safe(const char* src, char* dst, int compressedSize, int dstC
 done:
     pthread_mutex_unlock(&g_lock);
     return rc == LZ4B200_OK ? ret : -1;
+}
+
+int LZ4_decompress_safe(const char* src, char* dst, int compressedSize, int dstCapacity)
+{
+    /* lz4.c:2036, :2064-2069 decided on the host */
+    if (src == NULL || dstCapacity < 0) return -1;
+    if (dstCapacity == 0) return (compressedSize == 1 && src[0] == 0) ? 0 : -1;
+    if (compressedSize <= 0) return -1;
+    if (dst == NULL) return -1;
+    return one_block_decompress(src, dst, compressedSize, dstCapacity, 0);
+}
+
+int LZ4_decompress_safe_partial(const char* src, char* dst, int srcSize, int targetOutputSize, int dstCapacity)
+{
+    const int outputSize = targetOutputSize < dstCapacity ? targetOutputSize : dstCapacity;   /* lz4.c:2461 */
+    /* lz4.c:2036, :2066, :2069 decided on the host; a negative srcSize (undefined in the reference) and a NULL dst with
+     * room to write are rejected */
+    if (src == NULL || outputSize < 0) return -1;
+    if (outputSize == 0) return 0;
+    if (srcSize <= 0) return -1;
+    if (dst == NULL) return -1;
+    return one_block_decompress(src, dst, srcSize, outputSize, 1);
 }
 
 int LZ4_decompress_safe_usingDict(const char* src, char* dst, int compressedSize, int dstCapacity,

@@ -183,6 +183,16 @@ __device__ __forceinline__ WsView ws_view(const lz4k_decode_args& a)
     const bool wide = use_wide(a.dstCapArr, a.dstCap, a.nBlocks, a.workspaceBytes);
     return ws_view(a.workspace, a.nBlocks, mark_stride(a.dstCapArr, a.dstCap, wide), wide ? tiles_of(a.dstCap) : 0u);
 }
+/* The partial call (lz4k_launch_decode_partial; dstCapArr / dstCap hold the targets) never decodes in tiles, so its layout is
+ * the narrow one whatever the workspace: the smallest that LZ4B200_decompress_workspace_bytes_for sizes for the same
+ * arguments.  It never runs the split scan either, and its scratch region holds one word per block instead: the input
+ * bytes the scan consumed (partial_used), present whenever the batch has marks (markStride > 0: 2 x markStride words
+ * per block) -- a batch without marks sends every block to the generic kernel, which does not need it. */
+__device__ __forceinline__ WsView partial_view(const lz4k_decode_args& a)
+{
+    return ws_view(a.workspace, a.nBlocks, mark_stride(a.dstCapArr, a.dstCap), 0u);
+}
+__device__ __forceinline__ uint32_t* partial_used(const WsView& w) { return w.markStride ? w.scratch : nullptr; }
 
 /* a block the shared-memory expand kernel takes: input and output fit its 64 KB windows, marks for every sequence */
 __device__ __forceinline__ bool rows_eligible(int n, int cap, uint32_t nseq, uint32_t markStride)
@@ -222,6 +232,28 @@ __global__ void __launch_bounds__(128) lz4_scan_kernel(lz4k_decode_args a)
     MemPtr<true> mem{src};
     const int r = scan_block(mem, n, cap, &ns, scan_marks(w, b, n, cap), w.markStride);
     scan_result(a, w, b, n, cap, r, ns);
+}
+
+/* ---- scan of the partial call, one THREAD per block: LZ4_decompress_safe_partial with outputSize = the block's target ----
+ * The walk ends at the target, so its chain of dependent steps grows with the decoded prefix, not the block.  Marks are
+ * written for every target of at most 64 KB, whatever the input size: the rows kernel stages only the consumed prefix.
+ * Route P1 (lz4_expand_rows_partial_kernel): rows_eligible on (consumed, target); P2 (the generic kernel): the rest. */
+__global__ void __launch_bounds__(128) lz4_scan_partial_kernel(lz4k_decode_args a)
+{
+    int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= a.nBlocks) return;
+    const WsView w = partial_view(a);
+    const uint8_t* src = a.src + a.srcOff[b];
+    const int n = a.srcSize[b];
+    const int cap = a.dstCapArr ? a.dstCapArr[b] : a.dstCap;
+    uint32_t ns = 0, used = 0;
+    uint32_t* marks = (n > 0 && cap > 0 && cap <= 65536 && w.markStride > 0) ? w.marks + (size_t)b * w.markStride : nullptr;
+    MemPtr<true> mem{src};
+    const int r = scan_block<MemPtr<true>, true>(mem, n, cap, &ns, marks, w.markStride, &used);
+    a.outSize[b] = r;
+    w.nSeq[b] = ns;
+    if (uint32_t* u = partial_used(w)) u[b] = used;
+    if (r > 0 && !rows_eligible((int)used, cap, ns, w.markStride)) w.slowList[atomicAdd(&w.hdr->slowCount, 1u)] = (uint32_t)b;
 }
 
 /* ---- scan, kSsLanes lanes per block that merge (lz4_scan_split.h): the chain of dependent steps is kSsLanes times shorter ----
@@ -406,31 +438,37 @@ __global__ void __launch_bounds__(256) lz4_tile_index_kernel(lz4k_decode_args a)
 /* =============================================================================================
  * expand (generic): one warp per accepted block, any block size, straight to global memory
  * ============================================================================================= */
-__global__ void __launch_bounds__(128) lz4_expand_generic_kernel(lz4k_decode_args a)
+/* PARTIAL: the partial call's blocks (route P2): the decode stops at the scan's return value, and the literal and match
+ * runs that reach it are cut there (the scan's walk ended at the same place, lz4_scan_core.h: scan_tail) */
+template <bool PARTIAL>
+__device__ __forceinline__ void expand_generic(const lz4k_decode_args& a)
 {
     const int lane = threadIdx.x & 31;
     const int64_t warp0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nWarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    const WsView w = ws_view(a);
+    const WsView w = PARTIAL ? partial_view(a) : ws_view(a);
     const int64_t count = w.hdr->slowCount;       // only blocks the scan accepted and left to this kernel
     for (int64_t idx = warp0; idx < count; idx += nWarps) {
     const int64_t b = w.slowList[idx];
     const uint8_t* __restrict__ src = a.src + a.srcOff[b];
     uint8_t* dst = a.dst + (a.dstOff ? a.dstOff[b] : b * a.dstStride);
     const int64_t n = a.srcSize[b];
+    const int64_t total = PARTIAL ? a.outSize[b] : 0;
     int64_t ip = 0, op = 0;
 
     for (;;) {
         uint32_t token = ldb<true>(src + ip); ip++;
         int64_t ll = token >> 4;
         if (ll == 15) { uint32_t x; do { x = ldb<true>(src + ip); ip++; ll += x; } while (x == 255); }
+        if (PARTIAL && ll > total - op) ll = total - op;
         for (int64_t k = lane; k < ll; k += 32) dst[op + k] = (uint8_t)ldb<true>(src + ip + k);
         ip += ll; op += ll;
-        if (ip >= n) break;
+        if (PARTIAL ? op >= total : ip >= n) break;
         uint32_t offset = ld16<true>(src + ip); ip += 2;
         int64_t ml = token & 15;
         if (ml == 15) { uint32_t x; do { x = ldb<true>(src + ip); ip++; ml += x; } while (x == 255); }
         ml += kMinMatch;
+        if (PARTIAL && ml > total - op) ml = total - op;
         __syncwarp();                             // everything before `op` is now visible to all lanes
         if (offset == 0) {                        // reference zero-fills (lz4.c:2407, :500)
             for (int64_t k = lane; k < ml; k += 32) dst[op + k] = 0;
@@ -442,10 +480,14 @@ __global__ void __launch_bounds__(128) lz4_expand_generic_kernel(lz4k_decode_arg
             for (int64_t k = lane; k < ml; k += 32) dst[op + k] = from[k % offset];
         }
         op += ml;
+        if (PARTIAL && op >= total) break;
     }
     __syncwarp();
     }
 }
+
+__global__ void __launch_bounds__(128) lz4_expand_generic_kernel(lz4k_decode_args a) { expand_generic<false>(a); }
+__global__ void __launch_bounds__(128) lz4_expand_generic_partial_kernel(lz4k_decode_args a) { expand_generic<true>(a); }
 
 /* =============================================================================================
  * expand (rows): one CTA per 64 KB block, one output BYTE per thread, waves + run table
@@ -660,12 +702,16 @@ __device__ __forceinline__ void rows_store(uint8_t* dst, const uint8_t* out, con
     }
 }
 
-__global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_rows_kernel(lz4k_decode_args a)
+/* PARTIAL: the partial call's blocks (route P1).  The last sequence is rebuilt from its literal start and the return value
+ * (rw_parse<true>), so no run starts at or past the return value; only the consumed input prefix is staged, and
+ * eligibility is decided on (consumed, target) instead of (input size, capacity). */
+template <bool PARTIAL>
+__device__ __forceinline__ void expand_rows(const lz4k_decode_args& a)
 {
     extern __shared__ __align__(16) uint8_t smemRaw[];
     RowsSmem& S = *reinterpret_cast<RowsSmem*>(smemRaw);
     const int tid = threadIdx.x;
-    const WsView w = ws_view(a);
+    const WsView w = PARTIAL ? partial_view(a) : ws_view(a);
     const uint32_t le = lanemask_le();
     const uint32_t outA = (uint32_t)offsetof(RowsSmem, out);
     const int zeroDelta0 = (int)offsetof(RowsSmem, zero) - (int)outA;
@@ -682,7 +728,7 @@ __global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_rows_kernel(lz4k_d
         Raw r;
         r.b = b; r.off = 0; r.dOff = 0; r.n = 0; r.total = 0; r.cap = 0; r.ns = 0;
         if (b < a.nBlocks) {
-            r.n = a.srcSize[b]; r.total = a.outSize[b]; r.ns = w.nSeq[b]; r.off = a.srcOff[b];
+            r.n = PARTIAL ? (partial_used(w) ? (int)partial_used(w)[b] : 0) : a.srcSize[b]; r.total = a.outSize[b]; r.ns = w.nSeq[b]; r.off = a.srcOff[b];
             r.cap = a.dstCapArr ? a.dstCapArr[b] : a.dstCap;
             r.dOff = a.dstOff ? a.dstOff[b] : b * a.dstStride;
         }
@@ -750,13 +796,13 @@ __global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_rows_kernel(lz4k_d
         for (int i = 0; i < kRowsCache; i++) {
             const int k = tid + i * kRowsThreads;
             if (k < nseq) {
-                sq[i] = rw_parse(in, mk[i], k, k + 1 == nseq);
+                sq[i] = rw_parse<PARTIAL>(in, mk[i], k, k + 1 == nseq, total);
                 if (sq[i].ll > 0) setBit(sq[i].op, 0);
                 if (sq[i].mlen > 0) rw_match_runs(sq[i].m, sq[i].off, sq[i].mlen, zeroDelta0, setBit);
             }
         }
         for (int k = tid + kRowsCache * kRowsThreads; k < nseq; k += kRowsThreads) {
-            const RwSeq s = rw_parse(in, marks[k], k, k + 1 == nseq);
+            const RwSeq s = rw_parse<PARTIAL>(in, marks[k], k, k + 1 == nseq, total);
             if (s.ll > 0) setBit(s.op, 0);
             if (s.mlen > 0) rw_match_runs(s.m, s.off, s.mlen, zeroDelta0, setBit);
         }
@@ -785,7 +831,7 @@ __global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_rows_kernel(lz4k_d
                 if (k < nseq) emit(sq[i]);
             }
             for (int k = tid + kRowsCache * kRowsThreads; k < nseq; k += kRowsThreads) {
-                emit(rw_parse(in, marks[k], k, k + 1 == nseq));
+                emit(rw_parse<PARTIAL>(in, marks[k], k, k + 1 == nseq, total));
             }
             __syncthreads();
             PHASE_MARK(4);                                     // pass 2
@@ -814,6 +860,9 @@ __global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_rows_kernel(lz4k_d
     }
     if (tid == 0) tma_wait_all0();
 }
+
+__global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_rows_kernel(lz4k_decode_args a) { expand_rows<false>(a); }
+__global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_rows_partial_kernel(lz4k_decode_args a) { expand_rows<true>(a); }
 
 /* =============================================================================================
  * expand (tiles): blocks ABOVE 64 KB (lz4frame's 256 KB .. 4 MB blocks), one CTA per 60 KB OUTPUT TILE
@@ -1523,6 +1572,32 @@ int lz4k_launch_decode(const lz4k_decode_args* a, int phases, void* stream)
         lz4_expand_generic_kernel<<<(unsigned)grid2, threads, 0, s>>>(*a);
         g_launches++;
     }
+    return (int)cudaGetLastError();
+}
+
+/* LZ4_decompress_safe_partial per block, outputSize = dstCapArr[b] / dstCap: one-thread partial scan, then route P1 (rows
+ * kernel, targets <= 64 KB whose consumed prefix, sequences and runs fit it) and P2 (generic kernel, everything else).  Three
+ * launches; the tiles kernel is not used, so targets above 64 KB take the generic kernel (correct, not tuned). */
+int lz4k_launch_decode_partial(const lz4k_decode_args* a, void* stream)
+{
+    cudaStream_t s = (cudaStream_t)stream;
+    if (a->nBlocks == 0) return 0;
+    if (a->workspaceBytes < ws_bytes(a->nBlocks, mark_stride(a->dstCapArr, a->dstCap))) return (int)cudaErrorInvalidValue;
+    static int sms = 0;
+    if (sms == 0) {
+        cudaError_t e = cudaFuncSetAttribute(lz4_expand_rows_partial_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RowsSmem));
+        if (e != cudaSuccess) return (int)e;
+        sms = device_sms();
+    }
+    cudaError_t e = cudaMemsetAsync(a->workspace, 0, 256, s);         // WsHeader: list counter
+    if (e != cudaSuccess) return (int)e;
+    lz4_scan_partial_kernel<<<(unsigned)((a->nBlocks + 127) / 128), 128, 0, s>>>(*a);
+    const int64_t grid = a->nBlocks < sms ? a->nBlocks : sms;         // persistent: one CTA per SM
+    lz4_expand_rows_partial_kernel<<<(unsigned)grid, kRowsThreads, sizeof(RowsSmem), s>>>(*a);
+    int64_t grid2 = (a->nBlocks * 32 + 127) / 128;
+    if (grid2 > (int64_t)sms * 16) grid2 = (int64_t)sms * 16;
+    lz4_expand_generic_partial_kernel<<<(unsigned)grid2, 128, 0, s>>>(*a);
+    g_launches += 3;
     return (int)cudaGetLastError();
 }
 

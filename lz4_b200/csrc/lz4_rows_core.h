@@ -56,10 +56,34 @@ struct RwSeq {
 
 /* Sequence k from the scan's mark (token position | match start << 16, lz4_scan_core.h): the lane re-reads only its
  * own token -- literal length incl. extension bytes (lz4.c:1978-2014), the offset and the match length; the last
- * sequence has no match and its mark holds the end of its literals. */
-RW_FN RwSeq rw_parse(const uint8_t* in, uint32_t mk, int k, bool last)
+ * sequence has no match and its mark holds the end of its literals.
+ * PARTIAL (LZ4_decompress_safe_partial, lz4_scan_core.h: scan_tail): the last sequence's mark holds the START of its
+ * literals and the decode ended at `total`, so its literal run is min(token's length, total - start) bytes and, if the
+ * token's literals end before `total`, a match at their end fills the rest.  The match length comes from `total`, not
+ * from the token: the only input bytes read are the ones the scan read. */
+template <bool PARTIAL = false>
+RW_FN RwSeq rw_parse(const uint8_t* in, uint32_t mk, int k, bool last, int total = 0)
 {
     RwSeq s;
+    if (PARTIAL && last) {
+        const int tok = (int)(mk & 0xFFFFu);
+        int st = (int)(mk >> 16);
+        if (k != 0 && st == 0) st = 65536;             /* 16-bit wrap: a final token without bytes at 65536 */
+        const uint32_t t = in[tok];
+        int pp = tok + 1;
+        int ll = (int)(t >> 4);
+        if (ll == 15) { uint32_t x; do { x = in[pp++]; ll += (int)x; } while (x == 255); }
+        s.ls = pp; s.op = st;
+        s.ll = ll < total - st ? ll : total - st;
+        s.m = st + s.ll;
+        s.off = 0; s.mlen = 0;
+        if (s.ll == ll && s.m < total) {
+            pp += ll;
+            s.off = (int)((uint32_t)in[pp] | ((uint32_t)in[pp + 1] << 8));
+            s.mlen = total - s.m;
+        }
+        return s;
+    }
     const int tok = (int)(mk & 0xFFFFu);
     int m = (int)(mk >> 16);
     if (k != 0 && m == 0) m = 65536;                   /* 16-bit wrap: only the last sequence of a 64 KB block ends at 65536 */

@@ -258,8 +258,18 @@ template <class M> SC_FN bool scan_front(M& mem, int nIn, int capIn, ScanState& 
 }
 
 /* ---- the exact byte-wise walk (lz4.c:2083-2435) from the state `st` to the end of the block ---- */
-/* The marks go to `ms`; the caller flushes it. */
-template <class M> SC_FN int scan_tail(M& mem, int nIn, int capIn, const ScanState& st, uint32_t* nSeqOut, MarkSink<M>& ms)
+/* The marks go to `ms`; the caller flushes it.
+ * PARTIAL: the partial_decode instantiation (LZ4_decompress_safe_partial, lz4.c:2459-2465) with capIn = outputSize.  Only
+ * the output-dependent tail differs: a literal run near either end is cut to the input end and then to capIn, and the
+ * decode stops when it reaches capIn or fewer than 2 input bytes remain (lz4.c:2285-2330); a match near the output end is
+ * cut to capIn and the decode stops there (lz4.c:2392-2404), so the "last 5 bytes are literals" rule never fires.  A cut
+ * run belongs to the last sequence, which ends exactly at the return value.  The last sequence's mark holds the START of
+ * its literals instead of its match start (rw_parse<true> rebuilds its runs from it and the return value).  That start is
+ * at most the return value <= 65 536 for a block with marks; only a final token that produces no byte can sit at 65 536
+ * (a 16-bit 0 then), and every earlier sequence made >= 4 bytes, so a 0 in the mark of a sequence k > 0 means 65 536.
+ * *usedOut receives the input bytes the walk consumed (the return value's sequences end there). */
+template <class M, bool PARTIAL = false>
+SC_FN int scan_tail(M& mem, int nIn, int capIn, const ScanState& st, uint32_t* nSeqOut, MarkSink<M>& ms, uint32_t* usedOut = nullptr)
 {
     int64_t nextPrefetch = st.nextPrefetch;
     int64_t n = nIn, cap = capIn, ip = st.ip, op = st.op, ll = 0, ml = 0, add = 0, tokPos = 0, mop = 0;
@@ -315,12 +325,23 @@ template <class M> SC_FN int scan_tail(M& mem, int nIn, int capIn, const ScanSta
         }
 safe_literals:
         if (op + ll > cap - kMfLimit || ip + ll > n - (2 + 1 + kLastLiterals)) {   // lz4.c:2279
-            if (ip + ll != n || op + ll > cap) goto bad;               // lz4.c:2312
-            op += ll;
-            ms.commit((uint32_t)tokPos, (uint32_t)op);   /* last sequence: the end of its literals */
-            nseq++;
-            *nSeqOut = nseq;
-            return (int)op;                                            // lz4.c:2439
+            if (!PARTIAL) {
+                if (ip + ll != n || op + ll > cap) goto bad;           // lz4.c:2312
+                op += ll;
+                ms.commit((uint32_t)tokPos, (uint32_t)op);   /* last sequence: the end of its literals */
+                nseq++;
+                *nSeqOut = nseq;
+                return (int)op;                                        // lz4.c:2439
+            }
+            if (ip + ll > n) ll = n - ip;                              // lz4.c:2295-2304
+            if (op + ll > cap) ll = cap - op;
+            if (op + ll == cap || ip + ll >= n - 2) {                  // lz4.c:2328
+                ms.commit((uint32_t)tokPos, (uint32_t)op);   /* last sequence: the start of its literals */
+                nseq++;
+                *nSeqOut = nseq;
+                *usedOut = (uint32_t)(ip + ll);
+                return (int)(op + ll);
+            }
         }
         ip += ll; op += ll; mop = op;
         offset = mem.u16(ip); ip += 2;
@@ -332,7 +353,15 @@ match_length:
         ml += kMinMatch;
 safe_match:
         if ((int64_t)offset > op) goto bad;                            // lz4.c:2356
-        if (op + ml > cap - kLastLiterals) goto bad;                   // lz4.c:2421-2423
+        if (PARTIAL) {
+            if (op + ml >= cap) {                                      // lz4.c:2392-2404: cut to cap, stop there
+                ms.commit((uint32_t)tokPos, (uint32_t)(mop - ll));   /* last sequence: the start of its literals */
+                nseq++;
+                *nSeqOut = nseq;
+                *usedOut = (uint32_t)ip;
+                return (int)cap;
+            }
+        } else if (op + ml > cap - kLastLiterals) goto bad;            // lz4.c:2421-2423
         ms.commit((uint32_t)tokPos, (uint32_t)mop);
         op += ml; nseq++;
     }
@@ -341,13 +370,20 @@ bad:
     return (int)(-ip) - 1;                                             // lz4.c:2443
 }
 
-template <class M> SC_DEV int scan_block(M& mem, int nIn, int capIn, uint32_t* nSeqOut, uint32_t* marks, uint32_t markCap)
+/* PARTIAL: LZ4_decompress_safe_partial with capIn = outputSize (see scan_tail); *usedOut = input bytes consumed by an
+ * accepted block */
+template <class M, bool PARTIAL = false>
+SC_DEV int scan_block(M& mem, int nIn, int capIn, uint32_t* nSeqOut, uint32_t* marks, uint32_t markCap, uint32_t* usedOut = nullptr)
 {
     ScanState st;
     st.ip = 0; st.op = 0; st.nextPrefetch = 128; st.nseq = 0;
 
     if (capIn < 0) return -1;                                          // lz4.c:2036
-    if (capIn == 0) { if (nIn != 1) return -1; return mem.b(0) == 0 ? 0 : -1; }   // lz4.c:2064-2068
+    if (capIn == 0) {                                                  // lz4.c:2064-2068
+        if (PARTIAL) return 0;
+        if (nIn != 1) return -1;
+        return mem.b(0) == 0 ? 0 : -1;
+    }
     if (nIn <= 0) return -1;                                           // lz4.c:2069
     st.fast = (capIn >= 64);                                           // lz4.c:2076
 
@@ -357,7 +393,7 @@ template <class M> SC_DEV int scan_block(M& mem, int nIn, int capIn, uint32_t* n
         *nSeqOut = 0;
         r = (int)(-st.ip) - 1;                                         // lz4.c:2443
     } else {
-        r = scan_tail(mem, nIn, capIn, st, nSeqOut, ms);
+        r = scan_tail<M, PARTIAL>(mem, nIn, capIn, st, nSeqOut, ms, usedOut);
     }
     ms.flush();
     return r;
