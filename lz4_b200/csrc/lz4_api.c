@@ -161,10 +161,30 @@ done:
 /* ------------------------------------------------------------------------------------------ */
 /* batch layer: device pointers                                                                */
 /* ------------------------------------------------------------------------------------------ */
-size_t LZ4B200_decompress_workspace_bytes(int64_t nBlocks) { return lz4k_decode_workspace_bytes(nBlocks); }
+size_t LZ4B200_decompress_workspace_bytes(int64_t nBlocks) { return lz4k_decode_workspace_bytes(nBlocks, 1, 0, SIZE_MAX); }
 size_t LZ4B200_decompress_workspace_bytes_for(int64_t nBlocks, int perBlockCaps, int32_t dstCap)
 {
-    return lz4k_decode_workspace_bytes_for(nBlocks, perBlockCaps, dstCap);
+    return lz4k_decode_workspace_bytes(nBlocks, perBlockCaps, dstCap, SIZE_MAX);
+}
+
+/* the device decode calls (partial: LZ4_decompress_safe_partial, d_dstCap / dstCap hold the targets) */
+static int decode_call(int partial, const void* d_src, const int64_t* d_srcOff, const int32_t* d_srcSize, void* d_dst,
+                       const int64_t* d_dstOff, int64_t dstStride, const int32_t* d_dstCap, int32_t dstCap, int32_t* d_outSize,
+                       int64_t nBlocks, void* d_workspace, size_t workspaceBytes, int phases, void* stream)
+{
+    lz4k_decode_args a;
+    cudaError_t e;
+    if (nBlocks < 0) return LZ4B200_ERR_ARG;
+    if (nBlocks == 0) return LZ4B200_OK;
+    if (!d_src || !d_srcOff || !d_srcSize || !d_dst || !d_outSize || !d_workspace) return LZ4B200_ERR_ARG;
+    if (workspaceBytes < lz4k_decode_workspace_bytes(nBlocks, d_dstCap != NULL, dstCap, 0)) return LZ4B200_ERR_ARG;
+    if (phases < 1 || phases > 3) return LZ4B200_ERR_ARG;
+    a.src = (const uint8_t*)d_src; a.srcOff = d_srcOff; a.srcSize = d_srcSize;
+    a.dst = (uint8_t*)d_dst; a.dstOff = d_dstOff; a.dstStride = dstStride;
+    a.dstCapArr = d_dstCap; a.dstCap = dstCap; a.outSize = d_outSize; a.nBlocks = nBlocks;
+    a.workspace = d_workspace; a.workspaceBytes = workspaceBytes;
+    e = (cudaError_t)lz4k_launch_decode(&a, phases, partial, stream);
+    return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_decode");
 }
 
 int LZ4B200_decompress_blocks_phased(const void* d_src, const int64_t* d_srcOff, const int32_t* d_srcSize,
@@ -173,19 +193,8 @@ int LZ4B200_decompress_blocks_phased(const void* d_src, const int64_t* d_srcOff,
                               int32_t* d_outSize, int64_t nBlocks,
                               void* d_workspace, size_t workspaceBytes, int phases, void* stream)
 {
-    lz4k_decode_args a;
-    cudaError_t e;
-    if (nBlocks < 0) return LZ4B200_ERR_ARG;
-    if (nBlocks == 0) return LZ4B200_OK;
-    if (!d_src || !d_srcOff || !d_srcSize || !d_dst || !d_outSize || !d_workspace) return LZ4B200_ERR_ARG;
-    if (workspaceBytes < lz4k_decode_workspace_bytes_min(nBlocks, d_dstCap != NULL, dstCap)) return LZ4B200_ERR_ARG;
-    a.src = (const uint8_t*)d_src; a.srcOff = d_srcOff; a.srcSize = d_srcSize;
-    a.dst = (uint8_t*)d_dst; a.dstOff = d_dstOff; a.dstStride = dstStride;
-    a.dstCapArr = d_dstCap; a.dstCap = dstCap; a.outSize = d_outSize; a.nBlocks = nBlocks;
-    a.workspace = d_workspace; a.workspaceBytes = workspaceBytes;
-    if (phases < 1 || phases > 3) return LZ4B200_ERR_ARG;
-    e = (cudaError_t)lz4k_launch_decode(&a, phases, stream);
-    return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_decode");
+    return decode_call(0, d_src, d_srcOff, d_srcSize, d_dst, d_dstOff, dstStride, d_dstCap, dstCap, d_outSize, nBlocks,
+                       d_workspace, workspaceBytes, phases, stream);
 }
 
 int LZ4B200_decompress_blocks(const void* d_src, const int64_t* d_srcOff, const int32_t* d_srcSize,
@@ -194,8 +203,8 @@ int LZ4B200_decompress_blocks(const void* d_src, const int64_t* d_srcOff, const 
                               int32_t* d_outSize, int64_t nBlocks,
                               void* d_workspace, size_t workspaceBytes, void* stream)
 {
-    return LZ4B200_decompress_blocks_phased(d_src, d_srcOff, d_srcSize, d_dst, d_dstOff, dstStride, d_dstCap, dstCap,
-                                            d_outSize, nBlocks, d_workspace, workspaceBytes, 3, stream);
+    return decode_call(0, d_src, d_srcOff, d_srcSize, d_dst, d_dstOff, dstStride, d_dstCap, dstCap, d_outSize, nBlocks,
+                       d_workspace, workspaceBytes, 3, stream);
 }
 
 int LZ4B200_decompress_blocks_partial(const void* d_src, const int64_t* d_srcOff, const int32_t* d_srcSize,
@@ -204,18 +213,8 @@ int LZ4B200_decompress_blocks_partial(const void* d_src, const int64_t* d_srcOff
                                       int32_t* d_outSize, int64_t nBlocks,
                                       void* d_workspace, size_t workspaceBytes, void* stream)
 {
-    lz4k_decode_args a;
-    cudaError_t e;
-    if (nBlocks < 0) return LZ4B200_ERR_ARG;
-    if (nBlocks == 0) return LZ4B200_OK;
-    if (!d_src || !d_srcOff || !d_srcSize || !d_dst || !d_outSize || !d_workspace) return LZ4B200_ERR_ARG;
-    if (workspaceBytes < lz4k_decode_workspace_bytes_min(nBlocks, d_target != NULL, targetOutputSize)) return LZ4B200_ERR_ARG;
-    a.src = (const uint8_t*)d_src; a.srcOff = d_srcOff; a.srcSize = d_srcSize;
-    a.dst = (uint8_t*)d_dst; a.dstOff = d_dstOff; a.dstStride = dstStride;
-    a.dstCapArr = d_target; a.dstCap = targetOutputSize; a.outSize = d_outSize; a.nBlocks = nBlocks;   /* capacity = target */
-    a.workspace = d_workspace; a.workspaceBytes = workspaceBytes;
-    e = (cudaError_t)lz4k_launch_decode_partial(&a, stream);
-    return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_decode_partial");
+    return decode_call(1, d_src, d_srcOff, d_srcSize, d_dst, d_dstOff, dstStride, d_target, targetOutputSize, d_outSize,
+                       nBlocks, d_workspace, workspaceBytes, 3, stream);
 }
 
 int LZ4B200_compress_blocks(const void* d_src, int64_t srcStride, const int32_t* d_srcSize, int32_t srcSize,
@@ -344,7 +343,7 @@ int LZ4B200_decompress_blocks_host(const void* h_src, const int64_t* h_srcOff, c
         }
         inBytes = (size_t)(hi - lo);
         metaBytes = (size_t)cnt * (sizeof(int64_t) + 2 * sizeof(int32_t));
-        wsBytes = lz4k_decode_workspace_bytes_for(cnt, 0, dstCap);
+        wsBytes = LZ4B200_decompress_workspace_bytes_for(cnt, 0, dstCap);
         CU(cudaStreamSynchronize(st));                      /* slot reuse: previous chunk on it is finished */
         flush_slot(slot);
         if ((rc = grow(&g_ctx.d_in[slot], &g_ctx.in_cap[slot], inBytes + 16)) != LZ4B200_OK) goto done;
@@ -549,7 +548,7 @@ static int one_block_decompress(const char* src, char* dst, int compressedSize, 
     if ((rc = grow(&g_ctx.d_in[0], &g_ctx.in_cap[0], (size_t)compressedSize + 16)) != LZ4B200_OK) goto done;
     if ((rc = grow(&g_ctx.d_out[0], &g_ctx.out_cap[0], (size_t)dstCapacity + 16)) != LZ4B200_OK) goto done;
     if ((rc = grow(&g_ctx.d_meta[0], &g_ctx.meta_cap[0], 64)) != LZ4B200_OK) goto done;
-    if ((rc = grow(&g_ctx.d_ws[0], &g_ctx.ws_cap[0], lz4k_decode_workspace_bytes_for(1, 0, dstCapacity))) != LZ4B200_OK) goto done;
+    if ((rc = grow(&g_ctx.d_ws[0], &g_ctx.ws_cap[0], LZ4B200_decompress_workspace_bytes_for(1, 0, dstCapacity))) != LZ4B200_OK) goto done;
     d_off = (int64_t*)g_ctx.d_meta[0];
     d_size = (int32_t*)(d_off + 1);
     d_ret = d_size + 1;

@@ -49,6 +49,7 @@ __device__ unsigned long long g_loopStats[4];    // phase B: warp iterations, la
 #include "lz4_scan_par.h"
 #include "lz4_scan_split.h"
 #include "lz4_rows_core.h"
+#include "lz4_decode_plan.h"     /* a decode call's workspace layout (WsView), scan choice and block predicates */
 
 /* low 5 bytes at p (for the 5-byte hash, lz4.c:785-791) */
 __device__ __forceinline__ uint64_t ld40u(const uint8_t* p)
@@ -124,90 +125,6 @@ __device__ __forceinline__ int tma_stage(uint8_t* dst, const uint8_t* src, int n
 }
 
 
-/* workspace layout (lz4k_decode_workspace_bytes): header | nSeq[N] | slowList[N] | marks[N][markStride] */
-struct WsHeader { uint32_t slowCount, pad[3]; };
-
-struct WsView {
-    WsHeader* hdr; uint32_t* nSeq; uint32_t* slowList; uint32_t* marks; uint32_t* scratch; uint32_t markStride;
-    uint32_t* tileFirst; uint32_t* tileFlag; uint32_t tilesMax;    /* batches of blocks above 64 KB (wide marks): see lz4_expand_tiles_kernel */
-};
-constexpr int kTile = 61440;                       /* output bytes per tile of a block above 64 KB: 15 waves of 4096 */
-constexpr int32_t kTileMaxCap = 64 << 20;          /* larger capacities take the generic kernel (the marks would need 2 x capacity) */
-__host__ __device__ inline bool wide_batch(const int32_t* dstCapArr, int32_t dstCap) { return !dstCapArr && dstCap > 65536 && dstCap <= kTileMaxCap; }
-__host__ __device__ inline uint32_t tiles_of(int32_t bytes) { return ((uint32_t)bytes + (uint32_t)kTile - 1u) / (uint32_t)kTile; }
-/* mark slots per block: a block the shared-memory expand kernel may take (capacity <= 64 KB) has at most
- * capacity/4 + 1 sequences (every sequence but the last produces >= 4 bytes) and the scan visits at most one more;
- * batches of larger blocks need no marks at all */
-__host__ __device__ inline uint32_t mark_stride(const int32_t* dstCapArr, int32_t dstCap, bool wide = false)
-{
-    if (dstCapArr) return (uint32_t)kMaxSeqFast;               /* per-block capacities live on the device: worst case */
-    if (wide) return 2u * ((uint32_t)dstCap / 4u + 2u);        /* wide marks: two words per sequence */
-    if (dstCap <= 0 || dstCap > 65536) return 0u;
-    const uint32_t s = (uint32_t)dstCap / 4u + 2u;
-    return s < (uint32_t)kMaxSeqFast ? s : (uint32_t)kMaxSeqFast;
-}
-__host__ __device__ inline WsView ws_view(void* ws, int64_t n, uint32_t markStride, uint32_t tilesMax = 0)
-{
-    WsView v;
-    uint8_t* p = reinterpret_cast<uint8_t*>(ws);
-    v.hdr = reinterpret_cast<WsHeader*>(p); p += 256;
-    v.nSeq = reinterpret_cast<uint32_t*>(p); p += ((n * 4 + 255) / 256) * 256;
-    v.slowList = reinterpret_cast<uint32_t*>(p); p += ((n * 4 + 255) / 256) * 256;
-    v.marks = reinterpret_cast<uint32_t*>(p); p += (((size_t)n * markStride * 4 + 255) / 256) * 256;
-    v.scratch = reinterpret_cast<uint32_t*>(p);                /* split scan: 2 x markStride words per block */
-    v.markStride = markStride;
-    /* wide batches have no scratch lists: per block tilesMax + 1 first-sequence indices, tilesMax done flags + 1 "gave up" word */
-    v.tileFirst = reinterpret_cast<uint32_t*>(p); p += (((size_t)n * (tilesMax + 1) * 4 + 255) / 256) * 256;
-    v.tileFlag = reinterpret_cast<uint32_t*>(p);
-    v.tilesMax = tilesMax;
-    return v;
-}
-__host__ __device__ inline size_t ws_bytes(int64_t nBlocks, uint32_t markStride, uint32_t tilesMax = 0)
-{
-    const size_t lst = (((size_t)nBlocks * 4 + 255) / 256) * 256;
-    const size_t mk = (((size_t)nBlocks * markStride * sizeof(uint32_t) + 255) / 256) * 256;
-    if (tilesMax) {                                            /* header | nSeq | slowList | wide marks | tileFirst | tileFlag */
-        const size_t tl = (((size_t)nBlocks * (tilesMax + 1) * 4 + 255) / 256) * 256;
-        return 256 + 2 * lst + mk + 2 * tl + 256;
-    }
-    return 256 + 2 * lst + 3 * mk + 256;                      /* header | nSeq | slowList | marks | scratch (2 x marks) */
-}
-/* A batch of blocks above 64 KB is decoded in tiles when the caller's workspace has room for the wide marks
- * (LZ4B200_decompress_workspace_bytes_for says how much); with the small workspace it takes the generic kernel. */
-__host__ __device__ inline bool use_wide(const int32_t* dstCapArr, int32_t dstCap, int64_t nBlocks, size_t workspaceBytes)
-{
-    return wide_batch(dstCapArr, dstCap) && workspaceBytes >= ws_bytes(nBlocks, mark_stride(dstCapArr, dstCap, true), tiles_of(dstCap));
-}
-__device__ __forceinline__ WsView ws_view(const lz4k_decode_args& a)
-{
-    const bool wide = use_wide(a.dstCapArr, a.dstCap, a.nBlocks, a.workspaceBytes);
-    return ws_view(a.workspace, a.nBlocks, mark_stride(a.dstCapArr, a.dstCap, wide), wide ? tiles_of(a.dstCap) : 0u);
-}
-/* The partial call (lz4k_launch_decode_partial; dstCapArr / dstCap hold the targets) never decodes in tiles, so its layout is
- * the narrow one whatever the workspace: the smallest that LZ4B200_decompress_workspace_bytes_for sizes for the same
- * arguments.  It never runs the split scan either, and its scratch region holds one word per block instead: the input
- * bytes the scan consumed (partial_used), present whenever the batch has marks (markStride > 0: 2 x markStride words
- * per block) -- a batch without marks sends every block to the generic kernel, which does not need it. */
-__device__ __forceinline__ WsView partial_view(const lz4k_decode_args& a)
-{
-    return ws_view(a.workspace, a.nBlocks, mark_stride(a.dstCapArr, a.dstCap), 0u);
-}
-__device__ __forceinline__ uint32_t* partial_used(const WsView& w) { return w.markStride ? w.scratch : nullptr; }
-
-/* a block the shared-memory expand kernel takes: input and output fit its 64 KB windows, marks for every sequence */
-__device__ __forceinline__ bool rows_eligible(int n, int cap, uint32_t nseq, uint32_t markStride)
-{
-    return n > 0 && n <= 65535 && cap > 0 && cap <= 65536 && nseq <= (uint32_t)kMaxSeqFast && nseq <= markStride;
-}
-
-/* where a scan kernel leaves block b's marks: blocks the rows kernel may take have them, and so does every block of a
- * wide batch (two words per sequence, for the tiles kernel); nullptr: no marks */
-__device__ __forceinline__ uint32_t* scan_marks(const WsView& w, int64_t b, int n, int cap, bool wide = false)
-{
-    const bool want = wide ? n > 0 : (n > 0 && n <= 65535 && cap > 0 && cap <= 65536 && w.markStride > 0);
-    return want ? w.marks + (size_t)b * w.markStride : nullptr;
-}
-
 /* a scan kernel's result for block b: the decoder's return value and the sequence count; an accepted block that neither
  * the rows kernel nor (`tiled`) the tiles kernel takes goes on the generic kernel's list */
 __device__ __forceinline__ void scan_result(const lz4k_decode_args& a, const WsView& w, int64_t b, int n, int cap, int r,
@@ -220,17 +137,16 @@ __device__ __forceinline__ void scan_result(const lz4k_decode_args& a, const WsV
 
 /* ---- scan, one THREAD per block: reads through the read-only data cache with L1 prefetch hints, marks in 32-byte chunks ---- */
 
-__global__ void __launch_bounds__(128) lz4_scan_kernel(lz4k_decode_args a)
+__global__ void __launch_bounds__(128) lz4_scan_kernel(lz4k_decode_args a, WsView w)
 {
     int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= a.nBlocks) return;
-    const WsView w = ws_view(a);
     const uint8_t* src = a.src + a.srcOff[b];
     const int n = a.srcSize[b];
     int cap = a.dstCapArr ? a.dstCapArr[b] : a.dstCap;
     uint32_t ns = 0;
     MemPtr<true> mem{src};
-    const int r = scan_block(mem, n, cap, &ns, scan_marks(w, b, n, cap), w.markStride);
+    const int r = scan_block(mem, n, cap, &ns, block_marks(w, b, n, cap, kMarksNarrow), w.markStride);
     scan_result(a, w, b, n, cap, r, ns);
 }
 
@@ -238,22 +154,18 @@ __global__ void __launch_bounds__(128) lz4_scan_kernel(lz4k_decode_args a)
  * The walk ends at the target, so its chain of dependent steps grows with the decoded prefix, not the block.  Marks are
  * written for every target of at most 64 KB, whatever the input size: the rows kernel stages only the consumed prefix.
  * Route P1 (lz4_expand_rows_partial_kernel): rows_eligible on (consumed, target); P2 (the generic kernel): the rest. */
-__global__ void __launch_bounds__(128) lz4_scan_partial_kernel(lz4k_decode_args a)
+__global__ void __launch_bounds__(128) lz4_scan_partial_kernel(lz4k_decode_args a, WsView w)
 {
     int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= a.nBlocks) return;
-    const WsView w = partial_view(a);
     const uint8_t* src = a.src + a.srcOff[b];
     const int n = a.srcSize[b];
     const int cap = a.dstCapArr ? a.dstCapArr[b] : a.dstCap;
     uint32_t ns = 0, used = 0;
-    uint32_t* marks = (n > 0 && cap > 0 && cap <= 65536 && w.markStride > 0) ? w.marks + (size_t)b * w.markStride : nullptr;
     MemPtr<true> mem{src};
-    const int r = scan_block<MemPtr<true>, true>(mem, n, cap, &ns, marks, w.markStride, &used);
-    a.outSize[b] = r;
-    w.nSeq[b] = ns;
-    if (uint32_t* u = partial_used(w)) u[b] = used;
-    if (r > 0 && !rows_eligible((int)used, cap, ns, w.markStride)) w.slowList[atomicAdd(&w.hdr->slowCount, 1u)] = (uint32_t)b;
+    const int r = scan_block<MemPtr<true>, true>(mem, n, cap, &ns, block_marks(w, b, n, cap, kMarksPartial), w.markStride, &used);
+    if (w.used) w.used[b] = used;
+    scan_result(a, w, b, (int)used, cap, r, ns);
 }
 
 /* ---- scan, kSsLanes lanes per block that merge (lz4_scan_split.h): the chain of dependent steps is kSsLanes times shorter ----
@@ -261,20 +173,18 @@ __global__ void __launch_bounds__(128) lz4_scan_partial_kernel(lz4k_decode_args 
  * Lists go to the scratch part of the workspace (2 x markStride words per block), the per-block records to shared memory. */
 constexpr int kSplitThreads = 128;
 constexpr int kSplitBlocksPerCta = kSplitThreads / kSsLanes;
-constexpr int64_t kSplitMaxBlocks = 8192;         /* largest batch the split scan is the default for (H100, see below) */
 
-__global__ void __launch_bounds__(kSplitThreads, 10) lz4_scan_split_kernel(lz4k_decode_args a)
+__global__ void __launch_bounds__(kSplitThreads, 10) lz4_scan_split_kernel(lz4k_decode_args a, WsView w)
 {
     __shared__ SsBlock sh[kSplitBlocksPerCta];
     const int lane = threadIdx.x % kSsLanes, slot = threadIdx.x / kSsLanes;
     const int64_t b = (int64_t)blockIdx.x * kSplitBlocksPerCta + slot;
     if (b >= a.nBlocks) return;                                 /* (whole groups of kSsLanes lanes leave together) */
     const unsigned grp = ((1u << kSsLanes) - 1u) << ((threadIdx.x & 31) / kSsLanes * kSsLanes);   /* this block's lanes in the warp */
-    const WsView w = ws_view(a);
     const uint8_t* src = a.src + a.srcOff[b];
     const int n = a.srcSize[b];
     const int cap = a.dstCapArr ? a.dstCapArr[b] : a.dstCap;
-    uint32_t* marks = scan_marks(w, b, n, cap);
+    uint32_t* marks = block_marks(w, b, n, cap, kMarksNarrow);
     SsBlock& S = sh[slot];
     MemPtr<true> mem{src};
     int r = 0;
@@ -370,11 +280,10 @@ __device__ __forceinline__ void scan_par_block(ScanParSmem& S, M& mem, int n, in
     __syncthreads();
 }
 
-__global__ void __launch_bounds__(kScanLanes) lz4_scan_par_kernel(lz4k_decode_args a)
+__global__ void __launch_bounds__(kScanLanes) lz4_scan_par_kernel(lz4k_decode_args a, WsView w)
 {
     extern __shared__ __align__(16) uint8_t smemRaw[];
     ScanParSmem& S = *reinterpret_cast<ScanParSmem*>(smemRaw);
-    const WsView w = ws_view(a);
     const int tid = threadIdx.x;
     uint32_t parity = 0;
     if (tid == 0) mbar_init(&S.mbar, 1);
@@ -383,21 +292,19 @@ __global__ void __launch_bounds__(kScanLanes) lz4_scan_par_kernel(lz4k_decode_ar
         const uint8_t* src = a.src + a.srcOff[b];
         const int n = a.srcSize[b];
         const int cap = a.dstCapArr ? a.dstCapArr[b] : a.dstCap;
-        const bool wide = w.tilesMax != 0;                            /* a batch of blocks above 64 KB: two-word marks for the tiles kernel */
-        uint32_t* marks = scan_marks(w, b, n, cap, wide);
-        const uint32_t markCap = wide ? w.markStride / 2u : w.markStride;
+        uint32_t* marks = block_marks(w, b, n, cap, w.wide ? kMarksWide : kMarksNarrow);
         int r = -1;
         uint32_t ns = 0;
         /* the lanes' walk over `mem`; in a wide batch the marks are two words per sequence (MemPtr<G, true>) */
-        auto lanes = [&](auto mem) { scan_par_block(S, mem, n, cap, marks, markCap, r, ns); };
+        auto lanes = [&](auto mem) { scan_par_block(S, mem, n, cap, marks, mark_cap(w), r, ns); };
         if (n > 0 && n <= 65535 && cap > 0) {                     /* staged in shared memory */
             const int head = tma_stage(S.in, src, n, &S.mbar, tid == 0);
             while (!mbar_try_wait(&S.mbar, parity)) { }
             parity ^= 1;
-            if (wide) lanes(MemPtr<false, true>{S.in + head});
+            if (w.wide) lanes(MemPtr<false, true>{S.in + head});
             else lanes(MemPtr<false>{S.in + head});
         } else if (n > 65535 && cap >= 64) {                      /* walked in global memory */
-            if (wide) lanes(MemPtr<true, true>{src});
+            if (w.wide) lanes(MemPtr<true, true>{src});
             else lanes(MemPtr<true>{src});
         } else {                                                   /* degenerate arguments: the one-thread code decides (lz4.c:2036, :2064-2069) */
             if (tid == 0) { uint32_t q = 0; MemPtr<true> mem{src}; S.sp.ret = scan_block(mem, n, cap, &q, nullptr, 0u); S.sp.nseq = q; }
@@ -405,23 +312,22 @@ __global__ void __launch_bounds__(kScanLanes) lz4_scan_par_kernel(lz4k_decode_ar
             r = S.sp.ret; ns = S.sp.nseq;
             __syncthreads();
         }
-        if (tid == 0) scan_result(a, w, b, n, cap, r, ns, wide && ns <= markCap);   /* tiled: lz4_expand_tiles_kernel takes it */
+        if (tid == 0) scan_result(a, w, b, n, cap, r, ns, w.wide && tiles_eligible(w, ns));
     }
 }
 
 /* ---- wide batches: per tile of kTile output bytes the first sequence whose match starts in or beyond it ----
  * tileFirst[b][t] = min { k : matchStart(k) >= t * kTile } for t = 0 .. tiles(b) (nseq if none); done flags cleared.
  * The match starts are non-decreasing in k and the last mark holds the decoded size, so sequence k's neighbours decide. */
-__global__ void __launch_bounds__(256) lz4_tile_index_kernel(lz4k_decode_args a)
+__global__ void __launch_bounds__(256) lz4_tile_index_kernel(lz4k_decode_args a, WsView w)
 {
-    const WsView w = ws_view(a);
     for (int64_t b = blockIdx.x; b < a.nBlocks; b += gridDim.x) {
         uint32_t* first = w.tileFirst + (size_t)b * (w.tilesMax + 1);
         uint32_t* flag = w.tileFlag + (size_t)b * (w.tilesMax + 1);
         for (uint32_t t = threadIdx.x; t <= w.tilesMax; t += blockDim.x) flag[t] = 0u;
         const int total = a.outSize[b];
         const uint32_t ns = w.nSeq[b];
-        if (total <= 0 || ns == 0 || ns > w.markStride / 2u) continue;
+        if (total <= 0 || ns == 0 || !tiles_eligible(w, ns)) continue;
         const uint32_t nT = tiles_of(total);
         const uint32_t* marks = w.marks + (size_t)b * w.markStride;
         for (uint32_t k = threadIdx.x; k < ns; k += blockDim.x) {
@@ -441,12 +347,11 @@ __global__ void __launch_bounds__(256) lz4_tile_index_kernel(lz4k_decode_args a)
 /* PARTIAL: the partial call's blocks (route P2): the decode stops at the scan's return value, and the literal and match
  * runs that reach it are cut there (the scan's walk ended at the same place, lz4_scan_core.h: scan_tail) */
 template <bool PARTIAL>
-__device__ __forceinline__ void expand_generic(const lz4k_decode_args& a)
+__device__ __forceinline__ void expand_generic(const lz4k_decode_args& a, const WsView& w)
 {
     const int lane = threadIdx.x & 31;
     const int64_t warp0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nWarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    const WsView w = PARTIAL ? partial_view(a) : ws_view(a);
     const int64_t count = w.hdr->slowCount;       // only blocks the scan accepted and left to this kernel
     for (int64_t idx = warp0; idx < count; idx += nWarps) {
     const int64_t b = w.slowList[idx];
@@ -486,8 +391,8 @@ __device__ __forceinline__ void expand_generic(const lz4k_decode_args& a)
     }
 }
 
-__global__ void __launch_bounds__(128) lz4_expand_generic_kernel(lz4k_decode_args a) { expand_generic<false>(a); }
-__global__ void __launch_bounds__(128) lz4_expand_generic_partial_kernel(lz4k_decode_args a) { expand_generic<true>(a); }
+__global__ void __launch_bounds__(128) lz4_expand_generic_kernel(lz4k_decode_args a, WsView w) { expand_generic<false>(a, w); }
+__global__ void __launch_bounds__(128) lz4_expand_generic_partial_kernel(lz4k_decode_args a, WsView w) { expand_generic<true>(a, w); }
 
 /* =============================================================================================
  * expand (rows): one CTA per 64 KB block, one output BYTE per thread, waves + run table
@@ -706,12 +611,11 @@ __device__ __forceinline__ void rows_store(uint8_t* dst, const uint8_t* out, con
  * (rw_parse<true>), so no run starts at or past the return value; only the consumed input prefix is staged, and
  * eligibility is decided on (consumed, target) instead of (input size, capacity). */
 template <bool PARTIAL>
-__device__ __forceinline__ void expand_rows(const lz4k_decode_args& a)
+__device__ __forceinline__ void expand_rows(const lz4k_decode_args& a, const WsView& w)
 {
     extern __shared__ __align__(16) uint8_t smemRaw[];
     RowsSmem& S = *reinterpret_cast<RowsSmem*>(smemRaw);
     const int tid = threadIdx.x;
-    const WsView w = PARTIAL ? partial_view(a) : ws_view(a);
     const uint32_t le = lanemask_le();
     const uint32_t outA = (uint32_t)offsetof(RowsSmem, out);
     const int zeroDelta0 = (int)offsetof(RowsSmem, zero) - (int)outA;
@@ -728,7 +632,7 @@ __device__ __forceinline__ void expand_rows(const lz4k_decode_args& a)
         Raw r;
         r.b = b; r.off = 0; r.dOff = 0; r.n = 0; r.total = 0; r.cap = 0; r.ns = 0;
         if (b < a.nBlocks) {
-            r.n = PARTIAL ? (partial_used(w) ? (int)partial_used(w)[b] : 0) : a.srcSize[b]; r.total = a.outSize[b]; r.ns = w.nSeq[b]; r.off = a.srcOff[b];
+            r.n = PARTIAL ? (w.used ? (int)w.used[b] : 0) : a.srcSize[b]; r.total = a.outSize[b]; r.ns = w.nSeq[b]; r.off = a.srcOff[b];
             r.cap = a.dstCapArr ? a.dstCapArr[b] : a.dstCap;
             r.dOff = a.dstOff ? a.dstOff[b] : b * a.dstStride;
         }
@@ -861,8 +765,8 @@ __device__ __forceinline__ void expand_rows(const lz4k_decode_args& a)
     if (tid == 0) tma_wait_all0();
 }
 
-__global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_rows_kernel(lz4k_decode_args a) { expand_rows<false>(a); }
-__global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_rows_partial_kernel(lz4k_decode_args a) { expand_rows<true>(a); }
+__global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_rows_kernel(lz4k_decode_args a, WsView w) { expand_rows<false>(a, w); }
+__global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_rows_partial_kernel(lz4k_decode_args a, WsView w) { expand_rows<true>(a, w); }
 
 /* =============================================================================================
  * expand (tiles): blocks ABOVE 64 KB (lz4frame's 256 KB .. 4 MB blocks), one CTA per 60 KB OUTPUT TILE
@@ -895,12 +799,11 @@ __device__ __forceinline__ void st_release_gpu(uint32_t* p, uint32_t v)
     asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
-__global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_tiles_kernel(lz4k_decode_args a)
+__global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_tiles_kernel(lz4k_decode_args a, WsView w)
 {
     extern __shared__ __align__(16) uint8_t smemRaw[];
     RowsSmem& S = *reinterpret_cast<RowsSmem*>(smemRaw);
     const int tid = threadIdx.x;
-    const WsView w = ws_view(a);
     const uint32_t le = lanemask_le();
     const uint32_t sBase = smem_u32(smemRaw);
     const uint32_t outS = sBase + (uint32_t)offsetof(RowsSmem, out);
@@ -922,7 +825,7 @@ __global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_tiles_kernel(lz4k_
         const int total = a.outSize[b];
         const uint32_t nseq = w.nSeq[b];
         uint32_t* flags = w.tileFlag + (size_t)b * (tilesMax + 1);
-        if (!(total > 0 && nseq > 0 && nseq <= w.markStride / 2u && t < tiles_of(total))) {     /* (the same for every thread) */
+        if (!(total > 0 && nseq > 0 && tiles_eligible(w, nseq) && t < tiles_of(total))) {     /* (the same for every thread) */
             if (tid == 0 && pendFlag) publishPending();
             continue;
         }
@@ -1473,131 +1376,90 @@ int lz4k_debug_phase_cycles(unsigned long long* out8)   /* out8: 12 values (8 ph
     return (int)e;
 }
 
-static size_t ws_bytes_for(int64_t nBlocks, const int32_t* dstCapArr, int32_t dstCap)
+size_t lz4k_decode_workspace_bytes(int64_t nBlocks, int perBlockCaps, int32_t dstCap, size_t workspaceBytes)
 {
-    const bool wide = wide_batch(dstCapArr, dstCap);           /* the size that enables the tiles kernel */
-    return ws_bytes(nBlocks, mark_stride(dstCapArr, dstCap, wide), wide ? tiles_of(dstCap) : 0u);
+    return nBlocks < 0 ? 0 : plan_decode(nBlocks, perBlockCaps != 0, dstCap, workspaceBytes, kDecodeFull).bytes;
 }
 
-size_t lz4k_decode_workspace_bytes(int64_t nBlocks)               /* any capacities (worst case: 32 KB of marks per block) */
+/* once per process (every device of a process runs the same kernels): the decode kernels' opt-in to the large dynamic
+ * shared memory, the SMs the persistent kernels use, and the developer A/B switch of the scan */
+static int g_decodeSms = 0, g_scanImpl = -1;
+static cudaError_t decode_setup()
 {
-    return nBlocks < 0 ? 0 : ws_bytes(nBlocks, (uint32_t)kMaxSeqFast);
+    if (g_decodeSms) return cudaSuccess;
+    const int rowsSmem = (int)sizeof(RowsSmem);
+    cudaError_t e = cudaFuncSetAttribute(lz4_expand_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, rowsSmem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(lz4_expand_rows_partial_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, rowsSmem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(lz4_expand_tiles_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, rowsSmem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(lz4_scan_par_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ScanParSmem));
+    if (e != cudaSuccess) return e;
+    const char* env = getenv("LZ4K_SCAN_IMPL");                       /* "thread" | "par" | "split" */
+    g_scanImpl = env ? (env[0] == 'p' ? kScanPar : env[0] == 's' ? kScanSplit : kScanThread) : -1;
+    /* LZ4B200_RESERVE_SMS = k: the persistent expand kernels leave k SMs alone, for a communication kernel that runs
+     * concurrently (N > 1: NCCL's send/recv of the previous chunk; bench.py --reserve-sms) */
+    const int v = device_sms();
+    const char* rs = getenv("LZ4B200_RESERVE_SMS");
+    const int reserve = rs ? atoi(rs) : 0;
+    g_decodeSms = (reserve > 0 && reserve < v) ? v - reserve : v;
+    return cudaSuccess;
 }
 
-size_t lz4k_decode_workspace_bytes_for(int64_t nBlocks, int perBlockCaps, int32_t dstCap)
-{
-    static const int32_t one = 1;                                 /* any non-NULL pointer: "capacities are per block" */
-    return nBlocks < 0 ? 0 : ws_bytes_for(nBlocks, perBlockCaps ? &one : nullptr, dstCap);
-}
-
-size_t lz4k_decode_workspace_bytes_min(int64_t nBlocks, int perBlockCaps, int32_t dstCap)   /* smallest workspace a launch accepts */
-{
-    static const int32_t one = 1;
-    return nBlocks < 0 ? 0 : ws_bytes(nBlocks, mark_stride(perBlockCaps ? &one : nullptr, dstCap));
-}
-
-int lz4k_launch_decode(const lz4k_decode_args* a, int phases, void* stream)
+/* The full call: thread, split or parallel scan (plan_decode), then the rows or (wide batch) the tiles kernel, then the
+ * generic kernel.  The partial call: one-thread partial scan, then route P1 (rows kernel, targets <= 64 KB whose consumed
+ * prefix, sequences and runs fit it) and P2 (generic kernel, everything else); targets above 64 KB take the generic
+ * kernel (correct, not tuned). */
+int lz4k_launch_decode(const lz4k_decode_args* a, int phases, int partial, void* stream)
 {
     cudaStream_t s = (cudaStream_t)stream;
     if (a->nBlocks == 0) return 0;
-    if (a->workspaceBytes < ws_bytes(a->nBlocks, mark_stride(a->dstCapArr, a->dstCap))) return (int)cudaErrorInvalidValue;
-    const bool wide = use_wide(a->dstCapArr, a->dstCap, a->nBlocks, a->workspaceBytes);
-    static int sms = 0, scanImpl = -1;
-    if (sms == 0) {
-        const int v = device_sms();
-        /* opt in to the large dynamic shared memory (once; every device of a process runs the same kernels) */
-        cudaError_t e = cudaFuncSetAttribute(lz4_expand_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RowsSmem));
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(lz4_scan_par_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(ScanParSmem));
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(lz4_expand_tiles_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RowsSmem));
-        if (e != cudaSuccess) return (int)e;
-        const char* env = getenv("LZ4K_SCAN_IMPL");               /* developer A/B switch: "thread" | "par" | "split" */
-        scanImpl = env ? (env[0] == 'p' ? 1 : env[0] == 's' ? 2 : 0) : -1;
-        /* LZ4B200_RESERVE_SMS = k: the persistent expand kernels leave k SMs alone, for a communication kernel that runs
-         * concurrently (N > 1: NCCL's send/recv of the previous chunk; bench.py --reserve-sms) */
-        const char* rs = getenv("LZ4B200_RESERVE_SMS");
-        const int reserve = rs ? atoi(rs) : 0;
-        sms = (reserve > 0 && reserve < v) ? v - reserve : v;
-    }
+    cudaError_t e = decode_setup();
+    if (e != cudaSuccess) return (int)e;
+    DecodePlan p = plan_decode(a->nBlocks, a->dstCapArr != nullptr, a->dstCap, a->workspaceBytes, partial ? kDecodePartial : kDecodeFull);
+    /* the switch does not apply to a wide batch (only the parallel scan writes the wide marks) nor to the partial call */
+    if (!partial && g_scanImpl >= 0 && !p.wide) p.scan = (DecodeScan)g_scanImpl;
+    const WsView w = ws_view(p, a->workspace);
+    const int64_t sms = g_decodeSms;
     if (phases & 1) {
-        cudaError_t e = cudaMemsetAsync(a->workspace, 0, 256, s);     // WsHeader: list counter
+        e = cudaMemsetAsync(a->workspace, 0, 256, s);                   // WsHeader: list counter
         if (e != cudaSuccess) return (int)e;
-        /* the lanes of the parallel scan re-walk their segments several times (fix-up rounds), many times the instructions of
-         * the one-thread scan, so it only pays for blocks far beyond 64 KB (lz4frame's 4 MB blocks: 150 000 dependent steps for
-         * one thread) */
-        /* the switch does not apply to a wide batch: only the parallel scan writes the wide marks the tiles kernel reads */
-        const bool par = wide || (scanImpl >= 0 ? scanImpl == 1 : (a->dstCapArr == nullptr && a->dstCap > 65536));
-        /* blocks of 16..64 KB: kSsLanes merging lanes per block (smaller blocks have too few sequences to split).  Measured
-         * on an H100 SXM at a 700 W power limit (scan kernel alone, CUDA events, 64 KB P50 blocks, split against one thread
-         * per block, marks in 32-byte chunks): faster while the batch is small (1.20 against 2.13 ms for 4096 blocks, 1.72
-         * against 2.12 ms for 8192), slower beyond (2.51 against 2.10 ms for 12288, 3.47 against 2.14 ms for 16384, 30.6
-         * against 2.6 ms for 65536: the one-thread scan's time grows little with the batch, the split scan's does) */
-        const bool split = scanImpl >= 0 ? scanImpl == 2
-                                         : (a->dstCapArr == nullptr && a->dstCap >= 16384 && a->dstCap <= 65536 && a->nBlocks <= kSplitMaxBlocks);
-        if (split && !par) {
+        if (p.scan == kScanSplit) {
             const int64_t grid = (a->nBlocks + kSplitBlocksPerCta - 1) / kSplitBlocksPerCta;
-            lz4_scan_split_kernel<<<(unsigned)grid, kSplitThreads, 0, s>>>(*a);
-        } else if (par) {
-            const int64_t want = (int64_t)sms * 12;                   // 3 resident CTAs per SM, 4 rounds for balance
+            lz4_scan_split_kernel<<<(unsigned)grid, kSplitThreads, 0, s>>>(*a, w);
+        } else if (p.scan == kScanPar) {
+            const int64_t want = sms * 12;                              // 3 resident CTAs per SM, 4 rounds for balance
             const int64_t grid = a->nBlocks < want ? a->nBlocks : want;
-            lz4_scan_par_kernel<<<(unsigned)grid, kScanLanes, sizeof(ScanParSmem), s>>>(*a);
-            if (wide) {                                                // tiles kernel: first sequence of every tile, flags cleared
-                lz4_tile_index_kernel<<<(unsigned)(a->nBlocks < (int64_t)sms * 8 ? a->nBlocks : (int64_t)sms * 8), 256, 0, s>>>(*a);
+            lz4_scan_par_kernel<<<(unsigned)grid, kScanLanes, sizeof(ScanParSmem), s>>>(*a, w);
+            if (p.wide) {                                               // tiles kernel: first sequence of every tile, flags cleared
+                lz4_tile_index_kernel<<<(unsigned)(a->nBlocks < sms * 8 ? a->nBlocks : sms * 8), 256, 0, s>>>(*a, w);
                 g_launches++;
             }
         } else {
-            const int threads = 128;
-            const int64_t grid = (a->nBlocks + threads - 1) / threads;
-            lz4_scan_kernel<<<(unsigned)grid, threads, 0, s>>>(*a);
+            const unsigned grid = (unsigned)((a->nBlocks + 127) / 128);
+            if (partial) lz4_scan_partial_kernel<<<grid, 128, 0, s>>>(*a, w);
+            else lz4_scan_kernel<<<grid, 128, 0, s>>>(*a, w);
         }
         g_launches++;
     }
     if (phases & 2) {
-        if (wide) {                                                  // blocks above 64 KB: one CTA per 60 KB output tile
-            const int64_t units = a->nBlocks * (int64_t)tiles_of(a->dstCap);
-            const int64_t grid = units < sms ? units : sms;          // all CTAs resident: a tile may wait for its predecessor
-            {   /* the tiles' done flags start at 0 for THIS expand (the index kernel clears them too; an expand repeated after one scan must not see the last one's) */
-                const WsView wv = ws_view(a->workspace, a->nBlocks, mark_stride(a->dstCapArr, a->dstCap, true), tiles_of(a->dstCap));
-                cudaError_t e = cudaMemsetAsync(wv.tileFlag, 0, (size_t)a->nBlocks * (wv.tilesMax + 1) * sizeof(uint32_t), s);
-                if (e != cudaSuccess) return (int)e;
-            }
-            lz4_expand_tiles_kernel<<<(unsigned)grid, kRowsThreads, sizeof(RowsSmem), s>>>(*a);
+        if (p.wide) {                                                   // blocks above 64 KB: one CTA per 60 KB output tile
+            const int64_t units = a->nBlocks * (int64_t)p.tilesMax;
+            const int64_t grid = units < sms ? units : sms;             // all CTAs resident: a tile may wait for its predecessor
+            /* the tiles' done flags start at 0 for THIS expand (the index kernel clears them too; an expand repeated after one
+             * scan must not see the last one's) */
+            e = cudaMemsetAsync(w.tileFlag, 0, (size_t)a->nBlocks * (p.tilesMax + 1) * sizeof(uint32_t), s);
+            if (e != cudaSuccess) return (int)e;
+            lz4_expand_tiles_kernel<<<(unsigned)grid, kRowsThreads, sizeof(RowsSmem), s>>>(*a, w);
         } else {
-            int64_t grid = a->nBlocks < sms ? a->nBlocks : sms;      // persistent: one CTA per SM
-            lz4_expand_rows_kernel<<<(unsigned)grid, kRowsThreads, sizeof(RowsSmem), s>>>(*a);
+            const unsigned grid = (unsigned)(a->nBlocks < sms ? a->nBlocks : sms);   // persistent: one CTA per SM
+            if (partial) lz4_expand_rows_partial_kernel<<<grid, kRowsThreads, sizeof(RowsSmem), s>>>(*a, w);
+            else lz4_expand_rows_kernel<<<grid, kRowsThreads, sizeof(RowsSmem), s>>>(*a, w);
         }
-        g_launches++;
-        const int threads = 128;                                     // 4 warps = 4 blocks per CTA, grid-stride over the slow list
-        int64_t grid2 = (a->nBlocks * 32 + threads - 1) / threads;
-        if (grid2 > (int64_t)sms * 16) grid2 = (int64_t)sms * 16;
-        lz4_expand_generic_kernel<<<(unsigned)grid2, threads, 0, s>>>(*a);
-        g_launches++;
+        int64_t grid2 = (a->nBlocks * 32 + 127) / 128;                 // 4 warps = 4 blocks per CTA, grid-stride over the slow list
+        if (grid2 > sms * 16) grid2 = sms * 16;
+        if (partial) lz4_expand_generic_partial_kernel<<<(unsigned)grid2, 128, 0, s>>>(*a, w);
+        else lz4_expand_generic_kernel<<<(unsigned)grid2, 128, 0, s>>>(*a, w);
+        g_launches += 2;
     }
-    return (int)cudaGetLastError();
-}
-
-/* LZ4_decompress_safe_partial per block, outputSize = dstCapArr[b] / dstCap: one-thread partial scan, then route P1 (rows
- * kernel, targets <= 64 KB whose consumed prefix, sequences and runs fit it) and P2 (generic kernel, everything else).  Three
- * launches; the tiles kernel is not used, so targets above 64 KB take the generic kernel (correct, not tuned). */
-int lz4k_launch_decode_partial(const lz4k_decode_args* a, void* stream)
-{
-    cudaStream_t s = (cudaStream_t)stream;
-    if (a->nBlocks == 0) return 0;
-    if (a->workspaceBytes < ws_bytes(a->nBlocks, mark_stride(a->dstCapArr, a->dstCap))) return (int)cudaErrorInvalidValue;
-    static int sms = 0;
-    if (sms == 0) {
-        cudaError_t e = cudaFuncSetAttribute(lz4_expand_rows_partial_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RowsSmem));
-        if (e != cudaSuccess) return (int)e;
-        sms = device_sms();
-    }
-    cudaError_t e = cudaMemsetAsync(a->workspace, 0, 256, s);         // WsHeader: list counter
-    if (e != cudaSuccess) return (int)e;
-    lz4_scan_partial_kernel<<<(unsigned)((a->nBlocks + 127) / 128), 128, 0, s>>>(*a);
-    const int64_t grid = a->nBlocks < sms ? a->nBlocks : sms;         // persistent: one CTA per SM
-    lz4_expand_rows_partial_kernel<<<(unsigned)grid, kRowsThreads, sizeof(RowsSmem), s>>>(*a);
-    int64_t grid2 = (a->nBlocks * 32 + 127) / 128;
-    if (grid2 > (int64_t)sms * 16) grid2 = (int64_t)sms * 16;
-    lz4_expand_generic_partial_kernel<<<(unsigned)grid2, 128, 0, s>>>(*a);
-    g_launches += 3;
     return (int)cudaGetLastError();
 }
 

@@ -43,15 +43,13 @@ typedef struct {
                                   are left to another launch */
 } lz4k_encode_args;
 
-size_t lz4k_decode_workspace_bytes(int64_t nBlocks);   /* any capacities */
-/* tighter: per-block capacity array (perBlockCaps != 0) or one capacity for every block */
-size_t lz4k_decode_workspace_bytes_for(int64_t nBlocks, int perBlockCaps, int32_t dstCap);
-size_t lz4k_decode_workspace_bytes_min(int64_t nBlocks, int perBlockCaps, int32_t dstCap);   /* without the wide marks of the tiles kernel */
-/* phases: bit 0 = scan (validate, sizes), bit 1 = expand (move bytes; needs a prior scan's outSize) */
-int lz4k_launch_decode(const lz4k_decode_args* a, int phases, void* stream);
-/* LZ4_decompress_safe_partial per block with outputSize = (dstCapArr ? dstCapArr[i] : dstCap): scan and expand, three
- * launches; the workspace layout is the one lz4k_decode_workspace_bytes_min sizes */
-int lz4k_launch_decode_partial(const lz4k_decode_args* a, void* stream);
+/* the workspace a decode call of per-block capacities (perBlockCaps != 0) or one capacity dstCap for every block uses when
+ * it is given workspaceBytes: SIZE_MAX gives the size that enables the tiles kernel, 0 the smallest a call accepts (the
+ * partial call's layout) */
+size_t lz4k_decode_workspace_bytes(int64_t nBlocks, int perBlockCaps, int32_t dstCap, size_t workspaceBytes);
+/* phases: bit 0 = scan (validate, sizes), bit 1 = expand (move bytes; needs a prior scan's outSize).  partial:
+ * LZ4_decompress_safe_partial per block with outputSize = (dstCapArr ? dstCapArr[i] : dstCap), both phases */
+int lz4k_launch_decode(const lz4k_decode_args* a, int phases, int partial, void* stream);
 int lz4k_launch_encode(const lz4k_encode_args* a, void* stream);       /* byte-identical to LZ4_compress_fast */
 int lz4k_launch_encode_par(const lz4k_encode_args* a, void* stream);   /* parallel parse; blocks of <= 65 536 bytes */
 /* byte-identical to LZ4_compress_destSize_extState with targetDstSize = dstCap: outSize[i] its return value,

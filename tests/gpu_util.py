@@ -32,7 +32,7 @@ def pack_host_blocks(blocks):
 # decode calls
 # ------------------------------------------------------------------------------------------
 def ws_lists(ws, n):
-    """(nSeq[n], slow list) left in a decode workspace.  Layout (lz4_kernels.cu:149-164, ws_view): a 256-byte header
+    """(nSeq[n], slow list) left in a decode workspace.  Layout (plan_layout, lz4_decode_plan.h): a 256-byte header
     whose first word is the slow-list count, then nSeq[n] and slowList[n], each rounded up to 256 bytes."""
     lst = (n * 4 + 255) // 256 * 256
     w = ws[:256 + 2 * lst].cpu().numpy().view(np.uint32)
@@ -42,13 +42,13 @@ def ws_lists(ws, n):
 
 
 def route(n_blocks, cap=None, per_block_caps=False, ws_bytes=0):
-    """The decode route lz4k_launch_decode (lz4_kernels.cu:1381-1458) takes with LZ4K_SCAN_IMPL unset:
+    """The decode route lz4k_launch_decode takes with LZ4K_SCAN_IMPL unset (plan_decode, lz4_decode_plan.h):
       R1 per-block capacities: one-thread scan -> rows / generic
       R2 one capacity in [16 KB, 64 KB], <= 8 192 blocks: split scan -> rows / generic
       R3 one capacity in [16 KB, 64 KB], > 8 192 blocks: one-thread scan -> rows / generic
       R4 one capacity below 16 KB: one-thread scan -> rows / generic
-      R5 one capacity in (64 KB, 64 MB] and the workspace of LZ4B200_decompress_workspace_bytes_for (use_wide,
-         lz4_kernels.cu:177): parallel scan -> tile index -> tiles / generic
+      R5 one capacity in (64 KB, 64 MB] and the workspace of LZ4B200_decompress_workspace_bytes_for (the
+         plan's wide flag): parallel scan -> tile index -> tiles / generic
       R6 one capacity above 64 KB otherwise: parallel scan -> generic"""
     if per_block_caps:
         return "R1"
@@ -152,7 +152,7 @@ def decode_batch_uniform(blocks, cap, wide=True, stride=None, phases="one", dst_
 
 
 def wide_workspace(res, n, cap):
-    """Readers of what the scan and the tile index left in an R5 call's workspace (ws_view, lz4_kernels.cu): header |
+    """Readers of what the scan and the tile index left in an R5 call's workspace (plan_layout, lz4_decode_plan.h): header |
     nSeq | slowList | marks (2 * (cap / 4 + 2) words per block) | tileFirst (tiles_of(cap) + 1 words per block) |
     tileFlag.  Returns (marks(b, nseq): the first nseq wide marks of block b, flattened; tile_first(b, nt): its first
     nt + 1 tileFirst entries)."""

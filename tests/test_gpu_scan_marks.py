@@ -46,7 +46,7 @@ def host_scan(tmp_path_factory):
             pad = (-buf.ctypes.data) % 16 + 16
             buf[pad:pad + n] = np.frombuffer(block, dtype=np.uint8)
             table = np.full(stride + 8, SENT, dtype=np.uint32)
-            has_marks = 0 < n <= 65535 and 0 < cap <= 65536          # scan_marks (lz4_kernels.cu)
+            has_marks = 0 < n <= 65535 and 0 < cap <= 65536          # block_marks (lz4_decode_plan.h)
             ns = C.c_uint32(0)
             r = lib.scan_host_cap(buf.ctypes.data + pad, n, cap, C.byref(ns), table.ctypes.data if has_marks else None, stride)
             memo[key] = (r, ns.value, table[:stride].copy())
@@ -55,7 +55,7 @@ def host_scan(tmp_path_factory):
 
 
 def narrow_workspace(ws, n, stride):
-    """nSeq[n] and the narrow marks tables (n x stride words) of a workspace (ws_view, lz4_kernels.cu): a 256-byte
+    """nSeq[n] and the narrow marks tables (n x stride words) of a workspace (plan_layout, lz4_decode_plan.h): a 256-byte
     header, nSeq[n], slowList[n] (each rounded up to 256 bytes), then the marks"""
     r256 = lambda x: (x + 255) // 256 * 256
     w = ws.cpu().numpy().view(np.uint32)
