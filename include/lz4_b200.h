@@ -213,6 +213,29 @@ LZ4B200_API int LZ4B200_compress_blocks_destSize(const void* d_src, int64_t srcS
                                                  int32_t* d_outSize, int32_t* d_srcConsumed, int64_t nBlocks, void* stream);
 
 /*
+ * Compress every block at an HC level (the batched LZ4_compress_HC, lz4hc.h:63 / lz4hc.c:1519-1535):
+ *   block i input : d_src + i*srcStride, size n_i = (d_srcSize ? d_srcSize[i] : srcSize), any size the reference takes
+ *   block i output: d_dst + i*dstStride, capacity dstCap
+ *   d_outSize[i]  : LZ4_compress_HC(src_i, dst_i, n_i, dstCap, compressionLevel); block i's bytes are the reference's
+ * Levels follow LZ4HC_getCLevelParams (lz4hc.c:92-116): below 1 means 9; 1 and 2 take the lz4mid parse (lz4hc.c:522-773);
+ * 3 .. 9 the hash-chain parse (lz4hc.c:1121-1362) with 4 .. 256 searches, and pattern analysis at 9.  Routing is that of
+ * LZ4_compress_HC_extStateHC_fastReset (lz4hc.c:1500-1510): dstCap < LZ4_compressBound(n_i) limits the output (0 when the
+ * block does not fit); a size outside 0 .. LZ4_MAX_INPUT_SIZE gives 0; n_i == 0 gives the one byte 0x00 when dstCap >= 1.
+ * Nothing at or past dst_i + dstCap is written; a block that returns 0 may have written its slot below dstCap.  Every
+ * block starts from a fresh state, so the result does not depend on the batch, the order or the workspace.
+ * The input is read in aligned 4-byte words, each of which holds at least one byte of the block.
+ * The workspace is at least LZ4B200_compress_blocks_hc_workspace_bytes(nBlocks) bytes (256 KB per block, for at most
+ * 16 384 blocks); a larger one lets more blocks run at once.  One kernel launch; nBlocks == 0 returns LZ4B200_OK without
+ * one.  LZ4B200_ERR_ARG: compressionLevel >= 10 (the optimal parser of levels 10 .. 12 is not built), nBlocks < 0, a NULL
+ * d_dst, d_outSize or d_workspace, a NULL d_src with blocks present, or a workspace smaller than the size function asks.
+ */
+LZ4B200_API size_t LZ4B200_compress_blocks_hc_workspace_bytes(int64_t nBlocks);
+LZ4B200_API int LZ4B200_compress_blocks_hc(const void* d_src, int64_t srcStride, const int32_t* d_srcSize, int32_t srcSize,
+                                           void* d_dst, int64_t dstStride, int32_t dstCap, int compressionLevel,
+                                           int32_t* d_outSize, int64_t nBlocks,
+                                           void* d_workspace, size_t workspaceBytes, void* stream);
+
+/*
  * The same call with the PARALLEL PARSE (throughput mode): every block is a valid LZ4 block that
  * LZ4_decompress_safe expands to the input, the result is deterministic, but it is NOT byte-identical to
  * LZ4_compress_fast: every position is a match candidate (no skipping), matches are chosen by the same greedy

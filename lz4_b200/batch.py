@@ -137,6 +137,39 @@ def compress_blocks(src, block_size, acceleration=1, slots=None, slot_stride=Non
     return slots, out_sizes[:n], stride
 
 
+def compress_blocks_hc(src, block_size, level=9, slots=None, slot_stride=None, slot_capacity=None, out_sizes=None,
+                       stream=None):
+    """Compress src (u8 device tensor) as ceil(len/block_size) independent blocks at an HC level
+    (LZ4B200_compress_blocks_hc: block i is LZ4_compress_HC(block_i, slot_i, n_i, slot_capacity, level), byte for byte).
+
+    Levels 1 .. 9 (below 1 means 9); 10 .. 12 raise, their optimal parser is not built.
+    Returns (slots, out_sizes, slot_stride): block i's bytes are slots[i*slot_stride : i*slot_stride+out_sizes[i]].
+    """
+    lib = _lib.load()
+    _need_cuda(src, slots)
+    total = int(src.numel())
+    n = (total + block_size - 1) // block_size if total else 0
+    cap = int(slot_capacity if slot_capacity is not None else compress_bound(block_size))
+    stride = int(slot_stride if slot_stride is not None else ((cap + 15) // 16) * 16)
+    src_sizes = None
+    st = _stream(stream)
+    with torch.cuda.stream(st):
+        if slots is None:
+            slots = torch.empty(max(n, 1) * stride, dtype=torch.uint8, device=src.device)
+        if out_sizes is None:
+            out_sizes = torch.empty(max(n, 1), dtype=torch.int32, device=src.device)
+        if n and total != n * block_size:
+            src_sizes = torch.full((n,), block_size, dtype=torch.int32, device=src.device)
+            src_sizes[-1] = total - (n - 1) * block_size
+    workspace = _workspace(src.device, max(int(lib.LZ4B200_compress_blocks_hc_workspace_bytes(n)), 1), st)
+    rc = lib.LZ4B200_compress_blocks_hc(src.data_ptr(), int(block_size),
+                                        src_sizes.data_ptr() if src_sizes is not None else None, int(block_size),
+                                        slots.data_ptr(), stride, cap, int(level), out_sizes.data_ptr(), n,
+                                        workspace.data_ptr(), workspace.numel(), st.cuda_stream)
+    _lib.check(rc, "LZ4B200_compress_blocks_hc")
+    return slots, out_sizes[:n], stride
+
+
 def compress_blocks_dest_size(src, block_size, target, acceleration=1, slots=None, slot_stride=None, out_sizes=None,
                               consumed=None, src_sizes=None, stream=None):
     """Compress as much of each block of src as fits into `target` bytes (LZ4B200_compress_blocks_destSize: block i is

@@ -233,6 +233,29 @@ int LZ4B200_compress_blocks(const void* d_src, int64_t srcStride, const int32_t*
     return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_encode");
 }
 
+size_t LZ4B200_compress_blocks_hc_workspace_bytes(int64_t nBlocks)
+{
+    return lz4k_encode_hc_workspace_bytes(nBlocks);
+}
+
+int LZ4B200_compress_blocks_hc(const void* d_src, int64_t srcStride, const int32_t* d_srcSize, int32_t srcSize,
+                               void* d_dst, int64_t dstStride, int32_t dstCap, int compressionLevel,
+                               int32_t* d_outSize, int64_t nBlocks,
+                               void* d_workspace, size_t workspaceBytes, void* stream)
+{
+    lz4k_encode_args a;
+    cudaError_t e;
+    if (compressionLevel >= 10) return LZ4B200_ERR_ARG;     /* the optimal parser (lz4hc.c:1823-) is not built */
+    if (nBlocks < 0 || !d_dst || !d_outSize || !d_workspace) return LZ4B200_ERR_ARG;
+    if (nBlocks == 0) return LZ4B200_OK;
+    if (!d_src || workspaceBytes < lz4k_encode_hc_workspace_bytes(nBlocks)) return LZ4B200_ERR_ARG;
+    a.src = (const uint8_t*)d_src; a.srcStride = srcStride; a.srcSizeArr = d_srcSize; a.srcSize = srcSize;
+    a.dst = (uint8_t*)d_dst; a.dstStride = dstStride; a.dstCap = dstCap; a.acceleration = 0;
+    a.outSize = d_outSize; a.nBlocks = nBlocks; a.minSize = INT32_MIN; a.maxSize = INT32_MAX;
+    e = (cudaError_t)lz4k_launch_encode_hc(&a, compressionLevel, d_workspace, workspaceBytes, stream);
+    return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_encode_hc");
+}
+
 int LZ4B200_compress_blocks_destSize(const void* d_src, int64_t srcStride, const int32_t* d_srcSize, int32_t srcSize,
                                      void* d_dst, int64_t dstStride, int32_t targetDstSize, int acceleration,
                                      int32_t* d_outSize, int32_t* d_srcConsumed, int64_t nBlocks, void* stream)

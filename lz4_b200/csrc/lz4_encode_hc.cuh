@@ -1,0 +1,59 @@
+/*
+ * lz4_encode_hc.cuh -- LZ4_compress_HC at levels 1 .. 9 over a batch (included by lz4_kernels.cu).
+ *
+ * The HC parse is sequential within a block, so one THREAD compresses one block at a time with the parse of
+ * lz4_hc_core.h, and the parallelism is across blocks.  A block's state is a 2^15 x u32 hash table and a 64 K x u16
+ * chain table (256 KB), more than an SM's shared memory, so every thread owns one workspace slot in global memory and
+ * takes blocks t, t + slots, t + 2 * slots, ...  The hash table is zeroed before every block; the chain table is not
+ * (lz4_hc_core.h shows why no entry is read before it is written).  DESIGN.md section 3.7.
+ */
+
+constexpr int kHcThreads = 32;
+constexpr size_t kHcHashBytes = (size_t)hc::kHashEntries * sizeof(uint32_t);
+constexpr size_t kHcSlotBytes = kHcHashBytes + (size_t)hc::kChainEntries * sizeof(uint16_t);
+
+struct HcDevAcc {
+    const uint8_t* src;
+    uint8_t* dst;
+    uint32_t* ht;
+    uint16_t* ct;
+    /* 4 input bytes from the two aligned words holding them: both words hold bytes of the block */
+    __device__ __forceinline__ uint32_t in32(uint32_t p) const
+    {
+        const uintptr_t a = reinterpret_cast<uintptr_t>(src + p);
+        const uint32_t lo = __ldg(reinterpret_cast<const uint32_t*>(a & ~uintptr_t(3)));
+        const uint32_t hi = __ldg(reinterpret_cast<const uint32_t*>((a + 3) & ~uintptr_t(3)));
+        return __funnelshift_r(lo, hi, (uint32_t)(a & 3) * 8);
+    }
+    __device__ __forceinline__ uint32_t in8(uint32_t p) const { return __ldg(src + p); }
+    __device__ __forceinline__ uint64_t in64(uint32_t p) const { return (uint64_t)in32(p) | ((uint64_t)in32(p + 4) << 32); }
+    __device__ __forceinline__ uint32_t hash(uint32_t h) const { return ht[h]; }
+    __device__ __forceinline__ void set_hash(uint32_t h, uint32_t v) const { ht[h] = v; }
+    __device__ __forceinline__ uint32_t chain(uint32_t i) const { return ct[i]; }
+    __device__ __forceinline__ void set_chain(uint32_t i, uint32_t v) const { ct[i] = (uint16_t)v; }
+    __device__ __forceinline__ void out(int64_t o, uint32_t v) const { dst[o] = (uint8_t)v; }
+    __device__ __forceinline__ void copy(int64_t o, uint32_t p, uint32_t len) const
+    {
+        for (uint32_t k = 0; k < len; k++) dst[o + k] = __ldg(src + p + k);
+    }
+};
+
+/* slots = the threads that run: min(nBlocks, workspace slots) */
+__global__ void __launch_bounds__(kHcThreads) lz4_encode_hc_kernel(lz4k_encode_args a, uint8_t* ws, int64_t slots, int level)
+{
+    const int64_t t = (int64_t)blockIdx.x * kHcThreads + threadIdx.x;
+    if (t >= slots) return;
+    HcDevAcc acc;
+    acc.ht = reinterpret_cast<uint32_t*>(ws + t * kHcSlotBytes);
+    acc.ct = reinterpret_cast<uint16_t*>(ws + t * kHcSlotBytes + kHcHashBytes);
+    for (int64_t b = t; b < a.nBlocks; b += slots) {
+        const int n = a.srcSizeArr ? a.srcSizeArr[b] : a.srcSize;
+        acc.src = a.src + b * a.srcStride;
+        acc.dst = a.dst + b * a.dstStride;
+        if (n >= hc::kMinLength && (uint32_t)n <= hc::kMaxInput) {         // shorter blocks never touch the tables
+            uint4* h = reinterpret_cast<uint4*>(acc.ht);
+            for (int k = 0; k < (int)(kHcHashBytes / sizeof(uint4)); k++) h[k] = make_uint4(0, 0, 0, 0);
+        }
+        a.outSize[b] = hc::hc_compress_block(acc, n, a.dstCap, level);
+    }
+}

@@ -1,0 +1,450 @@
+/*
+ * lz4_hc_core.h -- the parse of LZ4_compress_HC (lz4hc.c, v1.10.0) at levels 1 .. 9, for host and device.
+ *
+ * One call compresses one block from a freshly initialised state, exactly as LZ4_compress_HC does with no dictionary,
+ * no chain swap and favorDecSpeed off (lz4hc.c:1500-1510): the same output bytes and the same return value.
+ *   levels 1 .. 2 (and the lz4mid entries of the level table): LZ4MID_compress, lz4hc.c:522-773
+ *   levels 3 .. 9 (and < 1 -> 9):                             LZ4HC_compress_hashChain, lz4hc.c:1121-1362
+ * Levels 10 .. 12 use the optimal parser, which is not built here: hc_compress_block returns kHcNoLevel for them.
+ *
+ * Positions are byte offsets into the block.  The reference's indices are position + kHcStart (LZ4HC_init_internal,
+ * lz4hc.c:242-259, starts a fresh state at 64 KB), so a zero hash entry is never a candidate.
+ *
+ * The parse reaches its input, its tables and its output through an accessor `A` with
+ *   uint32_t in8(uint32_t p), in32(uint32_t p)      byte / little-endian 32-bit word of the input at p
+ *   uint64_t in64(uint32_t p)                       little-endian 64-bit word of the input at p
+ *   uint32_t hash(uint32_t h); void set_hash(uint32_t h, uint32_t v)      2^15 entries, all 0 at the start of a block
+ *   uint32_t chain(uint32_t i); void set_chain(uint32_t i, uint32_t v)    2^16 16-bit entries, any content at the start
+ *   void out(int64_t o, uint32_t v); void copy(int64_t o, uint32_t p, uint32_t len)    output byte / literal copy
+ * The chain table needs no initial value: the hash-chain walk only reads the entry of an index in
+ * [ipIndex - 65535, ipIndex), and LZ4HC_Insert has written every such index before the walk, the entry of index i last.
+ * Nothing is written at or past the capacity: every output byte is written after the check that covers it.
+ */
+#ifndef LZ4_HC_CORE_H
+#define LZ4_HC_CORE_H
+
+#include <stdint.h>
+
+#if defined(__CUDACC__)
+#define HC_FN __host__ __device__ __forceinline__
+#else
+#define HC_FN static inline
+#endif
+
+namespace hc {
+
+constexpr int kMinMatch = 4;
+constexpr int kLastLiterals = 5;
+constexpr int kMfLimit = 12;
+constexpr int kMinLength = kMfLimit + 1;
+constexpr int kOptimalMl = 18;                    /* (ML_MASK - 1) + MINMATCH, lz4hc.c:76 */
+constexpr uint32_t kMaxDistance = 65535;          /* LZ4_DISTANCE_MAX */
+constexpr uint32_t kHcStart = 65536;              /* index of a fresh state's first byte, lz4hc.c:252 */
+constexpr uint32_t kMaxInput = 0x7E000000u;       /* LZ4_MAX_INPUT_SIZE */
+constexpr int kHashLog = 15;                      /* LZ4HC_HASH_LOG */
+constexpr int kMidHashLog = kHashLog - 1;         /* LZ4MID_HASHLOG: hash4 table, then hash8 table */
+constexpr uint32_t kMidHash8 = 1u << kMidHashLog;
+constexpr int kHashEntries = 1 << kHashLog;
+constexpr int kChainEntries = 1 << 16;
+constexpr int kMaxLevel = 9;                      /* above: the optimal parser */
+constexpr int kHcNoLevel = -1;
+
+struct Level { bool mid; int nbSearches; };
+
+/* LZ4HC_getCLevelParams (lz4hc.c:92-116) below the optimal parser */
+HC_FN Level level_params(int level)
+{
+    if (level < 1) level = 9;                     /* LZ4HC_CLEVEL_DEFAULT */
+    Level l;
+    l.mid = level <= 2;                           /* lz4mid, 2 searches (unused by the mid parse) */
+    l.nbSearches = l.mid ? 2 : 1 << (level - 1);  /* 3 -> 4, 4 -> 8, ..., 9 -> 256 */
+    return l;
+}
+
+HC_FN uint32_t hash4(uint32_t v) { return (v * 2654435761u) >> (32 - kHashLog); }
+HC_FN uint32_t mid_hash4(uint32_t v) { return (v * 2654435761u) >> (32 - kMidHashLog); }
+HC_FN uint32_t mid_hash8(uint64_t v) { return (uint32_t)(((v << 8) * 58295818150454627ull) >> (64 - kMidHashLog)); }
+
+HC_FN int ctz32(uint32_t x)
+{
+#if defined(__CUDA_ARCH__)
+    return __ffs((int)x) - 1;
+#else
+    return __builtin_ctz(x);
+#endif
+}
+
+/* LZ4_count: the common prefix of p and m, not reaching `limit` */
+template <class A> HC_FN uint32_t count(A& a, uint32_t p, uint32_t m, uint32_t limit)
+{
+    const uint32_t p0 = p;
+    while (p + 4 <= limit) {
+        const uint32_t x = a.in32(p) ^ a.in32(m);
+        if (x) return p - p0 + (uint32_t)(ctz32(x) >> 3);
+        p += 4; m += 4;
+    }
+    while (p < limit && a.in8(p) == a.in8(m)) { p++; m++; }
+    return p - p0;
+}
+
+/* LZ4HC_countBack: minus the common bytes before p and m, at most `most` of them */
+template <class A> HC_FN int count_back(A& a, uint32_t p, uint32_t m, uint32_t most)
+{
+    uint32_t k = 0;
+    while (k < most && a.in8(p - 1 - k) == a.in8(m - 1 - k)) k++;
+    return -(int)k;
+}
+
+/* LZ4HC_countPattern: bytes from p, before `end`, that continue the 4-byte pattern from its byte 0 */
+template <class A> HC_FN uint32_t count_pattern(A& a, uint32_t p, uint32_t end, uint32_t pattern)
+{
+    uint32_t k = 0;
+    while (p + k + 4 <= end && a.in32(p + k) == pattern) k += 4;
+    while (p + k < end && a.in8(p + k) == ((pattern >> ((k & 3) * 8)) & 0xFF)) k++;
+    return k;
+}
+
+/* LZ4HC_reverseCountPattern with iLow = the block start: bytes before p that continue the pattern backwards from its
+ * byte 3 */
+template <class A> HC_FN uint32_t reverse_count_pattern(A& a, uint32_t p, uint32_t pattern)
+{
+    uint32_t k = 0;
+    while (k + 4 <= p && a.in32(p - k - 4) == pattern) k += 4;
+    while (k < p && a.in8(p - 1 - k) == ((pattern >> ((3 - (k & 3)) * 8)) & 0xFF)) k++;
+    return k;
+}
+
+struct Out {
+    int64_t op;           /* bytes written */
+    int64_t cap;          /* dstCapacity */
+    bool limited;         /* limitedOutput */
+};
+
+/* the length bytes after a 15 in a token nibble */
+template <class A> HC_FN void put_length(A& a, Out& o, uint32_t len)
+{
+    for (; len >= 255; len -= 255) a.out(o.op++, 255);
+    a.out(o.op++, len);
+}
+
+/* LZ4HC_encodeSequence (lz4hc.c:268-354): literals [anchor, ip), then the match.  false when the output limit is hit
+ * (the caller's block then returns 0); on success ip and anchor move past the match. */
+template <class A> HC_FN bool encode_sequence(A& a, Out& o, uint32_t& ip, uint32_t& anchor, uint32_t mlen, uint32_t off)
+{
+    const int64_t token = o.op++;
+    const uint32_t ll = ip - anchor;
+    if (o.limited && o.op + ll / 255 + ll + (2 + 1 + kLastLiterals) > o.cap) return false;
+    uint32_t t;
+    if (ll >= 15) { t = 15u << 4; put_length(a, o, ll - 15); }
+    else t = ll << 4;
+    a.copy(o.op, anchor, ll);
+    o.op += ll;
+    a.out(o.op++, off & 0xFF);
+    a.out(o.op++, off >> 8);
+    uint32_t ml = mlen - kMinMatch;
+    if (o.limited && o.op + ml / 255 + (1 + kLastLiterals) > o.cap) return false;
+    if (ml >= 15) {
+        t += 15;
+        ml -= 15;
+        for (; ml >= 510; ml -= 510) { a.out(o.op++, 255); a.out(o.op++, 255); }
+        if (ml >= 255) { ml -= 255; a.out(o.op++, 255); }
+        a.out(o.op++, ml);
+    } else {
+        t += ml;
+    }
+    a.out(token, t);
+    ip += mlen;
+    anchor = ip;
+    return true;
+}
+
+/* the last literals (lz4hc.c:1308-1334, 707-735): the block's size, or 0 when they do not fit a limited output */
+template <class A> HC_FN int last_literals(A& a, Out& o, uint32_t anchor, uint32_t n)
+{
+    const uint32_t run = n - anchor;
+    const int64_t total = 1 + (int64_t)(run + 255 - 15) / 255 + run;
+    if (o.limited && o.op + total > o.cap) return 0;
+    if (run >= 15) { a.out(o.op++, 15u << 4); put_length(a, o, run - 15); }
+    else a.out(o.op++, run << 4);
+    a.copy(o.op, anchor, run);
+    o.op += run;
+    return (int)o.op;
+}
+
+/* LZ4MID_compress (lz4hc.c:522-773) without a dictionary.  Note that ipIndex keeps the search position's index when the
+ * catch-back or the ip + 1 match moves ip: the reference adds the next positions with it. */
+template <class A> HC_FN int mid_compress(A& a, Out& o, uint32_t n)
+{
+    uint32_t ip = 0, anchor = 0;
+    if (n < (uint32_t)kMinLength) return last_literals(a, o, anchor, n);
+    const uint32_t mflimit = n - kMfLimit, matchlimit = n - kLastLiterals;
+    const uint32_t ilimitIdx = n - 8 + kHcStart;                    /* LZ4MID_HASHSIZE */
+    while (ip <= mflimit) {
+        const uint32_t ipIndex = ip + kHcStart;
+        uint32_t mlen = 0, dist = 0;
+        bool found = false;
+        {   /* long match */
+            const uint32_t h8 = kMidHash8 + mid_hash8(a.in64(ip));
+            const uint32_t pos8 = a.hash(h8);
+            a.set_hash(h8, ipIndex);
+            if (ipIndex - pos8 <= kMaxDistance && pos8 >= kHcStart) {
+                mlen = count(a, ip, pos8 - kHcStart, matchlimit);
+                if (mlen >= (uint32_t)kMinMatch) { dist = ipIndex - pos8; found = true; }
+            }
+        }
+        if (!found) {   /* short match, then a longer one at ip + 1 */
+            const uint32_t h4 = mid_hash4(a.in32(ip));
+            const uint32_t pos4 = a.hash(h4);
+            a.set_hash(h4, ipIndex);
+            if (ipIndex - pos4 <= kMaxDistance && pos4 >= kHcStart) {
+                mlen = count(a, ip, pos4 - kHcStart, matchlimit);
+                if (mlen >= (uint32_t)kMinMatch) {
+                    const uint32_t h8 = kMidHash8 + mid_hash8(a.in64(ip + 1));
+                    const uint32_t pos8 = a.hash(h8);
+                    const uint32_t d2 = ipIndex + 1 - pos8;
+                    dist = ipIndex - pos4;
+                    found = true;
+                    if (d2 <= kMaxDistance && pos8 >= kHcStart && ip < mflimit) {
+                        const uint32_t ml2 = count(a, ip + 1, pos8 - kHcStart, matchlimit);
+                        if (ml2 > mlen) {
+                            a.set_hash(h8, ipIndex + 1);
+                            ip++;
+                            mlen = ml2;
+                            dist = d2;
+                        }
+                    }
+                }
+            }
+        }
+        if (!found) {
+            ip += 1 + ((ip - anchor) >> 9);
+            continue;
+        }
+        while (ip > anchor && ip > dist && a.in8(ip - 1) == a.in8(ip - 1 - dist)) { ip--; mlen++; }
+        a.set_hash(kMidHash8 + mid_hash8(a.in64(ip + 1)), ipIndex + 1);
+        a.set_hash(kMidHash8 + mid_hash8(a.in64(ip + 2)), ipIndex + 2);
+        a.set_hash(mid_hash4(a.in32(ip + 1)), ipIndex + 1);
+        if (!encode_sequence(a, o, ip, anchor, mlen, dist)) return 0;
+        const uint32_t end = ip + kHcStart;
+        if (end - 2 < ilimitIdx) {
+            if (ip > 5) a.set_hash(kMidHash8 + mid_hash8(a.in64(ip - 5)), end - 5);
+            a.set_hash(kMidHash8 + mid_hash8(a.in64(ip - 3)), end - 3);
+            a.set_hash(kMidHash8 + mid_hash8(a.in64(ip - 2)), end - 2);
+            a.set_hash(mid_hash4(a.in32(ip - 2)), end - 2);
+            a.set_hash(mid_hash4(a.in32(ip - 1)), end - 1);
+        }
+    }
+    return last_literals(a, o, anchor, n);
+}
+
+struct Match { int len, off, back; };
+
+struct ChainState {
+    uint32_t nextToUpdate;    /* index */
+    int nbSearches;
+    bool patternAnalysis;
+};
+
+/* LZ4HC_Insert (lz4hc.c:781-802): every index before `target` joins its hash chain */
+template <class A> HC_FN void insert(A& a, ChainState& s, uint32_t target)
+{
+    for (uint32_t idx = s.nextToUpdate; idx < target; idx++) {
+        const uint32_t h = hash4(a.in32(idx - kHcStart));
+        uint32_t delta = idx - a.hash(h);
+        if (delta > kMaxDistance) delta = kMaxDistance;
+        a.set_chain(idx & 0xFFFF, delta);
+        a.set_hash(h, idx);
+    }
+    s.nextToUpdate = target;
+}
+
+/* LZ4HC_InsertAndGetWiderMatch (lz4hc.c:884-1104) for one prefix, no chain swap, no favorDecSpeed: the longest match
+ * through ip that starts no earlier than iLow, is longer than `longest` and ends by iHigh.  The candidates are taken in
+ * the chain's order, and the 2-byte quick reject at longest - 1 comes first: it decides which later candidates count. */
+template <class A> HC_FN Match wider_match(A& a, ChainState& s, uint32_t ip, uint32_t iLow, uint32_t iHigh, int longest)
+{
+    const uint32_t ipIndex = ip + kHcStart;
+    const uint32_t lowest = (kHcStart + kMaxDistance + 1 > ipIndex) ? kHcStart : ipIndex - kMaxDistance;
+    const uint32_t lookBack = ip - iLow;
+    const uint32_t pattern = a.in32(ip);
+    int nb = s.nbSearches;
+    int repeat = 0;                       /* 0 untested, 1 not a repeat, 2 confirmed */
+    uint32_t srcPatternLength = 0;
+    Match r; r.len = longest; r.off = 0; r.back = 0;
+    insert(a, s, ipIndex);
+    uint32_t matchIndex = a.hash(hash4(pattern));
+    while (matchIndex >= lowest && nb > 0) {
+        nb--;
+        const uint32_t m = matchIndex - kHcStart;
+        const uint32_t q = (uint32_t)r.len - 1;
+        if (a.in8(iLow + q) == a.in8(m - lookBack + q) && a.in8(iLow + q + 1) == a.in8(m - lookBack + q + 1)
+            && a.in32(m) == pattern) {
+            const uint32_t most = lookBack < m ? lookBack : m;
+            const int back = lookBack ? count_back(a, ip, m, most) : 0;
+            const int len = kMinMatch + (int)count(a, ip + kMinMatch, m + kMinMatch, iHigh) - back;
+            if (len > r.len) { r.len = len; r.off = (int)(ipIndex - matchIndex); r.back = back; }
+        }
+        const uint32_t next = a.chain(matchIndex & 0xFFFF);
+        if (s.patternAnalysis && next == 1) {
+            const uint32_t cand = matchIndex - 1;
+            if (repeat == 0) {
+                if ((pattern & 0xFFFF) == (pattern >> 16) && (pattern & 0xFF) == (pattern >> 24)) {
+                    repeat = 2;
+                    srcPatternLength = count_pattern(a, ip + 4, iHigh, pattern) + 4;
+                } else {
+                    repeat = 1;
+                }
+            }
+            if (repeat == 2 && cand >= lowest) {
+                const uint32_t mp = cand - kHcStart;
+                if (a.in32(mp) == pattern) {
+                    const uint32_t fwd = count_pattern(a, mp + 4, iHigh, pattern) + 4;
+                    uint32_t backLength = reverse_count_pattern(a, mp, pattern);
+                    const uint32_t from = cand - backLength > lowest ? cand - backLength : lowest;
+                    backLength = cand - from;
+                    const uint32_t segment = backLength + fwd;
+                    if (segment >= srcPatternLength && fwd <= srcPatternLength) {
+                        matchIndex = cand + fwd - srcPatternLength;        /* the whole source pattern fits */
+                    } else {
+                        matchIndex = cand - backLength;                    /* the segment's farthest position */
+                        if (lookBack == 0) {
+                            const uint32_t maxML = segment < srcPatternLength ? segment : srcPatternLength;
+                            if ((uint32_t)r.len < maxML) {
+                                if (ipIndex - matchIndex > kMaxDistance) break;
+                                r.len = (int)maxML;
+                                r.off = (int)(ipIndex - matchIndex);
+                            }
+                            const uint32_t d = a.chain(matchIndex & 0xFFFF);
+                            if (d > matchIndex) break;
+                            matchIndex -= d;
+                        }
+                    }
+                    continue;
+                }
+            }
+        }
+        matchIndex -= next;
+    }
+    return r;
+}
+
+/* LZ4HC_compress_hashChain (lz4hc.c:1121-1362) without a dictionary: the _Search2 / _Search3 state machine */
+template <class A> HC_FN int chain_compress(A& a, Out& o, uint32_t n, int nbSearches)
+{
+    uint32_t anchor = 0;
+    if (n < (uint32_t)kMinLength) return last_literals(a, o, anchor, n);
+    ChainState s;
+    s.nextToUpdate = kHcStart;
+    s.nbSearches = nbSearches;
+    s.patternAnalysis = nbSearches > 128;
+    const int mflimit = (int)n - kMfLimit;
+    const uint32_t matchlimit = n - kLastLiterals;
+    int ip = 0, start0 = 0, start2 = 0, start3 = 0;
+    Match m0, m1, m2, m3;
+    const Match none = {0, 0, 0};
+    while (ip <= mflimit) {
+        m1 = wider_match(a, s, (uint32_t)ip, (uint32_t)ip, matchlimit, kMinMatch - 1);
+        if (m1.len < kMinMatch) { ip++; continue; }
+        start0 = ip; m0 = m1;
+        int state = 2;                        /* 2: _Search2, 3: _Search3, 0: back to the main loop */
+        while (state) {
+            if (state == 2) {
+                if (ip + m1.len <= mflimit) {
+                    start2 = ip + m1.len - 2;
+                    m2 = wider_match(a, s, (uint32_t)start2, (uint32_t)ip, matchlimit, m1.len);
+                    start2 += m2.back;
+                } else {
+                    m2 = none;
+                }
+                if (m2.len <= m1.len) {       /* no better match: ML1 goes out */
+                    uint32_t u = (uint32_t)ip, an = anchor;
+                    if (!encode_sequence(a, o, u, an, (uint32_t)m1.len, (uint32_t)m1.off)) return 0;
+                    ip = (int)u; anchor = an;
+                    state = 0;
+                    continue;
+                }
+                if (start0 < ip && start2 < ip + m0.len) { ip = start0; m1 = m0; }
+                if (start2 - ip < 3) { ip = start2; m1 = m2; continue; }     /* first match too short: dropped */
+                state = 3;
+            }
+            /* _Search3 */
+            if (start2 - ip < kOptimalMl) {
+                int newMl = m1.len > kOptimalMl ? kOptimalMl : m1.len;
+                if (ip + newMl > start2 + m2.len - kMinMatch) newMl = start2 - ip + m2.len - kMinMatch;
+                const int corr = newMl - (start2 - ip);
+                if (corr > 0) { start2 += corr; m2.len -= corr; }
+            }
+            if (start2 + m2.len <= mflimit) {
+                start3 = start2 + m2.len - 3;
+                m3 = wider_match(a, s, (uint32_t)start3, (uint32_t)start2, matchlimit, m2.len);
+                start3 += m3.back;
+            } else {
+                m3 = none;
+            }
+            if (m3.len <= m2.len) {           /* no better match: ML1 and ML2 go out */
+                if (start2 < ip + m1.len) m1.len = start2 - ip;
+                uint32_t u = (uint32_t)ip, an = anchor;
+                if (!encode_sequence(a, o, u, an, (uint32_t)m1.len, (uint32_t)m1.off)) return 0;
+                u = (uint32_t)start2;
+                if (!encode_sequence(a, o, u, an, (uint32_t)m2.len, (uint32_t)m2.off)) return 0;
+                ip = (int)u; anchor = an;
+                state = 0;
+                continue;
+            }
+            if (start3 < ip + m1.len + 3) {   /* no room for ML2 */
+                if (start3 >= ip + m1.len) {  /* ML1 goes out, ML3 becomes ML1 */
+                    if (start2 < ip + m1.len) {
+                        const int corr = ip + m1.len - start2;
+                        start2 += corr;
+                        m2.len -= corr;
+                        if (m2.len < kMinMatch) { start2 = start3; m2 = m3; }
+                    }
+                    uint32_t u = (uint32_t)ip, an = anchor;
+                    if (!encode_sequence(a, o, u, an, (uint32_t)m1.len, (uint32_t)m1.off)) return 0;
+                    anchor = an;
+                    ip = start3; m1 = m3;
+                    start0 = start2; m0 = m2;
+                    state = 2;
+                    continue;
+                }
+                start2 = start3; m2 = m3;
+                continue;                     /* _Search3 */
+            }
+            /* three ascending matches: ML1 goes out, shortened to meet ML2 */
+            if (start2 < ip + m1.len) {
+                if (start2 - ip < kOptimalMl) {
+                    if (m1.len > kOptimalMl) m1.len = kOptimalMl;
+                    if (ip + m1.len > start2 + m2.len - kMinMatch) m1.len = start2 - ip + m2.len - kMinMatch;
+                    const int corr = m1.len - (start2 - ip);
+                    if (corr > 0) { start2 += corr; m2.len -= corr; }
+                } else {
+                    m1.len = start2 - ip;
+                }
+            }
+            uint32_t u = (uint32_t)ip, an = anchor;
+            if (!encode_sequence(a, o, u, an, (uint32_t)m1.len, (uint32_t)m1.off)) return 0;
+            anchor = an;
+            ip = start2; m1 = m2;
+            start2 = start3; m2 = m3;
+        }
+    }
+    return last_literals(a, o, anchor, n);
+}
+
+/* LZ4_compress_HC(src, dst, n, cap, level) for level <= 9 from a fresh state; kHcNoLevel for levels above 9 */
+template <class A> HC_FN int hc_compress_block(A& a, int n, int cap, int level)
+{
+    if (level > kMaxLevel) return kHcNoLevel;
+    if ((uint32_t)n > kMaxInput) return 0;                                      /* lz4hc.c:1389 */
+    Out o;
+    o.op = 0;
+    o.cap = cap;
+    o.limited = cap < n + n / 255 + 16;                                         /* LZ4_compressBound, lz4hc.c:1506 */
+    const Level l = level_params(level);
+    return l.mid ? mid_compress(a, o, (uint32_t)n) : chain_compress(a, o, (uint32_t)n, l.nbSearches);
+}
+
+}  // namespace hc
+
+#undef HC_FN
+#endif

@@ -1247,6 +1247,8 @@ __global__ void __launch_bounds__(32) lz4_encode_dest_kernel(lz4k_encode_args a,
 }
 
 #include "lz4_encode_par.cuh"
+#include "lz4_hc_core.h"
+#include "lz4_encode_hc.cuh"
 
 /* =============================================================================================
  * pack: exclusive scan of sizes (+ optional 4-byte headers) and gather into a contiguous stream
@@ -1533,6 +1535,26 @@ int lz4k_launch_encode_par(const lz4k_encode_args* a, void* stream)
     }
     const int64_t grid = a->nBlocks < 2 * sms ? a->nBlocks : 2 * sms;        // persistent: two CTAs per SM, blocks c, c + grid, ...
     lz4_encode_par_kernel<<<(unsigned)grid, kEpThreads, sizeof(EncParSmem), s>>>(*a);
+    g_launches++;
+    return (int)cudaGetLastError();
+}
+
+/* The HC encoder's workspace slots: 16 384 x 256 KB = 4 GiB at most.  More slots in flight hide more of the chain
+ * walk's load latency; a caller that passes a larger workspace gets up to one slot per block. */
+constexpr int64_t kHcSlots = 16384;
+
+size_t lz4k_encode_hc_workspace_bytes(int64_t nBlocks)
+{
+    return nBlocks <= 0 ? 0 : (size_t)(nBlocks < kHcSlots ? nBlocks : kHcSlots) * kHcSlotBytes;
+}
+
+int lz4k_launch_encode_hc(const lz4k_encode_args* a, int level, void* workspace, size_t workspaceBytes, void* stream)
+{
+    if (a->nBlocks == 0) return 0;
+    const int64_t fit = (int64_t)(workspaceBytes / kHcSlotBytes);
+    const int64_t slots = a->nBlocks < fit ? a->nBlocks : fit;
+    const int64_t grid = (slots + kHcThreads - 1) / kHcThreads;
+    lz4_encode_hc_kernel<<<(unsigned)grid, kHcThreads, 0, (cudaStream_t)stream>>>(*a, (uint8_t*)workspace, slots, level);
     g_launches++;
     return (int)cudaGetLastError();
 }
