@@ -36,6 +36,40 @@ def compress_bound(n):
     return int(_lib.load().LZ4_compressBound(int(n)))
 
 
+def _decode_outputs(lib, comp, offsets, sizes, out_bytes, per_block, cap, out, out_sizes, workspace, st):
+    """out, out_sizes and the workspace of a decode call: the ones given, else new ones on the launch stream (the
+    workspace is sized by LZ4B200_decompress_workspace_bytes_for(n, per_block, cap))"""
+    n = int(sizes.numel())
+    with torch.cuda.stream(st):                     # temporaries belong to the stream the kernels run on
+        if out is None:
+            out = torch.empty(out_bytes, dtype=torch.uint8, device=comp.device)
+        if out_sizes is None:
+            out_sizes = torch.empty(n, dtype=torch.int32, device=comp.device)
+    ws_bytes = int(lib.LZ4B200_decompress_workspace_bytes_for(n, int(per_block), int(cap)))
+    if workspace is None or workspace.numel() < ws_bytes:
+        workspace = _workspace(comp.device, ws_bytes, st)
+    assert offsets.dtype == torch.int64 and sizes.dtype == torch.int32 and comp.dtype == torch.uint8
+    return out, out_sizes, workspace
+
+
+def _compress_layout(src, block_size, room, slots, slot_stride, out_sizes, src_sizes, st):
+    """The blocks of a compress call: ceil(len(src) / block_size) of them, in slots of slot_stride bytes (default: room
+    rounded up to 16).  slots, out_sizes and, for a short last block, the per-block src_sizes are allocated on the launch
+    stream unless given.  Returns (n, stride, slots, out_sizes, src_sizes)."""
+    total = int(src.numel())
+    n = (total + block_size - 1) // block_size if total else 0
+    stride = int(slot_stride if slot_stride is not None else ((room + 15) // 16) * 16)
+    with torch.cuda.stream(st):
+        if slots is None:
+            slots = torch.empty(max(n, 1) * stride, dtype=torch.uint8, device=src.device)
+        if out_sizes is None:
+            out_sizes = torch.empty(max(n, 1), dtype=torch.int32, device=src.device)
+        if src_sizes is None and n and total != n * block_size:
+            src_sizes = torch.full((n,), block_size, dtype=torch.int32, device=src.device)
+            src_sizes[-1] = total - (n - 1) * block_size
+    return n, stride, slots, out_sizes, src_sizes
+
+
 def decompress_blocks(comp, offsets, sizes, block_capacity, out=None, out_stride=None, out_sizes=None,
                       workspace=None, stream=None, phases=3):
     """Decode len(sizes) independent blocks.
@@ -49,15 +83,8 @@ def decompress_blocks(comp, offsets, sizes, block_capacity, out=None, out_stride
     n = int(sizes.numel())
     stride = int(out_stride if out_stride is not None else block_capacity)
     st = _stream(stream)
-    with torch.cuda.stream(st):                     # temporaries belong to the stream the kernels run on
-        if out is None:
-            out = torch.empty(n * stride, dtype=torch.uint8, device=comp.device)
-        if out_sizes is None:
-            out_sizes = torch.empty(n, dtype=torch.int32, device=comp.device)
-    ws_bytes = int(lib.LZ4B200_decompress_workspace_bytes_for(n, 0, int(block_capacity)))
-    if workspace is None or workspace.numel() < ws_bytes:
-        workspace = _workspace(comp.device, ws_bytes, st)
-    assert offsets.dtype == torch.int64 and sizes.dtype == torch.int32 and comp.dtype == torch.uint8
+    out, out_sizes, workspace = _decode_outputs(lib, comp, offsets, sizes, n * stride, 0, block_capacity, out, out_sizes,
+                                                workspace, st)
     rc = lib.LZ4B200_decompress_blocks_phased(comp.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), out.data_ptr(),
                                               None, stride, None, int(block_capacity), out_sizes.data_ptr(), n,
                                               workspace.data_ptr(), workspace.numel(), int(phases),
@@ -87,15 +114,8 @@ def decompress_blocks_partial(comp, offsets, sizes, target, out=None, out_stride
         uniform = biggest = int(target)
     stride = int(out_stride if out_stride is not None else max(biggest, 0))
     st = _stream(stream)
-    with torch.cuda.stream(st):
-        if out is None:
-            out = torch.empty(max(n * stride, 1), dtype=torch.uint8, device=comp.device)
-        if out_sizes is None:
-            out_sizes = torch.empty(n, dtype=torch.int32, device=comp.device)
-    ws_bytes = int(lib.LZ4B200_decompress_workspace_bytes_for(n, int(per_block), uniform))
-    if workspace is None or workspace.numel() < ws_bytes:
-        workspace = _workspace(comp.device, ws_bytes, st)
-    assert offsets.dtype == torch.int64 and sizes.dtype == torch.int32 and comp.dtype == torch.uint8
+    out, out_sizes, workspace = _decode_outputs(lib, comp, offsets, sizes, max(n * stride, 1), per_block, uniform, out,
+                                                out_sizes, workspace, st)
     rc = lib.LZ4B200_decompress_blocks_partial(comp.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), out.data_ptr(),
                                                None, stride, target.data_ptr() if per_block else None, uniform,
                                                out_sizes.data_ptr(), n, workspace.data_ptr(), workspace.numel(),
@@ -115,19 +135,10 @@ def compress_blocks(src, block_size, acceleration=1, slots=None, slot_stride=Non
     """
     lib = _lib.load()
     _need_cuda(src, slots)
-    total = int(src.numel())
-    n = (total + block_size - 1) // block_size if total else 0
     cap = int(slot_capacity if slot_capacity is not None else compress_bound(block_size))
-    stride = int(slot_stride if slot_stride is not None else ((cap + 15) // 16) * 16)
     st = _stream(stream)
-    with torch.cuda.stream(st):
-        if slots is None:
-            slots = torch.empty(max(n, 1) * stride, dtype=torch.uint8, device=src.device)
-        if out_sizes is None:
-            out_sizes = torch.empty(max(n, 1), dtype=torch.int32, device=src.device)
-        if src_sizes is None and n and total != n * block_size:
-            src_sizes = torch.full((n,), block_size, dtype=torch.int32, device=src.device)
-            src_sizes[-1] = total - (n - 1) * block_size
+    n, stride, slots, out_sizes, src_sizes = _compress_layout(src, block_size, cap, slots, slot_stride, out_sizes,
+                                                              src_sizes, st)
     if mode not in ("exact", "parallel"):
         raise ValueError("mode must be 'exact' or 'parallel'")
     fn = lib.LZ4B200_compress_blocks if mode == "exact" else lib.LZ4B200_compress_blocks_parallel
@@ -147,20 +158,9 @@ def compress_blocks_hc(src, block_size, level=9, slots=None, slot_stride=None, s
     """
     lib = _lib.load()
     _need_cuda(src, slots)
-    total = int(src.numel())
-    n = (total + block_size - 1) // block_size if total else 0
     cap = int(slot_capacity if slot_capacity is not None else compress_bound(block_size))
-    stride = int(slot_stride if slot_stride is not None else ((cap + 15) // 16) * 16)
-    src_sizes = None
     st = _stream(stream)
-    with torch.cuda.stream(st):
-        if slots is None:
-            slots = torch.empty(max(n, 1) * stride, dtype=torch.uint8, device=src.device)
-        if out_sizes is None:
-            out_sizes = torch.empty(max(n, 1), dtype=torch.int32, device=src.device)
-        if n and total != n * block_size:
-            src_sizes = torch.full((n,), block_size, dtype=torch.int32, device=src.device)
-            src_sizes[-1] = total - (n - 1) * block_size
+    n, stride, slots, out_sizes, src_sizes = _compress_layout(src, block_size, cap, slots, slot_stride, out_sizes, None, st)
     workspace = _workspace(src.device, max(int(lib.LZ4B200_compress_blocks_hc_workspace_bytes(n)), 1), st)
     rc = lib.LZ4B200_compress_blocks_hc(src.data_ptr(), int(block_size),
                                         src_sizes.data_ptr() if src_sizes is not None else None, int(block_size),
@@ -180,21 +180,13 @@ def compress_blocks_dest_size(src, block_size, target, acceleration=1, slots=Non
     """
     lib = _lib.load()
     _need_cuda(src, slots, src_sizes)
-    total = int(src.numel())
-    n = (total + block_size - 1) // block_size if total else 0
     room = max(min(int(target), compress_bound(block_size)), 1)
-    stride = int(slot_stride if slot_stride is not None else ((room + 15) // 16) * 16)
     st = _stream(stream)
-    with torch.cuda.stream(st):
-        if slots is None:
-            slots = torch.empty(max(n, 1) * stride, dtype=torch.uint8, device=src.device)
-        if out_sizes is None:
-            out_sizes = torch.empty(max(n, 1), dtype=torch.int32, device=src.device)
-        if consumed is None:
+    n, stride, slots, out_sizes, src_sizes = _compress_layout(src, block_size, room, slots, slot_stride, out_sizes,
+                                                              src_sizes, st)
+    if consumed is None:
+        with torch.cuda.stream(st):
             consumed = torch.empty(max(n, 1), dtype=torch.int32, device=src.device)
-        if src_sizes is None and n and total != n * block_size:
-            src_sizes = torch.full((n,), block_size, dtype=torch.int32, device=src.device)
-            src_sizes[-1] = total - (n - 1) * block_size
     rc = lib.LZ4B200_compress_blocks_destSize(src.data_ptr(), int(block_size),
                                               src_sizes.data_ptr() if src_sizes is not None else None, int(block_size),
                                               slots.data_ptr(), stride, int(target), int(acceleration),

@@ -92,22 +92,21 @@ int LZ4B200_device_count(void)
 
 #define N_PIPE 4   /* chunks in flight for the host-buffer batch calls */
 
-typedef struct {
-    int ready;
-    cudaStream_t stream[N_PIPE];
-    /* growable device buffers, one set per pipeline slot */
-    void* d_in[N_PIPE];   size_t in_cap[N_PIPE];
-    void* d_out[N_PIPE];  size_t out_cap[N_PIPE];
-    void* d_meta[N_PIPE]; size_t meta_cap[N_PIPE];
-    void* d_ws[N_PIPE];   size_t ws_cap[N_PIPE];
-    void* d_pack[N_PIPE]; size_t pack_cap[N_PIPE];   /* frame bodies assembled on the device */
-    /* pinned host staging for the per-block tables, so that every copy of a chunk is truly
-     * asynchronous (a pageable cudaMemcpyAsync blocks the host and serialises the pipeline) */
-    void* h_meta[N_PIPE]; size_t hmeta_cap[N_PIPE];
-    int32_t* pend_dst[N_PIPE]; int64_t pend_cnt[N_PIPE];   /* return values still to be handed to the caller */
-} host_ctx;
+typedef struct { void* p; size_t cap; } buf_t;   /* a growable buffer */
 
-static host_ctx g_ctx;
+/* One pipeline slot: the stream a chunk runs on, the chunk's buffers, and the return values it still owes the caller. */
+typedef struct {
+    cudaStream_t stream;
+    buf_t in, out, ws, pack;   /* device: input, output, decode workspace, frame bodies assembled on the device */
+    /* the chunk's per-block tables on the device and their pinned host staging, so that every copy of a chunk is truly
+     * asynchronous (a pageable cudaMemcpyAsync blocks the host and serialises the pipeline) */
+    buf_t d_tab, h_tab;
+    const int32_t* pend_ret;   /* pinned return values still to be handed over: pend_cnt of them to pend_dst */
+    int32_t* pend_dst;
+    int64_t pend_cnt;
+} slot_t;
+
+static struct { int ready; slot_t slot[N_PIPE]; } g_ctx;
 
 static int ctx_init(void)
 {
@@ -117,44 +116,84 @@ static int ctx_init(void)
         snprintf(g_cuda_error, sizeof(g_cuda_error), "no CUDA device: liblz4_b200 has no CPU fallback");
         return LZ4B200_ERR_CUDA;
     }
-    for (i = 0; i < N_PIPE; i++) CU(cudaStreamCreateWithFlags(&g_ctx.stream[i], cudaStreamNonBlocking));
+    for (i = 0; i < N_PIPE; i++) CU(cudaStreamCreateWithFlags(&g_ctx.slot[i].stream, cudaStreamNonBlocking));
     g_ctx.ready = 1;
 done:
     return rc;
 }
 
-static int grow_pinned(void** p, size_t* cap, size_t need)
+/* grow b to at least need bytes: device memory to the next 1 MiB above need, pinned host memory to a multiple of 64 KiB */
+static int reserve(buf_t* b, size_t need, int pinned)
 {
     int rc = LZ4B200_OK;
-    if (need <= *cap) return rc;
-    if (*p) { CU(cudaFreeHost(*p)); *p = NULL; *cap = 0; }
-    need = (need + 65535) & ~(size_t)65535;
-    CU(cudaHostAlloc(p, need, cudaHostAllocDefault));
-    *cap = need;
+    if (need <= b->cap) return rc;
+    if (b->p && pinned) CU(cudaFreeHost(b->p));
+    if (b->p && !pinned) CU(cudaFree(b->p));
+    b->p = NULL; b->cap = 0;
+    if (pinned) {
+        need = (need + 65535) & ~(size_t)65535;
+        CU(cudaHostAlloc(&b->p, need, cudaHostAllocDefault));
+    } else {
+        need = (need + (size_t)(1 << 20)) & ~(size_t)((1 << 20) - 1);
+        CU(cudaMalloc(&b->p, need));
+    }
+    b->cap = need;
 done:
     return rc;
 }
 
-/* hand the return values of the chunk that last used `slot` to the caller (its stream is idle) */
-static void flush_slot(int slot)
+/* Wait for the chunk that last used slot s, then hand its return values to the caller. */
+static int slot_wait(slot_t* s)
 {
-    if (g_ctx.pend_dst[slot]) {
-        const int64_t cnt = g_ctx.pend_cnt[slot];
-        const int32_t* h_ret = (const int32_t*)((char*)g_ctx.h_meta[slot] + (size_t)cnt * (sizeof(int64_t) + sizeof(int32_t)));
-        memcpy(g_ctx.pend_dst[slot], h_ret, (size_t)cnt * sizeof(int32_t));
-        g_ctx.pend_dst[slot] = NULL;
-    }
+    cudaError_t e = cudaStreamSynchronize(s->stream);
+    if (e == cudaSuccess && s->pend_dst) memcpy(s->pend_dst, s->pend_ret, (size_t)s->pend_cnt * sizeof(int32_t));
+    s->pend_dst = NULL;
+    return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "cudaStreamSynchronize");
 }
 
-static int grow(void** p, size_t* cap, size_t need)
+/* Make slot s ready for the next chunk: wait for the last one, then grow the buffers to the chunk's sizes (0: a buffer the
+ * chunk does not use).  The input, output and body buffers keep 16 bytes of slack, as the kernels read and write whole
+ * 16-byte granules at the ends of a block; the host table has the device table's size. */
+static int slot_take(slot_t* s, size_t inBytes, size_t outBytes, size_t wsBytes, size_t packBytes, size_t tabBytes)
+{
+    int rc = slot_wait(s);
+    if (rc == LZ4B200_OK) rc = reserve(&s->in, inBytes + 16, 0);
+    if (rc == LZ4B200_OK) rc = reserve(&s->out, outBytes + 16, 0);
+    if (rc == LZ4B200_OK && wsBytes) rc = reserve(&s->ws, wsBytes, 0);
+    if (rc == LZ4B200_OK && packBytes) rc = reserve(&s->pack, packBytes + 16, 0);
+    if (rc == LZ4B200_OK) rc = reserve(&s->d_tab, tabBytes, 0);
+    if (rc == LZ4B200_OK) rc = reserve(&s->h_tab, tabBytes, 1);
+    return rc;
+}
+
+/* Queue the copy of a chunk's cnt return values from d_ret to h_ret (both in the slot's tables); the next slot_wait of s
+ * hands them to dst. */
+static int slot_return(slot_t* s, int32_t* h_ret, const int32_t* d_ret, int32_t* dst, int64_t cnt)
 {
     int rc = LZ4B200_OK;
-    if (need <= *cap) return rc;
-    if (*p) { CU(cudaFree(*p)); *p = NULL; *cap = 0; }
-    need = (need + (size_t)(1 << 20)) & ~(size_t)((1 << 20) - 1);
-    CU(cudaMalloc(p, need));
-    *cap = need;
+    CU(cudaMemcpyAsync(h_ret, d_ret, (size_t)cnt * sizeof(int32_t), cudaMemcpyDeviceToHost, s->stream));
+    s->pend_ret = h_ret; s->pend_dst = dst; s->pend_cnt = cnt;
 done:
+    return rc;
+}
+
+/* Every host-pointer call that runs on the device is bracketed by host_begin and host_end: one call at a time owns the
+ * slots.  host_end(LZ4B200_OK) waits for every slot and hands over its results; host_end(error) drains every stream,
+ * drops what the slots still owe and keeps that first error.  Both unlock. */
+static int host_begin(void)
+{
+    pthread_mutex_lock(&g_lock);
+    return ctx_init();
+}
+
+static int host_end(int rc)
+{
+    int i;
+    for (i = 0; i < N_PIPE && g_ctx.ready; i++) {
+        if (rc == LZ4B200_OK) rc = slot_wait(&g_ctx.slot[i]);
+        else { cudaStreamSynchronize(g_ctx.slot[i].stream); g_ctx.slot[i].pend_dst = NULL; }
+    }
+    pthread_mutex_unlock(&g_lock);
     return rc;
 }
 
@@ -167,13 +206,18 @@ size_t LZ4B200_decompress_workspace_bytes_for(int64_t nBlocks, int perBlockCaps,
     return lz4k_decode_workspace_bytes(nBlocks, perBlockCaps, dstCap, SIZE_MAX);
 }
 
+/* a launcher's result: LZ4B200_OK, or LZ4B200_ERR_CUDA with the error recorded under `where` */
+static int launched(int e, const char* where)
+{
+    return e == cudaSuccess ? LZ4B200_OK : cuda_fail((cudaError_t)e, where);
+}
+
 /* the device decode calls (partial: LZ4_decompress_safe_partial, d_dstCap / dstCap hold the targets) */
 static int decode_call(int partial, const void* d_src, const int64_t* d_srcOff, const int32_t* d_srcSize, void* d_dst,
                        const int64_t* d_dstOff, int64_t dstStride, const int32_t* d_dstCap, int32_t dstCap, int32_t* d_outSize,
                        int64_t nBlocks, void* d_workspace, size_t workspaceBytes, int phases, void* stream)
 {
     lz4k_decode_args a;
-    cudaError_t e;
     if (nBlocks < 0) return LZ4B200_ERR_ARG;
     if (nBlocks == 0) return LZ4B200_OK;
     if (!d_src || !d_srcOff || !d_srcSize || !d_dst || !d_outSize || !d_workspace) return LZ4B200_ERR_ARG;
@@ -183,8 +227,7 @@ static int decode_call(int partial, const void* d_src, const int64_t* d_srcOff, 
     a.dst = (uint8_t*)d_dst; a.dstOff = d_dstOff; a.dstStride = dstStride;
     a.dstCapArr = d_dstCap; a.dstCap = dstCap; a.outSize = d_outSize; a.nBlocks = nBlocks;
     a.workspace = d_workspace; a.workspaceBytes = workspaceBytes;
-    e = (cudaError_t)lz4k_launch_decode(&a, phases, partial, stream);
-    return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_decode");
+    return launched(lz4k_launch_decode(&a, phases, partial, stream), "lz4k_launch_decode");
 }
 
 int LZ4B200_decompress_blocks_phased(const void* d_src, const int64_t* d_srcOff, const int32_t* d_srcSize,
@@ -217,20 +260,28 @@ int LZ4B200_decompress_blocks_partial(const void* d_src, const int64_t* d_srcOff
                        nBlocks, d_workspace, workspaceBytes, 3, stream);
 }
 
+/* the encode launch arguments, every block size included (a split launch narrows minSize .. maxSize) */
+static lz4k_encode_args encode_args(const void* d_src, int64_t srcStride, const int32_t* d_srcSize, int32_t srcSize,
+                                    void* d_dst, int64_t dstStride, int32_t dstCap, int acceleration,
+                                    int32_t* d_outSize, int64_t nBlocks)
+{
+    lz4k_encode_args a;
+    a.src = (const uint8_t*)d_src; a.srcStride = srcStride; a.srcSizeArr = d_srcSize; a.srcSize = srcSize;
+    a.dst = (uint8_t*)d_dst; a.dstStride = dstStride; a.dstCap = dstCap; a.acceleration = acceleration;
+    a.outSize = d_outSize; a.nBlocks = nBlocks; a.minSize = INT32_MIN; a.maxSize = INT32_MAX;
+    return a;
+}
+
 int LZ4B200_compress_blocks(const void* d_src, int64_t srcStride, const int32_t* d_srcSize, int32_t srcSize,
                             void* d_dst, int64_t dstStride, int32_t dstCap, int acceleration,
                             int32_t* d_outSize, int64_t nBlocks, void* stream)
 {
     lz4k_encode_args a;
-    cudaError_t e;
     if (nBlocks < 0) return LZ4B200_ERR_ARG;
     if (nBlocks == 0) return LZ4B200_OK;
     if (!d_dst || !d_outSize) return LZ4B200_ERR_ARG;
-    a.src = (const uint8_t*)d_src; a.srcStride = srcStride; a.srcSizeArr = d_srcSize; a.srcSize = srcSize;
-    a.dst = (uint8_t*)d_dst; a.dstStride = dstStride; a.dstCap = dstCap; a.acceleration = acceleration;
-    a.outSize = d_outSize; a.nBlocks = nBlocks; a.minSize = INT32_MIN; a.maxSize = INT32_MAX;
-    e = (cudaError_t)lz4k_launch_encode(&a, stream);
-    return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_encode");
+    a = encode_args(d_src, srcStride, d_srcSize, srcSize, d_dst, dstStride, dstCap, acceleration, d_outSize, nBlocks);
+    return launched(lz4k_launch_encode(&a, stream), "lz4k_launch_encode");
 }
 
 size_t LZ4B200_compress_blocks_hc_workspace_bytes(int64_t nBlocks)
@@ -244,16 +295,12 @@ int LZ4B200_compress_blocks_hc(const void* d_src, int64_t srcStride, const int32
                                void* d_workspace, size_t workspaceBytes, void* stream)
 {
     lz4k_encode_args a;
-    cudaError_t e;
     if (compressionLevel >= 10) return LZ4B200_ERR_ARG;     /* the optimal parser (lz4hc.c:1823-) is not built */
     if (nBlocks < 0 || !d_dst || !d_outSize || !d_workspace) return LZ4B200_ERR_ARG;
     if (nBlocks == 0) return LZ4B200_OK;
     if (!d_src || workspaceBytes < lz4k_encode_hc_workspace_bytes(nBlocks)) return LZ4B200_ERR_ARG;
-    a.src = (const uint8_t*)d_src; a.srcStride = srcStride; a.srcSizeArr = d_srcSize; a.srcSize = srcSize;
-    a.dst = (uint8_t*)d_dst; a.dstStride = dstStride; a.dstCap = dstCap; a.acceleration = 0;
-    a.outSize = d_outSize; a.nBlocks = nBlocks; a.minSize = INT32_MIN; a.maxSize = INT32_MAX;
-    e = (cudaError_t)lz4k_launch_encode_hc(&a, compressionLevel, d_workspace, workspaceBytes, stream);
-    return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_encode_hc");
+    a = encode_args(d_src, srcStride, d_srcSize, srcSize, d_dst, dstStride, dstCap, 0, d_outSize, nBlocks);
+    return launched(lz4k_launch_encode_hc(&a, compressionLevel, d_workspace, workspaceBytes, stream), "lz4k_launch_encode_hc");
 }
 
 int LZ4B200_compress_blocks_destSize(const void* d_src, int64_t srcStride, const int32_t* d_srcSize, int32_t srcSize,
@@ -261,15 +308,11 @@ int LZ4B200_compress_blocks_destSize(const void* d_src, int64_t srcStride, const
                                      int32_t* d_outSize, int32_t* d_srcConsumed, int64_t nBlocks, void* stream)
 {
     lz4k_encode_args a;
-    cudaError_t e;
     if (nBlocks < 0 || !d_dst || !d_outSize || !d_srcConsumed) return LZ4B200_ERR_ARG;
     if (nBlocks == 0) return LZ4B200_OK;
     if (!d_src) return LZ4B200_ERR_ARG;
-    a.src = (const uint8_t*)d_src; a.srcStride = srcStride; a.srcSizeArr = d_srcSize; a.srcSize = srcSize;
-    a.dst = (uint8_t*)d_dst; a.dstStride = dstStride; a.dstCap = targetDstSize; a.acceleration = acceleration;
-    a.outSize = d_outSize; a.nBlocks = nBlocks; a.minSize = INT32_MIN; a.maxSize = INT32_MAX;
-    e = (cudaError_t)lz4k_launch_encode_dest(&a, d_srcConsumed, stream);
-    return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_encode_dest");
+    a = encode_args(d_src, srcStride, d_srcSize, srcSize, d_dst, dstStride, targetDstSize, acceleration, d_outSize, nBlocks);
+    return launched(lz4k_launch_encode_dest(&a, d_srcConsumed, stream), "lz4k_launch_encode_dest");
 }
 
 int LZ4B200_compress_blocks_parallel(const void* d_src, int64_t srcStride, const int32_t* d_srcSize, int32_t srcSize,
@@ -277,47 +320,38 @@ int LZ4B200_compress_blocks_parallel(const void* d_src, int64_t srcStride, const
                                      int32_t* d_outSize, int64_t nBlocks, void* stream)
 {
     lz4k_encode_args a;
-    cudaError_t e;
+    int rc;
     if (nBlocks < 0) return LZ4B200_ERR_ARG;
     if (nBlocks == 0) return LZ4B200_OK;
     if (!d_dst || !d_outSize) return LZ4B200_ERR_ARG;
-    a.src = (const uint8_t*)d_src; a.srcStride = srcStride; a.srcSizeArr = d_srcSize; a.srcSize = srcSize;
-    a.dst = (uint8_t*)d_dst; a.dstStride = dstStride; a.dstCap = dstCap; a.acceleration = acceleration;
-    a.outSize = d_outSize; a.nBlocks = nBlocks; a.minSize = INT32_MIN; a.maxSize = INT32_MAX;
+    a = encode_args(d_src, srcStride, d_srcSize, srcSize, d_dst, dstStride, dstCap, acceleration, d_outSize, nBlocks);
     /* the parallel parse stages a whole block in shared memory: blocks above 64 KB take the byte-identical encoder.  With
      * per-block sizes each block goes by its own size (srcSize is not used): both kernels run, each on its blocks. */
-    if (!d_srcSize) {
-        e = (cudaError_t)(srcSize <= 65536 ? lz4k_launch_encode_par(&a, stream) : lz4k_launch_encode(&a, stream));
-        return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_encode_par");
-    }
+    if (!d_srcSize && srcSize <= 65536) return launched(lz4k_launch_encode_par(&a, stream), "lz4k_launch_encode_par");
+    if (!d_srcSize) return launched(lz4k_launch_encode(&a, stream), "lz4k_launch_encode");
     a.maxSize = 65536;
-    e = (cudaError_t)lz4k_launch_encode_par(&a, stream);
-    if (e != cudaSuccess) return cuda_fail(e, "lz4k_launch_encode_par");
+    if ((rc = launched(lz4k_launch_encode_par(&a, stream), "lz4k_launch_encode_par")) != LZ4B200_OK) return rc;
     a.minSize = 65537; a.maxSize = INT32_MAX;
-    e = (cudaError_t)lz4k_launch_encode(&a, stream);
-    return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_encode");
+    return launched(lz4k_launch_encode(&a, stream), "lz4k_launch_encode");
 }
 
 int LZ4B200_pack_blocks(const void* d_slots, int64_t slotStride, const int32_t* d_sizes, int64_t nBlocks,
                         void* d_packed, int64_t* d_outOff, int headerBytes, void* stream)
 {
-    cudaError_t e;
     if (nBlocks < 0 || !d_outOff || (headerBytes != 0 && headerBytes != 4)) return LZ4B200_ERR_ARG;
     if (nBlocks > 0 && (!d_slots || !d_sizes || !d_packed)) return LZ4B200_ERR_ARG;
-    e = (cudaError_t)lz4k_launch_pack((const uint8_t*)d_slots, slotStride, d_sizes, nBlocks, (uint8_t*)d_packed,
-                                      d_outOff, headerBytes, stream);
-    return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_pack");
+    return launched(lz4k_launch_pack((const uint8_t*)d_slots, slotStride, d_sizes, nBlocks, (uint8_t*)d_packed, d_outOff,
+                                     headerBytes, stream), "lz4k_launch_pack");
 }
 
 int LZ4B200_pack_frame_blocks(const void* d_slots, int64_t slotStride, const int32_t* d_sizes, const void* d_src, int64_t srcStride,
                               int32_t blockSize, int32_t lastSize, int64_t nBlocks, void* d_body, int64_t* d_outOff, void* stream)
 {
-    cudaError_t e;
     if (nBlocks < 0 || !d_outOff || blockSize <= 0 || lastSize < 0 || lastSize > blockSize) return LZ4B200_ERR_ARG;
     if (nBlocks > 0 && (!d_slots || !d_sizes || !d_src || !d_body)) return LZ4B200_ERR_ARG;
-    e = (cudaError_t)lz4k_launch_pack_frame((const uint8_t*)d_slots, slotStride, d_sizes, (const uint8_t*)d_src, srcStride,
-                                            blockSize, lastSize, nBlocks, (uint8_t*)d_body, d_outOff, stream);
-    return e == cudaSuccess ? LZ4B200_OK : cuda_fail(e, "lz4k_launch_pack_frame");
+    return launched(lz4k_launch_pack_frame((const uint8_t*)d_slots, slotStride, d_sizes, (const uint8_t*)d_src, srcStride,
+                                           blockSize, lastSize, nBlocks, (uint8_t*)d_body, d_outOff, stream),
+                    "lz4k_launch_pack_frame");
 }
 
 /* ------------------------------------------------------------------------------------------ */
@@ -342,127 +376,88 @@ int LZ4B200_decompress_blocks_host(const void* h_src, const int64_t* h_srcOff, c
                                    void* h_dst, int64_t dstStride, int32_t dstCap,
                                    int32_t* h_outSize, int64_t nBlocks)
 {
-    int rc = LZ4B200_OK;
+    int rc;
     int64_t perChunk, first;
-    int slot = 0, i;
+    int slot = 0;
     if (nBlocks < 0 || dstCap < 0 || dstStride < dstCap) return LZ4B200_ERR_ARG;
     if (nBlocks == 0) return LZ4B200_OK;
     if (!h_src || !h_srcOff || !h_srcSize || !h_dst || !h_outSize) return LZ4B200_ERR_ARG;
-    pthread_mutex_lock(&g_lock);
-    if ((rc = ctx_init()) != LZ4B200_OK) goto done;
+    if ((rc = host_begin()) != LZ4B200_OK) goto done;
 
     perChunk = CHUNK_OUT_BYTES / (dstStride > 0 ? dstStride : 1);
     if (perChunk < 1) perChunk = 1;
     for (first = 0; first < nBlocks; first += perChunk, slot = (slot + 1) % N_PIPE) {
         const int64_t cnt = (nBlocks - first < perChunk) ? nBlocks - first : perChunk;
-        cudaStream_t st = g_ctx.stream[slot];
+        slot_t* s = &g_ctx.slot[slot];
         int64_t lo = h_srcOff[first], hi = lo, k;
-        size_t inBytes, outBytes = (size_t)(cnt * dstStride), metaBytes, wsBytes;
+        int64_t *h_off, *d_off;
+        int32_t *h_size, *d_size;
         /* the chunk's compressed bytes span [lo, hi) of h_src (blocks may be in any order) */
         for (k = first; k < first + cnt; k++) {
             if (h_srcSize[k] < 0) { rc = LZ4B200_ERR_ARG; goto done; }
             if (h_srcOff[k] < lo) lo = h_srcOff[k];
             if (h_srcOff[k] + h_srcSize[k] > hi) hi = h_srcOff[k] + h_srcSize[k];
         }
-        inBytes = (size_t)(hi - lo);
-        metaBytes = (size_t)cnt * (sizeof(int64_t) + 2 * sizeof(int32_t));
-        wsBytes = LZ4B200_decompress_workspace_bytes_for(cnt, 0, dstCap);
-        CU(cudaStreamSynchronize(st));                      /* slot reuse: previous chunk on it is finished */
-        flush_slot(slot);
-        if ((rc = grow(&g_ctx.d_in[slot], &g_ctx.in_cap[slot], inBytes + 16)) != LZ4B200_OK) goto done;
-        if ((rc = grow(&g_ctx.d_out[slot], &g_ctx.out_cap[slot], outBytes + 16)) != LZ4B200_OK) goto done;
-        if ((rc = grow(&g_ctx.d_meta[slot], &g_ctx.meta_cap[slot], metaBytes + 16)) != LZ4B200_OK) goto done;
-        if ((rc = grow(&g_ctx.d_ws[slot], &g_ctx.ws_cap[slot], wsBytes)) != LZ4B200_OK) goto done;
-        if ((rc = grow_pinned(&g_ctx.h_meta[slot], &g_ctx.hmeta_cap[slot], metaBytes + 16)) != LZ4B200_OK) goto done;
-        {
-            int64_t* d_off = (int64_t*)g_ctx.d_meta[slot];
-            int32_t* d_size = (int32_t*)(d_off + cnt);
-            int32_t* d_ret = d_size + cnt;
-            int64_t* h_off = (int64_t*)g_ctx.h_meta[slot];          /* pinned: [offsets | sizes | return values] */
-            int32_t* h_size = (int32_t*)(h_off + cnt);
-            int32_t* h_ret = h_size + cnt;
-            for (k = 0; k < cnt; k++) h_off[k] = h_srcOff[first + k] - lo;   /* relative to the chunk's first byte */
-            memcpy(h_size, h_srcSize + first, (size_t)cnt * sizeof(int32_t));
-            CU(cudaMemcpyAsync(d_off, h_off, (size_t)cnt * (sizeof(int64_t) + sizeof(int32_t)), cudaMemcpyHostToDevice, st));
-            CU(cudaMemcpyAsync(g_ctx.d_in[slot], (const char*)h_src + lo, inBytes, cudaMemcpyHostToDevice, st));
-            rc = LZ4B200_decompress_blocks(g_ctx.d_in[slot], d_off, d_size, g_ctx.d_out[slot], NULL, dstStride,
-                                           NULL, dstCap, d_ret, cnt, g_ctx.d_ws[slot], g_ctx.ws_cap[slot], st);
-            if (rc != LZ4B200_OK) goto done;
-            CU(cudaMemcpyAsync((char*)h_dst + first * dstStride, g_ctx.d_out[slot], outBytes, cudaMemcpyDeviceToHost, st));
-            CU(cudaMemcpyAsync(h_ret, d_ret, (size_t)cnt * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-            g_ctx.pend_dst[slot] = h_outSize + first;
-            g_ctx.pend_cnt[slot] = cnt;
-        }
+        rc = slot_take(s, (size_t)(hi - lo), (size_t)(cnt * dstStride), LZ4B200_decompress_workspace_bytes_for(cnt, 0, dstCap), 0,
+                       (size_t)cnt * (sizeof(int64_t) + 2 * sizeof(int32_t)));
+        if (rc != LZ4B200_OK) goto done;
+        /* tables: [offsets i64 | sizes i32 | return values i32] */
+        h_off = (int64_t*)s->h_tab.p; h_size = (int32_t*)(h_off + cnt);
+        d_off = (int64_t*)s->d_tab.p; d_size = (int32_t*)(d_off + cnt);
+        for (k = 0; k < cnt; k++) h_off[k] = h_srcOff[first + k] - lo;   /* relative to the chunk's first byte */
+        memcpy(h_size, h_srcSize + first, (size_t)cnt * sizeof(int32_t));
+        CU(cudaMemcpyAsync(d_off, h_off, (size_t)cnt * (sizeof(int64_t) + sizeof(int32_t)), cudaMemcpyHostToDevice, s->stream));
+        CU(cudaMemcpyAsync(s->in.p, (const char*)h_src + lo, (size_t)(hi - lo), cudaMemcpyHostToDevice, s->stream));
+        rc = LZ4B200_decompress_blocks(s->in.p, d_off, d_size, s->out.p, NULL, dstStride, NULL, dstCap, d_size + cnt, cnt,
+                                       s->ws.p, s->ws.cap, s->stream);
+        if (rc != LZ4B200_OK) goto done;
+        CU(cudaMemcpyAsync((char*)h_dst + first * dstStride, s->out.p, (size_t)(cnt * dstStride), cudaMemcpyDeviceToHost, s->stream));
+        if ((rc = slot_return(s, h_size + cnt, d_size + cnt, h_outSize + first, cnt)) != LZ4B200_OK) goto done;
     }
-    for (i = 0; i < N_PIPE; i++) { CU(cudaStreamSynchronize(g_ctx.stream[i])); flush_slot(i); }
-    goto unlock;
 done:
-    for (i = 0; i < N_PIPE; i++) { cudaStreamSynchronize(g_ctx.stream[i]); g_ctx.pend_dst[i] = NULL; }
-unlock:
-    pthread_mutex_unlock(&g_lock);
-    return rc;
+    return host_end(rc);
 }
 
 int LZ4B200_compress_blocks_host(const void* h_src, int64_t srcStride, int32_t srcSize, int64_t lastSize,
                                  void* h_dst, int64_t dstStride, int32_t dstCap, int acceleration,
                                  int32_t* h_outSize, int64_t nBlocks)
 {
-    int rc = LZ4B200_OK;
+    int rc;
     int64_t perChunk, first;
-    int slot = 0, i;
+    int slot = 0;
     if (nBlocks < 0 || srcSize < 0 || lastSize < 0 || lastSize > srcSize || srcStride < srcSize) return LZ4B200_ERR_ARG;
     if (nBlocks == 0) return LZ4B200_OK;
     if (!h_dst || !h_outSize || (!h_src && srcSize > 0)) return LZ4B200_ERR_ARG;
-    pthread_mutex_lock(&g_lock);
-    if ((rc = ctx_init()) != LZ4B200_OK) goto done;
+    if ((rc = host_begin()) != LZ4B200_OK) goto done;
 
     perChunk = CHUNK_OUT_BYTES / (srcStride > 0 ? srcStride : 1);
     if (perChunk < 1) perChunk = 1;
     for (first = 0; first < nBlocks; first += perChunk, slot = (slot + 1) % N_PIPE) {
         const int64_t cnt = (nBlocks - first < perChunk) ? nBlocks - first : perChunk;
         const int isLast = (first + cnt == nBlocks);
-        cudaStream_t st = g_ctx.stream[slot];
-        size_t inBytes = (size_t)((cnt - 1) * srcStride + (isLast ? lastSize : srcSize));
-        size_t slotBytes = (size_t)(cnt * dstStride);
-        /* same table layout as the decode call: [unused i64 | source sizes i32 | return values i32] */
-        size_t metaBytes = (size_t)cnt * (sizeof(int64_t) + 2 * sizeof(int32_t));
-        int32_t *d_sizes, *d_ret, *h_sizes, *h_ret;
+        const int ragged = isLast && lastSize != srcSize;   /* a per-block size table only for the short final block */
+        slot_t* s = &g_ctx.slot[slot];
+        const size_t inBytes = (size_t)((cnt - 1) * srcStride + (isLast ? lastSize : srcSize));
+        int32_t *h_size, *d_size;
         int64_t k;
-        CU(cudaStreamSynchronize(st));
-        flush_slot(slot);
-        if ((rc = grow(&g_ctx.d_in[slot], &g_ctx.in_cap[slot], inBytes + 16)) != LZ4B200_OK) goto done;
-        if ((rc = grow(&g_ctx.d_out[slot], &g_ctx.out_cap[slot], slotBytes + 16)) != LZ4B200_OK) goto done;
-        if ((rc = grow(&g_ctx.d_meta[slot], &g_ctx.meta_cap[slot], metaBytes + 16)) != LZ4B200_OK) goto done;
-        if ((rc = grow_pinned(&g_ctx.h_meta[slot], &g_ctx.hmeta_cap[slot], metaBytes + 16)) != LZ4B200_OK) goto done;
-        d_sizes = (int32_t*)((int64_t*)g_ctx.d_meta[slot] + cnt);
-        d_ret = d_sizes + cnt;
-        h_sizes = (int32_t*)((int64_t*)g_ctx.h_meta[slot] + cnt);
-        h_ret = h_sizes + cnt;
-        if (inBytes) CU(cudaMemcpyAsync(g_ctx.d_in[slot], (const char*)h_src + first * srcStride, inBytes, cudaMemcpyHostToDevice, st));
-        if (isLast && lastSize != srcSize) {
-            /* per-block size table only needed for the ragged final block */
-            for (k = 0; k < cnt; k++) h_sizes[k] = srcSize;
-            h_sizes[cnt - 1] = (int32_t)lastSize;
-            CU(cudaMemcpyAsync(d_sizes, h_sizes, (size_t)cnt * sizeof(int32_t), cudaMemcpyHostToDevice, st));
-            rc = LZ4B200_compress_blocks(g_ctx.d_in[slot], srcStride, d_sizes, srcSize, g_ctx.d_out[slot], dstStride,
-                                         dstCap, acceleration, d_ret, cnt, st);
-        } else {
-            rc = LZ4B200_compress_blocks(g_ctx.d_in[slot], srcStride, NULL, srcSize, g_ctx.d_out[slot], dstStride,
-                                         dstCap, acceleration, d_ret, cnt, st);
-        }
+        rc = slot_take(s, inBytes, (size_t)(cnt * dstStride), 0, 0, (size_t)cnt * 2 * sizeof(int32_t));
         if (rc != LZ4B200_OK) goto done;
-        CU(cudaMemcpyAsync((char*)h_dst + first * dstStride, g_ctx.d_out[slot], slotBytes, cudaMemcpyDeviceToHost, st));
-        CU(cudaMemcpyAsync(h_ret, d_ret, (size_t)cnt * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-        g_ctx.pend_dst[slot] = h_outSize + first;
-        g_ctx.pend_cnt[slot] = cnt;
+        h_size = (int32_t*)s->h_tab.p;                       /* tables: [source sizes i32 | return values i32] */
+        d_size = (int32_t*)s->d_tab.p;
+        if (inBytes) CU(cudaMemcpyAsync(s->in.p, (const char*)h_src + first * srcStride, inBytes, cudaMemcpyHostToDevice, s->stream));
+        if (ragged) {
+            for (k = 0; k < cnt; k++) h_size[k] = srcSize;
+            h_size[cnt - 1] = (int32_t)lastSize;
+            CU(cudaMemcpyAsync(d_size, h_size, (size_t)cnt * sizeof(int32_t), cudaMemcpyHostToDevice, s->stream));
+        }
+        rc = LZ4B200_compress_blocks(s->in.p, srcStride, ragged ? d_size : NULL, srcSize, s->out.p, dstStride, dstCap,
+                                     acceleration, d_size + cnt, cnt, s->stream);
+        if (rc != LZ4B200_OK) goto done;
+        CU(cudaMemcpyAsync((char*)h_dst + first * dstStride, s->out.p, (size_t)(cnt * dstStride), cudaMemcpyDeviceToHost, s->stream));
+        if ((rc = slot_return(s, h_size + cnt, d_size + cnt, h_outSize + first, cnt)) != LZ4B200_OK) goto done;
     }
-    for (i = 0; i < N_PIPE; i++) { CU(cudaStreamSynchronize(g_ctx.stream[i])); flush_slot(i); }
-    goto unlock;
 done:
-    for (i = 0; i < N_PIPE; i++) { cudaStreamSynchronize(g_ctx.stream[i]); g_ctx.pend_dst[i] = NULL; }
-unlock:
-    pthread_mutex_unlock(&g_lock);
-    return rc;
+    return host_end(rc);
 }
 
 /* ------------------------------------------------------------------------------------------ */
@@ -473,47 +468,35 @@ unlock:
  * writes it (the fill route, lz4.c:1332 and :1369), and is left alone on the compress_fast route (lz4.c:1486-1487). */
 static int one_block_compress(const char* src, char* dst, int srcSize, int dstCapacity, int acceleration, int* srcSizePtr)
 {
-    int rc = LZ4B200_OK, ret = 0;
+    int rc, bound;
     int32_t res[2] = {0, 0};                 /* return value, consumed input */
-    int32_t* d_ret;
-    cudaStream_t st;
-    size_t capBytes;
+    slot_t* s = &g_ctx.slot[0];
+    int32_t* d_res;
     /* argument rules of LZ4_compress_generic, lz4.c:1360-1372, decided on the host so that a bad
      * size never reaches the device */
     if ((unsigned)srcSize > (unsigned)LZ4B200_MAX_INPUT_SIZE) return 0;
     if (dstCapacity <= 0) return 0;          /* nothing can be written (lz4.c:1362, :985 and the limited checks) */
     if (dst == NULL) return 0;
     if (srcSize > 0 && src == NULL) return 0;
-    pthread_mutex_lock(&g_lock);
-    if ((rc = ctx_init()) != LZ4B200_OK) goto done;
-    st = g_ctx.stream[0];
-    {
-        int bound = LZ4_compressBound(srcSize);
-        capBytes = (size_t)(dstCapacity < bound ? dstCapacity : bound);
-    }
-    if ((rc = grow(&g_ctx.d_in[0], &g_ctx.in_cap[0], (size_t)srcSize + 16)) != LZ4B200_OK) goto done;
-    if ((rc = grow(&g_ctx.d_out[0], &g_ctx.out_cap[0], capBytes + 16)) != LZ4B200_OK) goto done;
-    if ((rc = grow(&g_ctx.d_meta[0], &g_ctx.meta_cap[0], 64)) != LZ4B200_OK) goto done;
-    d_ret = (int32_t*)g_ctx.d_meta[0];
-    /* copy-in completes before any output is produced: in-place calls (lz4.h:619-678) are safe */
-    if (srcSize) CU(cudaMemcpyAsync(g_ctx.d_in[0], src, (size_t)srcSize, cudaMemcpyHostToDevice, st));
-    if (srcSizePtr)
-        rc = LZ4B200_compress_blocks_destSize(g_ctx.d_in[0], 0, NULL, srcSize, g_ctx.d_out[0], 0, dstCapacity, acceleration,
-                                              d_ret, d_ret + 1, 1, st);
-    else
-        rc = LZ4B200_compress_blocks(g_ctx.d_in[0], 0, NULL, srcSize, g_ctx.d_out[0], 0, dstCapacity, acceleration, d_ret, 1, st);
+    bound = LZ4_compressBound(srcSize);
+    if ((rc = host_begin()) != LZ4B200_OK) goto done;
+    rc = slot_take(s, (size_t)srcSize, (size_t)(dstCapacity < bound ? dstCapacity : bound), 0, 0, sizeof(res));
     if (rc != LZ4B200_OK) goto done;
-    CU(cudaMemcpyAsync(res, d_ret, (srcSizePtr ? 2 : 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    ret = res[0];
-    if (ret > 0) {
-        CU(cudaMemcpyAsync(dst, g_ctx.d_out[0], (size_t)ret, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
-        if (srcSizePtr && dstCapacity < LZ4_compressBound(srcSize)) *srcSizePtr = res[1];
-    }
+    d_res = (int32_t*)s->d_tab.p;
+    /* copy-in completes before any output is produced: in-place calls (lz4.h:619-678) are safe */
+    if (srcSize) CU(cudaMemcpyAsync(s->in.p, src, (size_t)srcSize, cudaMemcpyHostToDevice, s->stream));
+    if (srcSizePtr)
+        rc = LZ4B200_compress_blocks_destSize(s->in.p, 0, NULL, srcSize, s->out.p, 0, dstCapacity, acceleration,
+                                              d_res, d_res + 1, 1, s->stream);
+    else
+        rc = LZ4B200_compress_blocks(s->in.p, 0, NULL, srcSize, s->out.p, 0, dstCapacity, acceleration, d_res, 1, s->stream);
+    if (rc == LZ4B200_OK) rc = slot_return(s, (int32_t*)s->h_tab.p, d_res, res, srcSizePtr ? 2 : 1);
+    if (rc == LZ4B200_OK) rc = slot_wait(s);
+    if (rc == LZ4B200_OK && res[0] > 0) CU(cudaMemcpyAsync(dst, s->out.p, (size_t)res[0], cudaMemcpyDeviceToHost, s->stream));
 done:
-    pthread_mutex_unlock(&g_lock);
-    return rc == LZ4B200_OK ? ret : 0;
+    if (host_end(rc) != LZ4B200_OK) return 0;
+    if (srcSizePtr && res[0] > 0 && dstCapacity < bound) *srcSizePtr = res[1];
+    return res[0];
 }
 
 int LZ4_compress_fast(const char* src, char* dst, int srcSize, int dstCapacity, int acceleration)
@@ -561,41 +544,34 @@ int LZ4_compress_destSize_extState(void* state, const char* src, char* dst, int*
  * Only the returned bytes are copied back: dst is untouched for a rejected block. */
 static int one_block_decompress(const char* src, char* dst, int compressedSize, int dstCapacity, int partial)
 {
-    int rc = LZ4B200_OK, ret = -1;
-    cudaStream_t st;
-    int64_t* d_off; int32_t* d_size; int32_t* d_ret;
-    int64_t zero = 0;
-    pthread_mutex_lock(&g_lock);
-    if ((rc = ctx_init()) != LZ4B200_OK) goto done;
-    st = g_ctx.stream[0];
-    if ((rc = grow(&g_ctx.d_in[0], &g_ctx.in_cap[0], (size_t)compressedSize + 16)) != LZ4B200_OK) goto done;
-    if ((rc = grow(&g_ctx.d_out[0], &g_ctx.out_cap[0], (size_t)dstCapacity + 16)) != LZ4B200_OK) goto done;
-    if ((rc = grow(&g_ctx.d_meta[0], &g_ctx.meta_cap[0], 64)) != LZ4B200_OK) goto done;
-    if ((rc = grow(&g_ctx.d_ws[0], &g_ctx.ws_cap[0], LZ4B200_decompress_workspace_bytes_for(1, 0, dstCapacity))) != LZ4B200_OK) goto done;
-    d_off = (int64_t*)g_ctx.d_meta[0];
-    d_size = (int32_t*)(d_off + 1);
-    d_ret = d_size + 1;
-    CU(cudaMemcpyAsync(d_off, &zero, sizeof(zero), cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(d_size, &compressedSize, sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    int rc, ret = -1;
+    slot_t* s = &g_ctx.slot[0];
+    int64_t *h_off, *d_off;
+    int32_t *h_size, *d_size;
+    if ((rc = host_begin()) != LZ4B200_OK) goto done;
+    rc = slot_take(s, (size_t)compressedSize, (size_t)dstCapacity, LZ4B200_decompress_workspace_bytes_for(1, 0, dstCapacity), 0,
+                   sizeof(int64_t) + 2 * sizeof(int32_t));
+    if (rc != LZ4B200_OK) goto done;
+    /* tables: [offset i64 | size i32 | return value i32], as in LZ4B200_decompress_blocks_host */
+    h_off = (int64_t*)s->h_tab.p; h_size = (int32_t*)(h_off + 1);
+    d_off = (int64_t*)s->d_tab.p; d_size = (int32_t*)(d_off + 1);
+    *h_off = 0;
+    *h_size = compressedSize;
+    CU(cudaMemcpyAsync(d_off, h_off, sizeof(int64_t) + sizeof(int32_t), cudaMemcpyHostToDevice, s->stream));
     /* the whole input is on the device before the first output byte is written back: in-place
      * decompression (lz4.h:619-678, tests/fuzzer.c:1177-1187) needs no special handling */
-    CU(cudaMemcpyAsync(g_ctx.d_in[0], src, (size_t)compressedSize, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(s->in.p, src, (size_t)compressedSize, cudaMemcpyHostToDevice, s->stream));
     if (partial)
-        rc = LZ4B200_decompress_blocks_partial(g_ctx.d_in[0], d_off, d_size, g_ctx.d_out[0], NULL, 0, NULL, dstCapacity,
-                                               d_ret, 1, g_ctx.d_ws[0], g_ctx.ws_cap[0], st);
+        rc = LZ4B200_decompress_blocks_partial(s->in.p, d_off, d_size, s->out.p, NULL, 0, NULL, dstCapacity,
+                                               d_size + 1, 1, s->ws.p, s->ws.cap, s->stream);
     else
-        rc = LZ4B200_decompress_blocks(g_ctx.d_in[0], d_off, d_size, g_ctx.d_out[0], NULL, 0, NULL, dstCapacity,
-                                       d_ret, 1, g_ctx.d_ws[0], g_ctx.ws_cap[0], st);
-    if (rc != LZ4B200_OK) goto done;
-    CU(cudaMemcpyAsync(&ret, d_ret, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    if (ret > 0) {
-        CU(cudaMemcpyAsync(dst, g_ctx.d_out[0], (size_t)ret, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
-    }
+        rc = LZ4B200_decompress_blocks(s->in.p, d_off, d_size, s->out.p, NULL, 0, NULL, dstCapacity,
+                                       d_size + 1, 1, s->ws.p, s->ws.cap, s->stream);
+    if (rc == LZ4B200_OK) rc = slot_return(s, h_size + 1, d_size + 1, &ret, 1);
+    if (rc == LZ4B200_OK) rc = slot_wait(s);
+    if (rc == LZ4B200_OK && ret > 0) CU(cudaMemcpyAsync(dst, s->out.p, (size_t)ret, cudaMemcpyDeviceToHost, s->stream));
 done:
-    pthread_mutex_unlock(&g_lock);
-    return rc == LZ4B200_OK ? ret : -1;
+    return host_end(rc) == LZ4B200_OK ? ret : -1;
 }
 
 int LZ4_decompress_safe(const char* src, char* dst, int compressedSize, int dstCapacity)
@@ -712,60 +688,54 @@ int64_t LZ4B200_compressFrame_host(const void* h_src, int64_t srcSize, void* h_d
          * g+1 is issued before group g is retired, so its copies and kernels overlap g's D2H. */
         int64_t group = ((int64_t)256 << 20) / bs, nGroups, g;
         const int64_t slotStride = (bs + 15) & ~(int64_t)15;
-        int rc = LZ4B200_OK;
+        int rc;
         if (group < 1) group = 1;
         nGroups = (nBlocks + group - 1) / group;
-        pthread_mutex_lock(&g_lock);
-        if ((rc = ctx_init()) != LZ4B200_OK) { pthread_mutex_unlock(&g_lock); return rc; }
-        for (g = 0; g <= nGroups && rc == LZ4B200_OK; g++) {
+        if ((rc = host_begin()) != LZ4B200_OK) goto done;
+        for (g = 0; g <= nGroups; g++) {
             if (g < nGroups) {                                         /* ---- issue group g ---- */
-                const int slot = (int)(g % N_PIPE);
+                slot_t* s = &g_ctx.slot[g % N_PIPE];
                 const int64_t firstB = g * group;
                 const int64_t cnt = (nBlocks - firstB < group) ? nBlocks - firstB : group;
                 const int hasLast = (firstB + cnt == nBlocks) && lastSize > 0;
                 const int64_t inBytes = (cnt - 1) * bs + (hasLast ? lastSize : bs);
-                cudaStream_t st = g_ctx.stream[slot];
                 int64_t* d_off; int32_t* d_sz; int32_t* d_ssz;
-                if (cudaStreamSynchronize(st) != cudaSuccess) { rc = LZ4B200_ERR_CUDA; break; }
-                if ((rc = grow(&g_ctx.d_in[slot], &g_ctx.in_cap[slot], (size_t)inBytes + 16)) != LZ4B200_OK) break;
-                if ((rc = grow(&g_ctx.d_out[slot], &g_ctx.out_cap[slot], (size_t)(cnt * slotStride) + 16)) != LZ4B200_OK) break;
-                if ((rc = grow(&g_ctx.d_pack[slot], &g_ctx.pack_cap[slot], (size_t)(cnt * (bs + 4)) + 16)) != LZ4B200_OK) break;
-                if ((rc = grow(&g_ctx.d_meta[slot], &g_ctx.meta_cap[slot], (size_t)(cnt + 1) * 16 + 64)) != LZ4B200_OK) break;
-                if ((rc = grow_pinned(&g_ctx.h_meta[slot], &g_ctx.hmeta_cap[slot], (size_t)cnt * 4 + 64)) != LZ4B200_OK) break;
-                d_off = (int64_t*)g_ctx.d_meta[slot];
+                rc = slot_take(s, (size_t)inBytes, (size_t)(cnt * slotStride), 0, (size_t)(cnt * (bs + 4)),
+                               (size_t)(cnt + 1) * sizeof(int64_t) + (size_t)cnt * 2 * sizeof(int32_t));
+                if (rc != LZ4B200_OK) goto done;
+                /* tables: [body offsets i64 (cnt + 1) | compressed sizes i32 | source sizes i32]; the host's first word
+                 * receives the body size */
+                d_off = (int64_t*)s->d_tab.p;
                 d_sz = (int32_t*)(d_off + cnt + 1);
                 d_ssz = d_sz + cnt;
-                if (cudaMemcpyAsync(g_ctx.d_in[slot], src + firstB * bs, (size_t)inBytes, cudaMemcpyHostToDevice, st) != cudaSuccess) { rc = LZ4B200_ERR_CUDA; break; }
+                CU(cudaMemcpyAsync(s->in.p, src + firstB * bs, (size_t)inBytes, cudaMemcpyHostToDevice, s->stream));
                 if (hasLast) {                                           /* per-block sizes only for the group with the ragged block */
-                    int32_t* h_ssz = (int32_t*)((char*)g_ctx.h_meta[slot] + 64);
+                    int32_t* h_ssz = (int32_t*)((int64_t*)s->h_tab.p + cnt + 1) + cnt;
                     int64_t k;
                     for (k = 0; k < cnt; k++) h_ssz[k] = (int32_t)bs;
                     h_ssz[cnt - 1] = (int32_t)lastSize;
-                    if (cudaMemcpyAsync(d_ssz, h_ssz, (size_t)cnt * 4, cudaMemcpyHostToDevice, st) != cudaSuccess) { rc = LZ4B200_ERR_CUDA; break; }
+                    CU(cudaMemcpyAsync(d_ssz, h_ssz, (size_t)cnt * sizeof(int32_t), cudaMemcpyHostToDevice, s->stream));
                 }
-                rc = LZ4B200_compress_blocks(g_ctx.d_in[slot], bs, hasLast ? d_ssz : NULL, (int32_t)bs, g_ctx.d_out[slot], slotStride,
-                                             (int32_t)(bs - 1), accel, d_sz, cnt, st);
-                if (rc != LZ4B200_OK) break;
-                rc = LZ4B200_pack_frame_blocks(g_ctx.d_out[slot], slotStride, d_sz, g_ctx.d_in[slot], bs, (int32_t)bs,
-                                               hasLast ? (int32_t)lastSize : 0, cnt, g_ctx.d_pack[slot], d_off, st);
-                if (rc != LZ4B200_OK) break;
-                if (cudaMemcpyAsync(g_ctx.h_meta[slot], d_off + cnt, sizeof(int64_t), cudaMemcpyDeviceToHost, st) != cudaSuccess) { rc = LZ4B200_ERR_CUDA; break; }
+                rc = LZ4B200_compress_blocks(s->in.p, bs, hasLast ? d_ssz : NULL, (int32_t)bs, s->out.p, slotStride,
+                                             (int32_t)(bs - 1), accel, d_sz, cnt, s->stream);
+                if (rc != LZ4B200_OK) goto done;
+                rc = LZ4B200_pack_frame_blocks(s->out.p, slotStride, d_sz, s->in.p, bs, (int32_t)bs,
+                                               hasLast ? (int32_t)lastSize : 0, cnt, s->pack.p, d_off, s->stream);
+                if (rc != LZ4B200_OK) goto done;
+                CU(cudaMemcpyAsync(s->h_tab.p, d_off + cnt, sizeof(int64_t), cudaMemcpyDeviceToHost, s->stream));
             }
             if (g > 0) {                                               /* ---- retire group g-1: its size is known once its stream is idle ---- */
-                const int slot = (int)((g - 1) % N_PIPE);
-                cudaStream_t st = g_ctx.stream[slot];
+                slot_t* s = &g_ctx.slot[(g - 1) % N_PIPE];
                 int64_t total;
-                if (cudaStreamSynchronize(st) != cudaSuccess) { rc = LZ4B200_ERR_CUDA; break; }
-                total = *(const int64_t*)g_ctx.h_meta[slot];
-                if (op + total + 4 > dstCapacity) { rc = LZ4B200_ERR_DSTSIZE; break; }
-                if (cudaMemcpyAsync(dst + op, g_ctx.d_pack[slot], (size_t)total, cudaMemcpyDeviceToHost, st) != cudaSuccess) { rc = LZ4B200_ERR_CUDA; break; }
+                if ((rc = slot_wait(s)) != LZ4B200_OK) goto done;
+                total = *(const int64_t*)s->h_tab.p;
+                if (op + total + 4 > dstCapacity) { rc = LZ4B200_ERR_DSTSIZE; goto done; }
+                CU(cudaMemcpyAsync(dst + op, s->pack.p, (size_t)total, cudaMemcpyDeviceToHost, s->stream));
                 op += total;
             }
         }
-        {   int i; for (i = 0; i < N_PIPE; i++) if (cudaStreamSynchronize(g_ctx.stream[i]) != cudaSuccess && rc == LZ4B200_OK) rc = LZ4B200_ERR_CUDA; }
-        pthread_mutex_unlock(&g_lock);
-        if (rc == LZ4B200_ERR_CUDA) cuda_fail(cudaGetLastError(), "LZ4B200_compressFrame_host");
-        if (rc != LZ4B200_OK) return rc;
+    done:
+        if ((rc = host_end(rc)) != LZ4B200_OK) return rc;
     }
     wr_le32(dst + op, 0); op += 4;                                        /* EndMark, lz4frame.c:1222 */
     return op;
