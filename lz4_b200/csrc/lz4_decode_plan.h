@@ -22,6 +22,19 @@ constexpr int32_t kTileMaxCap = 64 << 20;          /* larger capacities take the
 constexpr int64_t kSplitMaxBlocks = 8192;          /* largest batch the split scan is the default for (H100, see plan_decode) */
 DP_FN uint32_t tiles_of(int32_t bytes) { return ((uint32_t)bytes + (uint32_t)kTile - 1u) / (uint32_t)kTile; }
 
+/* The tile index of a block of nT tiles and ns sequences with wide marks: first[t] = min { k : matchStart(k) >= t * kTile }
+ * for t = 0 .. nT (ns if none).  The match starts are non-decreasing in k and the last mark holds the decoded size, so
+ * sequence k and its predecessor decide which entries are k; calling this for every k < ns fills first[0 .. nT]. */
+DP_FN void tile_index_seq(uint32_t* first, const uint32_t* marks, uint32_t k, uint32_t ns, uint32_t nT)
+{
+    const uint32_t q1 = marks[2 * (size_t)k + 1] / (uint32_t)kTile;
+    const uint32_t t1 = q1 < nT ? q1 : nT;                 /* tiles t <= t1 start at or below the match start */
+    uint32_t t0 = 0;                                       /* first tile not yet served by k - 1 */
+    if (k) { const uint32_t q0 = marks[2 * (size_t)k - 1] / (uint32_t)kTile; t0 = (q0 < nT ? q0 : nT) + 1u; }
+    for (uint32_t t = t0; t <= t1; t++) first[t] = k;
+    if (k + 1 == ns) for (uint32_t t = t1 + 1; t <= nT; t++) first[t] = ns;
+}
+
 enum DecodeKind { kDecodeFull, kDecodePartial };    /* LZ4_decompress_safe, or LZ4_decompress_safe_partial (capacity = target) */
 enum DecodeScan { kScanThread, kScanPar, kScanSplit };
 

@@ -316,9 +316,8 @@ __global__ void __launch_bounds__(kScanLanes) lz4_scan_par_kernel(lz4k_decode_ar
     }
 }
 
-/* ---- wide batches: per tile of kTile output bytes the first sequence whose match starts in or beyond it ----
- * tileFirst[b][t] = min { k : matchStart(k) >= t * kTile } for t = 0 .. tiles(b) (nseq if none); done flags cleared.
- * The match starts are non-decreasing in k and the last mark holds the decoded size, so sequence k's neighbours decide. */
+/* ---- wide batches: per tile of kTile output bytes the first sequence whose match starts in or beyond it (tile_index_seq);
+ * done flags cleared ---- */
 __global__ void __launch_bounds__(256) lz4_tile_index_kernel(lz4k_decode_args a, WsView w)
 {
     for (int64_t b = blockIdx.x; b < a.nBlocks; b += gridDim.x) {
@@ -330,14 +329,7 @@ __global__ void __launch_bounds__(256) lz4_tile_index_kernel(lz4k_decode_args a,
         if (total <= 0 || ns == 0 || !tiles_eligible(w, ns)) continue;
         const uint32_t nT = tiles_of(total);
         const uint32_t* marks = w.marks + (size_t)b * w.markStride;
-        for (uint32_t k = threadIdx.x; k < ns; k += blockDim.x) {
-            const uint32_t m = marks[2 * (size_t)k + 1];
-            const uint32_t t1 = min(m / (uint32_t)kTile, nT);             /* tiles t <= t1 start at or below m */
-            uint32_t t0 = 0;                                                /* first tile not yet served by k - 1 */
-            if (k) t0 = min(marks[2 * (size_t)k - 1] / (uint32_t)kTile, nT) + 1u;
-            for (uint32_t t = t0; t <= t1; t++) first[t] = k;
-            if (k + 1 == ns) for (uint32_t t = t1 + 1; t <= nT; t++) first[t] = ns;
-        }
+        for (uint32_t k = threadIdx.x; k < ns; k += blockDim.x) tile_index_seq(first, marks, k, ns, nT);
     }
 }
 
@@ -469,6 +461,30 @@ __device__ __forceinline__ uint32_t lanemask_le()
 }
 
 /* ---- the phases of a window shared by lz4_expand_rows_kernel and lz4_expand_tiles_kernel ---- */
+
+/* runs pass 1 (PASS1: one bit per run start) or pass 2 (each run's delta at its rank) over the sequences [k0, k1):
+ * thread t takes k0 + t, k0 + t + 1024, ...  Pass 1 keeps the parse of the thread's first kRowsCache sequences in sq for
+ * pass 2.  parse(i, k) returns sequence k, the thread's i-th (i = kRowsCache for all past the cache); runs(s, f) calls
+ * f(start, delta) for each run of s in the window, in increasing start order, and first(s) is the first one's start
+ * (-1: none). */
+template <bool PASS1, class Parse, class First, class Runs>
+__device__ __forceinline__ void rows_runs_pass(RowsSmem& S, RwSeq (&sq)[kRowsCache], const int k0, const int k1,
+                                               Parse&& parse, First&& first, Runs&& runs)
+{
+    auto body = [&](const RwSeq& s) {
+        if constexpr (PASS1) runs(s, [&](int st, int) { atomicOr(&S.rows[st >> 5].x, 1u << (st & 31)); });
+        else rw_put_deltas(S.rows, S.tab, first(s), [&](auto f) { runs(s, f); });
+    };
+    #pragma unroll
+    for (int i = 0; i < kRowsCache; i++) {
+        const int k = k0 + (int)threadIdx.x + i * kRowsThreads;
+        if (k < k1) {
+            if constexpr (PASS1) sq[i] = parse(i, k);
+            body(sq[i]);
+        }
+    }
+    for (int k = k0 + (int)threadIdx.x + kRowsCache * kRowsThreads; k < k1; k += kRowsThreads) body(parse(kRowsCache, k));
+}
 
 /* rank: rows[r].y = (number of run starts in rows [0, r)) - 1.  Returns the number of runs. */
 __device__ __forceinline__ uint32_t rows_rank(RowsSmem& S)
@@ -693,23 +709,12 @@ __device__ __forceinline__ void expand_rows(const lz4k_decode_args& a, const WsV
 
         /* ---- runs, pass 1: one bit per run start ---- */
         const uint8_t* in = S.in + head;
-        const uint32_t inA = (uint32_t)offsetof(RowsSmem, in) + (uint32_t)head;
-        auto setBit = [&](int s, int) { atomicOr(&S.rows[s >> 5].x, 1u << (s & 31)); };
+        const int litDelta = (int)((uint32_t)offsetof(RowsSmem, in) + (uint32_t)head - outA);
+        auto parse = [&](int i, int k) { return rw_parse<PARTIAL>(in, i < kRowsCache ? mk[i] : marks[k], k, k + 1 == nseq, total); };
+        auto firstRun = [](const RwSeq& s) { return rw_seq_first(s); };
+        auto runs = [&](const RwSeq& s, auto f) { rw_seq_runs(s, litDelta, zeroDelta0, f); };
         RwSeq sq[kRowsCache];
-        #pragma unroll
-        for (int i = 0; i < kRowsCache; i++) {
-            const int k = tid + i * kRowsThreads;
-            if (k < nseq) {
-                sq[i] = rw_parse<PARTIAL>(in, mk[i], k, k + 1 == nseq, total);
-                if (sq[i].ll > 0) setBit(sq[i].op, 0);
-                if (sq[i].mlen > 0) rw_match_runs(sq[i].m, sq[i].off, sq[i].mlen, zeroDelta0, setBit);
-            }
-        }
-        for (int k = tid + kRowsCache * kRowsThreads; k < nseq; k += kRowsThreads) {
-            const RwSeq s = rw_parse<PARTIAL>(in, marks[k], k, k + 1 == nseq, total);
-            if (s.ll > 0) setBit(s.op, 0);
-            if (s.mlen > 0) rw_match_runs(s.m, s.off, s.mlen, zeroDelta0, setBit);
-        }
+        rows_runs_pass<true>(S, sq, 0, nseq, parse, firstRun, runs);
         __syncthreads();
         PHASE_MARK(2);                                     // pass 1
 
@@ -722,21 +727,7 @@ __device__ __forceinline__ void expand_rows(const lz4k_decode_args& a, const WsV
 
         if (!tooMany) {
             /* ---- runs, pass 2: delta of every run at its rank ---- */
-            auto emit = [&](const RwSeq& s) {
-                if (s.ll > 0) S.tab[rw_rank(S.rows, (uint32_t)s.op)] = (inA + (uint32_t)s.ls) - (outA + (uint32_t)s.op);
-                if (s.mlen > 0) {
-                    uint32_t j = rw_rank(S.rows, (uint32_t)s.m);
-                    rw_match_runs(s.m, s.off, s.mlen, zeroDelta0, [&](int, int dlt) { S.tab[j++] = (uint32_t)dlt; });
-                }
-            };
-            #pragma unroll
-            for (int i = 0; i < kRowsCache; i++) {
-                const int k = tid + i * kRowsThreads;
-                if (k < nseq) emit(sq[i]);
-            }
-            for (int k = tid + kRowsCache * kRowsThreads; k < nseq; k += kRowsThreads) {
-                emit(rw_parse<PARTIAL>(in, marks[k], k, k + 1 == nseq, total));
-            }
+            rows_runs_pass<false>(S, sq, 0, nseq, parse, firstRun, runs);
             __syncthreads();
             PHASE_MARK(4);                                     // pass 2
 
@@ -838,24 +829,15 @@ __global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_tiles_kernel(lz4k_
         const int k0 = f0 ? (int)f0 - 1 : 0, k1 = (int)min(f1 + 1u, nseq);
         const uint32_t litBase = kLitBase - outS + (uint32_t)os;
         const int zeroDelta0 = (int)(kZeroV - outS + (uint32_t)os);
-        auto parse = [&](int k) { return rw_parse_wide(src, marks[2 * (size_t)k], marks[2 * (size_t)k + 1], k + 1 == (int)nseq); };
+        auto parse = [&](int, int k) { return rw_parse_wide(src, marks[2 * (size_t)k], marks[2 * (size_t)k + 1], k + 1 == (int)nseq); };
+        auto firstRun = [&](const RwSeq& s) { return rw_tile_first(s, os, oe); };
+        auto runs = [&](const RwSeq& s, auto f) { rw_tile_runs(s, os, oe, litBase, zeroDelta0, f); };
 
         for (int k = tid; k < 2048; k += kRowsThreads) S.rows[k] = make_uint2(0u, 0u);
         __syncthreads();
         /* ---- runs, pass 1 (a thread's first sequences stay in registers for pass 2: parsing reads global memory) ---- */
         RwSeq sq[kRowsCache];
-        #pragma unroll
-        for (int i = 0; i < kRowsCache; i++) {
-            const int k = k0 + tid + i * kRowsThreads;
-            if (k < k1) {
-                sq[i] = parse(k);
-                rw_tile_runs(sq[i], os, oe, litBase, zeroDelta0, [&](int st, int) { atomicOr(&S.rows[st >> 5].x, 1u << (st & 31)); });
-            }
-        }
-        for (int k = k0 + tid + kRowsCache * kRowsThreads; k < k1; k += kRowsThreads) {
-            const RwSeq s = parse(k);
-            rw_tile_runs(s, os, oe, litBase, zeroDelta0, [&](int st, int) { atomicOr(&S.rows[st >> 5].x, 1u << (st & 31)); });
-        }
+        rows_runs_pass<true>(S, sq, k0, k1, parse, firstRun, runs);
         __syncthreads();
         const uint32_t nRuns = rows_rank(S);
         if (tid == 0) publishPending();                       /* the previous unit's store is complete: its flag goes up, `out` is free */
@@ -870,15 +852,7 @@ __global__ void __launch_bounds__(kRowsThreads, 1) lz4_expand_tiles_kernel(lz4k_
             continue;
         }
         /* ---- runs, pass 2 ---- */
-        #pragma unroll
-        for (int i = 0; i < kRowsCache; i++) {
-            const int k = k0 + tid + i * kRowsThreads;
-            if (k < k1) rw_tile_runs(sq[i], os, oe, litBase, zeroDelta0, [&](int st, int d) { S.tab[rw_rank(S.rows, (uint32_t)st)] = (uint32_t)d; });
-        }
-        for (int k = k0 + tid + kRowsCache * kRowsThreads; k < k1; k += kRowsThreads) {
-            const RwSeq s = parse(k);
-            rw_tile_runs(s, os, oe, litBase, zeroDelta0, [&](int st, int d) { S.tab[rw_rank(S.rows, (uint32_t)st)] = (uint32_t)d; });
-        }
+        rows_runs_pass<false>(S, sq, k0, k1, parse, firstRun, runs);
         __syncthreads();
         /* ---- the tile before this one must be in global memory ---- */
         if (t > 0) {

@@ -146,27 +146,46 @@ RW_FN void rw_match_runs(int m, int off, int len, int zeroDelta0, F f)
     for (long long step = 2LL * period; step < rem && step <= 65535; step *= 2) f(base + (int)step, -(int)step);
 }
 
+/* The runs of one sequence: calls f(start, delta) for its literal run, with delta = litDelta + ls - op (litDelta maps
+ * the compressed block's byte 0 into the caller's window), and then for the runs of its match (rw_match_runs), in
+ * increasing start order. */
+template <class F>
+RW_FN void rw_seq_runs(const RwSeq& s, int litDelta, int zeroDelta0, F f)
+{
+    if (s.ll > 0) f(s.op, (int)((uint32_t)litDelta + (uint32_t)(s.ls - s.op)));
+    if (s.mlen > 0) rw_match_runs(s.m, s.off, s.mlen, zeroDelta0, f);
+}
+
+/* start of the first run rw_seq_runs lists (op also when the literal run is empty: then m = op), -1 if it lists none */
+RW_FN int rw_seq_first(const RwSeq& s) { return s.ll > 0 || s.mlen > 0 ? s.op : -1; }
+
+/* start of the first run rw_tile_runs lists, -1 if the sequence's bytes [op, m + mlen) and the tile [os, oe) do not
+ * overlap (also when the sequence has no bytes) */
+RW_FN int rw_tile_first(const RwSeq& s, int os, int oe)
+{
+    const int lo = s.op > os ? s.op : os, hi = s.m + s.mlen < oe ? s.m + s.mlen : oe;
+    return hi > lo ? lo - os : -1;
+}
+
 /* The runs of one sequence CLIPPED to the output tile [os, oe) of a block above 64 KB, as f(start - os, delta), in
  * increasing start order.  Deltas keep the meaning "source = position + delta" in the tile's window (position counted
  * from the tile start): a match run's delta is the same number as in block coordinates (a source before the tile start
  * lies in an earlier tile = global memory); a literal run's delta is litBase + (ls - op), with litBase chosen by the
  * caller so that the sum lands in a virtual range that means "byte ls + (p - op) of the compressed block";
- * zeroDelta0 = what rw_match_runs needs for the always-zero cell, in the same convention. */
+ * zeroDelta0 = what rw_match_runs needs for the always-zero cell, in the same convention.  A sequence's runs are
+ * contiguous, so the last one that starts at or before the tile start covers it and is carried to offset 0. */
 template <class F>
 RW_FN void rw_tile_runs(const RwSeq& s, int os, int oe, uint32_t litBase, int zeroDelta0, F f)
 {
-    const int lo = s.op > os ? s.op : os, hi = (s.op + s.ll) < oe ? (s.op + s.ll) : oe;
-    if (hi > lo) f(lo - os, (int)(litBase + (uint32_t)(s.ls - s.op)));
-    if (s.mlen > 0 && s.m + s.mlen > os && s.m < oe) {
-        bool pend = false;                              /* the last piece that starts at or before the tile start covers it */
-        int pd = 0;
-        rw_match_runs(s.m, s.off, s.mlen, zeroDelta0, [&](int st, int d) {
-            if (st <= os) { pend = true; pd = d; return; }
-            if (pend) { f(0, pd); pend = false; }
-            if (st < oe) f(st - os, d);
-        });
-        if (pend) f(0, pd);
-    }
+    if (rw_tile_first(s, os, oe) < 0) return;
+    bool pend = false;
+    int pd = 0;
+    rw_seq_runs(s, (int)litBase, zeroDelta0, [&](int st, int d) {
+        if (st <= os) { pend = true; pd = d; return; }
+        if (pend) { f(0, pd); pend = false; }
+        if (st < oe) f(st - os, d);
+    });
+    if (pend) f(0, pd);
 }
 
 /* run index of output byte q: rows[r] = {bits of row r, (run starts before row r) - 1} */
@@ -176,16 +195,16 @@ RW_FN uint32_t rw_rank(const uint2* rows, uint32_t q)
     return r.y + (uint32_t)RW_POPC(r.x & (0xFFFFFFFFu >> (31u - (q & 31u))));
 }
 
-/* Source byte index (into `window`) of output byte p, given that everything below window index
- * `waveA` is final: follow sources that lie inside the current wave. */
-RW_FN uint32_t rw_resolve(const uint2* rows, const uint32_t* tab, uint32_t outA, uint32_t waveA, uint32_t p, uint32_t j)
+/* Runs pass 2 for one sequence: runs(f) calls f(start, delta) for the sequence's runs in increasing start order
+ * (rw_seq_runs, rw_tile_runs), the first of which starts at q0 (rw_seq_first, rw_tile_first; -1: there are none), and
+ * each delta goes to its run's rank in tab.  No other sequence starts a run between them, so they occupy consecutive
+ * ranks and only the first one is looked up. */
+template <class Runs>
+RW_FN void rw_put_deltas(const uint2* rows, uint32_t* tab, int q0, Runs runs)
 {
-    uint32_t a = outA + p + tab[j];
-    while (a >= waveA) {
-        const uint32_t q = a - outA;
-        a += tab[rw_rank(rows, q)];
-    }
-    return a;
+    if (q0 < 0) return;
+    uint32_t j = rw_rank(rows, (uint32_t)q0);
+    runs([&](int, int d) { tab[j++] = (uint32_t)d; });
 }
 
 #endif /* LZ4_ROWS_CORE_H */

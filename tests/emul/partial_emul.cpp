@@ -22,15 +22,11 @@ extern "C" int partial_emulate(const uint8_t* src, int n, int cap, uint32_t* nSe
     for (int k = 0; k < ns; k++) {
         const RwSeq s = rw_parse<true>(in, marks[k], k, k + 1 == ns, r);
         if (s.ls + s.ll > (int)*usedOut) return -1000002;
-        if (s.ll > 0 && (s.op >= r || s.op + s.ll > r)) return -1000001;
+        bool bad = (s.ll > 0 && s.op + s.ll > r) || (s.mlen > 0 && s.m + s.mlen > r);
+        rw_seq_runs(s, 0, 0, [&](int st, int) { if (st >= r) bad = true; });
+        if (bad) return -1000001;
         for (int i = 0; i < s.ll; i++) out[s.op + i] = in[s.ls + i];
-        if (s.mlen > 0) {
-            if (s.m + s.mlen > r) return -1000001;
-            bool bad = false;
-            rw_match_runs(s.m, s.off, s.mlen, 0, [&](int st, int) { if (st >= r) bad = true; });
-            if (bad) return -1000001;
-            for (int i = 0; i < s.mlen; i++) out[s.m + i] = s.off ? out[s.m + i - s.off] : 0;
-        }
+        for (int i = 0; i < s.mlen; i++) out[s.m + i] = s.off ? out[s.m + i - s.off] : 0;
     }
     return r;
 }

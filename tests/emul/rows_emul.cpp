@@ -39,17 +39,14 @@ extern "C" int rows_emulate(const uint8_t* comp, int n, int cap, uint8_t* out, i
     std::vector<uint2> rows(2048, uint2{0u, 0u});
     std::vector<uint32_t> tab(kRowsMaxRuns, 0xDEADBEEFu);
 
+    const int litDelta = (int)(inA - outA);
     auto seq = [&](int k) {
         return rw_parse(in, marks[k], k, k + 1 == nseq);
     };
     // pass 1
     for (int tid = 0; tid < kThreads; tid++)
-        for (int k = tid; k < nseq; k += kThreads) {
-            const RwSeq s = seq(k);
-            auto setBit = [&](int p, int) { rows[p >> 5].x |= 1u << (p & 31); };
-            if (s.ll > 0) setBit(s.op, 0);
-            if (s.mlen > 0) rw_match_runs(s.m, s.off, s.mlen, zeroDelta0, setBit);
-        }
+        for (int k = tid; k < nseq; k += kThreads)
+            rw_seq_runs(seq(k), litDelta, zeroDelta0, [&](int p, int) { rows[p >> 5].x |= 1u << (p & 31); });
     // rank
     uint32_t run = 0;
     for (int r = 0; r < 2048; r++) { rows[r].y = run - 1u; run += (uint32_t)__builtin_popcount(rows[r].x); }
@@ -59,11 +56,7 @@ extern "C" int rows_emulate(const uint8_t* comp, int n, int cap, uint8_t* out, i
     for (int tid = 0; tid < kThreads; tid++)
         for (int k = tid; k < nseq; k += kThreads) {
             const RwSeq s = seq(k);
-            if (s.ll > 0) tab[rw_rank(rows.data(), (uint32_t)s.op)] = (inA + (uint32_t)s.ls) - (outA + (uint32_t)s.op);
-            if (s.mlen > 0) {
-                uint32_t j = rw_rank(rows.data(), (uint32_t)s.m);
-                rw_match_runs(s.m, s.off, s.mlen, zeroDelta0, [&](int, int d) { tab[j++] = (uint32_t)d; });
-            }
+            rw_put_deltas(rows.data(), tab.data(), rw_seq_first(s), [&](auto f) { rw_seq_runs(s, litDelta, zeroDelta0, f); });
         }
     // waves
     const int wave = kThreads * rpt;

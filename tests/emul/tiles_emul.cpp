@@ -1,22 +1,22 @@
 // CPU emulator of the tiles expand kernel (lz4_b200/csrc/lz4_kernels.cu: lz4_expand_tiles_kernel): TEST INFRASTRUCTURE.
-// A block above 64 KB is decoded tile by tile with the arithmetic of lz4_rows_core.h (rw_parse_wide, rw_tile_runs: the same
-// text the device compiles): wide marks from the scan, the tile index (first sequence per tile), per tile runs pass 1,
-// rank, runs pass 2, waves with the kernel's three kinds of source -- compressed byte (virtual range), byte of this
-// tile (window), byte of an earlier tile (destination).  Checks what the kernel relies on: every source read from the
-// window was written in an earlier wave, every history read lies in an earlier tile.  Built by tests/test_tiles_emul.py.
+// A block above 64 KB is decoded tile by tile with the device's text (lz4_rows_core.h: rw_parse_wide, rw_tile_runs,
+// rw_put_deltas; lz4_decode_plan.h: tile_index_seq): wide marks from the scan, the tile index (first sequence per tile),
+// per tile runs pass 1, rank, runs pass 2, waves with the kernel's three kinds of source -- compressed byte (virtual
+// range), byte of this tile (window), byte of an earlier tile (destination).  Checks what the kernel relies on: every
+// source read from the window was written in an earlier wave, every history read lies in an earlier tile.  Built by
+// tests/test_tiles_emul.py.
 #include <stdint.h>
 #include <string.h>
 #include <vector>
 
 #include "../../lz4_b200/csrc/lz4_scan_core.h"
 #include "../../lz4_b200/csrc/lz4_rows_core.h"
+#include "../../lz4_b200/csrc/lz4_decode_plan.h"
 
 namespace {
 constexpr int kThreads = 1024;
-constexpr int kTile = 61440;
 constexpr uint32_t kOutS = 65616 + 4096;              // any window address above 65535 (the device's is sBase + offsetof(out))
 constexpr uint32_t kLitBase = 1u << 28, kZeroV = kLitBase + (1u << 27);
-uint32_t tiles_of(int bytes) { return ((uint32_t)bytes + (uint32_t)kTile - 1u) / (uint32_t)kTile; }
 }
 
 // returns LZ4_decompress_safe's value; out (cap bytes) receives the decoded bytes when it is > 0.
@@ -38,14 +38,7 @@ extern "C" int tiles_emulate(const uint8_t* comp, int n, int cap, uint8_t* out, 
     const uint32_t nT = tiles_of(total);
     stats[0] = nT;
     std::vector<uint32_t> first(nT + 1, 0xFFFFFFFFu);
-    for (uint32_t k = 0; k < nseqU; k++) {
-        const uint32_t m = marks[2 * (size_t)k + 1];
-        const uint32_t t1 = m / (uint32_t)kTile < nT ? m / (uint32_t)kTile : nT;
-        uint32_t t0 = 0;
-        if (k) { const uint32_t q = marks[2 * (size_t)k - 1] / (uint32_t)kTile; t0 = (q < nT ? q : nT) + 1u; }
-        for (uint32_t t = t0; t <= t1; t++) first[t] = k;
-        if (k + 1 == nseqU) for (uint32_t t = t1 + 1; t <= nT; t++) first[t] = nseqU;
-    }
+    for (uint32_t k = 0; k < nseqU; k++) tile_index_seq(first.data(), marks.data(), k, nseqU, nT);
     for (uint32_t t = 0; t <= nT; t++) if (first[t] == 0xFFFFFFFFu) return -1000005;
     // ---- tiles, in order ----
     std::vector<uint8_t> win(kOutS + 65536 + 16, 0xEE);
@@ -63,12 +56,14 @@ extern "C" int tiles_emulate(const uint8_t* comp, int n, int cap, uint8_t* out, 
         int covered = 0;
         for (int k = k0; k < k1; k++) {
             const RwSeq s = seq(k);
-            int last = -1;
+            int last = -1, firstSt = -1;
             rw_tile_runs(s, os, oe, litBase, zeroDelta0, [&](int st, int) {
                 if (st < 0 || st >= len || st <= last) { stats[3]++; return; }
+                if (last < 0) firstSt = st;
                 last = st;
                 rows[st >> 5].x |= 1u << (st & 31);
             });
+            if (firstSt != rw_tile_first(s, os, oe)) stats[3]++;      // pass 2 looks up the rank of this run only
             const int a = s.op > os ? s.op : os, b = (s.mlen ? s.m + s.mlen : s.op + s.ll) < oe ? (s.mlen ? s.m + s.mlen : s.op + s.ll) : oe;
             if (b > a) covered += b - a;
         }
@@ -80,7 +75,7 @@ extern "C" int tiles_emulate(const uint8_t* comp, int n, int cap, uint8_t* out, 
         if (!(rows[0].x & 1u)) return -1000007;                   // byte 0 of a tile starts a run
         for (int k = k0; k < k1; k++) {
             const RwSeq s = seq(k);
-            rw_tile_runs(s, os, oe, litBase, zeroDelta0, [&](int st, int d) { tab[rw_rank(rows.data(), (uint32_t)st)] = (uint32_t)d; });
+            rw_put_deltas(rows.data(), tab.data(), rw_tile_first(s, os, oe), [&](auto f) { rw_tile_runs(s, os, oe, litBase, zeroDelta0, f); });
         }
         const int wave = kThreads * rpt;
         std::vector<uint8_t> stage((size_t)wave);
