@@ -4,8 +4,13 @@
  * Plain-C restatement of the reference LZ4 block codec, written from the algorithm (index based,
  * byte-exact copies, no wild copies) rather than from the reference's pointer code.  Each
  * function cites the reference lines (lib/lz4.c of lz4 v1.10.0) whose behaviour it reproduces.
- * Pinned against the compiled reference (oracle/_ref) by tests/test_oracle_vs_ref.py and against
- * tests/golden/ fixtures by tests/test_oracle_golden.py.
+ * One parse (compress_generic) serves LZ4_compress_fast and LZ4_compress_destSize, one decoder
+ * (decompress_generic) LZ4_decompress_safe and LZ4_decompress_safe_partial.  The route functions
+ * hold the entry rules and pass the output directive and `partial` as constants, so the compiler
+ * may specialise the shared text per route.
+ * Pinned against the compiled reference (oracle/_ref) by tests/test_oracle_vs_ref.py,
+ * tests/test_destsize_oracle.py and tests/test_partial_oracle.py, and against tests/golden/
+ * fixtures by those files and tests/test_oracle_golden.py.
  */
 #include "lz4_oracle.h"
 #include <string.h>
@@ -25,6 +30,7 @@ enum {
     K_MATCH_SAFEGUARD = 12
 };
 #define K_MAX_INPUT 0x7E000000
+#define K_FILL_ACCEL_MAX ((1 << 25) - 1)
 
 static uint32_t load32(const uint8_t* p) { uint32_t v; memcpy(&v, p, 4); return v; }
 static uint64_t load64(const uint8_t* p) { uint64_t v; memcpy(&v, p, 8); return v; }
@@ -67,35 +73,28 @@ static int64_t put_runlength(uint8_t* dst, int64_t op, size_t len)
     return op;
 }
 
-int oracle_lz4_compress_fast(const uint8_t* src, uint8_t* dst, int srcSize, int dstCapacity, int acceleration)
+/* lz4.c:328-332: what the parse does at the end of dst */
+typedef enum { NOT_LIMITED, LIMITED_OUTPUT, FILL_OUTPUT } output_directive;
+
+/* lz4.c:930-1335 for 1 <= n <= LZ4_MAX_INPUT_SIZE, noDict / noDictIssue, 64-bit little-endian host.
+ * LIMITED_OUTPUT returns 0 where the output would pass dstCapacity; FILL_OUTPUT stops there instead,
+ * leaves the input it consumed in *consumed and the first output limit it met in *path. */
+static int compress_generic(const uint8_t* src, uint8_t* dst, int n, int dstCapacity, int acceleration,
+                            output_directive dir, int* consumed, int* path)
 {
     match_table T;
-    const int n = srcSize;
-    int limited;
-    size_t ip, anchor;
-    int64_t op, olimit;   /* signed: a negative dstCapacity must compare like the reference's pointer */
+    const int64_t olimit = dstCapacity;   /* signed: a negative dstCapacity must compare like the reference's pointer */
+    size_t ip, anchor, filled = 0;
+    int64_t op;
     size_t mflimit1, matchlimit;
     uint32_t fwdHash;
+    int first = ORACLE_DS_PATH_FILLED;    /* FILL_OUTPUT: the first output limit the parse meets */
 
-    /* lz4.c:1386-1388 */
-    if (acceleration < 1) acceleration = 1;
-    if (acceleration > K_ACCEL_MAX) acceleration = K_ACCEL_MAX;
-    limited = !(dstCapacity >= oracle_lz4_compress_bound(n));
-
-    /* lz4.c:1360-1372 */
-    if ((uint32_t)n > (uint32_t)K_MAX_INPUT) return 0;
-    if (n == 0) {
-        if (limited && dstCapacity <= 0) return 0;
-        dst[0] = 0;
-        return 1;
-    }
-
-    /* lz4.c:1389-1393 table choice; lz4.c:1558 zeroed table */
+    /* lz4.c:1389-1393, :1489-1494 table choice; lz4.c:1558, :1483 zeroed table */
     memset(T.slot, 0, sizeof(T.slot));
     T.small = (n < K_SMALL_LIMIT);
 
     ip = 0; anchor = 0; op = 0;
-    olimit = limited ? (int64_t)dstCapacity : 0;
     mflimit1 = (size_t)n - K_MFLIMIT + 1;      /* lz4.c:963, only meaningful when n >= 13 */
     matchlimit = (size_t)n - K_LASTLITERALS;   /* lz4.c:964 */
 
@@ -128,6 +127,7 @@ int oracle_lz4_compress_fast(const uint8_t* src, uint8_t* dst, int srcSize, int 
                 if (load32(src + cand) == load32(src + cur)) break;/* lz4.c:1096 */
             }
         }
+        if (dir == FILL_OUTPUT) filled = ip;                       /* lz4.c:1105 */
 
         /* --- backward extension (lz4.c:1107-1109) --- */
         while (ip > anchor && cand > 0 && src[ip - 1] == src[cand - 1]) { ip--; cand--; }
@@ -136,7 +136,15 @@ int oracle_lz4_compress_fast(const uint8_t* src, uint8_t* dst, int srcSize, int 
         {
             size_t lit = ip - anchor;
             tokenPos = op++;
-            if (limited && op + (int64_t)lit + (2 + 1 + K_LASTLITERALS) + (int64_t)(lit / 255) > olimit) return 0;
+            if (dir == LIMITED_OUTPUT && op + (int64_t)lit + (2 + 1 + K_LASTLITERALS) + (int64_t)(lit / 255) > olimit)
+                return 0;
+            /* lz4.c:1118-1122: no room for these literals, a match and the last literals: drop the token */
+            if (dir == FILL_OUTPUT
+                && op + (int64_t)((lit + 240) / 255) + (int64_t)lit + 2 + 1 + K_MFLIMIT - K_MINMATCH > olimit) {
+                op--;
+                if (first == ORACLE_DS_PATH_FILLED) first = ORACLE_DS_PATH_LITERALS;
+                goto tail;
+            }
             if (lit >= 15) {
                 dst[tokenPos] = 0xF0;
                 op = put_runlength(dst, op, lit - 15);
@@ -149,14 +157,33 @@ int oracle_lz4_compress_fast(const uint8_t* src, uint8_t* dst, int srcSize, int 
 
         for (;;) {   /* the "_next_match" chain: lz4.c:1138-1294 */
             uint32_t mcode;
-            size_t off = ip - cand;
+            size_t off;
+            /* lz4.c:1147-1152: the match would end too close to olimit: rewind to the token */
+            if (dir == FILL_OUTPUT && op + 2 + 1 + K_MFLIMIT - K_MINMATCH > olimit) {
+                op = tokenPos;
+                if (first == ORACLE_DS_PATH_FILLED) first = ORACLE_DS_PATH_NEXT_MATCH;
+                goto tail;
+            }
+            off = ip - cand;
             dst[op++] = (uint8_t)off;                              /* lz4.c:1162 LE16 */
             dst[op++] = (uint8_t)(off >> 8);
 
             mcode = common_prefix(src + ip + K_MINMATCH, src + cand + K_MINMATCH, src + matchlimit);  /* lz4.c:1182 */
             ip += (size_t)mcode + K_MINMATCH;
 
-            if (limited && op + (1 + K_LASTLITERALS) + (mcode + 240) / 255 > olimit) return 0;  /* lz4.c:1187-1211 */
+            if (dir != NOT_LIMITED && op + (1 + K_LASTLITERALS) + (mcode + 240) / 255 > olimit) {  /* lz4.c:1187-1211 */
+                uint32_t shorter;
+                if (dir == LIMITED_OUTPUT) return 0;
+                /* lz4.c:1189-1207: shorten the match to what fits, forget the positions hashed beyond it */
+                shorter = 15 - 1 + ((uint32_t)(olimit - op) - 1 - K_LASTLITERALS) * 255;
+                ip -= mcode - shorter;
+                mcode = shorter;
+                if (first == ORACLE_DS_PATH_FILLED) first = ORACLE_DS_PATH_REDUCED;
+                if (ip <= filled) {
+                    size_t p;
+                    for (p = ip; p <= filled; p++) T.slot[tbl_hash(&T, src + p)] = 0;
+                }
+            }
             if (mcode >= 15) {                                     /* lz4.c:1213-1225 */
                 dst[tokenPos] += 15;
                 op = put_runlength(dst, op, mcode - 15);
@@ -186,10 +213,16 @@ int oracle_lz4_compress_fast(const uint8_t* src, uint8_t* dst, int srcSize, int 
         fwdHash = tbl_hash(&T, src + ip);
     }
 
-tail:   /* lz4.c:1302-1329 */
+tail:   /* lz4.c:1302-1333 */
     {
         size_t last = (size_t)n - anchor;
-        if (limited && op + (int64_t)last + 1 + (int64_t)((last + 255 - 15) / 255) > olimit) return 0;
+        if (dir != NOT_LIMITED && op + (int64_t)last + 1 + (int64_t)((last + 255 - 15) / 255) > olimit) {
+            if (dir == LIMITED_OUTPUT) return 0;
+            /* lz4.c:1307-1311: as many literals as fit */
+            last = (size_t)(olimit - op) - 1;
+            last -= (last + 256 - 15) / 256;
+            if (first == ORACLE_DS_PATH_FILLED) first = ORACLE_DS_PATH_LAST_LITERALS;
+        }
         if (last >= 15) {
             dst[op++] = 0xF0;
             op = put_runlength(dst, op, last - 15);
@@ -198,8 +231,61 @@ tail:   /* lz4.c:1302-1329 */
         }
         memcpy(dst + op, src + anchor, last);
         op += (int64_t)last;
+        if (dir == FILL_OUTPUT) {
+            *consumed = (int)(anchor + last);                       /* lz4.c:1327, 1332 */
+            *path = first;
+        }
     }
     return (int)op;
+}
+
+int oracle_lz4_compress_fast(const uint8_t* src, uint8_t* dst, int srcSize, int dstCapacity, int acceleration)
+{
+    const int limited = !(dstCapacity >= oracle_lz4_compress_bound(srcSize));
+
+    /* lz4.c:1386-1388 */
+    if (acceleration < 1) acceleration = 1;
+    if (acceleration > K_ACCEL_MAX) acceleration = K_ACCEL_MAX;
+
+    /* lz4.c:1360-1372 */
+    if ((uint32_t)srcSize > (uint32_t)K_MAX_INPUT) return 0;
+    if (srcSize == 0) {
+        if (limited && dstCapacity <= 0) return 0;
+        dst[0] = 0;
+        return 1;
+    }
+    /* lz4.c:1389-1401 */
+    if (limited) return compress_generic(src, dst, srcSize, dstCapacity, acceleration, LIMITED_OUTPUT, NULL, NULL);
+    return compress_generic(src, dst, srcSize, dstCapacity, acceleration, NOT_LIMITED, NULL, NULL);
+}
+
+int oracle_lz4_compress_destSize_extState(const uint8_t* src, uint8_t* dst, int* srcSizePtr, int targetDstSize,
+                                          int acceleration, int* path)
+{
+    const int n = *srcSizePtr;
+    int unused;
+    if (path == NULL) path = &unused;
+
+    /* lz4.c:1486-1487: success is guaranteed, LZ4_compress_fast_extState (which clamps the acceleration) */
+    if (targetDstSize >= oracle_lz4_compress_bound(n)) {
+        *path = ORACLE_DS_PATH_FAST;
+        return oracle_lz4_compress_fast(src, dst, n, targetDstSize, acceleration);
+    }
+    /* lz4.c:1360-1372 with fillOutput */
+    if ((uint32_t)n > (uint32_t)K_MAX_INPUT) { *path = ORACLE_DS_PATH_BAD_SIZE; return 0; }
+    if (n == 0) {
+        *path = ORACLE_DS_PATH_EMPTY;
+        if (targetDstSize <= 0) return 0;
+        dst[0] = 0;
+        *srcSizePtr = 0;
+        return 1;
+    }
+    /* lz4.c:985 */
+    if (targetDstSize < 1) { *path = ORACLE_DS_PATH_NO_ROOM; return 0; }
+    /* lz4.c:1490-1493 pass the acceleration unclamped; the two ends are brought into range (see lz4_oracle.h) */
+    if (acceleration < 1) acceleration = 1;
+    if (acceleration > K_FILL_ACCEL_MAX) acceleration = K_FILL_ACCEL_MAX;
+    return compress_generic(src, dst, n, targetDstSize, acceleration, FILL_OUTPUT, srcSizePtr, path);
 }
 
 /* ------------------------------------------------------------------------------------------
@@ -231,18 +317,20 @@ static void copy_match(uint8_t* dst, int64_t op, int64_t offset, int64_t len)
     for (i = 0; i < len; i++) dst[op + i] = dst[op + i - offset];
 }
 
-int oracle_lz4_decompress_safe(const uint8_t* src, uint8_t* dst, int compressedSize, int dstCapacity)
+/* lz4.c:2071-2445, LZ4_decompress_generic after its entry checks (noDict, x86-64 build with
+ * LZ4_FAST_DEC_LOOP=1), for srcSize >= 1 and outputSize >= 1.  It follows the reference's control
+ * flow decision by decision, because the error value -(ip)-1 depends on which loop reads which
+ * byte, but copies bytes one at a time.  `partial` is partialDecoding: stop at outputSize instead
+ * of failing there; *lastPath then records how the decode stopped (see lz4_oracle.h). */
+static int decompress_generic(const uint8_t* src, uint8_t* dst, int srcSize, int outputSize, int partial,
+                              int* lastPath)
 {
-    const int64_t n = compressedSize, cap = dstCapacity;
+    const int64_t n = srcSize, cap = outputSize;
     int64_t ip = 0, op = 0;
     int64_t ll, ml, offset;
     uint32_t token;
 
-    if (src == NULL || dstCapacity < 0) return -1;                 /* lz4.c:2036 */
-    if (dstCapacity == 0) return (compressedSize == 1 && src[0] == 0) ? 0 : -1;   /* lz4.c:2064-2068 */
-    if (compressedSize == 0) return -1;                            /* lz4.c:2069 */
-
-    /* ---- fast loop region (lz4.c:2076-2209); x86-64 build has LZ4_FAST_DEC_LOOP ---- */
+    /* ---- fast loop region (lz4.c:2076-2209) ---- */
     if (cap - op >= K_FAST_DISTANCE) {
         for (;;) {
             token = src[ip++];
@@ -263,14 +351,12 @@ int oracle_lz4_decompress_safe(const uint8_t* src, uint8_t* dst, int compressedS
             if (ml == 15) {                                        /* lz4.c:2127-2139 */
                 int64_t add = read_runlength(src, &ip, n - 4, 0);
                 if (add < 0) goto error;
-                ml += add + K_MINMATCH;
-                if (op + ml >= cap - K_FAST_DISTANCE) goto safe_match;
-            } else {
-                ml += K_MINMATCH;
-                if (op + ml >= cap - K_FAST_DISTANCE) goto safe_match;
-                /* lz4.c:2148-2159: 18-byte shortcut performs no offset check of its own, but
-                 * is only entered when the match source is inside dst */
+                ml += add;
             }
+            /* lz4.c:2148-2159: the 18-byte shortcut performs no offset check of its own, but is only
+             * entered when the match source is inside dst */
+            ml += K_MINMATCH;
+            if (op + ml >= cap - K_FAST_DISTANCE) goto safe_match;
             if (offset > op) goto error;                           /* lz4.c:2161 */
             copy_match(dst, op, offset, ml);                       /* lz4.c:2199-2208 */
             op += ml;
@@ -304,13 +390,20 @@ int oracle_lz4_decompress_safe(const uint8_t* src, uint8_t* dst, int compressedS
 
 safe_literals:                                                     /* lz4.c:2273-2334 */
         if (op + ll > cap - K_MFLIMIT || ip + ll > n - (2 + 1 + K_LASTLITERALS)) {
-            if (ip + ll != n || op + ll > cap) goto error;         /* lz4.c:2312 */
+            if (partial) {
+                if (ip + ll > n) ll = n - ip;                      /* lz4.c:2295-2298 */
+                if (op + ll > cap) ll = cap - op;                  /* lz4.c:2301-2305 */
+            } else if (ip + ll != n || op + ll > cap) {
+                goto error;                                        /* lz4.c:2312 */
+            }
             memmove(dst + op, src + ip, (size_t)ll);
             ip += ll; op += ll;
-            break;                                                 /* end of block */
+            if (!partial) break;                                   /* end of block */
+            if (op == cap || ip >= n - 2) { *lastPath |= 1; break; }   /* lz4.c:2328 */
+        } else {
+            memcpy(dst + op, src + ip, (size_t)ll);
+            ip += ll; op += ll;
         }
-        memcpy(dst + op, src + ip, (size_t)ll);
-        ip += ll; op += ll;
 
         offset = src[ip] | (src[ip + 1] << 8); ip += 2;            /* lz4.c:2337 */
         ml = token & 15;
@@ -326,6 +419,14 @@ match_length:                                                      /* lz4.c:2344
 safe_match:                                                        /* lz4.c:2354-2434 */
         if (offset > op) goto error;                               /* lz4.c:2356 */
         if (op + ml > cap - K_MATCH_SAFEGUARD) {
+            if (partial) {                                         /* lz4.c:2392-2404 */
+                const int64_t m = ml < cap - op ? ml : cap - op;
+                copy_match(dst, op, offset, m);
+                if (offset == 0 && m > 0) *lastPath |= 4;
+                op += m;
+                if (op == cap) { *lastPath |= 2; break; }
+                continue;
+            }
             if (op + ml > cap - K_LASTLITERALS) goto error;        /* lz4.c:2423 */
         }
         copy_match(dst, op, offset, ml);
@@ -335,6 +436,25 @@ safe_match:                                                        /* lz4.c:2354
 
 error:
     return (int)(-ip) - 1;                                         /* lz4.c:2443 */
+}
+
+int oracle_lz4_decompress_safe(const uint8_t* src, uint8_t* dst, int compressedSize, int dstCapacity)
+{
+    if (src == NULL || dstCapacity < 0) return -1;                 /* lz4.c:2036 */
+    if (dstCapacity == 0) return (compressedSize == 1 && src[0] == 0) ? 0 : -1;   /* lz4.c:2064-2068 */
+    if (compressedSize == 0) return -1;                            /* lz4.c:2069 */
+    return decompress_generic(src, dst, compressedSize, dstCapacity, 0, NULL);
+}
+
+int oracle_lz4_decompress_safe_partial(const uint8_t* src, uint8_t* dst, int srcSize, int targetOutputSize,
+                                       int dstCapacity, int* lastPath)
+{
+    const int outputSize = targetOutputSize < dstCapacity ? targetOutputSize : dstCapacity;   /* lz4.c:2461 */
+    *lastPath = 0;
+    if (src == NULL || outputSize < 0) return -1;                  /* lz4.c:2036 */
+    if (outputSize == 0) return 0;                                 /* lz4.c:2066 */
+    if (srcSize <= 0) return -1;                                   /* lz4.c:2069, and a negative size */
+    return decompress_generic(src, dst, srcSize, outputSize, 1, lastPath);
 }
 
 /* Token walk over a VALID block (no bounds checking beyond the input length). */

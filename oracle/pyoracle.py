@@ -16,6 +16,11 @@ ORACLE_SO = os.path.join(HERE, "liboracle.so")
 REF_SO = os.path.join(HERE, "_ref", "libref_lz4.so")
 
 _u8p = C.POINTER(C.c_uint8)
+_ip = C.POINTER(C.c_int)
+
+# path codes of oracle_lz4_compress_destSize_extState (enum oracle_ds_path, lz4_oracle.h)
+PATHS = {0: "fast", 1: "empty", 2: "no_room", 3: "literals", 4: "next_match", 5: "reduced", 6: "last_literals",
+         7: "filled", 8: "bad_size"}
 
 
 def build(quiet=True):
@@ -39,7 +44,8 @@ def _as_u8(data):
 
 
 class _Codec:
-    """Common python surface over (compress_fast, decompress_safe, compress_bound)."""
+    """Common python surface over (compress_fast, decompress_safe, compress_bound, compress_destSize,
+    decompress_safe_partial)."""
 
     def compress_bound(self, n):
         return int(self._bound(int(n)))
@@ -65,6 +71,34 @@ class _Codec:
         assert (dst[max(cap, 0):] == 0xA5).all(), "decoder wrote past dstCapacity"
         return r, dst[:max(r, 0)].tobytes()
 
+    def compress_dest_size(self, data, target, acceleration=None):
+        """LZ4_compress_destSize (acceleration None) or LZ4_compress_destSize_extState (lz4.h:248-272, :613-617).  Returns
+        (ret, consumed, bytes, path): consumed is what the call leaves in *srcSizePtr, path the oracle's route code
+        (PATHS) or None for the reference."""
+        src = _as_u8(data)
+        room = max(int(target), 0)
+        dst = np.full(room + 64, 0xA5, dtype=np.uint8)
+        n = C.c_int(len(src))
+        r, path = self._dest_size(_ptr(src) if len(src) else None, _ptr(dst), n, int(target), acceleration)
+        assert (dst[room:] == 0xA5).all(), "destSize wrote at or past targetDstSize"
+        return r, n.value, dst[:max(r, 0)].tobytes(), path
+
+    def decompress_partial(self, data, target, capacity=None):
+        """LZ4_decompress_safe_partial(src, dst, len(data), target, capacity) (lz4.h:274-308), capacity defaulting to
+        target, into a zeroed dst.  Returns (ret, bytes)."""
+        return self._decompress_partial(data, target, capacity)[:2]
+
+    def _decompress_partial(self, data, target, capacity):
+        """(ret, bytes, lastPath) after checking that nothing at or past outputSize = min(target, capacity) was written"""
+        cap = int(target) if capacity is None else int(capacity)
+        src = _as_u8(data) if len(data) else np.zeros(1, dtype=np.uint8)
+        room = max(min(int(target), cap), 0)
+        dst = np.zeros(room + 64, dtype=np.uint8)
+        dst[room:] = 0xA5
+        r, last = self._partial(_ptr(src), _ptr(dst), len(data), int(target), cap)
+        assert (dst[room:] == 0xA5).all(), "partial decode wrote at or past outputSize"
+        return r, dst[:max(r, 0)].tobytes(), last
+
 
 class Oracle(_Codec):
     name = "port"
@@ -79,6 +113,10 @@ class Oracle(_Codec):
         lib.oracle_lz4_compress_fast.argtypes = [_u8p, _u8p, C.c_int, C.c_int, C.c_int]
         lib.oracle_lz4_decompress_safe.restype = C.c_int
         lib.oracle_lz4_decompress_safe.argtypes = [_u8p, _u8p, C.c_int, C.c_int]
+        lib.oracle_lz4_compress_destSize_extState.restype = C.c_int
+        lib.oracle_lz4_compress_destSize_extState.argtypes = [_u8p, _u8p, _ip, C.c_int, C.c_int, _ip]
+        lib.oracle_lz4_decompress_safe_partial.restype = C.c_int
+        lib.oracle_lz4_decompress_safe_partial.argtypes = [_u8p, _u8p, C.c_int, C.c_int, C.c_int, _ip]
         lib.oracle_datagen.restype = None
         lib.oracle_datagen.argtypes = [_u8p, C.c_size_t, C.c_double, C.c_double, C.c_uint]
         lib.oracle_datagen_mt.restype = None
@@ -98,6 +136,24 @@ class Oracle(_Codec):
         self._bound = lib.oracle_lz4_compress_bound
         self._compress = lib.oracle_lz4_compress_fast
         self._decompress = lib.oracle_lz4_decompress_safe
+
+    def _dest_size(self, sp, dp, n, target, acceleration):
+        path = C.c_int(-1)
+        acc = 1 if acceleration is None else int(acceleration)
+        r = self.lib.oracle_lz4_compress_destSize_extState(sp, dp, C.byref(n), target, acc, C.byref(path))
+        return int(r), path.value
+
+    def _partial(self, sp, dp, size, target, cap):
+        last = C.c_int(0)
+        r = self.lib.oracle_lz4_decompress_safe_partial(sp, dp, size, target, cap, C.byref(last))
+        return int(r), last.value
+
+    def decompress_partial_traced(self, data, target, capacity=None):
+        """decompress_partial plus how the decode ended: (ret, bytes, last_path, dst_dependent).  last_path is 1 after
+        literals, 2 inside a match, 0 otherwise; dst_dependent says whether the reference's bytes depend on what dst
+        held (an offset-0 match on its cut path, lz4.c:2392-2404), where the oracle writes zeros."""
+        r, out, last = self._decompress_partial(data, target, capacity)
+        return r, out, last & 3, bool(last & 4)
 
     # --- data generator (tests/datagen.c RDG_genBuffer) ---
     def datagen(self, size, proba=0.5, seed=0, lit_proba=0.0):
@@ -167,11 +223,27 @@ class Reference(_Codec):
         lib.LZ4_compress_fast.argtypes = [_u8p, _u8p, C.c_int, C.c_int, C.c_int]
         lib.LZ4_decompress_safe.restype = C.c_int
         lib.LZ4_decompress_safe.argtypes = [_u8p, _u8p, C.c_int, C.c_int]
+        lib.LZ4_compress_destSize.restype = C.c_int
+        lib.LZ4_compress_destSize.argtypes = [_u8p, _u8p, _ip, C.c_int]
+        lib.LZ4_compress_destSize_extState.restype = C.c_int
+        lib.LZ4_compress_destSize_extState.argtypes = [C.c_void_p, _u8p, _u8p, _ip, C.c_int, C.c_int]
+        lib.LZ4_decompress_safe_partial.restype = C.c_int
+        lib.LZ4_decompress_safe_partial.argtypes = [_u8p, _u8p, C.c_int, C.c_int, C.c_int]
         lib.RDG_genBuffer.restype = None
         lib.RDG_genBuffer.argtypes = [_u8p, C.c_size_t, C.c_double, C.c_double, C.c_uint]
         self._bound = lib.LZ4_compressBound
         self._compress = lib.LZ4_compress_fast
         self._decompress = lib.LZ4_decompress_safe
+        self.ext_state = np.zeros(16416 // 8, dtype=np.uint64)     # sizeof(LZ4_stream_t), lz4.h:729-733
+
+    def _dest_size(self, sp, dp, n, target, acceleration):
+        if acceleration is None:
+            return int(self.lib.LZ4_compress_destSize(sp, dp, C.byref(n), target)), None
+        return int(self.lib.LZ4_compress_destSize_extState(self.ext_state.ctypes.data, sp, dp, C.byref(n), target,
+                                                           int(acceleration))), None
+
+    def _partial(self, sp, dp, size, target, cap):
+        return int(self.lib.LZ4_decompress_safe_partial(sp, dp, size, target, cap)), 0
 
     def datagen(self, size, proba=0.5, seed=0, lit_proba=0.0):
         buf = np.empty(int(size), dtype=np.uint8)

@@ -16,9 +16,8 @@ import sys
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-for _p in (ROOT, os.path.join(ROOT, "tests")):
-    if _p not in sys.path:
-        sys.path.insert(0, _p)
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 OUT = os.path.join(HERE, "kat_destsize.json")
@@ -97,7 +96,6 @@ RUN_CASES, RUN_CHUNK = 3000, 250
 
 def main():
     from oracle.pyoracle import Reference
-    from destsize_oracle import reference_dest_size
     ref = Reference()
     ins, vecs = [], []
     for (iid, size, kind, seed) in inputs():
@@ -107,12 +105,12 @@ def main():
         for ti, t in enumerate(targets(size, fast)):
             # the plain entry point for every target, _extState with the accelerations in turn
             for acc in (None, ACCELS[(iid + ti) % len(ACCELS)]):
-                r, c, out, _ = reference_dest_size(ref, d, t, acc)
+                r, c, out, _ = ref.compress_dest_size(d, t, acc)
                 vecs.append([iid, t, acc, r, c, out.hex() if len(out) <= HEX_MAX else sha(out)])
     runs = []
     res = []
     for d, t, acc in random_cases(ref, RUN_CASES):
-        r, c, out, _ = reference_dest_size(ref, d, t, acc)
+        r, c, out, _ = ref.compress_dest_size(d, t, acc)
         res.append((r, c, out))
         if len(res) == RUN_CHUNK:
             runs.append(run_digest(res))

@@ -1,6 +1,7 @@
-"""LZ4_compress_destSize on the CPU: the fill parse of tests/destsize_oracle.c (oracle_lz4_compress_destSize) against the reference's
-results in tests/golden/kat_destsize.json (tests/golden/make_golden_destsize.py), its properties, a live differential
-against the compiled reference when it is present, and the drop-in's behaviour without a device."""
+"""LZ4_compress_destSize on the CPU: the fill parse of oracle/lz4_oracle.c (oracle_lz4_compress_destSize_extState)
+against the reference's results in tests/golden/kat_destsize.json (tests/golden/make_golden_destsize.py), its
+properties, a live differential against the compiled reference when it is present, and the drop-in's behaviour without
+a device."""
 import collections
 import ctypes as C
 import os
@@ -9,7 +10,7 @@ import numpy as np
 import pytest
 
 from conftest import load_golden
-from destsize_oracle import PATHS as PATHS_BY_CODE, DestSizeOracle, reference_dest_size
+from oracle.pyoracle import PATHS as PATHS_BY_CODE
 from golden.make_golden_destsize import ACCELS, inputs, make_input, random_cases, run_digest, sha, HEX_MAX
 
 PATHS = ["fast", "empty", "no_room", "literals", "next_match", "reduced", "last_literals", "filled"]
@@ -39,17 +40,12 @@ def path_name(code):
     return PATHS_BY_CODE[code]
 
 
-@pytest.fixture(scope="module")
-def ds():
-    return DestSizeOracle()
-
-
-def test_oracle_reproduces_every_golden_vector(kat, kat_inputs, oracle, ds):
+def test_oracle_reproduces_every_golden_vector(kat, kat_inputs, oracle):
     seen = collections.Counter()
     fill_accels = set()
     for iid, target, acc, ret, consumed, out in kat["vectors"]:
         d = kat_inputs[iid]
-        r, c, o, path = ds.compress_dest_size(d, target, acc)
+        r, c, o, path = oracle.compress_dest_size(d, target, acc)
         assert (r, c, _out_key(o)) == (ret, consumed, out), (iid, len(d), target, acc)
         seen[(path_name(path), len(d) < 65547)] += 1
         if path_name(path) in PATHS[3:]:
@@ -62,10 +58,10 @@ def test_oracle_reproduces_every_golden_vector(kat, kat_inputs, oracle, ds):
     assert fill_accels == set(ACCELS) | {None}
 
 
-def test_oracle_reproduces_the_run_digest(kat, oracle, ds):
+def test_oracle_reproduces_the_run_digest(kat, oracle):
     res, digests = [], []
     for d, t, acc in random_cases(oracle, kat["run_cases"]):
-        r, c, o, _ = ds.compress_dest_size(d, t, acc)
+        r, c, o, _ = oracle.compress_dest_size(d, t, acc)
         res.append((r, c, o))
         if len(res) == kat["run_chunk"]:
             digests.append(run_digest(res))
@@ -73,7 +69,7 @@ def test_oracle_reproduces_the_run_digest(kat, oracle, ds):
     assert digests == kat["run_digests"]
 
 
-def test_properties_over_random_cases(oracle, ds):
+def test_properties_over_random_cases(oracle):
     rng = np.random.default_rng(7)
     for k in range(600):
         n = int(rng.choice([1, 13, 50, 500, 5000, 65546, 65547, 90000]))
@@ -81,7 +77,7 @@ def test_properties_over_random_cases(oracle, ds):
         b = oracle.compress_bound(n)
         t = int(rng.integers(1, b + 2))
         acc = int(rng.choice(ACCELS))
-        r, c, o, path = ds.compress_dest_size(d, t, acc)
+        r, c, o, path = oracle.compress_dest_size(d, t, acc)
         assert 0 < r <= t and 0 <= c <= n, (n, t, acc, r, c)
         # the v1.9.2 guarantee (lz4.h:261-270): the output decodes with a capacity of exactly `consumed`
         assert oracle.decompress(o, c) == (c, d[:c].tobytes()), (n, t, acc)
@@ -90,21 +86,21 @@ def test_properties_over_random_cases(oracle, ds):
             assert (r, o) == oracle.compress(d, acc, t)
 
 
-def test_routes_in_front_of_the_parse(oracle, ds):
+def test_routes_in_front_of_the_parse(oracle):
     d = make_input(oracle, 1000, "p50", 1)
-    assert ds.compress_dest_size(d, 0, None)[:2] == (0, 1000)
-    assert ds.compress_dest_size(d, -5, 3)[:2] == (0, 1000)
-    assert ds.compress_dest_size(b"", 0, None)[:2] == (0, 0)
-    assert ds.compress_dest_size(b"", 1, None)[:3] == (1, 0, b"\x00")
-    assert ds.compress_dest_size(b"", 16, None)[:3] == (1, 0, b"\x00")
+    assert oracle.compress_dest_size(d, 0, None)[:2] == (0, 1000)
+    assert oracle.compress_dest_size(d, -5, 3)[:2] == (0, 1000)
+    assert oracle.compress_dest_size(b"", 0, None)[:2] == (0, 0)
+    assert oracle.compress_dest_size(b"", 1, None)[:3] == (1, 0, b"\x00")
+    assert oracle.compress_dest_size(b"", 16, None)[:3] == (1, 0, b"\x00")
     # the ends of the acceleration range are brought into it (documented deviations)
-    assert ds.compress_dest_size(d, 300, 0)[:3] == ds.compress_dest_size(d, 300, 1)[:3]
-    assert ds.compress_dest_size(d, 300, 1 << 30)[:3] == ds.compress_dest_size(d, 300, (1 << 25) - 1)[:3]
+    assert oracle.compress_dest_size(d, 300, 0)[:3] == oracle.compress_dest_size(d, 300, 1)[:3]
+    assert oracle.compress_dest_size(d, 300, 1 << 30)[:3] == oracle.compress_dest_size(d, 300, (1 << 25) - 1)[:3]
 
 
-def test_live_differential_against_the_reference(oracle, reference, ds):
+def test_live_differential_against_the_reference(oracle, reference):
     for k, (d, t, acc) in enumerate(random_cases(oracle, 400)):
-        assert ds.compress_dest_size(d, t, acc)[:3] == reference_dest_size(reference, d, t, acc)[:3], (k, len(d), t, acc)
+        assert oracle.compress_dest_size(d, t, acc)[:3] == reference.compress_dest_size(d, t, acc)[:3], (k, len(d), t, acc)
 
 
 def test_drop_in_without_a_device_leaves_srcsize_alone():

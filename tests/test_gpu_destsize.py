@@ -9,8 +9,8 @@ import pytest
 import torch
 
 from conftest import load_golden
-from destsize_oracle import PATHS, DestSizeOracle
 from golden.make_golden_destsize import ACCELS, HEX_MAX, inputs, make_input, sha
+from oracle.pyoracle import PATHS
 
 pytestmark = pytest.mark.gpu
 
@@ -26,11 +26,6 @@ def lib():
     if lib.LZ4B200_device_count() <= 0:
         pytest.skip("no CUDA device")
     return lib
-
-
-@pytest.fixture(scope="module")
-def ds():
-    return DestSizeOracle()
 
 
 def bound(n):
@@ -79,10 +74,10 @@ def dest_batch(lib, blocks, target, acc, src_phase=0, dst_phase=0, src_pad=0, ds
     return res
 
 
-def check_against_oracle(ds, blocks, target, acc, res):
+def check_against_oracle(oracle, blocks, target, acc, res):
     paths = collections.Counter()
     for i, (b, got) in enumerate(zip(blocks, res)):
-        r, c, o, p = ds.compress_dest_size(b, target, acc)
+        r, c, o, p = oracle.compress_dest_size(b, target, acc)
         assert got == (r, c, o), (i, len(b), target, acc, got[:2], (r, c))
         paths[p] += 1
     return paths
@@ -167,13 +162,13 @@ def test_golden_vectors_batch(lib, kat):
 TARGETS_64K = [-1, 0] + list(range(1, 21)) + [64, 100, 4096, 16384, 32768, 65535, bound(65536) - 1, bound(65536)]
 
 
-def test_64k_datagen_blocks_every_target_and_acceleration(lib, oracle, ds):
+def test_64k_datagen_blocks_every_target_and_acceleration(lib, oracle):
     blocks = [oracle.datagen(65536, p, 100 * k + s) for k, p in enumerate([0.0, 0.5, 0.9, 0.99]) for s in range(4)]
     paths = collections.Counter()
     for target in TARGETS_64K:
         for acc in (1, 2, 8, 65537, 65538, 1 << 20):
             res = dest_batch(lib, blocks, target, acc)
-            paths += check_against_oracle(ds, blocks, target, acc, res)
+            paths += check_against_oracle(oracle, blocks, target, acc, res)
             if target in (100, 4096, 32768):
                 assert_round_trip(lib, blocks, res)
     assert {PATHS[p] for p in paths} == {"fast", "no_room", "literals", "next_match", "reduced",
@@ -187,23 +182,23 @@ MIXED_SIZES = [0, 1, 12, 13, 14, 100, 4095, 65535, 65546, 65547, 65548, 200000, 
 
 @pytest.mark.parametrize("target,acc", [(1, 1), (20, 8), (4096, 1), (30000, 2), (65537, 65538), (1 << 20, 1),
                                         (bound(4 << 20), 1 << 20), (bound(4 << 20) - 1, (1 << 25) - 1)])
-def test_mixed_sizes_odd_strides_and_phases(lib, oracle, target, acc, ds):
+def test_mixed_sizes_odd_strides_and_phases(lib, oracle, target, acc):
     kinds = ["p50", "p90", "random", "period", "zero", "p0", "p99"]
     blocks = [make_input(oracle, n, kinds[i % len(kinds)], 300 + i) for i, n in enumerate(MIXED_SIZES)]
     res = dest_batch(lib, blocks, target, acc, src_phase=3, dst_phase=5, src_pad=7, dst_pad=9)
-    check_against_oracle(ds, blocks, target, acc, res)
+    check_against_oracle(oracle, blocks, target, acc, res)
     assert_round_trip(lib, blocks, res)
 
 
 # ---- 6. warps that compress many blocks of both table types, fill exits in between ----
 
-def test_warps_rezero_the_table_between_blocks(lib, oracle, ds):
+def test_warps_rezero_the_table_between_blocks(lib, oracle):
     nb = 3600                                       # above the grid (13 warps per SM): every warp takes 2-3 blocks
     big = oracle.datagen_mt(nb * 66000, 66000, 0.6, 11)
     sizes = [66000 if i % 3 == 0 else (100 if i % 4 == 3 else 20000) for i in range(nb)]
     blocks = [big[i * 66000:i * 66000 + sizes[i]] for i in range(nb)]
     res = dest_batch(lib, blocks, 5000, 1)
-    paths = check_against_oracle(ds, blocks, 5000, 1, res)
+    paths = check_against_oracle(oracle, blocks, 5000, 1, res)
     assert paths[0] > 0 and sum(paths.values()) - paths[0] > 1000
 
 
@@ -245,7 +240,7 @@ def test_launch_count_and_argument_errors(lib):
 # ---- 8. seeded fuzz loop through the drop-in entry points (fuzzer.c:399-420, 488-492, 1694-1704) ----
 
 @pytest.mark.parametrize("seed", [1, 2, 2026])
-def test_fuzz_drop_in(lib, oracle, seed, ds):
+def test_fuzz_drop_in(lib, oracle, seed):
     from lz4_b200 import block
     rng = np.random.default_rng(seed)
     state = np.zeros(2052, dtype=np.uint64)
@@ -274,4 +269,4 @@ def test_fuzz_drop_in(lib, oracle, seed, ds):
             assert oracle.decompress(dst[:r].tobytes(), cnt.value) == (cnt.value, d[:cnt.value].tobytes())
         if it % 3 == 1 and target > 0:
             assert cnt.value < n                                    # fuzzer.c:490: consumes less than the input
-        assert (r, cnt.value, dst[:r].tobytes()) == ds.compress_dest_size(d, target, acc)[:3], (seed, it, n, target, acc)
+        assert (r, cnt.value, dst[:r].tobytes()) == oracle.compress_dest_size(d, target, acc)[:3], (seed, it, n, target, acc)

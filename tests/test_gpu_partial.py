@@ -2,7 +2,7 @@
 
 Every case of tests/golden/kat_partial.json (results of the compiled reference) goes through the drop-in call and
 through batch calls, grouped by target and as one batch of per-block targets; the bytes are compared with the checker
-(tests/partial_oracle.c), itself pinned to the reference's digests.  The cases include srcSize = exact .. exact + 9 at
+(oracle_lz4_decompress_safe_partial), itself pinned to the reference's digests.  The cases include srcSize = exact .. exact + 9 at
 target = decoded size (the reference's tests/decompress-partial.c) and the exhaustive target sweeps.  Also: routes P1 / P2 through the slow list, guard bytes at and
 past every slot's return value, launch counts, argument errors, equality with the full decode, and a seeded fuzz loop.
 """
@@ -15,13 +15,11 @@ import pytest
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, HERE)
 sys.path.insert(0, os.path.join(HERE, "golden"))
 
 import make_golden_partial as mg  # noqa: E402
 from lz4_b200 import _lib, batch, block  # noqa: E402
 from oracle.pyoracle import Oracle  # noqa: E402
-from partial_oracle import PartialOracle, golden  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -30,7 +28,7 @@ GUARD = 0xA5
 
 @pytest.fixture(scope="module")
 def kat():
-    return golden()
+    return mg.golden()
 
 
 def pack(srcs):
@@ -78,23 +76,22 @@ def run_batch(srcs, targets, stride=None, shift=0, ws=None):
     return r, slots, slow
 
 
-def test_drop_in_matches_the_reference(kat):
+def test_drop_in_matches_the_reference(kat, oracle):
     _, groups = kat
-    po = PartialOracle()
     for name, cases, rets, digest in groups:
         res = []
         for src, t, c in cases:
             got = block.LZ4_decompress_safe_partial(src, t, c)
-            assert got == po.decompress_partial(src, t, c), (name, t, c)
-            res.append((got[0], None if po.dst_dependent else got[1]))
+            r, out, _, dst_dependent = oracle.decompress_partial_traced(src, t, c)
+            assert got == (r, out), (name, t, c)
+            res.append((got[0], None if dst_dependent else got[1]))
         assert [r for r, _ in res] == rets and mg.run_digest(res) == digest, name
 
 
-def test_batches_by_target_and_per_block(kat):
+def test_batches_by_target_and_per_block(kat, oracle):
     """every case with capacity = target: one batch per target, then one batch of per-block targets (the exhaustive
     sweeps included) at an odd stride and an unaligned base"""
     _, groups = kat
-    po = PartialOracle()
     flat = [(src, t, r) for _, cases, rets, _ in groups for (src, t, c), r in zip(cases, rets) if t == c]
     by_t = defaultdict(list)
     for x in flat:
@@ -102,17 +99,16 @@ def test_batches_by_target_and_per_block(kat):
     for t, xs in sorted(by_t.items()):
         rets, slots, _ = run_batch([x[0] for x in xs], t)
         for (src, _, want), r, s in zip(xs, rets, slots):
-            assert r == want and (r, s) == po.decompress_partial(src, t), (t, want, r)
+            assert r == want and (r, s) == oracle.decompress_partial(src, t), (t, want, r)
     small = [x for x in flat if x[1] <= 70000]
     rets, slots, _ = run_batch([x[0] for x in small], [x[1] for x in small], stride=70001, shift=3)
     for (src, t, want), r, s in zip(small, rets, slots):
-        assert r == want and (r, s) == po.decompress_partial(src, t), (t, want, r)
+        assert r == want and (r, s) == oracle.decompress_partial(src, t), (t, want, r)
 
 
-def test_stops_in_every_run_class():
+def test_stops_in_every_run_class(oracle):
     """literal stops, match stops at 0..13 bytes from its end, offsets 0, 1 and < 8, and the last 5 bytes as a match
     (which LZ4_decompress_safe rejects)"""
-    po = PartialOracle()
     rng = np.random.default_rng(5)
     lit = rng.integers(0, 256, 40, dtype=np.uint8).tobytes()
     cases = []
@@ -127,7 +123,7 @@ def test_stops_in_every_run_class():
     cases += [(blk, t) for t in (1, 5, 6, 100, 200, 289, 290)]
     rets, slots, _ = run_batch([c[0] for c in cases], [c[1] for c in cases], stride=400)
     for (b, t), r, s in zip(cases, rets, slots):
-        assert (r, s) == po.decompress_partial(b, t), (b[:4].hex(), t)
+        assert (r, s) == oracle.decompress_partial(b, t), (b[:4].hex(), t)
     assert block.LZ4_decompress_safe(blk, 300)[0] < 0
 
 
@@ -148,11 +144,11 @@ def test_routes():
     # > 8 192 sequences: 4-byte matches between single literals
     seqs = b"".join(bytes([0x10, 0x41 + (k % 20), 1, 0]) for k in range(9000)) + bytes([0x50]) + b"ABCDE"
     rets, slots, slow = run_batch([seqs], 45000 + 5)
-    assert slow == 1 and (rets[0], slots[0]) == PartialOracle().decompress_partial(seqs, 45005)
+    assert slow == 1 and (rets[0], slots[0]) == orc.decompress_partial(seqs, 45005)
     # > 20 480 runs with <= 8 192 sequences: 1 literal + an offset-0 match of 4 (4 runs each)
     runs = b"".join(bytes([0x10, 0x30 + (k % 9), 0, 0]) for k in range(6000)) + bytes([0x50]) + b"ABCDE"
     rets, slots, slow = run_batch([runs], 30005)
-    assert slow == 1 and (rets[0], slots[0]) == PartialOracle().decompress_partial(runs, 30005)
+    assert slow == 1 and (rets[0], slots[0]) == orc.decompress_partial(runs, 30005)
 
 
 def test_launch_counts_and_argument_errors():

@@ -15,12 +15,9 @@ import numpy as np
 import pytest
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, HERE)
 sys.path.insert(0, os.path.join(HERE, "golden"))
 
 import make_golden_partial as mg  # noqa: E402
-from oracle.pyoracle import Oracle  # noqa: E402
-from partial_oracle import PartialOracle, golden  # noqa: E402
 
 _u32p = C.POINTER(C.c_uint32)
 
@@ -50,27 +47,25 @@ def run(lib, src, cap):
     return r, ns.value, used.value, list(marks)[:min(ns.value, mcap)], out.raw[:r] if ok else None
 
 
-def test_emulated_partial_decode_matches_the_reference(emul):
-    _, groups = golden()
-    po = PartialOracle()
+def test_emulated_partial_decode_matches_the_reference(emul, oracle):
+    _, groups = mg.golden()
     rebuilt = 0
     for name, cases, rets, _ in groups:
         for (src, t, c), want in zip(cases, rets):
             r, _, used, _, out = run(emul, src, min(t, c))
             assert r == want, (name, t, c)
             if out is not None:
-                assert out == po.decompress_partial(src, t, c)[1] and used <= len(src), (name, t, c)
+                assert out == oracle.decompress_partial(src, t, c)[1] and used <= len(src), (name, t, c)
                 rebuilt += 1
     assert rebuilt > 10000
 
 
-def test_marks_and_last_sequence_encoding(emul):
-    orc = Oracle()
+def test_marks_and_last_sequence_encoding(emul, oracle):
     checked = 0
     for (bid, size, kind, seed) in mg.blocks():
         if not 0 < size <= 65536:
             continue
-        raw, comp = mg.make_block(orc, size, kind, seed)
+        raw, comp = mg.make_block(oracle, size, kind, seed)
         seqs = mg.sequences(comp)
         starts = [s[0] for s in seqs] + [seqs[-1][2] if seqs else 0]     # the final literal run starts after the last match
         for t in sorted(x for x in {1, 4, 5, 17, 64, 65, 1000, 4096, 65535, size} if x <= size):
@@ -101,13 +96,12 @@ def test_zero_byte_final_token_at_64k(emul):
     assert ns == 3 and used == len(blk) and marks[2] >> 16 == 0 and marks[2] & 0xFFFF == len(blk) - 1
 
 
-def test_big_blocks_take_the_rows_window_at_61440(emul):
-    orc = Oracle()
+def test_big_blocks_take_the_rows_window_at_61440(emul, oracle):
     n = 0
     for (bid, size, kind, seed) in mg.blocks():
         if size != 4 << 20:
             continue
-        raw, comp = mg.make_block(orc, size, kind, seed)
+        raw, comp = mg.make_block(oracle, size, kind, seed)
         for t in (4096, 30000, 61440):
             r, ns, used, _, out = run(emul, comp, t)
             assert r == t and (out is None or out == raw[:t])
