@@ -236,6 +236,31 @@ LZ4B200_API int LZ4B200_compress_blocks_hc(const void* d_src, int64_t srcStride,
                                            void* d_workspace, size_t workspaceBytes, void* stream);
 
 /*
+ * Compress as much of every block as fits a fixed-size destination at an HC level (the batched LZ4_compress_HC_destSize,
+ * lz4hc.h:83-94 / lz4hc.c:1538-1545):
+ *   block i input : d_src + i*srcStride, size n_i = (d_srcSize ? d_srcSize[i] : srcSize)
+ *   block i output: d_dst + i*dstStride; nothing at or past dst_i + min(targetDstSize, LZ4_compressBound(n_i)) is
+ *                   written, and the slot's bytes past d_outSize[i] below that limit are unspecified
+ *   d_outSize[i]    : LZ4_compress_HC_destSize(state, src_i, dst_i, &n_i, targetDstSize, compressionLevel)
+ *   d_srcConsumed[i]: what that call leaves in n_i -- the input bytes block i's output holds, or n_i itself where the
+ *                     reference leaves it alone (targetDstSize < 1, a size outside 0 .. LZ4_MAX_INPUT_SIZE)
+ * The bytes and both values are the reference's.  Levels are those of LZ4B200_compress_blocks_hc; unlike
+ * LZ4_compress_destSize there is no unlimited route: the fill parse (fillOutput, lz4hc.c:1340-1359 and 747-772) runs at
+ * every target from 1 up, the bound and above included.  Every block starts from a fresh state.
+ * The input is read in aligned 4-byte words, each of which holds at least one byte of the block.
+ * The workspace is at least LZ4B200_compress_blocks_hc_workspace_bytes(nBlocks) bytes, as for LZ4B200_compress_blocks_hc.
+ * One kernel launch; nBlocks == 0 returns LZ4B200_OK without one.  LZ4B200_ERR_ARG: compressionLevel >= 10, nBlocks < 0,
+ * a NULL d_dst, d_outSize, d_srcConsumed or d_workspace, a NULL d_src with blocks present, or a workspace smaller than
+ * the size function asks.  LZ4_compress_HC_destSize itself is not exported: the drop-in HC family keeps resolving to
+ * the reference until it serves every level.
+ */
+LZ4B200_API int LZ4B200_compress_blocks_hc_destSize(const void* d_src, int64_t srcStride, const int32_t* d_srcSize,
+                                                    int32_t srcSize, void* d_dst, int64_t dstStride, int32_t targetDstSize,
+                                                    int compressionLevel, int32_t* d_outSize, int32_t* d_srcConsumed,
+                                                    int64_t nBlocks, void* d_workspace, size_t workspaceBytes,
+                                                    void* stream);
+
+/*
  * The same call with the PARALLEL PARSE (throughput mode): every block is a valid LZ4 block that
  * LZ4_decompress_safe expands to the input, the result is deterministic, but it is NOT byte-identical to
  * LZ4_compress_fast: every position is a match candidate (no skipping), matches are chosen by the same greedy

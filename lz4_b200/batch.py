@@ -195,6 +195,34 @@ def compress_blocks_dest_size(src, block_size, target, acceleration=1, slots=Non
     return slots, out_sizes[:n], consumed[:n], stride
 
 
+def compress_blocks_hc_dest_size(src, block_size, target, level=9, slots=None, slot_stride=None, out_sizes=None,
+                                 consumed=None, src_sizes=None, stream=None):
+    """Compress as much of each block of src as fits into `target` bytes at an HC level
+    (LZ4B200_compress_blocks_hc_destSize: block i is LZ4_compress_HC_destSize(state, block_i, slot_i, &n_i, target, level)).
+
+    Levels 1 .. 9 (below 1 means 9); 10 .. 12 raise, their optimal parser is not built.
+    Returns (slots, out_sizes, consumed, slot_stride): block i's bytes are slots[i*slot_stride : i*slot_stride+out_sizes[i]]
+    and hold its first consumed[i] input bytes.
+    """
+    lib = _lib.load()
+    _need_cuda(src, slots, src_sizes)
+    room = max(min(int(target), compress_bound(block_size)), 1)
+    st = _stream(stream)
+    n, stride, slots, out_sizes, src_sizes = _compress_layout(src, block_size, room, slots, slot_stride, out_sizes,
+                                                              src_sizes, st)
+    if consumed is None:
+        with torch.cuda.stream(st):
+            consumed = torch.empty(max(n, 1), dtype=torch.int32, device=src.device)
+    workspace = _workspace(src.device, max(int(lib.LZ4B200_compress_blocks_hc_workspace_bytes(n)), 1), st)
+    rc = lib.LZ4B200_compress_blocks_hc_destSize(src.data_ptr(), int(block_size),
+                                                 src_sizes.data_ptr() if src_sizes is not None else None,
+                                                 int(block_size), slots.data_ptr(), stride, int(target), int(level),
+                                                 out_sizes.data_ptr(), consumed.data_ptr(), n, workspace.data_ptr(),
+                                                 workspace.numel(), st.cuda_stream)
+    _lib.check(rc, "LZ4B200_compress_blocks_hc_destSize")
+    return slots, out_sizes[:n], consumed[:n], stride
+
+
 def pack_blocks(slots, slot_stride, sizes, header_bytes=0, packed=None, stream=None):
     """Gather variable-size blocks into one contiguous stream.  Returns (packed, offsets[n+1])."""
     lib = _lib.load()

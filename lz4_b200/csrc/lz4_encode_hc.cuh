@@ -5,7 +5,8 @@
  * lz4_hc_core.h, and the parallelism is across blocks.  A block's state is a 2^15 x u32 hash table and a 64 K x u16
  * chain table (256 KB), more than an SM's shared memory, so every thread owns one workspace slot in global memory and
  * takes blocks t, t + slots, t + 2 * slots, ...  The hash table is zeroed before every block; the chain table is not
- * (lz4_hc_core.h shows why no entry is read before it is written).  DESIGN.md section 3.7.
+ * (lz4_hc_core.h shows why no entry is read before it is written).  lz4_encode_hc_dest_kernel runs the fill parse of
+ * LZ4_compress_HC_destSize on the same layout.  DESIGN.md section 3.7.
  */
 
 constexpr int kHcThreads = 32;
@@ -38,11 +39,12 @@ struct HcDevAcc {
     }
 };
 
-/* slots = the threads that run: min(nBlocks, workspace slots) */
-__global__ void __launch_bounds__(kHcThreads) lz4_encode_hc_kernel(lz4k_encode_args a, uint8_t* ws, int64_t slots, int level)
+/* One slot's blocks: t, t + slots, ...  FILL: LZ4_compress_HC_destSize with targetDstSize = a.dstCap, which also writes
+ * srcConsumed[b]. */
+template <bool FILL>
+__device__ __forceinline__ void hc_slot_blocks(const lz4k_encode_args& a, int32_t* srcConsumed, uint8_t* ws, int64_t t,
+                                               int64_t slots, int level)
 {
-    const int64_t t = (int64_t)blockIdx.x * kHcThreads + threadIdx.x;
-    if (t >= slots) return;
     HcDevAcc acc;
     acc.ht = reinterpret_cast<uint32_t*>(ws + t * kHcSlotBytes);
     acc.ct = reinterpret_cast<uint16_t*>(ws + t * kHcSlotBytes + kHcHashBytes);
@@ -54,6 +56,30 @@ __global__ void __launch_bounds__(kHcThreads) lz4_encode_hc_kernel(lz4k_encode_a
             uint4* h = reinterpret_cast<uint4*>(acc.ht);
             for (int k = 0; k < (int)(kHcHashBytes / sizeof(uint4)); k++) h[k] = make_uint4(0, 0, 0, 0);
         }
-        a.outSize[b] = hc::hc_compress_block(acc, n, a.dstCap, level);
+        if (FILL) {
+            int consumed;
+            a.outSize[b] = hc::hc_compress_block_dest(acc, n, a.dstCap, level, consumed);
+            srcConsumed[b] = consumed;
+        } else {
+            a.outSize[b] = hc::hc_compress_block(acc, n, a.dstCap, level);
+        }
     }
+}
+
+/* slots = the threads that run: min(nBlocks, workspace slots) */
+__global__ void __launch_bounds__(kHcThreads) lz4_encode_hc_kernel(lz4k_encode_args a, uint8_t* ws, int64_t slots, int level)
+{
+    const int64_t t = (int64_t)blockIdx.x * kHcThreads + threadIdx.x;
+    if (t >= slots) return;
+    hc_slot_blocks<false>(a, nullptr, ws, t, slots, level);
+}
+
+/* the same slots and grid, LZ4_compress_HC_destSize per block: the parse stops at the target, so a block costs the input
+ * it consumes */
+__global__ void __launch_bounds__(kHcThreads) lz4_encode_hc_dest_kernel(lz4k_encode_args a, int32_t* srcConsumed, uint8_t* ws,
+                                                                        int64_t slots, int level)
+{
+    const int64_t t = (int64_t)blockIdx.x * kHcThreads + threadIdx.x;
+    if (t >= slots) return;
+    hc_slot_blocks<true>(a, srcConsumed, ws, t, slots, level);
 }

@@ -6,6 +6,8 @@
  *   levels 1 .. 2 (and the lz4mid entries of the level table): LZ4MID_compress, lz4hc.c:522-773
  *   levels 3 .. 9 (and < 1 -> 9):                             LZ4HC_compress_hashChain, lz4hc.c:1121-1362
  * Levels 10 .. 12 use the optimal parser, which is not built here: hc_compress_block returns kHcNoLevel for them.
+ * Both parses take the reference's fillOutput directive as the template flag FILL: hc_compress_block_dest is
+ * LZ4_compress_HC_destSize (lz4hc.c:1538-1545), which compresses as much input as fits a fixed-size output.
  *
  * Positions are byte offsets into the block.  The reference's indices are position + kHcStart (LZ4HC_init_internal,
  * lz4hc.c:242-259, starts a fresh state at 64 KB), so a zero hash entry is never a candidate.
@@ -18,7 +20,8 @@
  *   void out(int64_t o, uint32_t v); void copy(int64_t o, uint32_t p, uint32_t len)    output byte / literal copy
  * The chain table needs no initial value: the hash-chain walk only reads the entry of an index in
  * [ipIndex - 65535, ipIndex), and LZ4HC_Insert has written every such index before the walk, the entry of index i last.
- * Nothing is written at or past the capacity: every output byte is written after the check that covers it.
+ * Nothing is written at or past the capacity: every output byte is written after the check that covers it (the fill
+ * parse's unchecked last sequence after its room test against oend - 3).
  */
 #ifndef LZ4_HC_CORE_H
 #define LZ4_HC_CORE_H
@@ -114,10 +117,13 @@ template <class A> HC_FN uint32_t reverse_count_pattern(A& a, uint32_t p, uint32
     return k;
 }
 
+/* Offsets are signed: the fill parse's end lies LASTLITERALS before the target while it parses, before dst for targets
+ * below 8, and every comparison with it must then come out "does not fit". */
 struct Out {
     int64_t op;           /* bytes written */
-    int64_t cap;          /* dstCapacity */
-    bool limited;         /* limitedOutput */
+    int64_t cap;          /* dstCapacity; oend - LASTLITERALS while the fill parse runs (lz4hc.c:565, 1154) */
+    bool limited;         /* limitedOutput (fillOutput included) */
+    uint32_t consumed;    /* the fill parse: the input bytes the output holds */
 };
 
 /* the length bytes after a 15 in a token nibble */
@@ -158,12 +164,22 @@ template <class A> HC_FN bool encode_sequence(A& a, Out& o, uint32_t& ip, uint32
     return true;
 }
 
-/* the last literals (lz4hc.c:1308-1334, 707-735): the block's size, or 0 when they do not fit a limited output */
-template <class A> HC_FN int last_literals(A& a, Out& o, uint32_t anchor, uint32_t n)
+/* the last literals (lz4hc.c:1308-1337, 707-741): the block's size, or 0 when they do not fit a limited output.  The
+ * fill parse restores its end and takes as many literals as fit there. */
+template <bool FILL, class A> HC_FN int last_literals(A& a, Out& o, uint32_t anchor, uint32_t n)
 {
-    const uint32_t run = n - anchor;
+    uint32_t run = n - anchor;
     const int64_t total = 1 + (int64_t)(run + 255 - 15) / 255 + run;
-    if (o.limited && o.op + total > o.cap) return 0;
+    if (FILL) {
+        o.cap += kLastLiterals;
+        if (o.op + total > o.cap) {
+            const int64_t room = o.cap - o.op - 1;                     /* >= 0: the parse leaves a byte for the token */
+            run = (uint32_t)(room - (room + 256 - 15) / 256);
+        }
+        o.consumed = anchor + run;
+    } else if (o.limited && o.op + total > o.cap) {
+        return 0;
+    }
     if (run >= 15) { a.out(o.op++, 15u << 4); put_length(a, o, run - 15); }
     else a.out(o.op++, run << 4);
     a.copy(o.op, anchor, run);
@@ -171,12 +187,34 @@ template <class A> HC_FN int last_literals(A& a, Out& o, uint32_t anchor, uint32
     return (int)o.op;
 }
 
+/* The fill parse's end after a sequence that does not fit (lz4hc.c:747-769, 1340-1358): the output goes back to `saved`,
+ * before the sequence.  When its literals fit below maxLitPos = oend - 3, the match is clamped to the room left and
+ * the sequence goes out unchecked if the MFLIMIT test holds; the last literals follow. */
+template <class A> HC_FN int fill_overflow(A& a, Out& o, int64_t saved, uint32_t ip, uint32_t anchor, uint32_t mlen,
+                                           uint32_t off, uint32_t n)
+{
+    o.op = saved;
+    const int64_t ll = ip - anchor;
+    const int64_t llTotal = 1 + (ll + 240) / 255 + ll;
+    const int64_t maxLitPos = o.cap - 3;
+    if (o.op + llTotal <= maxLitPos) {
+        const int64_t maxMl = kMinMatch + 14 + (maxLitPos - (o.op + llTotal)) * 255;
+        if ((int64_t)mlen > maxMl) mlen = (uint32_t)maxMl;
+        if ((o.cap + kLastLiterals) - (o.op + llTotal + 2) - 1 + (int64_t)mlen >= kMfLimit) {
+            o.limited = false;
+            encode_sequence(a, o, ip, anchor, mlen, off);
+            o.limited = true;
+        }
+    }
+    return last_literals<true>(a, o, anchor, n);
+}
+
 /* LZ4MID_compress (lz4hc.c:522-773) without a dictionary.  Note that ipIndex keeps the search position's index when the
  * catch-back or the ip + 1 match moves ip: the reference adds the next positions with it. */
-template <class A> HC_FN int mid_compress(A& a, Out& o, uint32_t n)
+template <bool FILL, class A> HC_FN int mid_compress(A& a, Out& o, uint32_t n)
 {
     uint32_t ip = 0, anchor = 0;
-    if (n < (uint32_t)kMinLength) return last_literals(a, o, anchor, n);
+    if (n < (uint32_t)kMinLength) return last_literals<FILL>(a, o, anchor, n);
     const uint32_t mflimit = n - kMfLimit, matchlimit = n - kLastLiterals;
     const uint32_t ilimitIdx = n - 8 + kHcStart;                    /* LZ4MID_HASHSIZE */
     while (ip <= mflimit) {
@@ -224,7 +262,9 @@ template <class A> HC_FN int mid_compress(A& a, Out& o, uint32_t n)
         a.set_hash(kMidHash8 + mid_hash8(a.in64(ip + 1)), ipIndex + 1);
         a.set_hash(kMidHash8 + mid_hash8(a.in64(ip + 2)), ipIndex + 2);
         a.set_hash(mid_hash4(a.in32(ip + 1)), ipIndex + 1);
-        if (!encode_sequence(a, o, ip, anchor, mlen, dist)) return 0;
+        const int64_t saved = o.op;
+        if (!encode_sequence(a, o, ip, anchor, mlen, dist))
+            return FILL ? fill_overflow(a, o, saved, ip, anchor, mlen, dist, n) : 0;
         const uint32_t end = ip + kHcStart;
         if (end - 2 < ilimitIdx) {
             if (ip > 5) a.set_hash(kMidHash8 + mid_hash8(a.in64(ip - 5)), end - 5);
@@ -234,7 +274,7 @@ template <class A> HC_FN int mid_compress(A& a, Out& o, uint32_t n)
             a.set_hash(mid_hash4(a.in32(ip - 1)), end - 1);
         }
     }
-    return last_literals(a, o, anchor, n);
+    return last_literals<FILL>(a, o, anchor, n);
 }
 
 struct Match { int len, off, back; };
@@ -328,11 +368,13 @@ template <class A> HC_FN Match wider_match(A& a, ChainState& s, uint32_t ip, uin
     return r;
 }
 
-/* LZ4HC_compress_hashChain (lz4hc.c:1121-1362) without a dictionary: the _Search2 / _Search3 state machine */
-template <class A> HC_FN int chain_compress(A& a, Out& o, uint32_t n, int nbSearches)
+/* LZ4HC_compress_hashChain (lz4hc.c:1121-1362) without a dictionary: the _Search2 / _Search3 state machine.  The fill
+ * parse restores the output to optr, before the sequence that overflows: for the second of the ML1 and ML2 pair that
+ * is m2 at start2 (lz4hc.c:1231-1237). */
+template <bool FILL, class A> HC_FN int chain_compress(A& a, Out& o, uint32_t n, int nbSearches)
 {
     uint32_t anchor = 0;
-    if (n < (uint32_t)kMinLength) return last_literals(a, o, anchor, n);
+    if (n < (uint32_t)kMinLength) return last_literals<FILL>(a, o, anchor, n);
     ChainState s;
     s.nextToUpdate = kHcStart;
     s.nbSearches = nbSearches;
@@ -358,7 +400,9 @@ template <class A> HC_FN int chain_compress(A& a, Out& o, uint32_t n, int nbSear
                 }
                 if (m2.len <= m1.len) {       /* no better match: ML1 goes out */
                     uint32_t u = (uint32_t)ip, an = anchor;
-                    if (!encode_sequence(a, o, u, an, (uint32_t)m1.len, (uint32_t)m1.off)) return 0;
+                    const int64_t optr = o.op;
+                    if (!encode_sequence(a, o, u, an, (uint32_t)m1.len, (uint32_t)m1.off))
+                        return FILL ? fill_overflow(a, o, optr, u, an, (uint32_t)m1.len, (uint32_t)m1.off, n) : 0;
                     ip = (int)u; anchor = an;
                     state = 0;
                     continue;
@@ -384,9 +428,13 @@ template <class A> HC_FN int chain_compress(A& a, Out& o, uint32_t n, int nbSear
             if (m3.len <= m2.len) {           /* no better match: ML1 and ML2 go out */
                 if (start2 < ip + m1.len) m1.len = start2 - ip;
                 uint32_t u = (uint32_t)ip, an = anchor;
-                if (!encode_sequence(a, o, u, an, (uint32_t)m1.len, (uint32_t)m1.off)) return 0;
+                int64_t optr = o.op;
+                if (!encode_sequence(a, o, u, an, (uint32_t)m1.len, (uint32_t)m1.off))
+                    return FILL ? fill_overflow(a, o, optr, u, an, (uint32_t)m1.len, (uint32_t)m1.off, n) : 0;
                 u = (uint32_t)start2;
-                if (!encode_sequence(a, o, u, an, (uint32_t)m2.len, (uint32_t)m2.off)) return 0;
+                optr = o.op;
+                if (!encode_sequence(a, o, u, an, (uint32_t)m2.len, (uint32_t)m2.off))
+                    return FILL ? fill_overflow(a, o, optr, u, an, (uint32_t)m2.len, (uint32_t)m2.off, n) : 0;
                 ip = (int)u; anchor = an;
                 state = 0;
                 continue;
@@ -400,7 +448,9 @@ template <class A> HC_FN int chain_compress(A& a, Out& o, uint32_t n, int nbSear
                         if (m2.len < kMinMatch) { start2 = start3; m2 = m3; }
                     }
                     uint32_t u = (uint32_t)ip, an = anchor;
-                    if (!encode_sequence(a, o, u, an, (uint32_t)m1.len, (uint32_t)m1.off)) return 0;
+                    const int64_t optr = o.op;
+                    if (!encode_sequence(a, o, u, an, (uint32_t)m1.len, (uint32_t)m1.off))
+                        return FILL ? fill_overflow(a, o, optr, u, an, (uint32_t)m1.len, (uint32_t)m1.off, n) : 0;
                     anchor = an;
                     ip = start3; m1 = m3;
                     start0 = start2; m0 = m2;
@@ -422,13 +472,15 @@ template <class A> HC_FN int chain_compress(A& a, Out& o, uint32_t n, int nbSear
                 }
             }
             uint32_t u = (uint32_t)ip, an = anchor;
-            if (!encode_sequence(a, o, u, an, (uint32_t)m1.len, (uint32_t)m1.off)) return 0;
+            const int64_t optr = o.op;
+            if (!encode_sequence(a, o, u, an, (uint32_t)m1.len, (uint32_t)m1.off))
+                return FILL ? fill_overflow(a, o, optr, u, an, (uint32_t)m1.len, (uint32_t)m1.off, n) : 0;
             anchor = an;
             ip = start2; m1 = m2;
             start2 = start3; m2 = m3;
         }
     }
-    return last_literals(a, o, anchor, n);
+    return last_literals<FILL>(a, o, anchor, n);
 }
 
 /* LZ4_compress_HC(src, dst, n, cap, level) for level <= 9 from a fresh state; kHcNoLevel for levels above 9 */
@@ -441,7 +493,27 @@ template <class A> HC_FN int hc_compress_block(A& a, int n, int cap, int level)
     o.cap = cap;
     o.limited = cap < n + n / 255 + 16;                                         /* LZ4_compressBound, lz4hc.c:1506 */
     const Level l = level_params(level);
-    return l.mid ? mid_compress(a, o, (uint32_t)n) : chain_compress(a, o, (uint32_t)n, l.nbSearches);
+    return l.mid ? mid_compress<false>(a, o, (uint32_t)n) : chain_compress<false>(a, o, (uint32_t)n, l.nbSearches);
+}
+
+/* LZ4_compress_HC_destSize(state, src, dst, &n, target, level) for level <= 9 from a fresh state, kHcNoLevel for levels
+ * above 9.  `consumed` is what the reference leaves in *srcSizePtr: the input bytes the output holds, or n where it
+ * leaves it alone (lz4hc.c:1388-1389).  The fill parse runs at every target from 1 up, the bound and above included. */
+template <class A> HC_FN int hc_compress_block_dest(A& a, int n, int target, int level, int& consumed)
+{
+    consumed = n;
+    if (level > kMaxLevel) return kHcNoLevel;
+    if (target < 1) return 0;                                                   /* lz4hc.c:1388 */
+    if ((uint32_t)n > kMaxInput) return 0;                                      /* lz4hc.c:1389 */
+    Out o;
+    o.op = 0;
+    o.cap = (int64_t)target - kLastLiterals;
+    o.limited = true;
+    o.consumed = 0;
+    const Level l = level_params(level);
+    const int r = l.mid ? mid_compress<true>(a, o, (uint32_t)n) : chain_compress<true>(a, o, (uint32_t)n, l.nbSearches);
+    consumed = (int)o.consumed;
+    return r;
 }
 
 }  // namespace hc
