@@ -19,7 +19,9 @@
  * behind a mutex).  The host-pointer calls (layers 1, 3, 4) run on the CUDA device that is current
  * in the calling thread at their FIRST use in the process; the device-pointer calls (layer 2) run
  * on the current device / the given stream, and calls that overlap in time must use different
- * workspaces.
+ * workspaces.  The device-pointer calls do no host synchronisation: they only enqueue work on
+ * `stream`, from any thread, and can be captured into a CUDA graph (the first call of a process
+ * included).
  */
 #ifndef LZ4_B200_H
 #define LZ4_B200_H
@@ -118,7 +120,8 @@ LZ4B200_API int LZ4_decompress_safe_usingDict(const char* src, char* dst, int co
 /* Library / device introspection. */
 LZ4B200_API int LZ4B200_device_count(void);
 LZ4B200_API const char* LZ4B200_last_cuda_error(void);
-/* Number of kernel launches issued by this library since load (bench.py's gpu_launches). */
+/* Number of kernel launches issued by this library since load (bench.py's gpu_launches).  A call captured into a
+ * CUDA graph counts when it is captured; replays of the graph do not count. */
 LZ4B200_API uint64_t LZ4B200_launch_count(void);
 
 /* Bytes of device workspace LZ4B200_decompress_blocks needs for nBlocks blocks of ANY capacity

@@ -2,6 +2,17 @@
 
 torch is plumbing here: it owns the device memory and the stream; all work is done by
 LZ4B200_* in liblz4_b200.so on raw pointers.
+
+Every call is enqueued on `stream` (default: the current stream) and does no host synchronisation, so it can be
+captured into a CUDA graph.  The workspace rule of the calls that need one (the decoders and the HC compressors):
+  - `workspace=` is the caller's: it must hold what the call needs (ValueError otherwise), and calls that overlap in
+    time must use different ones;
+  - without it the call draws on a workspace the module owns, one per (device, stream): it is only ever used on the
+    stream it was allocated on, so calls on different streams never share one, and calls on one stream are ordered by
+    that stream;
+  - a phased decode (phases 1 or 2) and any call under stream capture need their own: the expand consumes what its
+    scan left in the workspace, which a call in between would overwrite, and a graph keeps the workspace's address,
+    which the module's cache may free when it grows.
 """
 import torch
 
@@ -12,17 +23,27 @@ def _stream(stream=None):
     return stream if stream is not None else torch.cuda.current_stream()
 
 
-_workspaces = {}        # device index -> cached decode workspace (grown on demand, reused by later calls)
+_workspaces = {}        # (device index, stream handle) -> workspace owned by this module (grown on demand)
 
 
-def _workspace(device, nbytes, stream):
-    """One workspace per device, allocated on the launch stream: calls on the same stream are ordered by the
-    stream; a caller that decodes on several streams at once passes its own `workspace`."""
-    ws = _workspaces.get(device.index)
+def _workspace(device, nbytes, stream, given, what):
+    """The workspace of one call: `given` if the caller passed one (ValueError when it is smaller than nbytes), else the
+    one this module keeps for (device, stream), allocated on that stream and used on no other.  A call that has to keep
+    its workspace past its return -- under stream capture, or a scan whose expand comes later -- must bring its own."""
+    if given is not None:
+        _need_cuda(given)
+        if given.numel() < nbytes:
+            raise ValueError("%s: workspace of %d bytes, the call needs %d" % (what, given.numel(), nbytes))
+        return given
+    if torch.cuda.is_current_stream_capturing():
+        raise ValueError("%s under stream capture needs its own workspace= (the graph would keep a cached one's "
+                         "address)" % what)
+    key = (device.index, stream.cuda_stream)
+    ws = _workspaces.get(key)
     if ws is None or ws.numel() < nbytes:
         with torch.cuda.stream(stream):
             ws = torch.empty(nbytes, dtype=torch.uint8, device=device)
-        _workspaces[device.index] = ws
+        _workspaces[key] = ws
     return ws
 
 
@@ -36,18 +57,17 @@ def compress_bound(n):
     return int(_lib.load().LZ4_compressBound(int(n)))
 
 
-def _decode_outputs(lib, comp, offsets, sizes, out_bytes, per_block, cap, out, out_sizes, workspace, st):
+def _decode_outputs(lib, comp, offsets, sizes, out_bytes, per_block, cap, out, out_sizes, workspace, st, what):
     """out, out_sizes and the workspace of a decode call: the ones given, else new ones on the launch stream (the
-    workspace is sized by LZ4B200_decompress_workspace_bytes_for(n, per_block, cap))"""
+    workspace is sized by LZ4B200_decompress_workspace_bytes_for(n, per_block, cap); see _workspace)"""
     n = int(sizes.numel())
+    ws_bytes = int(lib.LZ4B200_decompress_workspace_bytes_for(n, int(per_block), int(cap)))
+    workspace = _workspace(comp.device, ws_bytes, st, workspace, what)
     with torch.cuda.stream(st):                     # temporaries belong to the stream the kernels run on
         if out is None:
             out = torch.empty(out_bytes, dtype=torch.uint8, device=comp.device)
         if out_sizes is None:
             out_sizes = torch.empty(n, dtype=torch.int32, device=comp.device)
-    ws_bytes = int(lib.LZ4B200_decompress_workspace_bytes_for(n, int(per_block), int(cap)))
-    if workspace is None or workspace.numel() < ws_bytes:
-        workspace = _workspace(comp.device, ws_bytes, st)
     assert offsets.dtype == torch.int64 and sizes.dtype == torch.int32 and comp.dtype == torch.uint8
     return out, out_sizes, workspace
 
@@ -76,15 +96,20 @@ def decompress_blocks(comp, offsets, sizes, block_capacity, out=None, out_stride
 
     comp: u8[*] device buffer; block i = comp[offsets[i] : offsets[i]+sizes[i]] (int64 / int32 device
     tensors).  Block i is written to out[i*out_stride : ...] with capacity block_capacity.
+    phases: 3 decodes; 1 only scans (out_sizes gets the sizes), 2 expands what the scan with the same arguments left
+    in `workspace`, which both phases must be given (ValueError otherwise).
     Returns (out, out_sizes) -- out_sizes[i] is LZ4_decompress_safe's return value.
     """
     lib = _lib.load()
     _need_cuda(comp, offsets, sizes, out)
+    if int(phases) in (1, 2) and workspace is None:
+        raise ValueError("decompress_blocks: phases %d needs workspace= (the expand reads what the scan left there)"
+                         % int(phases))
     n = int(sizes.numel())
     stride = int(out_stride if out_stride is not None else block_capacity)
     st = _stream(stream)
     out, out_sizes, workspace = _decode_outputs(lib, comp, offsets, sizes, n * stride, 0, block_capacity, out, out_sizes,
-                                                workspace, st)
+                                                workspace, st, "decompress_blocks")
     rc = lib.LZ4B200_decompress_blocks_phased(comp.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), out.data_ptr(),
                                               None, stride, None, int(block_capacity), out_sizes.data_ptr(), n,
                                               workspace.data_ptr(), workspace.numel(), int(phases),
@@ -99,7 +124,8 @@ def decompress_blocks_partial(comp, offsets, sizes, target, out=None, out_stride
     LZ4_decompress_safe_partial(block_i, slot_i, sizes[i], t_i, t_i)).
 
     target: one int for every block, or an int32 device tensor of per-block targets.  Block i is written to
-    out[i*out_stride : i*out_stride + out_sizes[i]] (out_stride defaults to the largest target).
+    out[i*out_stride : i*out_stride + out_sizes[i]] (out_stride defaults to the largest target: with per-block targets
+    that reads target.max() on the host, so a captured call passes out_stride).
     Returns (out, out_sizes) -- out_sizes[i] is LZ4_decompress_safe_partial's return value.
     """
     lib = _lib.load()
@@ -109,13 +135,16 @@ def decompress_blocks_partial(comp, offsets, sizes, target, out=None, out_stride
     if per_block:
         assert target.dtype == torch.int32 and target.numel() == n
         uniform = 0
-        biggest = int(target.max()) if n else 0
+        if out_stride is None:
+            if torch.cuda.is_current_stream_capturing():
+                raise ValueError("decompress_blocks_partial under stream capture with per-block targets needs out_stride")
+            biggest = int(target.max()) if n else 0
     else:
         uniform = biggest = int(target)
     stride = int(out_stride if out_stride is not None else max(biggest, 0))
     st = _stream(stream)
     out, out_sizes, workspace = _decode_outputs(lib, comp, offsets, sizes, max(n * stride, 1), per_block, uniform, out,
-                                                out_sizes, workspace, st)
+                                                out_sizes, workspace, st, "decompress_blocks_partial")
     rc = lib.LZ4B200_decompress_blocks_partial(comp.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), out.data_ptr(),
                                                None, stride, target.data_ptr() if per_block else None, uniform,
                                                out_sizes.data_ptr(), n, workspace.data_ptr(), workspace.numel(),
@@ -149,11 +178,12 @@ def compress_blocks(src, block_size, acceleration=1, slots=None, slot_stride=Non
 
 
 def compress_blocks_hc(src, block_size, level=9, slots=None, slot_stride=None, slot_capacity=None, out_sizes=None,
-                       stream=None):
+                       workspace=None, stream=None):
     """Compress src (u8 device tensor) as ceil(len/block_size) independent blocks at an HC level
     (LZ4B200_compress_blocks_hc: block i is LZ4_compress_HC(block_i, slot_i, n_i, slot_capacity, level), byte for byte).
 
-    Levels 1 .. 9 (below 1 means 9); 10 .. 12 raise, their optimal parser is not built.
+    Levels 1 .. 9 (below 1 means 9); 10 .. 12 raise, their optimal parser is not built.  workspace: at least
+    LZ4B200_compress_blocks_hc_workspace_bytes(n) bytes (the module's rule above).
     Returns (slots, out_sizes, slot_stride): block i's bytes are slots[i*slot_stride : i*slot_stride+out_sizes[i]].
     """
     lib = _lib.load()
@@ -161,7 +191,8 @@ def compress_blocks_hc(src, block_size, level=9, slots=None, slot_stride=None, s
     cap = int(slot_capacity if slot_capacity is not None else compress_bound(block_size))
     st = _stream(stream)
     n, stride, slots, out_sizes, src_sizes = _compress_layout(src, block_size, cap, slots, slot_stride, out_sizes, None, st)
-    workspace = _workspace(src.device, max(int(lib.LZ4B200_compress_blocks_hc_workspace_bytes(n)), 1), st)
+    workspace = _workspace(src.device, max(int(lib.LZ4B200_compress_blocks_hc_workspace_bytes(n)), 1), st, workspace,
+                           "compress_blocks_hc")
     rc = lib.LZ4B200_compress_blocks_hc(src.data_ptr(), int(block_size),
                                         src_sizes.data_ptr() if src_sizes is not None else None, int(block_size),
                                         slots.data_ptr(), stride, cap, int(level), out_sizes.data_ptr(), n,
@@ -196,11 +227,12 @@ def compress_blocks_dest_size(src, block_size, target, acceleration=1, slots=Non
 
 
 def compress_blocks_hc_dest_size(src, block_size, target, level=9, slots=None, slot_stride=None, out_sizes=None,
-                                 consumed=None, src_sizes=None, stream=None):
+                                 consumed=None, src_sizes=None, workspace=None, stream=None):
     """Compress as much of each block of src as fits into `target` bytes at an HC level
     (LZ4B200_compress_blocks_hc_destSize: block i is LZ4_compress_HC_destSize(state, block_i, slot_i, &n_i, target, level)).
 
-    Levels 1 .. 9 (below 1 means 9); 10 .. 12 raise, their optimal parser is not built.
+    Levels 1 .. 9 (below 1 means 9); 10 .. 12 raise, their optimal parser is not built.  workspace: as for
+    compress_blocks_hc.
     Returns (slots, out_sizes, consumed, slot_stride): block i's bytes are slots[i*slot_stride : i*slot_stride+out_sizes[i]]
     and hold its first consumed[i] input bytes.
     """
@@ -213,7 +245,8 @@ def compress_blocks_hc_dest_size(src, block_size, target, level=9, slots=None, s
     if consumed is None:
         with torch.cuda.stream(st):
             consumed = torch.empty(max(n, 1), dtype=torch.int32, device=src.device)
-    workspace = _workspace(src.device, max(int(lib.LZ4B200_compress_blocks_hc_workspace_bytes(n)), 1), st)
+    workspace = _workspace(src.device, max(int(lib.LZ4B200_compress_blocks_hc_workspace_bytes(n)), 1), st, workspace,
+                           "compress_blocks_hc_dest_size")
     rc = lib.LZ4B200_compress_blocks_hc_destSize(src.data_ptr(), int(block_size),
                                                  src_sizes.data_ptr() if src_sizes is not None else None,
                                                  int(block_size), slots.data_ptr(), stride, int(target), int(level),

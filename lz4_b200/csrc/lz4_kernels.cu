@@ -16,6 +16,8 @@
 #include <stdint.h>
 #include <stdlib.h>
 #include <stddef.h>
+#include <atomic>
+#include <mutex>
 #include "lz4_kernels.h"
 
 namespace {
@@ -31,7 +33,8 @@ constexpr int kAccelMax = 65537;                 // lz4.c:58
 constexpr uint32_t kMaxInput = 0x7E000000u;      // lz4.h:214
 constexpr unsigned kFull = 0xFFFFFFFFu;
 
-unsigned long long g_launches = 0;
+/* kernel launches since load (LZ4B200_launch_count): the device-pointer calls run without a lock, from any thread */
+std::atomic<unsigned long long> g_launches{0};
 
 /* optional phase timing of the fast expand kernel (thread 0 of each CTA; enabled with -DLZ4K_PHASE_TIMING) */
 __device__ unsigned long long g_phaseCycles[8];
@@ -1339,7 +1342,7 @@ static int launch_pack(const uint8_t* slots, int64_t slotStride, const int32_t* 
 
 extern "C" {
 
-uint64_t lz4k_launch_count(void) { return g_launches; }
+uint64_t lz4k_launch_count(void) { return g_launches.load(); }
 
 /* debug: read and reset the phase-cycle counters (all zero unless built with -DLZ4K_PHASE_TIMING) */
 int lz4k_debug_phase_cycles(unsigned long long* out8)   /* out8: 12 values (8 phase cycles + 4 loop statistics) */
@@ -1359,10 +1362,14 @@ size_t lz4k_decode_workspace_bytes(int64_t nBlocks, int perBlockCaps, int32_t ds
 
 /* once per process (every device of a process runs the same kernels): the decode kernels' opt-in to the large dynamic
  * shared memory, the SMs the persistent kernels use, and the developer A/B switch of the scan */
-static int g_decodeSms = 0, g_scanImpl = -1;
+static std::mutex g_setupLock;
+static std::atomic<int> g_decodeSms{0};
+static int g_scanImpl = -1;                                           // written before g_decodeSms is published
 static cudaError_t decode_setup()
 {
-    if (g_decodeSms) return cudaSuccess;
+    if (g_decodeSms.load(std::memory_order_acquire)) return cudaSuccess;
+    std::lock_guard<std::mutex> hold(g_setupLock);                    // first calls from several threads: one sets up
+    if (g_decodeSms.load(std::memory_order_relaxed)) return cudaSuccess;
     const int rowsSmem = (int)sizeof(RowsSmem);
     cudaError_t e = cudaFuncSetAttribute(lz4_expand_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, rowsSmem);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(lz4_expand_rows_partial_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, rowsSmem);
@@ -1376,7 +1383,7 @@ static cudaError_t decode_setup()
     const int v = device_sms();
     const char* rs = getenv("LZ4B200_RESERVE_SMS");
     const int reserve = rs ? atoi(rs) : 0;
-    g_decodeSms = (reserve > 0 && reserve < v) ? v - reserve : v;
+    g_decodeSms.store((reserve > 0 && reserve < v) ? v - reserve : v, std::memory_order_release);
     return cudaSuccess;
 }
 
@@ -1501,11 +1508,16 @@ int lz4k_launch_encode_par(const lz4k_encode_args* a, void* stream)
 {
     cudaStream_t s = (cudaStream_t)stream;
     if (a->nBlocks == 0) return 0;
+    static std::atomic<int> ready{0};
     static int sms = 0;
-    if (sms == 0) {
-        cudaError_t e = cudaFuncSetAttribute(lz4_encode_par_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(EncParSmem));
-        if (e != cudaSuccess) return (int)e;
-        sms = device_sms();
+    if (!ready.load(std::memory_order_acquire)) {
+        std::lock_guard<std::mutex> hold(g_setupLock);
+        if (!ready.load(std::memory_order_relaxed)) {
+            cudaError_t e = cudaFuncSetAttribute(lz4_encode_par_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(EncParSmem));
+            if (e != cudaSuccess) return (int)e;
+            sms = device_sms();
+            ready.store(1, std::memory_order_release);
+        }
     }
     const int64_t grid = a->nBlocks < 2 * sms ? a->nBlocks : 2 * sms;        // persistent: two CTAs per SM, blocks c, c + grid, ...
     lz4_encode_par_kernel<<<(unsigned)grid, kEpThreads, sizeof(EncParSmem), s>>>(*a);

@@ -26,6 +26,7 @@ def main():
     offs = offs[:-1].contiguous()
     out = torch.empty_like(src)
     rets = torch.empty(n_blocks, dtype=torch.int32, device="cuda")
+    ws = torch.empty(int(_lib.load().LZ4B200_decompress_workspace_bytes_for(n_blocks, 0, bs)), dtype=torch.uint8, device="cuda")
     for _ in range(3):
         batch.decompress_blocks(packed, offs, sizes, bs, out=out, out_sizes=rets)
     torch.cuda.synchronize()
@@ -33,10 +34,10 @@ def main():
     raw.LZ4B200_debug_phase_cycles(buf)
     reps = 5
     t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    batch.decompress_blocks(packed, offs, sizes, bs, out=out, out_sizes=rets, phases=1)
+    batch.decompress_blocks(packed, offs, sizes, bs, out=out, out_sizes=rets, workspace=ws, phases=1)
     t0.record()
     for _ in range(reps):
-        batch.decompress_blocks(packed, offs, sizes, bs, out=out, out_sizes=rets, phases=2)
+        batch.decompress_blocks(packed, offs, sizes, bs, out=out, out_sizes=rets, workspace=ws, phases=2)
     t1.record()
     torch.cuda.synchronize()
     raw.LZ4B200_debug_phase_cycles(buf)
