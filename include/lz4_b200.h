@@ -264,6 +264,38 @@ LZ4B200_API int LZ4B200_compress_blocks_hc_destSize(const void* d_src, int64_t s
                                                     void* stream);
 
 /*
+ * The two calls above at LZ4HC levels 10 .. 12, the optimal parser (LZ4HC_compress_optimal, lz4hc.c:1823-2123):
+ *   LZ4B200_compress_blocks_hc_opt          takes the arguments of LZ4B200_compress_blocks_hc:
+ *       d_outSize[i] = LZ4_compress_HC(src_i, dst_i, n_i, dstCap, compressionLevel), routed as there (a capacity below
+ *       LZ4_compressBound(n_i) limits the output, 0 when the block does not fit); nothing at or past dst_i + dstCap
+ *       is written
+ *   LZ4B200_compress_blocks_hc_opt_destSize takes the arguments of LZ4B200_compress_blocks_hc_destSize:
+ *       d_outSize[i] = LZ4_compress_HC_destSize(state, src_i, dst_i, &n_i, targetDstSize, compressionLevel) and
+ *       d_srcConsumed[i] what it leaves in n_i, as there; nothing at or past dst_i + min(targetDstSize,
+ *       LZ4_compressBound(n_i)) is written
+ * The bytes and values are the reference's, from a fresh state per block.  Levels: 10 (96 searches, matches over 64
+ * bytes taken at once), 11 (512, 128) and 12 (16 384 searches, every position searched); above 12 reads as 12.  Levels
+ * below 10, including <= 0 (which the reference reads as 9), belong to the calls above and give LZ4B200_ERR_ARG here.
+ * The input is read in aligned 4-byte words, each of which holds at least one byte of the block.
+ * The workspace is at least LZ4B200_compress_blocks_hc_opt_workspace_bytes(nBlocks) bytes: 327 728 bytes per slot (the
+ * 256 KB of tables and 4 099 x 16 bytes of prices) for min(nBlocks, 16 384) slots; a larger one gets up to one slot
+ * per block.  One kernel launch; nBlocks == 0 returns LZ4B200_OK without one.  LZ4B200_ERR_ARG: compressionLevel < 10
+ * (checked first), then the rules of the matching call above.
+ * Cost: one thread parses a block, so a call takes as long as its slowest block, and large blocks at levels 11 and 12
+ * take a long time.
+ */
+LZ4B200_API size_t LZ4B200_compress_blocks_hc_opt_workspace_bytes(int64_t nBlocks);
+LZ4B200_API int LZ4B200_compress_blocks_hc_opt(const void* d_src, int64_t srcStride, const int32_t* d_srcSize,
+                                               int32_t srcSize, void* d_dst, int64_t dstStride, int32_t dstCap,
+                                               int compressionLevel, int32_t* d_outSize, int64_t nBlocks,
+                                               void* d_workspace, size_t workspaceBytes, void* stream);
+LZ4B200_API int LZ4B200_compress_blocks_hc_opt_destSize(const void* d_src, int64_t srcStride, const int32_t* d_srcSize,
+                                                        int32_t srcSize, void* d_dst, int64_t dstStride,
+                                                        int32_t targetDstSize, int compressionLevel, int32_t* d_outSize,
+                                                        int32_t* d_srcConsumed, int64_t nBlocks, void* d_workspace,
+                                                        size_t workspaceBytes, void* stream);
+
+/*
  * The same call with the PARALLEL PARSE (throughput mode): every block is a valid LZ4 block that
  * LZ4_decompress_safe expands to the input, the result is deterministic, but it is NOT byte-identical to
  * LZ4_compress_fast: every position is a match candidate (no skipping), matches are chosen by the same greedy

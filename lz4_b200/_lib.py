@@ -41,6 +41,11 @@ PROTOTYPES = [
     ("LZ4B200_compress_blocks_hc", C.c_int, [_vp, _i64, _vp, _i32, _vp, _i64, _i32, C.c_int, _vp, _i64, _vp, _sz, _vp]),
     ("LZ4B200_compress_blocks_hc_destSize", C.c_int, [_vp, _i64, _vp, _i32, _vp, _i64, _i32, C.c_int, _vp, _vp, _i64, _vp,
                                                       _sz, _vp]),
+    ("LZ4B200_compress_blocks_hc_opt_workspace_bytes", _sz, [_i64]),
+    ("LZ4B200_compress_blocks_hc_opt", C.c_int, [_vp, _i64, _vp, _i32, _vp, _i64, _i32, C.c_int, _vp, _i64, _vp, _sz,
+                                                 _vp]),
+    ("LZ4B200_compress_blocks_hc_opt_destSize", C.c_int, [_vp, _i64, _vp, _i32, _vp, _i64, _i32, C.c_int, _vp, _vp, _i64,
+                                                          _vp, _sz, _vp]),
     ("LZ4B200_compress_blocks_parallel",C.c_int, [_vp, _i64, _vp, _i32, _vp, _i64, _i32, C.c_int, _vp, _i64, _vp]),
     ("LZ4B200_pack_blocks", C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, C.c_int, _vp]),
     ("LZ4B200_pack_frame_blocks", C.c_int, [_vp, _i64, _vp, _vp, _i64, _i32, _i32, _i64, _vp, _vp, _vp]),

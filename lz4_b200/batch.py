@@ -256,6 +256,60 @@ def compress_blocks_hc_dest_size(src, block_size, target, level=9, slots=None, s
     return slots, out_sizes[:n], consumed[:n], stride
 
 
+def compress_blocks_hc_opt(src, block_size, level=12, slots=None, slot_stride=None, slot_capacity=None, out_sizes=None,
+                           workspace=None, stream=None):
+    """compress_blocks_hc at levels 10 .. 12, the optimal parser (LZ4B200_compress_blocks_hc_opt: block i is
+    LZ4_compress_HC(block_i, slot_i, n_i, slot_capacity, level), byte for byte).
+
+    Levels above 12 read as 12; levels below 10 raise (they are compress_blocks_hc's).  workspace: at least
+    LZ4B200_compress_blocks_hc_opt_workspace_bytes(n) bytes (the module's rule above).  One thread parses a block, so
+    large blocks at levels 11 and 12 take a long time.
+    Returns (slots, out_sizes, slot_stride): block i's bytes are slots[i*slot_stride : i*slot_stride+out_sizes[i]].
+    """
+    lib = _lib.load()
+    _need_cuda(src, slots)
+    cap = int(slot_capacity if slot_capacity is not None else compress_bound(block_size))
+    st = _stream(stream)
+    n, stride, slots, out_sizes, src_sizes = _compress_layout(src, block_size, cap, slots, slot_stride, out_sizes, None, st)
+    workspace = _workspace(src.device, max(int(lib.LZ4B200_compress_blocks_hc_opt_workspace_bytes(n)), 1), st, workspace,
+                           "compress_blocks_hc_opt")
+    rc = lib.LZ4B200_compress_blocks_hc_opt(src.data_ptr(), int(block_size),
+                                            src_sizes.data_ptr() if src_sizes is not None else None, int(block_size),
+                                            slots.data_ptr(), stride, cap, int(level), out_sizes.data_ptr(), n,
+                                            workspace.data_ptr(), workspace.numel(), st.cuda_stream)
+    _lib.check(rc, "LZ4B200_compress_blocks_hc_opt")
+    return slots, out_sizes[:n], stride
+
+
+def compress_blocks_hc_opt_dest_size(src, block_size, target, level=12, slots=None, slot_stride=None, out_sizes=None,
+                                     consumed=None, src_sizes=None, workspace=None, stream=None):
+    """compress_blocks_hc_dest_size at levels 10 .. 12, the optimal parser (LZ4B200_compress_blocks_hc_opt_destSize:
+    block i is LZ4_compress_HC_destSize(state, block_i, slot_i, &n_i, target, level)).
+
+    Levels as for compress_blocks_hc_opt; workspace: as for compress_blocks_hc_opt.
+    Returns (slots, out_sizes, consumed, slot_stride): block i's bytes are slots[i*slot_stride : i*slot_stride+out_sizes[i]]
+    and hold its first consumed[i] input bytes.
+    """
+    lib = _lib.load()
+    _need_cuda(src, slots, src_sizes)
+    room = max(min(int(target), compress_bound(block_size)), 1)
+    st = _stream(stream)
+    n, stride, slots, out_sizes, src_sizes = _compress_layout(src, block_size, room, slots, slot_stride, out_sizes,
+                                                              src_sizes, st)
+    if consumed is None:
+        with torch.cuda.stream(st):
+            consumed = torch.empty(max(n, 1), dtype=torch.int32, device=src.device)
+    workspace = _workspace(src.device, max(int(lib.LZ4B200_compress_blocks_hc_opt_workspace_bytes(n)), 1), st, workspace,
+                           "compress_blocks_hc_opt_dest_size")
+    rc = lib.LZ4B200_compress_blocks_hc_opt_destSize(src.data_ptr(), int(block_size),
+                                                     src_sizes.data_ptr() if src_sizes is not None else None,
+                                                     int(block_size), slots.data_ptr(), stride, int(target), int(level),
+                                                     out_sizes.data_ptr(), consumed.data_ptr(), n, workspace.data_ptr(),
+                                                     workspace.numel(), st.cuda_stream)
+    _lib.check(rc, "LZ4B200_compress_blocks_hc_opt_destSize")
+    return slots, out_sizes[:n], consumed[:n], stride
+
+
 def pack_blocks(slots, slot_stride, sizes, header_bytes=0, packed=None, stream=None):
     """Gather variable-size blocks into one contiguous stream.  Returns (packed, offsets[n+1])."""
     lib = _lib.load()

@@ -318,6 +318,41 @@ int LZ4B200_compress_blocks_hc_destSize(const void* d_src, int64_t srcStride, co
                     "lz4k_launch_encode_hc_dest");
 }
 
+size_t LZ4B200_compress_blocks_hc_opt_workspace_bytes(int64_t nBlocks)
+{
+    return lz4k_encode_hc_opt_workspace_bytes(nBlocks);
+}
+
+int LZ4B200_compress_blocks_hc_opt(const void* d_src, int64_t srcStride, const int32_t* d_srcSize, int32_t srcSize,
+                                   void* d_dst, int64_t dstStride, int32_t dstCap, int compressionLevel,
+                                   int32_t* d_outSize, int64_t nBlocks,
+                                   void* d_workspace, size_t workspaceBytes, void* stream)
+{
+    lz4k_encode_args a;
+    if (compressionLevel < 10) return LZ4B200_ERR_ARG;      /* levels 1 .. 9 (and <= 0, read as 9): the hash-chain calls */
+    if (nBlocks < 0 || !d_dst || !d_outSize || !d_workspace) return LZ4B200_ERR_ARG;
+    if (nBlocks == 0) return LZ4B200_OK;
+    if (!d_src || workspaceBytes < lz4k_encode_hc_opt_workspace_bytes(nBlocks)) return LZ4B200_ERR_ARG;
+    a = encode_args(d_src, srcStride, d_srcSize, srcSize, d_dst, dstStride, dstCap, 0, d_outSize, nBlocks);
+    return launched(lz4k_launch_encode_hc_opt(&a, compressionLevel, d_workspace, workspaceBytes, stream),
+                    "lz4k_launch_encode_hc_opt");
+}
+
+int LZ4B200_compress_blocks_hc_opt_destSize(const void* d_src, int64_t srcStride, const int32_t* d_srcSize,
+                                            int32_t srcSize, void* d_dst, int64_t dstStride, int32_t targetDstSize,
+                                            int compressionLevel, int32_t* d_outSize, int32_t* d_srcConsumed,
+                                            int64_t nBlocks, void* d_workspace, size_t workspaceBytes, void* stream)
+{
+    lz4k_encode_args a;
+    if (compressionLevel < 10) return LZ4B200_ERR_ARG;      /* levels 1 .. 9 (and <= 0, read as 9): the hash-chain calls */
+    if (nBlocks < 0 || !d_dst || !d_outSize || !d_srcConsumed || !d_workspace) return LZ4B200_ERR_ARG;
+    if (nBlocks == 0) return LZ4B200_OK;
+    if (!d_src || workspaceBytes < lz4k_encode_hc_opt_workspace_bytes(nBlocks)) return LZ4B200_ERR_ARG;
+    a = encode_args(d_src, srcStride, d_srcSize, srcSize, d_dst, dstStride, targetDstSize, 0, d_outSize, nBlocks);
+    return launched(lz4k_launch_encode_hc_opt_dest(&a, d_srcConsumed, compressionLevel, d_workspace, workspaceBytes,
+                                                   stream), "lz4k_launch_encode_hc_opt_dest");
+}
+
 int LZ4B200_compress_blocks_destSize(const void* d_src, int64_t srcStride, const int32_t* d_srcSize, int32_t srcSize,
                                      void* d_dst, int64_t dstStride, int32_t targetDstSize, int acceleration,
                                      int32_t* d_outSize, int32_t* d_srcConsumed, int64_t nBlocks, void* stream)

@@ -1,13 +1,15 @@
 /*
- * lz4_hc_core.h -- the parse of LZ4_compress_HC (lz4hc.c, v1.10.0) at levels 1 .. 9, for host and device.
+ * lz4_hc_core.h -- the parses of LZ4_compress_HC (lz4hc.c, v1.10.0) at every level, for host and device.
  *
- * One call compresses one block from a freshly initialised state, exactly as LZ4_compress_HC does with no dictionary,
- * no chain swap and favorDecSpeed off (lz4hc.c:1500-1510): the same output bytes and the same return value.
+ * One call compresses one block from a freshly initialised state, exactly as LZ4_compress_HC does with no dictionary
+ * and favorDecSpeed off (lz4hc.c:1500-1510): the same output bytes and the same return value.
  *   levels 1 .. 2 (and the lz4mid entries of the level table): LZ4MID_compress, lz4hc.c:522-773
  *   levels 3 .. 9 (and < 1 -> 9):                             LZ4HC_compress_hashChain, lz4hc.c:1121-1362
- * Levels 10 .. 12 use the optimal parser, which is not built here: hc_compress_block returns kHcNoLevel for them.
- * Both parses take the reference's fillOutput directive as the template flag FILL: hc_compress_block_dest is
- * LZ4_compress_HC_destSize (lz4hc.c:1538-1545), which compresses as much input as fits a fixed-size output.
+ *   levels 10 .. 12 (and > 12 -> 12):                         LZ4HC_compress_optimal, lz4hc.c:1823-2123
+ * hc_compress_block serves levels up to 9 and returns kHcNoLevel above; hc_compress_block_opt serves 10 and above and
+ * returns kHcNoLevel below.  Every parse takes the reference's fillOutput directive as the template flag FILL:
+ * hc_compress_block_dest and hc_compress_block_opt_dest are LZ4_compress_HC_destSize (lz4hc.c:1538-1545), which
+ * compresses as much input as fits a fixed-size output.
  *
  * Positions are byte offsets into the block.  The reference's indices are position + kHcStart (LZ4HC_init_internal,
  * lz4hc.c:242-259, starts a fresh state at 64 KB), so a zero hash entry is never a candidate.
@@ -18,8 +20,15 @@
  *   uint32_t hash(uint32_t h); void set_hash(uint32_t h, uint32_t v)      2^15 entries, all 0 at the start of a block
  *   uint32_t chain(uint32_t i); void set_chain(uint32_t i, uint32_t v)    2^16 16-bit entries, any content at the start
  *   void out(int64_t o, uint32_t v); void copy(int64_t o, uint32_t p, uint32_t len)    output byte / literal copy
+ *   Opt& opt(int r)                                 the optimal parser's table, kOptEntries entries, any content at the
+ *                                                   start (only hc_compress_block_opt* call it)
  * The chain table needs no initial value: the hash-chain walk only reads the entry of an index in
  * [ipIndex - 65535, ipIndex), and LZ4HC_Insert has written every such index before the walk, the entry of index i last.
+ * The chain swap reads the entries of [matchIndex, matchIndex + longest - 4], and only when matchIndex + longest <=
+ * ipIndex: with matchIndex >= lowest they all lie in [lowest, ipIndex), which the walk's rule covers.
+ * The optimal parser's table needs none either: a step writes entries 0 .. last + 3 before it reads any, and every
+ * later write that moves `last` writes the positions it newly covers (a match reaching past last + 3 is always
+ * stored), so no read in [0, last + 3] finds an entry from an earlier step or from before the block.
  * Nothing is written at or past the capacity: every output byte is written after the check that covers it (the fill
  * parse's unchecked last sequence after its room test against oend - 3).
  */
@@ -50,7 +59,14 @@ constexpr uint32_t kMidHash8 = 1u << kMidHashLog;
 constexpr int kHashEntries = 1 << kHashLog;
 constexpr int kChainEntries = 1 << 16;
 constexpr int kMaxLevel = 9;                      /* above: the optimal parser */
+constexpr int kMinOptLevel = 10;                  /* LZ4HC_CLEVEL_OPT_MIN */
 constexpr int kHcNoLevel = -1;
+constexpr int kOptNum = 4096;                     /* LZ4_OPT_NUM */
+constexpr int kTrailingLiterals = 3;
+constexpr int kOptEntries = kOptNum + kTrailingLiterals;
+
+/* LZ4HC_optimal_t: one position of the optimal parser's price table */
+struct Opt { int price, off, mlen, litlen; };
 
 struct Level { bool mid; int nbSearches; };
 
@@ -298,10 +314,14 @@ template <class A> HC_FN void insert(A& a, ChainState& s, uint32_t target)
     s.nextToUpdate = target;
 }
 
-/* LZ4HC_InsertAndGetWiderMatch (lz4hc.c:884-1104) for one prefix, no chain swap, no favorDecSpeed: the longest match
- * through ip that starts no earlier than iLow, is longer than `longest` and ends by iHigh.  The candidates are taken in
- * the chain's order, and the 2-byte quick reject at longest - 1 comes first: it decides which later candidates count. */
-template <class A> HC_FN Match wider_match(A& a, ChainState& s, uint32_t ip, uint32_t iLow, uint32_t iHigh, int longest)
+/* LZ4HC_InsertAndGetWiderMatch (lz4hc.c:884-1104) for one prefix, no favorDecSpeed: the longest match through ip that
+ * starts no earlier than iLow, is longer than `longest` and ends by iHigh.  The candidates are taken in the chain's
+ * order, and the 2-byte quick reject at longest - 1 comes first: it decides which later candidates count.
+ * SWAP is the chain swap of the optimal parser (lz4hc.c:964-985, called with iLow == ip): a candidate whose length ties
+ * or sets the best so far moves the walk to the chain, among the best match's positions, that reaches farthest back.
+ * chainPos (matchChainPos) is never reset: once set it shuts the repeat-pattern branch and shifts every later step. */
+template <bool SWAP = false, class A>
+HC_FN Match wider_match(A& a, ChainState& s, uint32_t ip, uint32_t iLow, uint32_t iHigh, int longest)
 {
     const uint32_t ipIndex = ip + kHcStart;
     const uint32_t lowest = (kHcStart + kMaxDistance + 1 > ipIndex) ? kHcStart : ipIndex - kMaxDistance;
@@ -310,6 +330,7 @@ template <class A> HC_FN Match wider_match(A& a, ChainState& s, uint32_t ip, uin
     int nb = s.nbSearches;
     int repeat = 0;                       /* 0 untested, 1 not a repeat, 2 confirmed */
     uint32_t srcPatternLength = 0;
+    uint32_t chainPos = 0;
     Match r; r.len = longest; r.off = 0; r.back = 0;
     insert(a, s, ipIndex);
     uint32_t matchIndex = a.hash(hash4(pattern));
@@ -323,9 +344,30 @@ template <class A> HC_FN Match wider_match(A& a, ChainState& s, uint32_t ip, uin
             const int back = lookBack ? count_back(a, ip, m, most) : 0;
             const int len = kMinMatch + (int)count(a, ip + kMinMatch, m + kMinMatch, iHigh) - back;
             if (len > r.len) { r.len = len; r.off = (int)(ipIndex - matchIndex); r.back = back; }
+            /* the swap fires on matchLength == longest after the update, ties included; a rejected candidate's
+             * matchLength is 0 and never does */
+            if constexpr (SWAP) {
+                if (len == r.len && matchIndex + (uint32_t)r.len <= ipIndex) {
+                    /* the entries of [matchIndex, matchIndex + longest - 4], with a stride that grows while none is
+                     * larger */
+                    uint32_t farthest = 1;
+                    const int end = r.len - kMinMatch + 1;
+                    int step = 1, accel = 1 << 4;
+                    for (int pos = 0; pos < end; pos += step) {
+                        const uint32_t d = a.chain((matchIndex + (uint32_t)pos) & 0xFFFF);
+                        step = accel++ >> 4;
+                        if (d > farthest) { farthest = d; chainPos = (uint32_t)pos; accel = 1 << 4; }
+                    }
+                    if (farthest > 1) {
+                        if (farthest > matchIndex) break;
+                        matchIndex -= farthest;
+                        continue;
+                    }
+                }
+            }
         }
         const uint32_t next = a.chain(matchIndex & 0xFFFF);
-        if (s.patternAnalysis && next == 1) {
+        if (s.patternAnalysis && next == 1 && (!SWAP || chainPos == 0)) {
             const uint32_t cand = matchIndex - 1;
             if (repeat == 0) {
                 if ((pattern & 0xFFFF) == (pattern >> 16) && (pattern & 0xFF) == (pattern >> 24)) {
@@ -363,7 +405,8 @@ template <class A> HC_FN Match wider_match(A& a, ChainState& s, uint32_t ip, uin
                 }
             }
         }
-        matchIndex -= next;
+        if constexpr (SWAP) matchIndex -= a.chain((matchIndex + chainPos) & 0xFFFF);
+        else matchIndex -= next;
     }
     return r;
 }
@@ -483,6 +526,135 @@ template <bool FILL, class A> HC_FN int chain_compress(A& a, Out& o, uint32_t n,
     return last_literals<FILL>(a, o, anchor, n);
 }
 
+/* LZ4HC_literalsPrice / LZ4HC_sequencePrice (lz4hc.c:1778-1800): bytes of a literal run, and of a sequence (mlen >= 4) */
+HC_FN int literals_price(int litlen) { return litlen >= 15 ? litlen + 1 + (litlen - 15) / 255 : litlen; }
+HC_FN int sequence_price(int litlen, int mlen)
+{
+    return 3 + literals_price(litlen) + (mlen >= 15 + kMinMatch ? 1 + (mlen - 15 - kMinMatch) / 255 : 0);
+}
+
+/* LZ4HC_FindLongerMatch (lz4hc.c:1802-1820) without favorDecSpeed: a match at ip longer than minLen (pattern analysis
+ * and the chain swap on), else {0, 0, 0} */
+template <class A> HC_FN Match longer_match(A& a, ChainState& s, uint32_t ip, uint32_t iHigh, int minLen)
+{
+    Match m = wider_match<true>(a, s, ip, ip, iHigh, minLen);
+    if (m.len <= minLen) { m.len = 0; m.off = 0; }
+    return m;
+}
+
+struct OptLevel { int nbSearches, sufficient; bool fullUpdate; };
+
+/* the level table for 10 .. 12 (lz4hc.c:103-105; above 12 reads as 12), targetLength clamped to LZ4_OPT_NUM - 1
+ * (lz4hc.c:1861), and ultra mode from the level as given (lz4hc.c:1409) */
+HC_FN OptLevel opt_level_params(int level)
+{
+    OptLevel l;
+    l.nbSearches = level == 10 ? 96 : level == 11 ? 512 : 16384;
+    l.sufficient = level == 10 ? 64 : level == 11 ? 128 : kOptNum - 1;
+    l.fullUpdate = level >= 12;
+    return l;
+}
+
+/* LZ4HC_compress_optimal (lz4hc.c:1823-2123) without a dictionary or favorDecSpeed.  Each step prices every position up
+ * to the end of the matches found so far (a.opt(r) for r = 0 .. last + 3), walks the cheapest path back and encodes it.
+ * Literal runs and prices grow with ip - anchor, so they stay 32-bit.  The fill parse restores the output to `saved`,
+ * before the sequence that overflows. */
+template <bool FILL, class A> HC_FN int opt_compress(A& a, Out& o, uint32_t n, const OptLevel l)
+{
+    uint32_t ip = 0, anchor = 0;
+    /* below 13 bytes the reference's loop runs at most one search, at position 0 of an empty table, and finds nothing */
+    if (n < (uint32_t)kMinLength) return last_literals<FILL>(a, o, anchor, n);
+    ChainState s;
+    s.nextToUpdate = kHcStart;
+    s.nbSearches = l.nbSearches;
+    s.patternAnalysis = true;
+    const uint32_t mflimit = n - kMfLimit, matchlimit = n - kLastLiterals;
+    while (ip <= mflimit) {
+        const int llen = (int)(ip - anchor);
+        const Match first = longer_match(a, s, ip, matchlimit, kMinMatch - 1);
+        if (first.len == 0) { ip++; continue; }
+        if (first.len > l.sufficient) {                              /* good enough: encoded at once */
+            const int64_t saved = o.op;
+            if (!encode_sequence(a, o, ip, anchor, (uint32_t)first.len, (uint32_t)first.off))
+                return FILL ? fill_overflow(a, o, saved, ip, anchor, (uint32_t)first.len, (uint32_t)first.off, n) : 0;
+            continue;
+        }
+        for (int r = 0; r < kMinMatch; r++) {
+            Opt& e = a.opt(r);
+            e.mlen = 1; e.off = 0; e.litlen = llen + r; e.price = literals_price(llen + r);
+        }
+        for (int ml = kMinMatch; ml <= first.len; ml++) {
+            Opt& e = a.opt(ml);
+            e.mlen = ml; e.off = first.off; e.litlen = llen; e.price = sequence_price(llen, ml);
+        }
+        int last = first.len;
+        for (int k = 1; k <= kTrailingLiterals; k++) {
+            Opt& e = a.opt(last + k);
+            e.mlen = 1; e.off = 0; e.litlen = k; e.price = a.opt(last).price + literals_price(k);
+        }
+        int cur, bestLen = 0, bestOff = 0;
+        bool now = false;                                            /* a match at cur is encoded at once */
+        for (cur = 1; cur < last; cur++) {
+            if (ip + cur > mflimit) break;
+            const int pc = a.opt(cur).price;
+            if (a.opt(cur + 1).price <= pc && (!l.fullUpdate || a.opt(cur + kMinMatch).price < pc + 3)) continue;
+            const Match m = longer_match(a, s, ip + cur, matchlimit, l.fullUpdate ? kMinMatch - 1 : last - cur);
+            if (m.len == 0) continue;
+            if (m.len > l.sufficient || m.len + cur >= kOptNum) {
+                bestLen = m.len; bestOff = m.off; last = cur + 1; now = true;
+                break;
+            }
+            const int baseLit = a.opt(cur).litlen;
+            for (int lit = 1; lit < kMinMatch; lit++) {                  /* literals before the match: strictly cheaper */
+                const int price = pc - literals_price(baseLit) + literals_price(baseLit + lit);
+                Opt& e = a.opt(cur + lit);
+                if (price < e.price) { e.mlen = 1; e.off = 0; e.litlen = baseLit + lit; e.price = price; }
+            }
+            const bool afterLit = a.opt(cur).mlen == 1;
+            const int ll = afterLit ? baseLit : 0;
+            const int base = afterLit ? (cur > ll ? a.opt(cur - ll).price : 0) : pc;
+            for (int ml = kMinMatch; ml <= m.len; ml++) {                /* the match: ties win, and so does past last + 3 */
+                const int pos = cur + ml;
+                const int price = base + sequence_price(ll, ml);
+                if (pos > last + kTrailingLiterals || price <= a.opt(pos).price) {
+                    if (ml == m.len && last < pos) last = pos;
+                    Opt& e = a.opt(pos);
+                    e.mlen = ml; e.off = m.off; e.litlen = ll; e.price = price;
+                }
+            }
+            for (int k = 1; k <= kTrailingLiterals; k++) {
+                Opt& e = a.opt(last + k);
+                e.mlen = 1; e.off = 0; e.litlen = k; e.price = a.opt(last).price + literals_price(k);
+            }
+        }
+        if (!now) {
+            bestLen = a.opt(last).mlen;
+            bestOff = a.opt(last).off;
+            cur = last - bestLen;
+        }
+        {   /* the path back from cur: each position takes the step that leaves it */
+            int pos = cur, ml = bestLen, off = bestOff;
+            for (;;) {
+                Opt& e = a.opt(pos);
+                const int nml = e.mlen, noff = e.off;
+                e.mlen = ml; e.off = off;
+                ml = nml; off = noff;
+                if (nml > pos) break;
+                pos -= nml;
+            }
+        }
+        for (int r = 0; r < last;) {
+            const int ml = a.opt(r).mlen, off = a.opt(r).off;
+            if (ml == 1) { ip++; r++; continue; }
+            r += ml;
+            const int64_t saved = o.op;
+            if (!encode_sequence(a, o, ip, anchor, (uint32_t)ml, (uint32_t)off))
+                return FILL ? fill_overflow(a, o, saved, ip, anchor, (uint32_t)ml, (uint32_t)off, n) : 0;
+        }
+    }
+    return last_literals<FILL>(a, o, anchor, n);
+}
+
 /* LZ4_compress_HC(src, dst, n, cap, level) for level <= 9 from a fresh state; kHcNoLevel for levels above 9 */
 template <class A> HC_FN int hc_compress_block(A& a, int n, int cap, int level)
 {
@@ -512,6 +684,37 @@ template <class A> HC_FN int hc_compress_block_dest(A& a, int n, int target, int
     o.consumed = 0;
     const Level l = level_params(level);
     const int r = l.mid ? mid_compress<true>(a, o, (uint32_t)n) : chain_compress<true>(a, o, (uint32_t)n, l.nbSearches);
+    consumed = (int)o.consumed;
+    return r;
+}
+
+/* LZ4_compress_HC(src, dst, n, cap, level) for level >= 10 from a fresh state (above 12 reads as 12); kHcNoLevel for
+ * levels below 10, which belong to hc_compress_block */
+template <class A> HC_FN int hc_compress_block_opt(A& a, int n, int cap, int level)
+{
+    if (level < kMinOptLevel) return kHcNoLevel;
+    if ((uint32_t)n > kMaxInput) return 0;                                      /* lz4hc.c:1389 */
+    Out o;
+    o.op = 0;
+    o.cap = cap;
+    o.limited = cap < n + n / 255 + 16;                                         /* LZ4_compressBound, lz4hc.c:1506 */
+    return opt_compress<false>(a, o, (uint32_t)n, opt_level_params(level));
+}
+
+/* LZ4_compress_HC_destSize(state, src, dst, &n, target, level) for level >= 10 from a fresh state, kHcNoLevel below;
+ * `consumed` as for hc_compress_block_dest */
+template <class A> HC_FN int hc_compress_block_opt_dest(A& a, int n, int target, int level, int& consumed)
+{
+    consumed = n;
+    if (level < kMinOptLevel) return kHcNoLevel;
+    if (target < 1) return 0;                                                   /* lz4hc.c:1388 */
+    if ((uint32_t)n > kMaxInput) return 0;                                      /* lz4hc.c:1389 */
+    Out o;
+    o.op = 0;
+    o.cap = (int64_t)target - kLastLiterals;
+    o.limited = true;
+    o.consumed = 0;
+    const int r = opt_compress<true>(a, o, (uint32_t)n, opt_level_params(level));
     consumed = (int)o.consumed;
     return r;
 }

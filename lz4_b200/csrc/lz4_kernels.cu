@@ -1558,6 +1558,38 @@ int lz4k_launch_encode_hc_dest(const lz4k_encode_args* a, int32_t* srcConsumed, 
     return (int)cudaGetLastError();
 }
 
+/* The optimal parser's slots: kHcOptSlotBytes each, for the same count of slots */
+size_t lz4k_encode_hc_opt_workspace_bytes(int64_t nBlocks)
+{
+    return nBlocks <= 0 ? 0 : (size_t)(nBlocks < kHcSlots ? nBlocks : kHcSlots) * kHcOptSlotBytes;
+}
+
+int lz4k_launch_encode_hc_opt(const lz4k_encode_args* a, int level, void* workspace, size_t workspaceBytes, void* stream)
+{
+    if (a->nBlocks == 0) return 0;
+    const int64_t fit = (int64_t)(workspaceBytes / kHcOptSlotBytes);
+    const int64_t slots = a->nBlocks < fit ? a->nBlocks : fit;
+    const int64_t grid = (slots + kHcThreads - 1) / kHcThreads;
+    lz4_encode_hc_opt_kernel<<<(unsigned)grid, kHcThreads, 0, (cudaStream_t)stream>>>(*a, (uint8_t*)workspace, slots,
+                                                                                      level);
+    g_launches++;
+    return (int)cudaGetLastError();
+}
+
+int lz4k_launch_encode_hc_opt_dest(const lz4k_encode_args* a, int32_t* srcConsumed, int level, void* workspace,
+                                   size_t workspaceBytes, void* stream)
+{
+    if (a->nBlocks == 0) return 0;
+    const int64_t fit = (int64_t)(workspaceBytes / kHcOptSlotBytes);
+    const int64_t slots = a->nBlocks < fit ? a->nBlocks : fit;
+    const int64_t grid = (slots + kHcThreads - 1) / kHcThreads;
+    lz4_encode_hc_opt_dest_kernel<<<(unsigned)grid, kHcThreads, 0, (cudaStream_t)stream>>>(*a, srcConsumed,
+                                                                                           (uint8_t*)workspace, slots,
+                                                                                           level);
+    g_launches++;
+    return (int)cudaGetLastError();
+}
+
 int lz4k_launch_pack(const uint8_t* slots, int64_t slotStride, const int32_t* sizes, int64_t nBlocks,
                      uint8_t* packed, int64_t* outOff, int headerBytes, void* stream)
 {

@@ -63,6 +63,12 @@ int lz4k_launch_encode_hc(const lz4k_encode_args* a, int level, void* workspace,
  * return value, srcConsumed[i] what it leaves in n_i; the workspace as for lz4k_launch_encode_hc, one launch */
 int lz4k_launch_encode_hc_dest(const lz4k_encode_args* a, int32_t* srcConsumed, int level, void* workspace,
                                size_t workspaceBytes, void* stream);
+/* the two calls above for level >= 10 (the caller rejects the others), the optimal parser; the workspace holds
+ * lz4k_encode_hc_opt_workspace_bytes(nBlocks) bytes or more, one launch */
+size_t lz4k_encode_hc_opt_workspace_bytes(int64_t nBlocks);
+int lz4k_launch_encode_hc_opt(const lz4k_encode_args* a, int level, void* workspace, size_t workspaceBytes, void* stream);
+int lz4k_launch_encode_hc_opt_dest(const lz4k_encode_args* a, int32_t* srcConsumed, int level, void* workspace,
+                                   size_t workspaceBytes, void* stream);
 int lz4k_launch_pack(const uint8_t* slots, int64_t slotStride, const int32_t* sizes, int64_t nBlocks,
                      uint8_t* packed, int64_t* outOff, int headerBytes, void* stream);
 /* the body of an LZ4 frame: [LE32 block header][payload] per block; blocks whose compression did not gain are stored raw */
