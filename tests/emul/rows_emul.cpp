@@ -2,7 +2,7 @@
 // Runs the kernel's phases -- scan marks, runs pass 1, rank, runs pass 2, waves -- with the arithmetic of
 // lz4_b200/csrc/lz4_rows_core.h (the same text the device compiles), one "thread" after the other, and
 // checks the property the kernel relies on: a byte read from the output window during a wave was written
-// in an EARLIER wave.  Built by tests/test_rows_emul.py (g++).
+// in an EARLIER wave.  Checked by tests/test_rows_emul.py.
 #include <stdint.h>
 #include <string.h>
 #include <vector>

@@ -5,14 +5,11 @@
 #include <string.h>
 #include "../../lz4_b200/csrc/lz4_scan_par.h"
 
-static int g_lanes = 128;
-extern "C" void scan_par_set_lanes(int nl) { g_lanes = nl; }
-
-// stats[0] = fix-up rounds, stats[1] = lane walks in the fix-up rounds, stats[2] = lane that finished the block
+// nl lanes (at most kSpMaxLanes); stats[0] = fix-up rounds, stats[1] = lane walks in the fix-up rounds, stats[2] = lane
+// that finished the block
 template <class M>
-static int run_par(M& mem, int n, int cap, uint32_t* nSeqOut, uint32_t* marks, uint32_t markCap, int* stats)
+static int run_par(M& mem, int n, int cap, uint32_t* nSeqOut, uint32_t* marks, uint32_t markCap, int* stats, int nl)
 {
-    const int nl = g_lanes;
     *nSeqOut = 0;
     stats[0] = stats[1] = 0; stats[2] = -1;
     if (cap < 64 || n < kSpMinBytes) return scan_block(mem, n, cap, nSeqOut, marks, markCap);   // lane 0, one-thread scan
@@ -41,16 +38,18 @@ static int run_par(M& mem, int n, int cap, uint32_t* nSeqOut, uint32_t* marks, u
     *nSeqOut = S.nseq;
     return S.ret;
 }
-extern "C" int scan_par_host(const uint8_t* src, int n, int cap, uint32_t* nSeqOut, uint32_t* marks, int* stats)
+extern "C" int scan_par_host(const uint8_t* src, int n, int cap, uint32_t* nSeqOut, uint32_t* marks, int* stats,
+                             int nl)
 {
     MemPtr<true> mem{src};
-    return run_par(mem, n, cap, nSeqOut, marks, (uint32_t)kMaxSeqFast, stats);
+    return run_par(mem, n, cap, nSeqOut, marks, (uint32_t)kMaxSeqFast, stats, nl);
 }
 // blocks above 64 KB: wide marks (two words per sequence), parallel scan and one-thread scan
-extern "C" int scan_par_host_wide(const uint8_t* src, int n, int cap, uint32_t* nSeqOut, uint32_t* marks, uint32_t markCap, int* stats)
+extern "C" int scan_par_host_wide(const uint8_t* src, int n, int cap, uint32_t* nSeqOut, uint32_t* marks, uint32_t markCap,
+                                  int* stats, int nl)
 {
     MemPtr<true, true> mem{src};
-    return run_par(mem, n, cap, nSeqOut, marks, markCap, stats);
+    return run_par(mem, n, cap, nSeqOut, marks, markCap, stats, nl);
 }
 extern "C" int scan_thread_host_wide(const uint8_t* src, int n, int cap, uint32_t* nSeqOut, uint32_t* marks, uint32_t markCap)
 {
@@ -59,12 +58,13 @@ extern "C" int scan_thread_host_wide(const uint8_t* src, int n, int cap, uint32_
 }
 
 // In-process differential fuzz: mutate a (valid) compressed block `iters` times, pick a capacity, and
-// compare the parallel scan with the one-thread scan (return value, sequence count, marks).
+// compare the parallel scan on nl lanes with the one-thread scan (return value, sequence count, marks).
 // Returns the number of cases run, or -(1 + index) of the first mismatching case.
 namespace {
 struct FuzzRng { uint64_t s; uint32_t next() { s = s * 6364136223846793005ull + 1442695040888963407ull; return (uint32_t)(s >> 33); } };
 }
-extern "C" long long scan_par_fuzz(const uint8_t* base, int n, int rawSize, int iters, uint64_t seed, long long* nErrors)
+extern "C" long long scan_par_fuzz(const uint8_t* base, int n, int rawSize, int iters, uint64_t seed, long long* nErrors,
+                                   int nl)
 {
     FuzzRng r{seed * 0x9E3779B97F4A7C15ull + 1};
     uint8_t* buf = new uint8_t[(size_t)n + 64];
@@ -95,7 +95,7 @@ extern "C" long long scan_par_fuzz(const uint8_t* base, int n, int rawSize, int 
         for (int i = 0; i < kMaxSeqFast; i++) { m1[i] = 0xABABABABu; m2[i] = 0xABABABABu; }
         MemPtr<true> memP{p};
         const int r1 = scan_block(memP, (int)len, cap, &ns1, wm ? m1 : nullptr, (uint32_t)kMaxSeqFast);
-        const int r2 = scan_par_host(p, (int)len, cap, &ns2, wm ? m2 : nullptr, st);
+        const int r2 = scan_par_host(p, (int)len, cap, &ns2, wm ? m2 : nullptr, st, nl);
         const uint32_t k = ns1 < (uint32_t)kMaxSeqFast ? ns1 : (uint32_t)kMaxSeqFast;
         if (r1 != r2 || (r1 > 0 && ns1 != ns2) || (r1 > 0 && wm && memcmp(m1, m2, sizeof(uint32_t) * k) != 0)) bad = -(1 + (long long)it);
         cases++;

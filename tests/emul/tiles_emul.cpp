@@ -3,7 +3,7 @@
 // rw_put_deltas; lz4_decode_plan.h: tile_index_seq): wide marks from the scan, the tile index (first sequence per tile),
 // per tile runs pass 1, rank, runs pass 2, waves with the kernel's three kinds of source -- compressed byte (virtual
 // range), byte of this tile (window), byte of an earlier tile (destination).  Checks what the kernel relies on: every
-// source read from the window was written in an earlier wave, every history read lies in an earlier tile.  Built by
+// source read from the window was written in an earlier wave, every history read lies in an earlier tile.  Checked by
 // tests/test_tiles_emul.py.
 #include <stdint.h>
 #include <string.h>

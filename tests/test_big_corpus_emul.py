@@ -13,44 +13,24 @@ silently losing its edge cases:
     the emulators' marks, and the tile index kernel's neighbour rule, on every accepted block.
 """
 import ctypes as C
-import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
 from oracle.pyoracle import Oracle
 import big_corpus as bc
+import host_build
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 HANDOFF = -1000002                   # the emulators' code for "more runs than the table holds: generic kernel"
 ROWS_MAX_RUNS = 20480
 CAPS = (65537, 122880, 300000, 4 << 20)
 
 
-def _build(tmp_path_factory, name):
-    gxx = shutil.which("g++")
-    if not gxx:
-        pytest.skip("g++ not available")
-    so = str(tmp_path_factory.mktemp(name) / ("lib%s.so" % name))
-    subprocess.run([gxx, "-O2", "-std=c++17", "-Wall", "-shared", "-fPIC", "-o", so,
-                    os.path.join(HERE, "emul", name + ".cpp")], check=True)
-    return C.CDLL(so)
-
-
 @pytest.fixture(scope="module")
-def scans(tmp_path_factory):
+def scans():
     """(par, thread): scan_par_host_wide with 128 lanes / scan_thread_host_wide -> (return value, nseq, marks, lane)"""
-    lib = _build(tmp_path_factory, "scan_par_emul")
-    lib.scan_par_set_lanes.argtypes = [C.c_int]
-    lib.scan_par_set_lanes(bc.LANES)
-    lib.scan_par_host_wide.restype = C.c_int
-    lib.scan_par_host_wide.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_uint32), C.c_void_p, C.c_uint32,
-                                       C.POINTER(C.c_int)]
-    lib.scan_thread_host_wide.restype = C.c_int
-    lib.scan_thread_host_wide.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_uint32), C.c_void_p, C.c_uint32]
+    lib = host_build.require()
 
     def run(par, blk, cap):
         mcap = cap // 4 + 2
@@ -59,7 +39,8 @@ def scans(tmp_path_factory):
         ns = C.c_uint32(0)
         st = (C.c_int * 3)(0, 0, -7)
         if par:
-            r = lib.scan_par_host_wide(buf.ctypes.data, len(blk), cap, C.byref(ns), marks.ctypes.data, mcap, st)
+            r = lib.scan_par_host_wide(buf.ctypes.data, len(blk), cap, C.byref(ns), marks.ctypes.data, mcap, st,
+                                       bc.LANES)
         else:
             r = lib.scan_thread_host_wide(buf.ctypes.data, len(blk), cap, C.byref(ns), marks.ctypes.data, mcap)
         return r, ns.value, marks[:2 * min(ns.value, mcap)], st[2]
@@ -67,10 +48,8 @@ def scans(tmp_path_factory):
 
 
 @pytest.fixture(scope="module")
-def tiles(tmp_path_factory):
-    lib = _build(tmp_path_factory, "tiles_emul")
-    lib.tiles_emulate.restype = C.c_int
-    lib.tiles_emulate.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_char_p, C.c_int, C.POINTER(C.c_longlong)]
+def tiles():
+    lib = host_build.require()
 
     def run(comp, cap):
         out = C.create_string_buffer(cap)

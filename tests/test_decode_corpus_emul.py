@@ -9,36 +9,21 @@ edge cases:
   - the event blocks are rejected by the oracle where the corpus says they are.
 """
 import ctypes as C
-import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
+import host_build
 from oracle.pyoracle import Oracle
 from gpu_util import (RUNS_ABOVE, RUNS_BELOW, event_block, hostile_corpus, run_block, seq_count_block)
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 ROWS_MAX_RUNS = 20480
 HANDOFF = -1000002                   # the emulators' code for "more runs than the table holds: generic kernel"
 
 
-def _build(tmp_path_factory, name):
-    gxx = shutil.which("g++")
-    if not gxx:
-        pytest.skip("g++ not available")
-    so = str(tmp_path_factory.mktemp(name) / ("lib%s.so" % name))
-    subprocess.run([gxx, "-O2", "-std=c++17", "-Wall", "-shared", "-fPIC", "-o", so,
-                    os.path.join(HERE, "emul", name + ".cpp")], check=True)
-    return C.CDLL(so)
-
-
 @pytest.fixture(scope="module")
-def rows(tmp_path_factory):
-    lib = _build(tmp_path_factory, "rows_emul")
-    lib.rows_emulate.restype = C.c_int
-    lib.rows_emulate.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_char_p, C.c_int, C.c_int, C.POINTER(C.c_longlong)]
+def rows():
+    lib = host_build.require()
 
     def run(comp, cap):
         out = C.create_string_buffer(cap)
@@ -49,10 +34,8 @@ def rows(tmp_path_factory):
 
 
 @pytest.fixture(scope="module")
-def scan(tmp_path_factory):
-    lib = _build(tmp_path_factory, "scan_emul")
-    lib.scan_host.restype = C.c_int
-    lib.scan_host.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_uint32), C.c_void_p]
+def scan():
+    lib = host_build.require()
 
     def run(comp, cap):
         buf = np.zeros(len(comp) + 64, dtype=np.uint8)
@@ -65,10 +48,8 @@ def scan(tmp_path_factory):
 
 
 @pytest.fixture(scope="module")
-def tiles(tmp_path_factory):
-    lib = _build(tmp_path_factory, "tiles_emul")
-    lib.tiles_emulate.restype = C.c_int
-    lib.tiles_emulate.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_char_p, C.c_int, C.POINTER(C.c_longlong)]
+def tiles():
+    lib = host_build.require()
 
     def run(comp, cap):
         out = C.create_string_buffer(cap)

@@ -10,9 +10,6 @@ the size for any capacities and one byte less than sized-for, the plan must agre
   - gpu_util.route's R1 .. R6 for the wide flag and the scan kernel.
 """
 import ctypes as C
-import os
-import shutil
-import subprocess
 import types
 
 import numpy as np
@@ -20,9 +17,9 @@ import pytest
 import torch
 
 import gpu_util
+import host_build
 from test_gpu_scan_marks import narrow_workspace
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 SIZE_MAX = 2**64 - 1
 THREAD, PAR, SPLIT = 0, 1, 2                                  # DecodeScan
 FIELDS = ("wide", "markStride", "tilesMax", "scan", "nSeq", "slowList", "marks", "scratch", "used", "tileFirst",
@@ -56,16 +53,8 @@ READ_BACK_MAX = 64 << 20                                      # workspaces the r
 
 
 @pytest.fixture(scope="module")
-def plan(tmp_path_factory):
-    gxx = shutil.which("g++")
-    if not gxx:
-        pytest.skip("g++ not available")
-    so = str(tmp_path_factory.mktemp("planemul") / "libplanemul.so")
-    subprocess.run([gxx, "-O2", "-std=c++17", "-Wall", "-shared", "-fPIC", "-o", so,
-                    os.path.join(HERE, "emul", "plan_emul.cpp")], check=True)
-    lib = C.CDLL(so)
-    lib.plan_host.restype = None
-    lib.plan_host.argtypes = [C.c_int64, C.c_int, C.c_int32, C.c_uint64, C.c_int, C.POINTER(C.c_uint64)]
+def plan():
+    lib = host_build.require()
 
     def run(n, per_block, cap, ws_bytes, partial=False):
         out = (C.c_uint64 * len(FIELDS))()

@@ -64,7 +64,7 @@ def hc_batch(lib, blocks, cap, level, src_phase=0, dst_phase=0, src_pad=0, dst_p
 def test_golden_vectors(lib, oracle):
     """Every capacity of every vector up to 256 KB.  A block is compressed by one thread, so the 1 MB and 4 MB inputs
     are checked at the bound only, all in one call per level (their other capacities are the CPU suite's)."""
-    doc, ins = he.golden()
+    doc, ins = he.golden("kat_hc.json")
     by_level, big = {}, {}
     for iid, lv, rb, rets, dig in doc["vectors"]:
         (big if ins[iid]["size"] > (256 << 10) else by_level).setdefault(lv, []).append((iid, rb, rets, dig))
@@ -92,7 +92,7 @@ def test_golden_vectors(lib, oracle):
 
 
 def test_run_digests(lib, oracle):
-    doc, _ = he.golden()
+    doc, _ = he.golden("kat_hc.json")
     cases = list(mg.random_cases(oracle, doc["run_cases"]))
     got = [None] * len(cases)
     groups = {}

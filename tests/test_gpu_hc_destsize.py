@@ -1,13 +1,13 @@
 """LZ4B200_compress_blocks_hc_destSize on the GPU through the C ABI: the reference's results
-(tests/golden/kat_hc_destsize.json) and the host build of the same parse (tests/hc_dest_emul.py), with mixed sizes, odd
+(tests/golden/kat_hc_destsize.json) and the host build of the same parse (tests/hc_emul.py), with mixed sizes, odd
 strides and phases, guard bytes at and past every slot's limit, targets at and below zero, workspace sizes, two calls on
 one workspace, round trips through the GPU decoder, argument errors, launch counts, the Python wrapper and a fuzz loop."""
 import numpy as np
 import pytest
 import torch
 
-import hc_dest_emul as hd
-from hc_dest_emul import host_hc_dest, mg, mgd
+import hc_emul as he
+from hc_emul import host_hc_dest, mg, mgd
 
 pytestmark = pytest.mark.gpu
 
@@ -33,7 +33,7 @@ def hcd_batch(lib, blocks, target, level, src_phase=0, dst_phase=0, src_pad=0, d
     nb = len(blocks)
     sizes = [len(b) for b in blocks]
     src_stride = max(max(sizes), 1) + src_pad
-    room = [hd.room(n, target) for n in sizes]
+    room = [he.room(n, target) for n in sizes]
     dst_stride = max(max(room), 1) + dst_pad
     src_h = np.zeros(src_phase + nb * src_stride + 16, dtype=np.uint8)
     for i, b in enumerate(blocks):
@@ -79,7 +79,7 @@ def grouped(lib, cases):
 def test_golden_vectors(lib, oracle):
     """Every target of every vector up to 64 KB.  A block is compressed by one thread, so the larger inputs are checked
     at the targets up to 65 536, where the parse stops early, and at 2^30 (their other targets are the CPU suite's)."""
-    doc, ins = hd.golden()
+    doc, ins = he.golden("kat_hc_destsize.json")
     data = {iid: mg.make_input(oracle, i["size"], i["kind"], i["seed"]) for iid, i in ins.items()}
     cases, want = [], []
     for iid, lv, rb, rets, cons, dig in doc["vectors"]:
@@ -103,7 +103,7 @@ def test_golden_vectors(lib, oracle):
 
 
 def test_run_digests(lib, oracle):
-    doc, _ = hd.golden()
+    doc, _ = he.golden("kat_hc_destsize.json")
     got = grouped(lib, list(mgd.random_cases(oracle, doc["run_cases"])))
     chunk = doc["run_chunk"]
     assert [mgd.run_digest(got[k:k + chunk]) for k in range(0, len(got), chunk)] == doc["run_digests"]

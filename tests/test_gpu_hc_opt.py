@@ -1,6 +1,6 @@
 """LZ4B200_compress_blocks_hc_opt and LZ4B200_compress_blocks_hc_opt_destSize (LZ4HC levels 10 .. 12) on the GPU through
 the C ABI: the reference's results (tests/golden/kat_hc_opt.json) and the host build of the same parse
-(tests/hc_opt_emul.py), with mixed sizes, odd strides and phases, guard bytes at and past every slot's limit, poisoned
+(tests/hc_emul.py), with mixed sizes, odd strides and phases, guard bytes at and past every slot's limit, poisoned
 and small workspaces, two calls on one workspace, round trips through the GPU decoder, side streams and graph capture,
 argument errors, launch counts and the Python wrappers.
 
@@ -11,8 +11,8 @@ import numpy as np
 import pytest
 import torch
 
-import hc_opt_emul as he
-from hc_opt_emul import host_hc_opt, host_hc_opt_dest, mg, mgd, mgo
+import hc_emul as he
+from hc_emul import host_hc_opt, host_hc_opt_dest, mg, mgd, mgo
 
 pytestmark = pytest.mark.gpu
 
@@ -113,7 +113,7 @@ def host(data, limit, level, fill):
 
 @pytest.fixture(scope="module")
 def golden(oracle):
-    doc, ins = he.golden()
+    doc, ins = he.golden("kat_hc_opt.json")
     return doc, ins, {iid: mg.make_input(oracle, i["size"], i["kind"], i["seed"]) for iid, i in ins.items()}
 
 
@@ -153,7 +153,7 @@ def test_golden_vectors_fill(lib, golden):
 
 
 def test_run_digests(lib, oracle):
-    doc, _ = he.golden()
+    doc, _ = he.golden("kat_hc_opt.json")
     chunk = doc["run_chunk"]
     got = grouped(lib, list(mgo.random_cases(oracle, doc["run_cases"], mgo.PLAIN_SEED)), False)
     assert [mg.run_digest(got[k:k + chunk]) for k in range(0, len(got), chunk)] == doc["run_digests"]

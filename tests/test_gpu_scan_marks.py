@@ -10,31 +10,21 @@ all when the block goes to the generic kernel; so these tests read the narrow ma
 Blocks sit at all 16 source phases; the corpus is gpu_util.hostile_corpus plus datagen blocks.  Return values and
 bytes are checked against the oracle, the sequence counts against the host scan."""
 import ctypes as C
-import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+import host_build
 from gpu_util import dev, hostile_corpus, to_dev
 
 pytestmark = pytest.mark.gpu
-HERE = os.path.dirname(os.path.abspath(__file__))
 SENT = 0xEEEEEEEE
 
 
 @pytest.fixture(scope="module")
-def host_scan(tmp_path_factory):
-    gxx = shutil.which("g++")
-    if not gxx:
-        pytest.skip("g++ not available")
-    so = str(tmp_path_factory.mktemp("scanmarks") / "libscanmarks.so")
-    subprocess.run([gxx, "-O2", "-std=c++17", "-Wall", "-shared", "-fPIC", "-o", so,
-                    os.path.join(HERE, "emul", "scan_marks_emul.cpp")], check=True)
-    lib = C.CDLL(so)
-    lib.scan_host_cap.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_uint32), C.c_void_p, C.c_uint32]
+def host_scan():
+    lib = host_build.require()
     memo = {}
 
     def run(block, cap, stride):

@@ -10,7 +10,7 @@ and target tables, strides) is final before the sleep, so a wrong stream can onl
 out of range.
 
 Every result is compared with a reference: the oracle for decodes, partial decodes, compress and destSize; the host
-builds of the HC parses (hc_emul, hc_dest_emul); the parallel compressor's host model (encpar_model); the pack
+build of the HC parses (hc_emul); the parallel compressor's host model (encpar_model); the pack
 restatement (gpu_util.pack_model); the frame restatement (frame_oracle).  Guard bytes are checked as the route tests
 do: a rejected block's slot and the bytes past every returned size stay as they were.
 
@@ -35,8 +35,7 @@ for _p in (ROOT, HERE):
 import encpar_model  # noqa: E402
 import frame_oracle  # noqa: E402
 from gpu_util import GUARD, hostile_corpus, odd_stride, pack_host_blocks, pack_model, route  # noqa: E402
-from hc_dest_emul import host_hc_dest  # noqa: E402
-from hc_emul import host_hc  # noqa: E402
+from hc_emul import host_hc, host_hc_dest  # noqa: E402
 from lz4_b200 import _lib, batch  # noqa: E402
 
 pytestmark = pytest.mark.gpu

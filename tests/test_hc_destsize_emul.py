@@ -1,19 +1,12 @@
-"""CPU check of the HC fill parse the GPU runs: the host build of lz4_b200/csrc/lz4_hc_core.h (tests/emul/hc_dest_emul.cpp)
+"""CPU check of the HC fill parse the GPU runs: the host build of lz4_b200/csrc/lz4_hc_core.h (tests/emul/hc_emul.cpp)
 must give the reference's LZ4_compress_HC_destSize results (ret, consumed and bytes) on every vector and run digest of
 tests/golden/kat_hc_destsize.json, whatever the chain table holds at the start, write nothing at or past
 min(target, bound), and every output must decode through the oracle's decoder to exactly the first `consumed` input
 bytes.  Where oracle/_ref exists, extra seeded cases are compared with the reference live."""
 import numpy as np
-import pytest
 
-import hc_dest_emul as hd
-from hc_dest_emul import host_hc_dest, mg, mgd
-
-
-@pytest.fixture(scope="module", autouse=True)
-def emul():
-    if hd.load() is None:
-        pytest.skip("g++ not available")
+import hc_emul as he
+from hc_emul import host_hc_dest, mg, mgd
 
 
 def check_decodes(oracle, out, consumed, data):
@@ -21,7 +14,7 @@ def check_decodes(oracle, out, consumed, data):
 
 
 def test_vectors_match_the_reference(oracle):
-    doc, ins = hd.golden()
+    doc, ins = he.golden("kat_hc_destsize.json")
     data = {}
     checked = 0
     for iid, lv, rb, rets, cons, dig in doc["vectors"]:
@@ -45,7 +38,7 @@ def test_vectors_match_the_reference(oracle):
 
 
 def test_run_digests_match_the_reference(oracle):
-    doc, _ = hd.golden()
+    doc, _ = he.golden("kat_hc_destsize.json")
     runs, res = [], []
     for d, t, lv in mgd.random_cases(oracle, doc["run_cases"]):
         res.append(host_hc_dest(d, t, lv, chain_fill=0x1234))

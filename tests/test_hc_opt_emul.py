@@ -1,26 +1,20 @@
 """CPU check of the HC optimal parse (levels 10 .. 12) the GPU runs: the host build of lz4_b200/csrc/lz4_hc_core.h
-(tests/emul/hc_opt_emul.cpp) must give the reference's LZ4_compress_HC and LZ4_compress_HC_destSize results on every
+(tests/emul/hc_emul.cpp) must give the reference's LZ4_compress_HC and LZ4_compress_HC_destSize results on every
 vector and run digest of tests/golden/kat_hc_opt.json, whatever the chain table and the price table hold at the start,
 write nothing past its limit, and every output must decode through the oracle's decoder (at the input's size, or at
 `consumed` for the fill mode).  Where oracle/_ref exists, extra seeded cases are compared with the reference live."""
 import numpy as np
 import pytest
 
-import hc_opt_emul as he
-from hc_opt_emul import host_hc_opt, host_hc_opt_dest, mg, mgd, mgo
+import hc_emul as he
+from hc_emul import host_hc_opt, host_hc_opt_dest, mg, mgd, mgo
 
 FILLS = [(0xFFFF, 0), (0x3C5A, 0x7FFFFFFF), (0x0001, 0x80000000), (0x1234, 0xFFFFFFFF)]
 
 
-@pytest.fixture(scope="module", autouse=True)
-def emul():
-    if he.load() is None:
-        pytest.skip("g++ not available")
-
-
 @pytest.fixture(scope="module")
 def inputs(oracle):
-    doc, ins = he.golden()
+    doc, ins = he.golden("kat_hc_opt.json")
     data = {}
     for iid, i in ins.items():
         data[iid] = mg.make_input(oracle, i["size"], i["kind"], i["seed"])
@@ -57,7 +51,7 @@ def test_fill_vectors_match_the_reference(oracle, inputs):
 
 
 def test_run_digests_match_the_reference(oracle):
-    doc, _ = he.golden()
+    doc, _ = he.golden("kat_hc_opt.json")
     runs, res = [], []
     for d, cap, lv in mgo.random_cases(oracle, doc["run_cases"], mgo.PLAIN_SEED):
         res.append(host_hc_opt(d, cap, lv, chain_fill=0x5555, opt_fill=0x01010101))

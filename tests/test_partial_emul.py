@@ -7,33 +7,22 @@ the last sequence (16 bits).  4 MB blocks at targets up to 61 440 must fit the r
 """
 import ctypes as C
 import os
-import shutil
-import subprocess
 import sys
 
 import numpy as np
 import pytest
+
+import host_build
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 
 import make_golden_partial as mg  # noqa: E402
 
-_u32p = C.POINTER(C.c_uint32)
-
 
 @pytest.fixture(scope="module")
-def emul(tmp_path_factory):
-    gxx = shutil.which("g++")
-    if not gxx:
-        pytest.skip("g++ not available")
-    so = str(tmp_path_factory.mktemp("partialemul") / "libpartialemul.so")
-    subprocess.run([gxx, "-O2", "-std=c++17", "-Wall", "-shared", "-fPIC", "-o", so,
-                    os.path.join(HERE, "emul", "partial_emul.cpp")], check=True)
-    lib = C.CDLL(so)
-    lib.partial_emulate.restype = C.c_int
-    lib.partial_emulate.argtypes = [C.c_char_p, C.c_int, C.c_int, _u32p, _u32p, _u32p, C.c_uint32, C.c_char_p]
-    return lib
+def emul():
+    return host_build.require()
 
 
 def run(lib, src, cap):

@@ -8,29 +8,19 @@ compared with the oracle's LZ4_decompress_safe: return value and bytes.  This pi
 """
 import ctypes as C
 import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
+import host_build
 from oracle.pyoracle import Oracle, Reference, have_reference
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 @pytest.fixture(scope="module")
-def emul(tmp_path_factory):
-    gxx = shutil.which("g++")
-    if not gxx:
-        pytest.skip("g++ not available")
-    so = str(tmp_path_factory.mktemp("rowsemul") / "librowsemul.so")
-    subprocess.run([gxx, "-O2", "-std=c++17", "-Wall", "-shared", "-fPIC", "-o", so,
-                    os.path.join(HERE, "emul", "rows_emul.cpp")], check=True)
-    lib = C.CDLL(so)
-    lib.rows_emulate.restype = C.c_int
-    lib.rows_emulate.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_char_p, C.c_int, C.c_int, C.POINTER(C.c_longlong)]
-    return lib
+def emul():
+    return host_build.require()
 
 
 def run(lib, comp, cap, head=0, rpt=4):

@@ -6,28 +6,19 @@ sequences and the per-sequence marks.  Test infrastructure only: the library nev
 import ctypes as C
 import json
 import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
+import host_build
 from oracle.pyoracle import Oracle, Reference, have_reference
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 @pytest.fixture(scope="module")
-def scan(tmp_path_factory):
-    gxx = shutil.which("g++")
-    if not gxx:
-        pytest.skip("g++ not available")
-    so = str(tmp_path_factory.mktemp("scanemul") / "libscanemul.so")
-    subprocess.run([gxx, "-O2", "-std=c++17", "-Wall", "-shared", "-fPIC", "-o", so,
-                    os.path.join(HERE, "emul", "scan_emul.cpp")], check=True)
-    lib = C.CDLL(so)
-    lib.scan_host.restype = C.c_int
-    lib.scan_host.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_uint32), C.c_void_p]
+def scan():
+    lib = host_build.require()
     entry = lib.scan_host
     max_seq = lib.scan_host_max_seq()
 

@@ -9,13 +9,12 @@ capacity-limited block the same words whatever the phase.  The split and the par
 chunks at the edges of their parts) must leave the one-thread scan's marks."""
 import ctypes as C
 import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
 import big_corpus as bc
+import host_build
 from gpu_util import corrupt, lz4_seq, seq_count_block
 from oracle.pyoracle import Oracle
 from test_scan_core_host import true_marks
@@ -26,25 +25,8 @@ GUARD = 16                      # sentinel words on either side of a table
 
 
 @pytest.fixture(scope="module")
-def libs(tmp_path_factory):
-    gxx = shutil.which("g++")
-    if not gxx:
-        pytest.skip("g++ not available")
-    out = {}
-    for name in ("scan_marks_emul", "scan_split_emul", "scan_par_emul"):
-        so = str(tmp_path_factory.mktemp(name) / ("lib%s.so" % name))
-        subprocess.run([gxx, "-O1", "-std=c++17", "-Wall", "-shared", "-fPIC", "-o", so,
-                        os.path.join(HERE, "emul", name + ".cpp")], check=True)
-        out[name] = C.CDLL(so)
-    u32p = C.POINTER(C.c_uint32)
-    out["scan_marks_emul"].scan_host_cap.argtypes = [C.c_void_p, C.c_int, C.c_int, u32p, C.c_void_p, C.c_uint32]
-    out["scan_split_emul"].scan_split_host.argtypes = [C.c_void_p, C.c_int, C.c_int, u32p, C.c_void_p, C.c_uint32,
-                                                      C.POINTER(C.c_int)]
-    out["scan_par_emul"].scan_par_host.argtypes = [C.c_void_p, C.c_int, C.c_int, u32p, C.c_void_p, C.POINTER(C.c_int)]
-    out["scan_par_emul"].scan_thread_host_wide.argtypes = [C.c_void_p, C.c_int, C.c_int, u32p, C.c_void_p, C.c_uint32]
-    out["scan_par_emul"].scan_par_host_wide.argtypes = [C.c_void_p, C.c_int, C.c_int, u32p, C.c_void_p, C.c_uint32,
-                                                       C.POINTER(C.c_int)]
-    return out
+def lib():
+    return host_build.require()
 
 
 def place_block(block, shift):
@@ -56,7 +38,7 @@ def place_block(block, shift):
     return buf, buf.ctypes.data + pad
 
 
-def run(libs, which, block, cap, mark_cap, phase, shift=0):
+def run(lib, which, block, cap, mark_cap, phase, shift=0):
     """-> (ret, nseq, the words of a table of mark_cap words at word `phase` of a 32-byte chunk, with GUARD sentinel
     words before and after it)"""
     buf, src = place_block(block, shift)
@@ -67,27 +49,27 @@ def run(libs, which, block, cap, mark_cap, phase, shift=0):
     st = (C.c_int * 3)()
     n = len(block)
     if which == "thread":
-        r = libs["scan_marks_emul"].scan_host_cap(src, n, cap, C.byref(ns), table, mark_cap)
+        r = lib.scan_host_cap(src, n, cap, C.byref(ns), table, mark_cap)
     elif which == "split":
-        r = libs["scan_split_emul"].scan_split_host(src, n, cap, C.byref(ns), table, mark_cap, st)
+        r = lib.scan_split_host(src, n, cap, C.byref(ns), table, mark_cap, st)
     elif which == "par":
         assert mark_cap == 8192
-        r = libs["scan_par_emul"].scan_par_host(src, n, cap, C.byref(ns), table, st)
+        r = lib.scan_par_host(src, n, cap, C.byref(ns), table, st, bc.LANES)
     elif which == "thread-wide":
-        r = libs["scan_par_emul"].scan_thread_host_wide(src, n, cap, C.byref(ns), table, mark_cap // 2)
+        r = lib.scan_thread_host_wide(src, n, cap, C.byref(ns), table, mark_cap // 2)
     else:
-        r = libs["scan_par_emul"].scan_par_host_wide(src, n, cap, C.byref(ns), table, mark_cap // 2, st)
+        r = lib.scan_par_host_wide(src, n, cap, C.byref(ns), table, mark_cap // 2, st, bc.LANES)
     del buf
     return r, ns.value, words[first - GUARD:first + mark_cap + GUARD].copy()
 
 
-def check_block(libs, block, cap, mark_cap, shifts=(0,), scans=("thread",), orc=None):
+def check_block(lib, block, cap, mark_cap, shifts=(0,), scans=("thread",), orc=None):
     """every scan at every phase and source shift leaves the same words; an accepted block's are its true marks"""
     want = None
     for which in scans:
         for shift in shifts:
             for phase in range(8):
-                r, ns, w = run(libs, which, block, cap, mark_cap, phase, shift)
+                r, ns, w = run(lib, which, block, cap, mark_cap, phase, shift)
                 assert (w[:GUARD] == SENT).all() and (w[GUARD + mark_cap:] == SENT).all(), \
                     (which, phase, shift, "wrote outside the block's table")
                 table = w[GUARD:GUARD + mark_cap]
@@ -113,14 +95,14 @@ def check_block(libs, block, cap, mark_cap, shifts=(0,), scans=("thread",), orc=
     return want
 
 
-def test_fixture_block_every_phase_and_shift(libs):
+def test_fixture_block_every_phase_and_shift(lib):
     blk = open(os.path.join(HERE, "golden", "p50_seed0_64k.lz4block"), "rb").read()
-    r, ns, _ = check_block(libs, blk, 65536, 8192, shifts=range(16), scans=("thread", "split", "par"))
+    r, ns, _ = check_block(lib, blk, 65536, 8192, shifts=range(16), scans=("thread", "split", "par"))
     assert r == 65536 and ns > 2000
 
 
 @pytest.mark.parametrize("cap", [1000, 16383, 20000, 65536])
-def test_capacities_with_odd_mark_strides(libs, cap):
+def test_capacities_with_odd_mark_strides(lib, cap):
     """markStride = cap / 4 + 2 (252, 4 097, 5 002, 16 386 -> 8 192): a block's table starts mid-chunk"""
     orc = Oracle()
     mark_cap = min(cap // 4 + 2, 8192)
@@ -130,23 +112,23 @@ def test_capacities_with_odd_mark_strides(libs, cap):
         raw = orc.datagen(cap, p, int(rng.integers(0, 1 << 30)))
         _, c = orc.compress(raw, 1)
         c = bytes(c)
-        check_block(libs, c, cap, mark_cap, shifts=(0, 5, 15), scans=scans, orc=orc)
+        check_block(lib, c, cap, mark_cap, shifts=(0, 5, 15), scans=scans, orc=orc)
         for k in range(6):                                     # rejected and capacity-limited blocks
-            check_block(libs, corrupt(rng, c), cap, mark_cap, shifts=(k,), orc=orc)
+            check_block(lib, corrupt(rng, c), cap, mark_cap, shifts=(k,), orc=orc)
         for c2 in (cap - 1, cap - 70, cap // 2):
-            check_block(libs, c, c2, mark_cap, shifts=(3,), orc=orc)
+            check_block(lib, c, c2, mark_cap, shifts=(3,), orc=orc)
 
 
-def test_last_byte_at_every_granule_offset(libs):
+def test_last_byte_at_every_granule_offset(lib):
     """source shifts 0..15 put a block's last byte at every offset of its granule"""
     orc = Oracle()
     for size in (777, 4096, 30001):
         raw = orc.datagen(size, 0.5, size)
         _, c = orc.compress(raw, 1)
-        check_block(libs, bytes(c), size, size // 4 + 2, shifts=range(16), orc=orc)
+        check_block(lib, bytes(c), size, size // 4 + 2, shifts=range(16), orc=orc)
 
 
-def test_long_runs_and_extension_bytes(libs):
+def test_long_runs_and_extension_bytes(lib):
     """literal runs and matches of 1 .. 3 extension bytes, their lengths and offsets at every position of a granule"""
     orc = Oracle()
     rng = np.random.default_rng(7)
@@ -161,23 +143,23 @@ def test_long_runs_and_extension_bytes(libs):
         size = orc.decompress(blk, 1 << 20)[0]
         assert size > 0
         cap = min(size, 65536)
-        check_block(libs, blk, cap, min(cap // 4 + 2, 8192), shifts=(lead, 15 - lead), orc=orc)
+        check_block(lib, blk, cap, min(cap // 4 + 2, 8192), shifts=(lead, 15 - lead), orc=orc)
 
 
-def test_blocks_at_the_mark_cap(libs):
+def test_blocks_at_the_mark_cap(lib):
     """8 191 .. 8 200 sequences against the 8 192-word table: the table fills, nothing is written past it"""
     for ns in (8191, 8192, 8193, 8200):
-        r, got, table = check_block(libs, seq_count_block(ns), 65536, 8192, shifts=(0, 9), scans=("thread", "split", "par"))
+        r, got, table = check_block(lib, seq_count_block(ns), 65536, 8192, shifts=(0, 9), scans=("thread", "split", "par"))
         assert r == 4 * ns + 13 and got == ns
 
 
-def test_wide_marks(libs):
+def test_wide_marks(lib):
     """two words per sequence (blocks above 64 KB): the one-thread and the parallel scan leave the same words"""
     orc = Oracle()
     raw = orc.datagen(300000, 0.5, 3)
     _, c = orc.compress(raw, 1)
     mark_cap = 2 * (300000 // 4 + 2)
-    r, ns, table = check_block(libs, bytes(c), 300000, mark_cap, shifts=(0, 7), scans=("thread-wide", "par-wide"))
+    r, ns, table = check_block(lib, bytes(c), 300000, mark_cap, shifts=(0, 7), scans=("thread-wide", "par-wide"))
     assert r == 300000
     assert table[:2 * ns].tolist() == bc.wide_marks(bc.seq_list(bytes(c))).tolist()
     assert (table[2 * ns:] == SENT).all()

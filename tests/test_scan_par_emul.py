@@ -8,12 +8,11 @@ tests/test_scan_core_host.py): return value, sequence count, and the marks of ev
 """
 import ctypes as C
 import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
+import host_build
 from oracle.pyoracle import Oracle, Reference, have_reference
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -21,37 +20,16 @@ MAX_SEQ = 8192
 
 
 @pytest.fixture(scope="module")
-def libs(tmp_path_factory):
-    gxx = shutil.which("g++")
-    if not gxx:
-        pytest.skip("g++ not available")
-    d = tmp_path_factory.mktemp("scanpar")
-    out = []
-    for name in ("scan_emul", "scan_par_emul"):
-        so = str(d / ("lib%s.so" % name))
-        subprocess.run([gxx, "-O2", "-std=c++17", "-Wall", "-shared", "-fPIC", "-o", so,
-                        os.path.join(HERE, "emul", name + ".cpp")], check=True)
-        out.append(C.CDLL(so))
-    one, v2 = out
-    one.scan_host.restype = C.c_int
-    one.scan_host.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_uint32), C.c_void_p]
-    v2.scan_par_host.restype = C.c_int
-    v2.scan_par_host.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_uint32), C.c_void_p, C.POINTER(C.c_int)]
-    v2.scan_par_fuzz.restype = C.c_longlong
-    v2.scan_par_fuzz.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_uint64, C.POINTER(C.c_longlong)]
-    v2.scan_par_set_lanes.restype = None
-    v2.scan_par_set_lanes.argtypes = [C.c_int]
-    return one, v2
+def lib():
+    return host_build.require()
 
 
 @pytest.fixture(params=[32, 128, 256])
-def lanes(request, libs):
-    libs[1].scan_par_set_lanes(request.param)
+def lanes(request):
     return request.param
 
 
-def both(libs, block, cap, shift=0, with_marks=True):
-    one, v2 = libs
+def both(lib, lanes, block, cap, shift=0, with_marks=True):
     n = len(block)
     buf = np.full(n + 32, 0xEE, dtype=np.uint8)
     base = buf.ctypes.data
@@ -61,8 +39,8 @@ def both(libs, block, cap, shift=0, with_marks=True):
     m2 = np.full(MAX_SEQ, 0xABABABAB, dtype=np.uint32)
     n1, n2 = C.c_uint32(0), C.c_uint32(0)
     stats = (C.c_int * 3)()
-    r1 = one.scan_host(base + pad, n, cap, C.byref(n1), m1.ctypes.data if with_marks else None)
-    r2 = v2.scan_par_host(base + pad, n, cap, C.byref(n2), m2.ctypes.data if with_marks else None, stats)
+    r1 = lib.scan_host(base + pad, n, cap, C.byref(n1), m1.ctypes.data if with_marks else None)
+    r2 = lib.scan_par_host(base + pad, n, cap, C.byref(n2), m2.ctypes.data if with_marks else None, stats, lanes)
     k = min(n1.value, MAX_SEQ)
     return (r1, n1.value, m1[:k]), (r2, n2.value, m2[:k]), list(stats)
 
@@ -83,7 +61,7 @@ def corrupt(rng, comp):
     return bytes(b)
 
 
-def test_parallel_scan_equals_one_thread_scan(libs, lanes):
+def test_parallel_scan_equals_one_thread_scan(lib, lanes):
     orc = Oracle()
     gen = Reference() if have_reference() else orc
     rng = np.random.default_rng(20260924)
@@ -95,7 +73,7 @@ def test_parallel_scan_equals_one_thread_scan(libs, lanes):
             comp = bytes(comp)
             caps = {size, size + 1, size + 64, size + 1000, size - 1, size - 70, size // 2, 64, 63}
             for cap in caps:
-                a, b, st = both(libs, comp, cap, shift=int(rng.integers(0, 4)), with_marks=(len(comp) <= 65535 and cap <= 65536))
+                a, b, st = both(lib, lanes, comp, cap, shift=int(rng.integers(0, 4)), with_marks=(len(comp) <= 65535 and cap <= 65536))
                 assert a[0] == b[0] and a[1] == b[1], (proba, size, cap, a[:2], b[:2], st)
                 assert np.array_equal(a[2], b[2]), (proba, size, cap, st)
                 if cap == size:
@@ -107,7 +85,7 @@ def test_parallel_scan_equals_one_thread_scan(libs, lanes):
             for _ in range(10 if size <= 70000 else 3):
                 bad = corrupt(rng, comp)
                 cap = int(rng.choice([size, size + 64, size + 1000, max(size - 5, 0)]))
-                a, b, st = both(libs, bad, cap, shift=int(rng.integers(0, 4)), with_marks=(len(bad) <= 65535 and cap <= 65536))
+                a, b, st = both(lib, lanes, bad, cap, shift=int(rng.integers(0, 4)), with_marks=(len(bad) <= 65535 and cap <= 65536))
                 assert a[0] == b[0] and a[1] == b[1], (proba, size, cap, a[:2], b[:2], st)
                 assert np.array_equal(a[2], b[2])
                 errors += a[0] < 0
@@ -116,11 +94,11 @@ def test_parallel_scan_equals_one_thread_scan(libs, lanes):
     assert rounds <= {32: 4, 128: 16, 256: 32}[lanes]   # P50: the re-walks die out after a few rounds (longest run of unsynchronised lanes)
 
 
-def test_fixture_block_and_special_shapes(libs, lanes):
+def test_fixture_block_and_special_shapes(lib, lanes):
     blk = open(os.path.join(HERE, "golden", "p50_seed0_64k.lz4block"), "rb").read()
     for cap in (65536, 65536 + 64, 65535, 65536 - 64, 70000, 100, 64, 0, -1):
         for shift in range(4):
-            a, b, st = both(libs, blk, cap, shift)
+            a, b, st = both(lib, lanes, blk, cap, shift)
             assert a[0] == b[0] and a[1] == b[1] and np.array_equal(a[2], b[2]), (cap, shift, a[:2], b[:2], st)
     # long literal runs (chains jump over whole segments), long matches, RLE, text
     rng = np.random.default_rng(5)
@@ -132,14 +110,13 @@ def test_fixture_block_and_special_shapes(libs, lanes):
     for raw in shapes:
         _, comp = orc.compress(raw, 1)
         for cap in (len(raw), len(raw) + 64, len(raw) + 5000, len(raw) - 1):
-            a, b, st = both(libs, bytes(comp), cap, 1, with_marks=(len(comp) <= 65535 and cap <= 65536))
+            a, b, st = both(lib, lanes, bytes(comp), cap, 1, with_marks=(len(comp) <= 65535 and cap <= 65536))
             assert a[0] == b[0] and a[1] == b[1] and np.array_equal(a[2], b[2]), (len(raw), cap, a[:2], b[:2], st)
 
 
-def test_differential_fuzz_in_process(libs, lanes):
+def test_differential_fuzz_in_process(lib, lanes):
     """Tens of thousands of mutated blocks, compared inside the emulator library (fast): the warp scan
     must agree with the one-thread scan on the return value (incl. every error code), count and marks."""
-    _, v2 = libs
     gen = Reference() if have_reference() else Oracle()
     total = errors = 0
     k = 1 if lanes == 128 else 4
@@ -148,21 +125,16 @@ def test_differential_fuzz_in_process(libs, lanes):
         raw = bytes(gen.datagen(size, proba, seed))
         _, comp = gen.compress(raw, 1)
         ne = C.c_longlong(0)
-        n = v2.scan_par_fuzz(bytes(comp), len(comp), size, iters, seed, C.byref(ne))
+        n = lib.scan_par_fuzz(bytes(comp), len(comp), size, iters, seed, C.byref(ne), lanes)
         assert n == iters, (proba, size, "first mismatch at case %d" % (-n - 1))
         total += n
         errors += ne.value
     assert total > 30000 // k and errors > 10000 // k
 
 
-def test_wide_marks_of_big_blocks(libs, lanes):
+def test_wide_marks_of_big_blocks(lib, lanes):
     """Blocks above 64 KB get two-word marks {token position, match start} for the tiles kernel: the parallel scan and the
     one-thread scan must write the same ones, on valid, truncated and corrupted blocks."""
-    _, v2 = libs
-    v2.scan_par_host_wide.restype = C.c_int
-    v2.scan_par_host_wide.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_uint32), C.c_void_p, C.c_uint32, C.POINTER(C.c_int)]
-    v2.scan_thread_host_wide.restype = C.c_int
-    v2.scan_thread_host_wide.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_uint32), C.c_void_p, C.c_uint32]
     gen = Reference() if have_reference() else Oracle()
     rng = np.random.default_rng(lanes)
     for proba, size, seed in ((0.5, 1 << 20, 1), (0.9, 300000, 2), (0.0, 150000, 3), (0.5, 4 << 20, 4)):
@@ -180,8 +152,8 @@ def test_wide_marks_of_big_blocks(libs, lanes):
             m2 = np.full(2 * mcap, 0xABABABAB, dtype=np.uint32)
             n1, n2 = C.c_uint32(0), C.c_uint32(0)
             st = (C.c_int * 3)()
-            r1 = v2.scan_thread_host_wide(buf.ctypes.data, len(blk), cap, C.byref(n1), m1.ctypes.data, mcap)
-            r2 = v2.scan_par_host_wide(buf.ctypes.data, len(blk), cap, C.byref(n2), m2.ctypes.data, mcap, st)
+            r1 = lib.scan_thread_host_wide(buf.ctypes.data, len(blk), cap, C.byref(n1), m1.ctypes.data, mcap)
+            r2 = lib.scan_par_host_wide(buf.ctypes.data, len(blk), cap, C.byref(n2), m2.ctypes.data, mcap, st, lanes)
             assert r1 == r2 and n1.value == n2.value, (proba, size, cap, r1, r2, n1.value, n2.value)
             if r1 > 0:
                 k = min(n1.value, mcap)

@@ -7,12 +7,11 @@ sequence count, and the marks of every sequence.
 """
 import ctypes as C
 import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
+import host_build
 from oracle.pyoracle import Oracle, Reference, have_reference
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -20,29 +19,11 @@ MAX_SEQ = 8192
 
 
 @pytest.fixture(scope="module")
-def libs(tmp_path_factory):
-    gxx = shutil.which("g++")
-    if not gxx:
-        pytest.skip("g++ not available")
-    d = tmp_path_factory.mktemp("scansplit")
-    out = []
-    for name in ("scan_emul", "scan_split_emul"):
-        so = str(d / ("lib%s.so" % name))
-        subprocess.run([gxx, "-O2", "-std=c++17", "-Wall", "-shared", "-fPIC", "-o", so,
-                        os.path.join(HERE, "emul", name + ".cpp")], check=True)
-        out.append(C.CDLL(so))
-    one, sp = out
-    one.scan_host.restype = C.c_int
-    one.scan_host.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_uint32), C.c_void_p]
-    sp.scan_split_host.restype = C.c_int
-    sp.scan_split_host.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_uint32), C.c_void_p, C.c_uint32, C.POINTER(C.c_int)]
-    sp.scan_split_fuzz.restype = C.c_longlong
-    sp.scan_split_fuzz.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_uint64, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]
-    return one, sp
+def lib():
+    return host_build.require()
 
 
-def both(libs, block, cap, shift=0):
-    one, sp = libs
+def both(lib, block, cap, shift=0):
     n = len(block)
     buf = np.full(n + 80, 0xEE, dtype=np.uint8)
     base = buf.ctypes.data
@@ -52,8 +33,8 @@ def both(libs, block, cap, shift=0):
     m2 = np.full(MAX_SEQ, 0xABABABAB, dtype=np.uint32)
     n1, n2 = C.c_uint32(0), C.c_uint32(0)
     stats = (C.c_int * 3)()
-    r1 = one.scan_host(base + pad, n, cap, C.byref(n1), m1.ctypes.data)
-    r2 = sp.scan_split_host(base + pad, n, cap, C.byref(n2), m2.ctypes.data, MAX_SEQ, stats)
+    r1 = lib.scan_host(base + pad, n, cap, C.byref(n1), m1.ctypes.data)
+    r2 = lib.scan_split_host(base + pad, n, cap, C.byref(n2), m2.ctypes.data, MAX_SEQ, stats)
     k = min(n1.value, MAX_SEQ)
     return (r1, n1.value, m1[:k]), (r2, n2.value, m2[:k]), list(stats)
 
@@ -74,7 +55,7 @@ def corrupt(rng, comp):
     return bytes(b)[:65535]
 
 
-def test_split_scan_equals_one_thread_scan(libs):
+def test_split_scan_equals_one_thread_scan(lib):
     orc = Oracle()
     gen = Reference() if have_reference() else orc
     rng = np.random.default_rng(20260925)
@@ -89,7 +70,7 @@ def test_split_scan_equals_one_thread_scan(libs):
             for cap in {size, size + 1, size + 64, min(size + 1000, 65536), size - 1, size - 70, size // 2, 64, 63, 65536}:
                 if cap > 65536:
                     continue
-                a, b, st = both(libs, comp, cap, shift=int(rng.integers(0, 16)))
+                a, b, st = both(lib, comp, cap, shift=int(rng.integers(0, 16)))
                 assert a[0] == b[0] and a[1] == b[1], (proba, size, cap, a[:2], b[:2], st)
                 assert np.array_equal(a[2], b[2]), (proba, size, cap, st)
                 if cap == size:
@@ -100,7 +81,7 @@ def test_split_scan_equals_one_thread_scan(libs):
             for _ in range(12):
                 bad = corrupt(rng, comp)
                 cap = int(rng.choice([size, min(size + 64, 65536), min(size + 1000, 65536), max(size - 5, 1)]))
-                a, b, st = both(libs, bad, cap, shift=int(rng.integers(0, 16)))
+                a, b, st = both(lib, bad, cap, shift=int(rng.integers(0, 16)))
                 assert a[0] == b[0] and a[1] == b[1], (proba, size, cap, a[:2], b[:2], st)
                 assert np.array_equal(a[2], b[2])
                 errors += a[0] < 0
@@ -109,11 +90,11 @@ def test_split_scan_equals_one_thread_scan(libs):
     assert fallbacks == 0                                  # well-formed data never needs the one-thread scan
 
 
-def test_fixture_block_and_special_shapes(libs):
+def test_fixture_block_and_special_shapes(lib):
     blk = open(os.path.join(HERE, "golden", "p50_seed0_64k.lz4block"), "rb").read()
     for cap in (65536, 65535, 65536 - 64, 65536 - 65, 40000, 100, 64):
         for shift in range(4):
-            a, b, st = both(libs, blk, cap, shift)
+            a, b, st = both(lib, blk, cap, shift)
             assert a[0] == b[0] and a[1] == b[1] and np.array_equal(a[2], b[2]), (cap, shift, a[:2], b[:2], st)
     rng = np.random.default_rng(5)
     orc = Oracle()
@@ -126,13 +107,12 @@ def test_fixture_block_and_special_shapes(libs):
         if len(comp) > 65535:
             continue
         for cap in (len(raw), min(len(raw) + 64, 65536), len(raw) - 1, len(raw) // 3):
-            a, b, st = both(libs, bytes(comp), cap, 1)
+            a, b, st = both(lib, bytes(comp), cap, 1)
             assert a[0] == b[0] and a[1] == b[1] and np.array_equal(a[2], b[2]), (len(raw), cap, a[:2], b[:2], st)
 
 
-def test_differential_fuzz_in_process(libs):
+def test_differential_fuzz_in_process(lib):
     """Tens of thousands of mutated blocks, compared inside the emulator library (fast)."""
-    _, sp = libs
     gen = Reference() if have_reference() else Oracle()
     total = errors = 0
     for seed, (proba, size, iters) in enumerate(((0.5, 65536, 12000), (0.9, 65536, 8000), (0.2, 65536, 4000), (0.0, 60000, 1500),
@@ -142,7 +122,7 @@ def test_differential_fuzz_in_process(libs):
         if len(comp) > 65535:
             continue
         ne, nf = C.c_longlong(0), C.c_longlong(0)
-        n = sp.scan_split_fuzz(bytes(comp), len(comp), size, iters, seed, C.byref(ne), C.byref(nf))
+        n = lib.scan_split_fuzz(bytes(comp), len(comp), size, iters, seed, C.byref(ne), C.byref(nf))
         assert n == iters, (proba, size, "first mismatch at case %d" % (-n - 1))
         total += n
         errors += ne.value

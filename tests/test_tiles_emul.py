@@ -8,12 +8,11 @@ byte of this tile, byte of an earlier tile) before the kernel runs on a GPU.
 """
 import ctypes as C
 import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
+import host_build
 from oracle.pyoracle import Oracle, Reference, have_reference
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -21,17 +20,8 @@ TILE = 61440
 
 
 @pytest.fixture(scope="module")
-def emul(tmp_path_factory):
-    gxx = shutil.which("g++")
-    if not gxx:
-        pytest.skip("g++ not available")
-    so = str(tmp_path_factory.mktemp("tilesemul") / "libtilesemul.so")
-    subprocess.run([gxx, "-O2", "-std=c++17", "-Wall", "-shared", "-fPIC", "-o", so,
-                    os.path.join(HERE, "emul", "tiles_emul.cpp")], check=True)
-    lib = C.CDLL(so)
-    lib.tiles_emulate.restype = C.c_int
-    lib.tiles_emulate.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_char_p, C.c_int, C.POINTER(C.c_longlong)]
-    return lib
+def emul():
+    return host_build.require()
 
 
 def run(lib, comp, cap, rpt=4):
