@@ -3,7 +3,7 @@
  *
  * Two layers, both plain C (pointers and sizes only, no torch / C++ types):
  *
- *  1. DROP-IN layer: the one-shot block API of the reference's lib/lz4.h, same names, argument
+ *  1. DROP-IN layer: the one-shot block API of the reference's lib/lz4.h and lib/lz4hc.h, same names, argument
  *     meaning, return values and error behaviour, host pointers, synchronous.  A program built
  *     against the reference's own lz4.h links against this library unchanged for these symbols
  *     (each declaration cites the lz4.h / lz4.c line it replaces; v1.10.0).
@@ -46,6 +46,7 @@ extern "C" {
 #define LZ4B200_VERSION_NUMBER 11000          /* == LZ4_VERSION_NUMBER, lz4.h:131-135 */
 #define LZ4B200_MAX_INPUT_SIZE 0x7E000000     /* == LZ4_MAX_INPUT_SIZE, lz4.h:214 */
 #define LZ4B200_STATE_BYTES    16416          /* == sizeof(LZ4_stream_t), lz4.h:729-733 */
+#define LZ4B200_STATEHC_BYTES  262200         /* == sizeof(LZ4_streamHC_t) == LZ4_STREAMHC_MINSIZE, lz4hc.h:252-256 */
 
 /* lz4.h:142 / lz4.c:749 */
 LZ4B200_API int LZ4_versionNumber(void);
@@ -87,6 +88,41 @@ LZ4B200_API int LZ4_compress_destSize(const char* src, char* dst, int* srcSizePt
  * 0 and leaves *srcSizePtr untouched. */
 LZ4B200_API int LZ4_compress_destSize_extState(void* state, const char* src, char* dst, int* srcSizePtr, int targetDstSize,
                                                int acceleration);
+
+/* The one-shot API of the reference's lib/lz4hc.h at every level, each call one block through the batched HC calls of
+ * section 2: levels <= 9 (below 1 means 9) through LZ4B200_compress_blocks_hc(_destSize), levels >= 10 (above 12 means
+ * 12) through LZ4B200_compress_blocks_hc_opt(_destSize).  Return values, written bytes and *srcSizePtr are the
+ * reference's for every size, capacity and level.  The whole input is on the device before any byte is written back, so
+ * src and dst may overlap (in-place calls); only the returned bytes are written to dst (nothing for a 0 result), never a
+ * byte at or past dst + dstCapacity (targetDstSize).  Decided on the host without a launch: a size outside
+ * 0 .. LZ4_MAX_INPUT_SIZE and a capacity (target) below 1 give 0; an empty input gives the one byte 0x00.
+ * Cost: one GPU thread parses the block, which is far slower than the reference on one CPU core at levels 10 and up
+ * (INTEGRATION.md section 1); batches belong on the section 2 calls.
+ * Without a CUDA device the calls that would launch return 0 and leave dst and *srcSizePtr untouched. */
+/* lz4hc.h:79 / lz4hc.c:1486 */
+LZ4B200_API int LZ4_sizeofStateHC(void);
+/* lz4hc.h:66 / lz4hc.c:1519-1535.  Routed as LZ4_compress_HC_extStateHC_fastReset (lz4hc.c:1506-1509): dstCapacity below
+ * LZ4_compressBound(srcSize) limits the output, 0 when the block does not fit. */
+LZ4B200_API int LZ4_compress_HC(const char* src, char* dst, int srcSize, int dstCapacity, int compressionLevel);
+/* lz4hc.h:80 / lz4hc.c:1512-1517.  `state` is checked as LZ4_initStreamHC checks it (lz4hc.c:1573-1586): NULL or not
+ * aligned like LZ4_streamHC_t (8 bytes, lz4hc.c:1488-1496) returns 0 and is not written.  A valid state is left as
+ * LZ4_initStreamHC leaves it (its first 262 192 bytes zero but the compression level, 9), so the reference's
+ * LZ4_resetStreamHC_fast / LZ4_compress_HC_continue accept it afterwards (lz4hc.h:373-382).  Deviation: the reference's
+ * state also keeps the block just compressed, which a following LZ4_compress_HC_continue uses as its dictionary; a
+ * stream continued from this state starts without one. */
+LZ4B200_API int LZ4_compress_HC_extStateHC(void* state, const char* src, char* dst, int srcSize, int dstCapacity,
+                                           int compressionLevel);
+/* lz4hc.h:392-406 / lz4hc.c:1500-1510.  Only the alignment of `state` is checked, and the state is neither read nor
+ * written.  Deviation: a NULL state returns 0 (the reference dereferences it). */
+LZ4B200_API int LZ4_compress_HC_extStateHC_fastReset(void* state, const char* src, char* dst, int srcSize, int dstCapacity,
+                                                     int compressionLevel);
+/* lz4hc.h:83-94 / lz4hc.c:1538-1545.  The fill parse at every targetDstSize from 1 up, the bound and above included:
+ * returns the bytes written (<= targetDstSize) and sets *srcSizePtr to the input bytes they hold.  `state` is checked
+ * and initialised as for LZ4_compress_HC_extStateHC.  targetDstSize < 1 or *srcSizePtr outside 0 .. LZ4_MAX_INPUT_SIZE:
+ * 0 with *srcSizePtr left alone.  Deviations: a NULL srcSizePtr or dst returns 0 (the reference dereferences them), and
+ * so does a NULL src with *srcSizePtr > 0. */
+LZ4B200_API int LZ4_compress_HC_destSize(void* state, const char* src, char* dst, int* srcSizePtr, int targetDstSize,
+                                         int cLevel);
 
 /* lz4.h:208 / lz4.c:2451.  Returns the number of bytes decoded into dst (<= dstCapacity), or a
  * negative value for malformed input / too small dst -- the same value -(position)-1 as the
@@ -254,8 +290,7 @@ LZ4B200_API int LZ4B200_compress_blocks_hc(const void* d_src, int64_t srcStride,
  * The workspace is at least LZ4B200_compress_blocks_hc_workspace_bytes(nBlocks) bytes, as for LZ4B200_compress_blocks_hc.
  * One kernel launch; nBlocks == 0 returns LZ4B200_OK without one.  LZ4B200_ERR_ARG: compressionLevel >= 10, nBlocks < 0,
  * a NULL d_dst, d_outSize, d_srcConsumed or d_workspace, a NULL d_src with blocks present, or a workspace smaller than
- * the size function asks.  LZ4_compress_HC_destSize itself is not exported: the drop-in HC family keeps resolving to
- * the reference until it serves every level.
+ * the size function asks.
  */
 LZ4B200_API int LZ4B200_compress_blocks_hc_destSize(const void* d_src, int64_t srcStride, const int32_t* d_srcSize,
                                                     int32_t srcSize, void* d_dst, int64_t dstStride, int32_t targetDstSize,

@@ -24,6 +24,11 @@ PROTOTYPES = [
     ("LZ4_compress_fast_extState_fastReset", C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int, C.c_int]),
     ("LZ4_compress_destSize", C.c_int, [_vp, _vp, C.POINTER(C.c_int), C.c_int]),
     ("LZ4_compress_destSize_extState", C.c_int, [_vp, _vp, _vp, C.POINTER(C.c_int), C.c_int, C.c_int]),
+    ("LZ4_sizeofStateHC", C.c_int, []),
+    ("LZ4_compress_HC", C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int]),
+    ("LZ4_compress_HC_extStateHC", C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int, C.c_int]),
+    ("LZ4_compress_HC_extStateHC_fastReset", C.c_int, [_vp, _vp, _vp, C.c_int, C.c_int, C.c_int]),
+    ("LZ4_compress_HC_destSize", C.c_int, [_vp, _vp, _vp, C.POINTER(C.c_int), C.c_int, C.c_int]),
     ("LZ4_decompress_safe", C.c_int, [_vp, _vp, C.c_int, C.c_int]),
     ("LZ4_decompress_safe_partial", C.c_int, [_vp, _vp, C.c_int, C.c_int, C.c_int]),
     ("LZ4_decompress_safe_usingDict", C.c_int, [_vp, _vp, C.c_int, C.c_int, _vp, C.c_int]),

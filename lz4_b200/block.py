@@ -1,4 +1,4 @@
-"""One-shot block API: the Python face of the drop-in C functions (lib/lz4.h:191,208,236).
+"""One-shot block API: the Python face of the drop-in C functions (lib/lz4.h:191,208,236, lib/lz4hc.h:66,91).
 
 Same names, argument meaning and error behaviour as the reference's C API; data are host bytes.
 Each call is LZ4_* in liblz4_b200.so: host -> device copy, CUDA kernels, device -> host copy.
@@ -55,6 +55,29 @@ def LZ4_compress_destSize(src, target, acceleration=None):
         state = np.empty(16416 // 8, dtype=np.uint64)          # LZ4_sizeofState(), 8-byte aligned
         r = int(lib.LZ4_compress_destSize_extState(state.ctypes.data, sp, dst.ctypes.data, C.byref(n), int(target),
                                                    int(acceleration)))
+    return r, int(n.value), dst[:max(r, 0)].tobytes()
+
+
+def LZ4_compress_HC(src, level=9, dst_capacity=None):
+    """Returns (ret, bytes): ret bytes written at LZ4HC level `level`, 0 on failure -- lz4hc.h:66."""
+    lib = _lib.load()
+    s = _u8(src)
+    cap = LZ4_compressBound(len(s)) if dst_capacity is None else int(dst_capacity)
+    dst = np.empty(max(cap, 1), dtype=np.uint8)
+    r = int(lib.LZ4_compress_HC(s.ctypes.data if len(s) else None, dst.ctypes.data, len(s), cap, int(level)))
+    return r, dst[:max(r, 0)].tobytes()
+
+
+def LZ4_compress_HC_destSize(src, target, level=9):
+    """Returns (ret, consumed, bytes): ret bytes written (<= target) at LZ4HC level `level`, consumed = what the call
+    leaves in *srcSizePtr -- lz4hc.h:83-94."""
+    lib = _lib.load()
+    s = _u8(src)
+    dst = np.empty(max(int(target), 1), dtype=np.uint8)
+    n = C.c_int(len(s))
+    state = np.empty(lib.LZ4_sizeofStateHC() // 8, dtype=np.uint64)      # 8-byte aligned, like LZ4_streamHC_t
+    r = int(lib.LZ4_compress_HC_destSize(state.ctypes.data, s.ctypes.data if len(s) else None, dst.ctypes.data,
+                                         C.byref(n), int(target), int(level)))
     return r, int(n.value), dst[:max(r, 0)].tobytes()
 
 

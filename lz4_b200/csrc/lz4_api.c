@@ -589,6 +589,103 @@ int LZ4_compress_destSize_extState(void* state, const char* src, char* dst, int*
     return one_block_compress(src, dst, *srcSizePtr, targetDstSize, acceleration, srcSizePtr);
 }
 
+/* ------------------------------------------------------------------------------------------ */
+/* drop-in HC layer (lz4hc.c:1486-1545): one block, host pointers, synchronous                 */
+/* ------------------------------------------------------------------------------------------ */
+/* LZ4_initStreamHC (lz4hc.c:1573-1586) zeroes the LZ4HC_CCtx_internal at the head of LZ4_streamHC_t (lz4hc.h:235-250:
+ * 262 192 bytes on LP64 targets; the union's last 8 bytes are left alone) and sets its compressionLevel (offset
+ * 262 180) to LZ4HC_CLEVEL_DEFAULT.  The alignment is LZ4_streamHC_t's (lz4hc.c:1488-1496), 8 bytes: pointer members. */
+#define HC_STATE_INIT_BYTES   262192
+#define HC_STATE_LEVEL_OFFSET 262180
+#define HC_STATE_ALIGN        8u
+
+static int hc_state_is_aligned(const void* state) { return (((uintptr_t)state) & (HC_STATE_ALIGN - 1)) == 0; }
+
+/* LZ4_initStreamHC's checks and writes: 1 for a state that is non-NULL, aligned and now initialised, else 0 */
+static int hc_state_init(void* state)
+{
+    const short level = 9;
+    if (state == NULL || !hc_state_is_aligned(state)) return 0;
+    memset(state, 0, HC_STATE_INIT_BYTES);
+    memcpy((char*)state + HC_STATE_LEVEL_OFFSET, &level, sizeof level);
+    return 1;
+}
+
+int LZ4_sizeofStateHC(void) { return LZ4B200_STATEHC_BYTES; }
+
+/* srcSizePtr == NULL: LZ4_compress_HC_extStateHC_fastReset's routing (lz4hc.c:1506-1509: a capacity below the bound
+ * limits the output).  Otherwise LZ4_compress_HC_destSize's fill parse (lz4hc.c:1544) with srcSize = *srcSizePtr and
+ * targetDstSize = dstCapacity; *srcSizePtr receives the consumed input.  Levels <= 9 go to the hash-chain launchers,
+ * levels >= 10 to the optimal parser's.  Like one_block_compress: the whole input is on the device before any byte is
+ * written back, only the returned bytes are copied to dst, and the rules the reference decides without parsing are
+ * decided here without a launch (lz4hc.c:1388-1389; an empty input is one 0x00 token). */
+static int one_block_compress_hc(const char* src, char* dst, int srcSize, int dstCapacity, int level, int* srcSizePtr)
+{
+    int rc, bound;
+    int32_t res[2] = {0, 0};                 /* return value, consumed input */
+    slot_t* s = &g_ctx.slot[0];
+    int32_t* d_res;
+    void* ws;
+    size_t wsBytes;
+    if ((unsigned)srcSize > (unsigned)LZ4B200_MAX_INPUT_SIZE) return 0;
+    if (dstCapacity < 1) return 0;           /* fillOutput: lz4hc.c:1388; limited output: not even a token fits */
+    if (dst == NULL) return 0;
+    if (srcSize > 0 && src == NULL) return 0;
+    if (srcSize == 0) { dst[0] = 0; return 1; }   /* the last-literals token of an empty block; *srcSizePtr stays 0 */
+    bound = LZ4_compressBound(srcSize);
+    if ((rc = host_begin()) != LZ4B200_OK) goto done;
+    rc = slot_take(s, (size_t)srcSize, (size_t)(dstCapacity < bound ? dstCapacity : bound),
+                   LZ4B200_compress_blocks_hc_opt_workspace_bytes(1), 0, sizeof(res));
+    if (rc != LZ4B200_OK) goto done;
+    d_res = (int32_t*)s->d_tab.p;
+    ws = s->ws.p; wsBytes = s->ws.cap;
+    /* copy-in completes before any output is produced: in-place and overlapping buffers are safe */
+    CU(cudaMemcpyAsync(s->in.p, src, (size_t)srcSize, cudaMemcpyHostToDevice, s->stream));
+    if (srcSizePtr && level >= 10)
+        rc = LZ4B200_compress_blocks_hc_opt_destSize(s->in.p, 0, NULL, srcSize, s->out.p, 0, dstCapacity, level,
+                                                     d_res, d_res + 1, 1, ws, wsBytes, s->stream);
+    else if (srcSizePtr)
+        rc = LZ4B200_compress_blocks_hc_destSize(s->in.p, 0, NULL, srcSize, s->out.p, 0, dstCapacity, level,
+                                                 d_res, d_res + 1, 1, ws, wsBytes, s->stream);
+    else if (level >= 10)
+        rc = LZ4B200_compress_blocks_hc_opt(s->in.p, 0, NULL, srcSize, s->out.p, 0, dstCapacity, level, d_res, 1,
+                                            ws, wsBytes, s->stream);
+    else
+        rc = LZ4B200_compress_blocks_hc(s->in.p, 0, NULL, srcSize, s->out.p, 0, dstCapacity, level, d_res, 1,
+                                        ws, wsBytes, s->stream);
+    if (rc == LZ4B200_OK) rc = slot_return(s, (int32_t*)s->h_tab.p, d_res, res, srcSizePtr ? 2 : 1);
+    if (rc == LZ4B200_OK) rc = slot_wait(s);
+    if (rc == LZ4B200_OK && res[0] > 0) CU(cudaMemcpyAsync(dst, s->out.p, (size_t)res[0], cudaMemcpyDeviceToHost, s->stream));
+done:
+    if (host_end(rc) != LZ4B200_OK) return 0;
+    if (srcSizePtr) *srcSizePtr = res[1];
+    return res[0];
+}
+
+int LZ4_compress_HC(const char* src, char* dst, int srcSize, int dstCapacity, int compressionLevel)
+{
+    return one_block_compress_hc(src, dst, srcSize, dstCapacity, compressionLevel, NULL);
+}
+
+int LZ4_compress_HC_extStateHC(void* state, const char* src, char* dst, int srcSize, int dstCapacity, int compressionLevel)
+{
+    if (!hc_state_init(state)) return 0;
+    return one_block_compress_hc(src, dst, srcSize, dstCapacity, compressionLevel, NULL);
+}
+
+int LZ4_compress_HC_extStateHC_fastReset(void* state, const char* src, char* dst, int srcSize, int dstCapacity,
+                                         int compressionLevel)
+{
+    if (state == NULL || !hc_state_is_aligned(state)) return 0;
+    return one_block_compress_hc(src, dst, srcSize, dstCapacity, compressionLevel, NULL);
+}
+
+int LZ4_compress_HC_destSize(void* state, const char* src, char* dst, int* srcSizePtr, int targetDstSize, int cLevel)
+{
+    if (!hc_state_init(state) || srcSizePtr == NULL) return 0;
+    return one_block_compress_hc(src, dst, *srcSizePtr, targetDstSize, cLevel, srcSizePtr);
+}
+
 /* One block through the batch layer: LZ4_decompress_safe (partial == 0) or LZ4_decompress_safe_partial with outputSize =
  * dstCapacity.  The caller has decided the argument rules (compressedSize > 0, dstCapacity > 0, src and dst non-NULL).
  * Only the returned bytes are copied back: dst is untouched for a rejected block. */
