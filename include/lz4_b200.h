@@ -223,6 +223,44 @@ LZ4B200_API int LZ4B200_decompress_blocks_partial(const void* d_src, const int64
                                                   void* d_workspace, size_t workspaceBytes, void* stream);
 
 /*
+ * Decode nFrames LZ4 frames that are already in device memory (the batched LZ4B200_decompressFrame_host of section 4):
+ *   frame f input : d_src + d_srcOff[f], d_srcSize[f] bytes
+ *   frame f output: d_dst + d_dstOff[f], capacity d_dstCap[f]
+ *   d_result[f]   : what LZ4B200_decompressFrame_host(src_f, d_srcSize[f], dst_f, d_dstCap[f], &c) returns for that frame
+ *                   alone -- the decoded byte count, or its error code in its order: argument (LZ4B200_ERR_ARG: a negative
+ *                   size or capacity), header, chain, then per block in order (decode failure, LZ4B200_ERR_DSTSIZE
+ *                   against the capacity, the content size) -- or LZ4B200_ERR_LIMIT (below)
+ *   d_consumed[f] : (may be NULL) the frame's length when its header and chain of blocks are valid, else 0 (0 as well
+ *                   for a frame with LZ4B200_ERR_LIMIT)
+ * The decoded bytes are the host call's: blocks are placed one after the other, short middle blocks closed up.  Nothing
+ * is written outside [dst_f, dst_f + d_dstCap[f]); inside a failed frame's region the bytes are unspecified.  Output
+ * regions must not overlap.  Frames are accepted exactly where the host call accepts them: independent blocks, no
+ * checksums, no dictID, no skippable frames; stored-raw blocks and the content size are supported.  Same readable
+ * padding as LZ4B200_decompress_blocks: 16 bytes before and after every frame.
+ *
+ * The budget: maxBlocks (a host array) bounds the blocks the call decodes from frames of block size ID 4 + c
+ * (maxBlocks[0 .. 3]: 64 KB, 256 KB, 1 MB, 4 MB blocks); the workspace is sized by it, so that the host plans every
+ * step and the call never synchronises (it can be captured into a CUDA graph).  A frame gets LZ4B200_ERR_LIMIT when the
+ * blocks of the earlier frames (lower index) of its class that passed the header and chain checks, plus its own, exceed
+ * maxBlocks[c] -- whatever the scheduling.  A frame's chain walk stops after maxBlocks[c] + 1 blocks, which bounds the
+ * work of an untrusted frame of empty blocks; the order is therefore: header errors, then chain errors within the first
+ * maxBlocks[c] + 1 blocks, then LZ4B200_ERR_LIMIT.
+ *
+ * Kernel launches: 5, plus 3 for maxBlocks[0] > 0 and 4 for each of maxBlocks[1 .. 3] > 0 (the two phases of
+ * LZ4B200_decompress_blocks_phased per class).  nFrames == 0 returns LZ4B200_OK without one.  LZ4B200_ERR_ARG: nFrames < 0,
+ * a NULL maxBlocks or an entry outside 0 .. 2^31 - 1, a NULL pointer other than d_consumed, or a workspace smaller than
+ * LZ4B200_decompress_frames_workspace_bytes asks (0 for arguments the call rejects).  The workspace is about
+ * 2 x maxBlocks[c] x the block size for classes 1 .. 3 (the tiles kernel's marks) and 48 bytes per frame.
+ */
+#define LZ4B200_ERR_LIMIT (-6)   /* per-frame result: the frame needs more blocks than the call's budget for its block size */
+LZ4B200_API size_t LZ4B200_decompress_frames_workspace_bytes(int64_t nFrames, const int64_t maxBlocks[4]);
+LZ4B200_API int LZ4B200_decompress_frames(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
+                                          void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
+                                          int64_t* d_result, int64_t* d_consumed,
+                                          int64_t nFrames, const int64_t maxBlocks[4],
+                                          void* d_workspace, size_t workspaceBytes, void* stream);
+
+/*
  * Compress nBlocks independent blocks (the batched LZ4_compress_fast; replaces bench.c:464-493 and
  * lz4frame.c:1046-1055).
  *   block i input : d_src + i*srcStride, size (d_srcSize ? d_srcSize[i] : srcSize)

@@ -14,6 +14,8 @@ captured into a CUDA graph.  The workspace rule of the calls that need one (the 
     scan left in the workspace, which a call in between would overwrite, and a graph keeps the workspace's address,
     which the module's cache may free when it grows.
 """
+import ctypes as C
+
 import torch
 
 from . import _lib
@@ -151,6 +153,61 @@ def decompress_blocks_partial(comp, offsets, sizes, target, out=None, out_stride
                                                st.cuda_stream)
     _lib.check(rc, "LZ4B200_decompress_blocks_partial")
     return out, out_sizes
+
+
+def _budget(max_blocks):
+    """the per-class budget (64 KB, 256 KB, 1 MB, 4 MB blocks) as the C array the frame calls take"""
+    mb = [int(x) for x in max_blocks]
+    if len(mb) != 4:
+        raise ValueError("max_blocks: one budget per block size ID 4 .. 7 (4 values)")
+    return (C.c_int64 * 4)(*mb)
+
+
+def decompress_frames_workspace_bytes(n_frames, max_blocks):
+    """LZ4B200_decompress_frames_workspace_bytes: the workspace decompress_frames needs (0: arguments it rejects)"""
+    return int(_lib.load().LZ4B200_decompress_frames_workspace_bytes(int(n_frames), _budget(max_blocks)))
+
+
+def decompress_frames(comp, offsets, sizes, capacities, max_blocks, out=None, out_offsets=None, results=None,
+                      consumed=None, workspace=None, stream=None):
+    """Decode len(sizes) LZ4 frames held in device memory (LZ4B200_decompress_frames).
+
+    comp: u8[*] device buffer; frame f = comp[offsets[f] : offsets[f]+sizes[f]] (int64 device tensors), with 16
+    readable bytes before and after it.  Frame f decodes to out[out_offsets[f] : out_offsets[f]+capacities[f]]
+    (int64 device tensors).  out_offsets defaults to the exclusive sum of capacities, and out to their total (read on
+    the host: a captured call passes out).  max_blocks: the blocks the call decodes at most from frames of each block
+    size ID 4 .. 7 (4 host ints); a frame past its class's budget gets LZ4B200_ERR_LIMIT (-6).
+    Returns (out, results, consumed): results[f] is LZ4B200_decompressFrame_host's return value for frame f (decoded
+    bytes or a negative error code), consumed[f] the frame's length when its header and chain are valid, else 0.
+    """
+    lib = _lib.load()
+    _need_cuda(comp, offsets, sizes, capacities, out, out_offsets, results, consumed)
+    assert comp.dtype == torch.uint8 and offsets.dtype == torch.int64 and sizes.dtype == torch.int64
+    assert capacities.dtype == torch.int64
+    n = int(sizes.numel())
+    budget = _budget(max_blocks)
+    st = _stream(stream)
+    ws_bytes = int(lib.LZ4B200_decompress_frames_workspace_bytes(n, budget))
+    if ws_bytes == 0:
+        raise ValueError("decompress_frames: budgets must be 0 .. 2^31 - 1")
+    workspace = _workspace(comp.device, ws_bytes, st, workspace, "decompress_frames")
+    with torch.cuda.stream(st):                     # temporaries belong to the stream the kernels run on
+        if out_offsets is None:
+            out_offsets = torch.cumsum(capacities, 0) - capacities
+        if out is None:
+            if torch.cuda.is_current_stream_capturing():
+                raise ValueError("decompress_frames under stream capture needs out=")
+            out = torch.empty(max(int(capacities.sum()) if n else 0, 1), dtype=torch.uint8, device=comp.device)
+        if results is None:
+            results = torch.empty(n, dtype=torch.int64, device=comp.device)
+        if consumed is None:
+            consumed = torch.empty(n, dtype=torch.int64, device=comp.device)
+    rc = lib.LZ4B200_decompress_frames(comp.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), out.data_ptr(),
+                                       out_offsets.data_ptr(), capacities.data_ptr(), results.data_ptr(),
+                                       consumed.data_ptr(), n, budget, workspace.data_ptr(), workspace.numel(),
+                                       st.cuda_stream)
+    _lib.check(rc, "LZ4B200_decompress_frames")
+    return out, results, consumed
 
 
 def compress_blocks(src, block_size, acceleration=1, slots=None, slot_stride=None, slot_capacity=None,

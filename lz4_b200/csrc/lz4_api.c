@@ -8,6 +8,7 @@
  */
 #include "../../include/lz4_b200.h"
 #include "lz4_kernels.h"
+#include "lz4_frame_core.h"
 
 #include <cuda_runtime_api.h>
 #include <pthread.h>
@@ -258,6 +259,96 @@ int LZ4B200_decompress_blocks_partial(const void* d_src, const int64_t* d_srcOff
 {
     return decode_call(1, d_src, d_srcOff, d_srcSize, d_dst, d_dstOff, dstStride, d_target, targetOutputSize, d_outSize,
                        nBlocks, d_workspace, workspaceBytes, 3, stream);
+}
+
+/* The workspace of LZ4B200_decompress_frames, from the budget alone: the frame records, the block table of every class
+ * (entries tabBase[c] .. tabBase[c] + maxBlocks[c] - 1), then one decode workspace per class with a budget, each the
+ * size that gives the class's uniform capacity its own route (LZ4B200_decompress_workspace_bytes_for(maxBlocks[c], 0,
+ * block size)).  Regions start on 256 bytes from a base rounded up to 256 (the 256 bytes of slack in `bytes`). */
+#define FRAMES_MAX_BUDGET 0x7FFFFFFF
+typedef struct {
+    size_t frames, srcOff, dstOff, srcSize, outSize, rawLen, decode[4], decodeBytes[4], bytes;
+    int64_t tabBase[4], nEntries;
+} frames_plan_t;
+
+static size_t up256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+/* 0 for arguments the call rejects (nFrames < 0, a NULL budget, an entry outside 0 .. FRAMES_MAX_BUDGET) */
+static int frames_plan(int64_t nFrames, const int64_t* maxBlocks, frames_plan_t* p)
+{
+    size_t at = 0;
+    int c;
+    if (nFrames < 0 || !maxBlocks) return 0;
+    p->nEntries = 0;
+    for (c = 0; c < 4; c++) {
+        if (maxBlocks[c] < 0 || maxBlocks[c] > FRAMES_MAX_BUDGET) return 0;
+        p->tabBase[c] = p->nEntries;
+        p->nEntries += maxBlocks[c];
+    }
+    p->frames = at;  at = up256(at + (size_t)nFrames * sizeof(fc_frame_rec));
+    p->srcOff = at;  at = up256(at + (size_t)p->nEntries * sizeof(int64_t));
+    p->dstOff = at;  at = up256(at + (size_t)p->nEntries * sizeof(int64_t));
+    p->srcSize = at; at = up256(at + (size_t)p->nEntries * sizeof(int32_t));
+    p->outSize = at; at = up256(at + (size_t)p->nEntries * sizeof(int32_t));
+    p->rawLen = at;  at = up256(at + (size_t)p->nEntries * sizeof(int32_t));
+    for (c = 0; c < 4; c++) {
+        p->decodeBytes[c] = maxBlocks[c] ? lz4k_decode_workspace_bytes(maxBlocks[c], 0, (int32_t)fc_block_bytes(4 + c), SIZE_MAX) : 0;
+        p->decode[c] = at;
+        at = up256(at + p->decodeBytes[c]);
+    }
+    p->bytes = at + 256;
+    return 1;
+}
+
+size_t LZ4B200_decompress_frames_workspace_bytes(int64_t nFrames, const int64_t maxBlocks[4])
+{
+    frames_plan_t p;
+    return frames_plan(nFrames, maxBlocks, &p) ? p.bytes : 0;
+}
+
+/* index -> per class: scan (phase 1) -> verdict -> per class: expand (phase 2) -> raw blocks.  Every class decodes its
+ * whole table (maxBlocks[c] entries, unused ones with size 0) at the uniform capacity of its block size, the capacity
+ * lz4frame.c:1901-1904 and LZ4B200_decompressFrame_host decode with. */
+int LZ4B200_decompress_frames(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
+                              void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
+                              int64_t* d_result, int64_t* d_consumed,
+                              int64_t nFrames, const int64_t maxBlocks[4],
+                              void* d_workspace, size_t workspaceBytes, void* stream)
+{
+    frames_plan_t p;
+    lz4k_frames_args a;
+    uint8_t* ws;
+    int c, ph, rc;
+    if (!frames_plan(nFrames, maxBlocks, &p)) return LZ4B200_ERR_ARG;
+    if (nFrames == 0) return LZ4B200_OK;
+    if (!d_src || !d_srcOff || !d_srcSize || !d_dst || !d_dstOff || !d_dstCap || !d_result || !d_workspace)
+        return LZ4B200_ERR_ARG;
+    if (workspaceBytes < p.bytes) return LZ4B200_ERR_ARG;
+    ws = (uint8_t*)(((uintptr_t)d_workspace + 255) & ~(uintptr_t)255);
+    memset(&a, 0, sizeof a);
+    a.src = (const uint8_t*)d_src; a.srcOff = d_srcOff; a.srcSize = d_srcSize;
+    a.dst = (uint8_t*)d_dst; a.dstOff = d_dstOff; a.dstCap = d_dstCap;
+    a.result = d_result; a.consumed = d_consumed; a.nFrames = nFrames;
+    for (c = 0; c < 4; c++) { a.maxBlocks[c] = maxBlocks[c]; a.tabBase[c] = p.tabBase[c]; }
+    a.nEntries = p.nEntries;
+    a.frames = ws + p.frames;
+    a.tabSrcOff = (int64_t*)(ws + p.srcOff); a.tabDstOff = (int64_t*)(ws + p.dstOff);
+    a.tabSrcSize = (int32_t*)(ws + p.srcSize); a.tabOutSize = (int32_t*)(ws + p.outSize); a.tabRawLen = (int32_t*)(ws + p.rawLen);
+
+    if ((rc = launched(lz4k_launch_frames_index(&a, stream), "lz4k_launch_frames_index")) != LZ4B200_OK) return rc;
+    for (ph = 1; ph <= 2; ph++) {
+        if (ph == 2 && (rc = launched(lz4k_launch_frames_verdict(&a, stream), "lz4k_launch_frames_verdict")) != LZ4B200_OK)
+            return rc;
+        for (c = 0; c < 4; c++) {
+            const int64_t t = p.tabBase[c];
+            if (!maxBlocks[c]) continue;
+            rc = LZ4B200_decompress_blocks_phased(d_src, a.tabSrcOff + t, a.tabSrcSize + t, d_dst, a.tabDstOff + t, 0, NULL,
+                                                  (int32_t)fc_block_bytes(4 + c), a.tabOutSize + t, maxBlocks[c],
+                                                  ws + p.decode[c], p.decodeBytes[c], ph, stream);
+            if (rc != LZ4B200_OK) return rc;
+        }
+    }
+    return launched(lz4k_launch_frames_raw(&a, stream), "lz4k_launch_frames_raw");
 }
 
 /* the encode launch arguments, every block size included (a split launch narrows minSize .. maxSize) */
@@ -754,27 +845,7 @@ int LZ4_decompress_safe_usingDict(const char* src, char* dst, int compressedSize
 /* ------------------------------------------------------------------------------------------ */
 /* frame layer (SURVEY section 8 f-1): independent-block LZ4 frames over host buffers          */
 /* ------------------------------------------------------------------------------------------ */
-#define FRAME_MAGIC 0x184D2204u            /* lz4frame.c: LZ4F_MAGICNUMBER */
-#define FRAME_MAGIC_SKIPPABLE 0x184D2A50u  /* .. LZ4F_MAGIC_SKIPPABLE_START */
-
-static uint32_t rd_le32(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
 static void wr_le32(uint8_t* p, uint32_t v) { p[0] = (uint8_t)v; p[1] = (uint8_t)(v >> 8); p[2] = (uint8_t)(v >> 16); p[3] = (uint8_t)(v >> 24); }
-static uint32_t rotl32(uint32_t x, int r) { return (x << r) | (x >> (32 - r)); }
-
-/* XXH32 of a short message (len < 16), as published in the xxHash specification; the frame header
- * checksum is its second byte (lz4frame.c:781-809: HC = (XXH32(descriptor, 0) >> 8) & 0xFF). */
-static uint32_t xxh32_short(const uint8_t* p, size_t len, uint32_t seed)
-{
-    const uint32_t P1 = 2654435761u, P2 = 2246822519u, P3 = 3266489917u, P4 = 668265263u, P5 = 374761393u;
-    const uint8_t* end = p + len;
-    uint32_t h = seed + P5 + (uint32_t)len;
-    while (p + 4 <= end) { h += rd_le32(p) * P3; h = rotl32(h, 17) * P4; p += 4; }
-    while (p < end) { h += (uint32_t)(*p) * P5; h = rotl32(h, 11) * P1; p++; }
-    h ^= h >> 15; h *= P2; h ^= h >> 13; h *= P3; h ^= h >> 16;
-    return h;
-}
-
-static int64_t frame_block_bytes(int bsid) { return (int64_t)1 << (8 + 2 * bsid); }   /* 4..7 -> 64 KB..4 MB (lz4frame.c:333-342) */
 
 /* LZ4F_optimalBSID, lz4frame.c:362-373 */
 static int frame_optimal_bsid(int requested, int64_t srcSize)
@@ -795,7 +866,7 @@ int64_t LZ4B200_compressFrameBound(int64_t srcSize, int blockSizeID)
     if (srcSize < 0) return LZ4B200_ERR_ARG;
     if (blockSizeID == 0) blockSizeID = 4;
     if (blockSizeID < 4 || blockSizeID > 7) return LZ4B200_ERR_ARG;
-    bs = frame_block_bytes(blockSizeID);
+    bs = fc_block_bytes(blockSizeID);
     nBlocks = srcSize / bs + 1;
     return 19 + nBlocks * 4 + srcSize + 4 + 4;     /* max header + block headers + data + EndMark (+ slack) */
 }
@@ -814,15 +885,15 @@ int64_t LZ4B200_compressFrame_host(const void* h_src, int64_t srcSize, void* h_d
     if (dstCapacity < LZ4B200_compressFrameBound(srcSize, blockSizeID)) return LZ4B200_ERR_DSTSIZE;
     accel = compressionLevel < 0 ? -compressionLevel + 1 : 1;           /* lz4frame.c:913 */
     bsid = frame_optimal_bsid(blockSizeID, srcSize);                     /* lz4frame.c:447 */
-    bs = frame_block_bytes(bsid);
+    bs = fc_block_bytes(bsid);
     if (srcSize == 0) contentSizeFlag = 0;                               /* lz4frame.c:445: contentSize = srcSize = 0 -> no field */
 
     /* frame header, lz4frame.c:781-809 */
-    wr_le32(dst, FRAME_MAGIC); op = 4;
+    wr_le32(dst, FC_MAGIC); op = 4;
     dst[op++] = (uint8_t)((1u << 6) | (1u << 5) | ((contentSizeFlag ? 1u : 0u) << 3));   /* version 01, B.Indep */
     dst[op++] = (uint8_t)((uint32_t)bsid << 4);
     if (contentSizeFlag) { int i; for (i = 0; i < 8; i++) dst[op++] = (uint8_t)((uint64_t)srcSize >> (8 * i)); }
-    dst[op] = (uint8_t)(xxh32_short(dst + 4, (size_t)(op - 4), 0) >> 8);
+    dst[op] = (uint8_t)(fc_xxh32_short(dst + 4, (size_t)(op - 4), 0) >> 8);
     op++;
 
     nFull = srcSize / bs;
@@ -893,37 +964,19 @@ int64_t LZ4B200_decompressFrame_host(const void* h_src, int64_t srcSize, void* h
 {
     const uint8_t* src = (const uint8_t*)h_src;
     uint8_t* dst = (uint8_t*)h_dst;
-    int64_t ip, bs, nBlocks = 0, capBlocks = 0, k, total = 0, contentSize = -1;
+    int64_t ip, at, sz, bs, nBlocks = 0, capBlocks = 0, k, total = 0, contentSize;
     int64_t* off = NULL; int32_t* csz = NULL; int32_t* rets = NULL; uint8_t* raw = NULL;
     int64_t result = LZ4B200_ERR_FRAME;
-    uint32_t flg, bd, hdrLen;
-    int bsid;
-    if (!h_src || srcSize < 0 || dstCapacity < 0 || (!h_dst && dstCapacity > 0)) return LZ4B200_ERR_ARG;
-    if (srcSize < 7) return LZ4B200_ERR_FRAME;                            /* minFHSize, lz4frame.h:280 */
-    if ((rd_le32(src) & 0xFFFFFFF0u) == FRAME_MAGIC_SKIPPABLE) return LZ4B200_ERR_UNSUPPORTED;
-    if (rd_le32(src) != FRAME_MAGIC) return LZ4B200_ERR_FRAME;
-    flg = src[4];
-    if (((flg >> 6) & 3) != 1 || ((flg >> 1) & 1)) return LZ4B200_ERR_FRAME;   /* version, reserved bit */
-    hdrLen = 7 + ((flg >> 3) & 1 ? 8 : 0) + ((flg & 1) ? 4 : 0);
-    if (srcSize < hdrLen) return LZ4B200_ERR_FRAME;
-    bd = src[5];
-    bsid = (int)((bd >> 4) & 7);
-    if ((bd >> 7) || (bd & 15) || bsid < 4) return LZ4B200_ERR_FRAME;     /* lz4frame.c:1406-1412 */
-    if ((uint8_t)(xxh32_short(src + 4, hdrLen - 5, 0) >> 8) != src[hdrLen - 1]) return LZ4B200_ERR_FRAME;
-    if (!((flg >> 5) & 1)) return LZ4B200_ERR_UNSUPPORTED;                 /* linked blocks (f-4) */
-    if (((flg >> 4) & 1) || ((flg >> 2) & 1) || (flg & 1)) return LZ4B200_ERR_UNSUPPORTED;   /* checksums (f-3), dictID */
-    if ((flg >> 3) & 1) { int i; uint64_t v = 0; for (i = 0; i < 8; i++) v |= (uint64_t)src[6 + i] << (8 * i); contentSize = (int64_t)v; }
-    bs = frame_block_bytes(bsid);
+    fc_header_t hdr;
+    int isRaw, step;
+    if (!h_src || (!h_dst && dstCapacity > 0)) return LZ4B200_ERR_ARG;
+    if ((step = fc_frame_header(src, srcSize, dstCapacity, &hdr)) != LZ4B200_OK) return step;   /* lz4frame.c:1340-1425 */
+    contentSize = hdr.contentSize;
+    bs = fc_block_bytes(hdr.bsid);
 
     /* walk the chain of block headers (serial, O(#blocks)), lz4frame.c:1729-1758 */
-    ip = hdrLen;
-    for (;;) {
-        uint32_t h; int64_t sz;
-        if (ip + 4 > srcSize) goto done;
-        h = rd_le32(src + ip); ip += 4;
-        if (h == 0) break;                                                /* EndMark */
-        sz = (int64_t)(h & 0x7FFFFFFFu);
-        if (sz > bs || ip + sz > srcSize) goto done;                       /* lz4frame.c:1745: maxBlockSize_invalid */
+    ip = hdr.hdrLen;
+    while ((step = fc_next_block(src, srcSize, bs, &ip, &at, &sz, &isRaw)) == 1) {
         if (nBlocks == capBlocks) {
             int64_t* o2; int32_t* c2; uint8_t* r2;
             capBlocks = capBlocks ? capBlocks * 2 : 1024;
@@ -935,12 +988,12 @@ int64_t LZ4B200_decompressFrame_host(const void* h_src, int64_t srcSize, void* h
             if (r2) raw = r2;
             if (!o2 || !c2 || !r2) { result = LZ4B200_ERR_ARG; goto done; }     /* (the old blocks are freed at `done`) */
         }
-        off[nBlocks] = ip; csz[nBlocks] = (int32_t)sz; raw[nBlocks] = (uint8_t)(h >> 31);
+        off[nBlocks] = at; csz[nBlocks] = (int32_t)sz; raw[nBlocks] = (uint8_t)isRaw;
         nBlocks++;
-        ip += sz;
     }
+    if (step < 0) goto done;
     if (consumed) *consumed = ip;
-    if (nBlocks == 0) { result = (contentSize > 0) ? LZ4B200_ERR_FRAME : 0; goto done; }
+    if (nBlocks == 0) { result = fc_frame_result(0, contentSize); goto done; }
 
     /* Every block is decoded with dstCapacity = maxBlockSize like lz4frame.c:1901-1904 does.  The frame is untrusted
      * input, so memory is bounded whatever it claims: blocks are decoded in GROUPS of at most ~256 MiB of block slots,
@@ -976,10 +1029,9 @@ int64_t LZ4B200_decompressFrame_host(const void* h_src, int64_t srcSize, void* h
                 int64_t r;
                 if (raw[g0 + k]) { memcpy(base + k * bs, src + off[g0 + k], (size_t)csz[g0 + k]); rets[g0 + k] = csz[g0 + k]; }
                 r = rets[g0 + k];
-                if (r < 0) { free(bounce); free(tmpSz); goto done; }      /* a block failed to decode */
-                if (pos + r > dstCapacity || (contentSize >= 0 && pos + r > contentSize)) {
+                if ((step = fc_block_verdict(pos, r, dstCapacity, contentSize)) != LZ4B200_OK) {
                     free(bounce); free(tmpSz);
-                    result = (pos + r > dstCapacity) ? LZ4B200_ERR_DSTSIZE : LZ4B200_ERR_FRAME;
+                    result = step;
                     goto done;
                 }
                 if (dst + pos != base + k * bs) memmove(dst + pos, base + k * bs, (size_t)r);      /* close the gap (moves left) */
@@ -989,8 +1041,7 @@ int64_t LZ4B200_decompressFrame_host(const void* h_src, int64_t srcSize, void* h
         }
         free(bounce); free(tmpSz);
     }
-    if (contentSize >= 0 && contentSize != total) goto done;              /* lz4frame.c: frameSize_wrong */
-    result = total;
+    result = fc_frame_result(total, contentSize);                        /* lz4frame.c: frameSize_wrong */
 done:
     free(off); free(csz); free(raw); free(rets);
     return result;

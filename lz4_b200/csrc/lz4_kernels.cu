@@ -19,6 +19,7 @@
 #include <atomic>
 #include <mutex>
 #include "lz4_kernels.h"
+#include "../../include/lz4_b200.h"   /* (the error codes lz4_frame_core.h returns; included here, outside the namespace) */
 
 namespace {
 
@@ -53,6 +54,7 @@ __device__ unsigned long long g_loopStats[4];    // phase B: warp iterations, la
 #include "lz4_scan_split.h"
 #include "lz4_rows_core.h"
 #include "lz4_decode_plan.h"     /* a decode call's workspace layout (WsView), scan choice and block predicates */
+#include "lz4_frame_core.h"      /* the frame rules of the batched frame decode, shared with lz4_api.c */
 
 /* low 5 bytes at p (for the 5-byte hash, lz4.c:785-791) */
 __device__ __forceinline__ uint64_t ld40u(const uint8_t* p)
@@ -350,6 +352,7 @@ __device__ __forceinline__ void expand_generic(const lz4k_decode_args& a, const 
     const int64_t count = w.hdr->slowCount;       // only blocks the scan accepted and left to this kernel
     for (int64_t idx = warp0; idx < count; idx += nWarps) {
     const int64_t b = w.slowList[idx];
+    if (a.outSize[b] <= 0) continue;              // dropped after the scan (the frame decode's verdict: a failed frame)
     const uint8_t* __restrict__ src = a.src + a.srcOff[b];
     uint8_t* dst = a.dst + (a.dstOff ? a.dstOff[b] : b * a.dstStride);
     const int64_t n = a.srcSize[b];
@@ -1245,6 +1248,32 @@ __device__ __forceinline__ int pack_payload(const FrameRule& fr, const int32_t* 
     return isRaw ? sz : c;
 }
 
+/* s bytes from -> to by the whole CTA: destination-aligned 16-byte stores, the source read through aligned words (up to 3
+ * bytes past its end: readable padding) */
+__device__ __forceinline__ void cta_copy(uint8_t* to, const uint8_t* from, int s)
+{
+    const uintptr_t ta = reinterpret_cast<uintptr_t>(to);
+    int head = (int)((16 - (ta & 15)) & 15);
+    if (head > s) head = s;
+    for (int k = threadIdx.x; k < head; k += blockDim.x) to[k] = from[k];
+    const int body = (s - head) >> 4;
+    const uint8_t* fb = from + head;
+    uint4* tb = reinterpret_cast<uint4*>(to + head);
+    const uintptr_t fa = reinterpret_cast<uintptr_t>(fb);
+    const uint32_t sh = (uint32_t)(fa & 3) * 8;
+    const uint32_t* fw = reinterpret_cast<const uint32_t*>(fa & ~uintptr_t(3));
+    for (int k = threadIdx.x; k < body; k += blockDim.x) {
+        const uint32_t* w = fw + 4 * k;
+        uint32_t w0 = __ldg(w), w1 = __ldg(w + 1), w2 = __ldg(w + 2), w3 = __ldg(w + 3);
+        uint32_t w4 = sh ? __ldg(w + 4) : 0u;
+        uint4 v;
+        v.x = __funnelshift_r(w0, w1, sh); v.y = __funnelshift_r(w1, w2, sh);
+        v.z = __funnelshift_r(w2, w3, sh); v.w = __funnelshift_r(w3, w4, sh);
+        tb[k] = v;
+    }
+    for (int k = head + (body << 4) + threadIdx.x; k < s; k += blockDim.x) to[k] = from[k];
+}
+
 __global__ void __launch_bounds__(1024) lz4_pack_scan_kernel(const int32_t* __restrict__ sizes, int64_t n,
                                                              int64_t* __restrict__ outOff, int headerBytes, FrameRule fr)
 {
@@ -1288,28 +1317,107 @@ __global__ void __launch_bounds__(256) lz4_pack_gather_kernel(const uint8_t* __r
         uint8_t* to = packed + outOff[b];
         const uint32_t hw = (uint32_t)s | (isRaw ? 0x80000000u : 0u);
         if (headerBytes == 4 && threadIdx.x < 4) to[threadIdx.x] = (uint8_t)(hw >> (8 * threadIdx.x));   // lz4frame.c:896-907 LE32
-        to += headerBytes;
-        /* destination-aligned 16-byte stores, source read through aligned words */
-        const uintptr_t ta = reinterpret_cast<uintptr_t>(to);
-        int head = (int)((16 - (ta & 15)) & 15);
-        if (head > s) head = s;
-        for (int k = threadIdx.x; k < head; k += blockDim.x) to[k] = from[k];
-        const int body = (s - head) >> 4;
-        const uint8_t* fb = from + head;
-        uint4* tb = reinterpret_cast<uint4*>(to + head);
-        const uintptr_t fa = reinterpret_cast<uintptr_t>(fb);
-        const uint32_t sh = (uint32_t)(fa & 3) * 8;
-        const uint32_t* fw = reinterpret_cast<const uint32_t*>(fa & ~uintptr_t(3));
-        for (int k = threadIdx.x; k < body; k += blockDim.x) {
-            const uint32_t* w = fw + 4 * k;
-            uint32_t w0 = __ldg(w), w1 = __ldg(w + 1), w2 = __ldg(w + 2), w3 = __ldg(w + 3);
-            uint32_t w4 = sh ? __ldg(w + 4) : 0u;
-            uint4 v;
-            v.x = __funnelshift_r(w0, w1, sh); v.y = __funnelshift_r(w1, w2, sh);
-            v.z = __funnelshift_r(w2, w3, sh); v.w = __funnelshift_r(w3, w4, sh);
-            tb[k] = v;
+        cta_copy(to + headerBytes, from, s);
+    }
+}
+
+/* =============================================================================================
+ * batched frame decode (LZ4B200_decompress_frames): the frame rules of lz4_frame_core.h, one frame per thread, around the
+ * decode of every class's block table (lz4k_launch_decode, by the caller)
+ *   index  : pass 1 -- header rules and chain walk, one thread per frame
+ *   scan   : one CTA -- per class, the exclusive sum of the block counts in frame order: each frame's base in its class's
+ *            table, and LZ4B200_ERR_LIMIT where the budget runs out
+ *   fill   : pass 2 -- the chain walked again, the table written (after the table is cleared)
+ *   verdict: between the scan and the expand of the blocks -- tight offsets, results, failed frames' blocks dropped
+ *   raw    : one CTA per stored-raw block of a frame that passed
+ * ============================================================================================= */
+__device__ __forceinline__ fc_block_tab frames_tab(const lz4k_frames_args& a, int cls)
+{
+    const int64_t t = cls >= 0 ? a.tabBase[cls] : 0;
+    return fc_block_tab{a.tabSrcOff + t, a.tabDstOff + t, a.tabSrcSize + t, a.tabOutSize + t, a.tabRawLen + t};
+}
+
+__global__ void __launch_bounds__(128) lz4_frames_index_kernel(lz4k_frames_args a)
+{
+    const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= a.nFrames) return;
+    fc_index_frame(a.src + a.srcOff[f], a.srcSize[f], a.dstCap[f], a.maxBlocks, static_cast<fc_frame_rec*>(a.frames) + f);
+}
+
+constexpr int kFsThreads = 1024, kFsItems = 4;            /* frames scan: kFsItems consecutive frames per thread */
+
+__global__ void __launch_bounds__(kFsThreads) lz4_frames_scan_kernel(lz4k_frames_args a)
+{
+    __shared__ int64_t warpSums[4][32];
+    __shared__ int64_t carry[4];
+    fc_frame_rec* rec = static_cast<fc_frame_rec*>(a.frames);
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    if (threadIdx.x < 4) carry[threadIdx.x] = 0;
+    __syncthreads();
+    for (int64_t base = 0; base < a.nFrames; base += kFsThreads * kFsItems) {
+        const int64_t f0 = base + (int64_t)threadIdx.x * kFsItems;
+        int64_t v[4] = {0, 0, 0, 0}, x[4];
+        #pragma unroll
+        for (int i = 0; i < kFsItems; i++) {
+            if (f0 + i >= a.nFrames) break;
+            const int64_t n = fc_scan_count(&rec[f0 + i]);
+            const int cls = rec[f0 + i].cls;
+            #pragma unroll
+            for (int c = 0; c < 4; c++) v[c] += cls == c ? n : 0;
         }
-        for (int k = head + (body << 4) + threadIdx.x; k < s; k += blockDim.x) to[k] = from[k];
+        #pragma unroll
+        for (int c = 0; c < 4; c++) {
+            x[c] = v[c];
+            for (int d = 1; d < 32; d <<= 1) { const int64_t y = __shfl_up_sync(kFull, x[c], d); if (lane >= d) x[c] += y; }
+            if (lane == 31) warpSums[c][wid] = x[c];
+        }
+        __syncthreads();
+        if (wid < 4) {                                        /* warp c scans class c's warp sums */
+            int64_t s = warpSums[wid][lane];
+            for (int d = 1; d < 32; d <<= 1) { const int64_t y = __shfl_up_sync(kFull, s, d); if (lane >= d) s += y; }
+            warpSums[wid][lane] = s;
+        }
+        __syncthreads();
+        int64_t pre[4];
+        #pragma unroll
+        for (int c = 0; c < 4; c++) pre[c] = carry[c] + (wid ? warpSums[c][wid - 1] : 0) + x[c] - v[c];
+        #pragma unroll
+        for (int i = 0; i < kFsItems; i++) {
+            if (f0 + i >= a.nFrames) break;
+            fc_frame_rec* r = &rec[f0 + i];
+            const int64_t n = fc_scan_count(r);
+            #pragma unroll
+            for (int c = 0; c < 4; c++)
+                if (r->cls == c) { fc_place_frame(r, pre[c], a.maxBlocks); pre[c] += n; }
+        }
+        __syncthreads();                                      /* every thread has read carry */
+        if (threadIdx.x == kFsThreads - 1) for (int c = 0; c < 4; c++) carry[c] = pre[c];
+        __syncthreads();
+    }
+}
+
+__global__ void __launch_bounds__(128) lz4_frames_fill_kernel(lz4k_frames_args a)
+{
+    const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= a.nFrames) return;
+    const fc_frame_rec* r = static_cast<const fc_frame_rec*>(a.frames) + f;
+    if (r->status != LZ4B200_OK) return;
+    fc_fill_frame(a.src + a.srcOff[f], a.srcOff[f], a.srcSize[f], r, frames_tab(a, r->cls));
+}
+
+__global__ void __launch_bounds__(128) lz4_frames_verdict_kernel(lz4k_frames_args a)
+{
+    const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= a.nFrames) return;
+    const fc_frame_rec* r = static_cast<const fc_frame_rec*>(a.frames) + f;
+    fc_verdict_frame(r, a.dstOff[f], a.dstCap[f], frames_tab(a, r->cls), a.result + f, a.consumed ? a.consumed + f : nullptr);
+}
+
+__global__ void __launch_bounds__(256) lz4_frames_raw_kernel(lz4k_frames_args a)
+{
+    for (int64_t b = blockIdx.x; b < a.nEntries; b += gridDim.x) {
+        const int len = a.tabRawLen[b];
+        if (len > 0) cta_copy(a.dst + a.tabDstOff[b], a.src + a.tabSrcOff[b], len);
     }
 }
 
@@ -1343,6 +1451,39 @@ static int launch_pack(const uint8_t* slots, int64_t slotStride, const int32_t* 
 extern "C" {
 
 uint64_t lz4k_launch_count(void) { return g_launches.load(); }
+
+static unsigned frames_grid(int64_t n) { return (unsigned)((n + 127) / 128); }
+
+int lz4k_launch_frames_index(const lz4k_frames_args* a, void* stream)
+{
+    cudaStream_t s = (cudaStream_t)stream;
+    lz4_frames_index_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);
+    lz4_frames_scan_kernel<<<1, kFsThreads, 0, s>>>(*a);
+    g_launches += 2;
+    /* unused entries decode nothing: size 0 (the scan rejects them) and no raw bytes */
+    cudaError_t e = cudaMemsetAsync(a->tabSrcSize, 0, (size_t)a->nEntries * sizeof(int32_t), s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(a->tabRawLen, 0xFF, (size_t)a->nEntries * sizeof(int32_t), s);
+    if (e != cudaSuccess) return (int)e;
+    lz4_frames_fill_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);
+    g_launches++;
+    return (int)cudaGetLastError();
+}
+
+int lz4k_launch_frames_verdict(const lz4k_frames_args* a, void* stream)
+{
+    lz4_frames_verdict_kernel<<<frames_grid(a->nFrames), 128, 0, (cudaStream_t)stream>>>(*a);
+    g_launches++;
+    return (int)cudaGetLastError();
+}
+
+int lz4k_launch_frames_raw(const lz4k_frames_args* a, void* stream)
+{
+    const int64_t cap = (int64_t)device_sms() * 16;
+    const int64_t grid = a->nEntries < 1 ? 1 : a->nEntries < cap ? a->nEntries : cap;
+    lz4_frames_raw_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(*a);
+    g_launches++;
+    return (int)cudaGetLastError();
+}
 
 /* debug: read and reset the phase-cycle counters (all zero unless built with -DLZ4K_PHASE_TIMING) */
 int lz4k_debug_phase_cycles(unsigned long long* out8)   /* out8: 12 values (8 phase cycles + 4 loop statistics) */

@@ -74,6 +74,30 @@ int lz4k_launch_pack(const uint8_t* slots, int64_t slotStride, const int32_t* si
 /* the body of an LZ4 frame: [LE32 block header][payload] per block; blocks whose compression did not gain are stored raw */
 int lz4k_launch_pack_frame(const uint8_t* slots, int64_t slotStride, const int32_t* sizes, const uint8_t* src, int64_t srcStride,
                            int32_t blockSize, int32_t lastSize, int64_t nBlocks, uint8_t* packed, int64_t* outOff, void* stream);
+/* the batched frame decode's own steps (lz4_frame_core.h); the decode of the blocks between them is the caller's */
+typedef struct {
+    const uint8_t* src;        /* the call's frames: frame f is src + srcOff[f], srcSize[f] bytes */
+    const int64_t* srcOff;
+    const int64_t* srcSize;
+    uint8_t* dst;              /* frame f decodes to dst + dstOff[f], dstCap[f] bytes of room */
+    const int64_t* dstOff;
+    const int64_t* dstCap;
+    int64_t* result;           /* [nFrames] */
+    int64_t* consumed;         /* [nFrames] or NULL */
+    int64_t nFrames;
+    int64_t maxBlocks[4];      /* the budget of every class */
+    int64_t tabBase[4];        /* class c's entries of the block table start at tabBase[c] */
+    int64_t nEntries;          /* entries of the block table (sum of maxBlocks) */
+    void* frames;              /* fc_frame_rec[nFrames] */
+    int64_t* tabSrcOff; int64_t* tabDstOff; int32_t* tabSrcSize; int32_t* tabOutSize; int32_t* tabRawLen;
+} lz4k_frames_args;
+
+/* pass 1 (index), the per-class scan with the budget rule, then the table cleared and filled (pass 2) */
+int lz4k_launch_frames_index(const lz4k_frames_args* a, void* stream);
+/* the verdict on every frame, once the scans of every class have run; the expands follow it */
+int lz4k_launch_frames_verdict(const lz4k_frames_args* a, void* stream);
+/* the stored-raw blocks of the frames that passed, to their place */
+int lz4k_launch_frames_raw(const lz4k_frames_args* a, void* stream);
 uint64_t lz4k_launch_count(void);
 int lz4k_debug_poison_smem(uint32_t pattern, int lo, int hi, void* stream);   /* developer tool */
 int lz4k_launch_ceiling(const lz4k_decode_args* a, int mode, void* stream);   /* developer tool: skeleton of the rows kernel without the decode */
