@@ -261,6 +261,42 @@ LZ4B200_API int LZ4B200_decompress_frames(const void* d_src, const int64_t* d_sr
                                           void* d_workspace, size_t workspaceBytes, void* stream);
 
 /*
+ * LZ4B200_decompress_frames for frames that may carry XXH32 checksums -- what the reference `lz4` tool writes by default
+ * (a content checksum) and any producer with blockChecksumFlag or contentChecksumFlag set.  Same arguments, budget,
+ * LZ4B200_ERR_LIMIT rule, readable padding, argument errors and workspace (LZ4B200_decompress_frames_workspace_bytes);
+ * it never synchronises and can be captured into a CUDA graph.
+ *
+ * Frames: everything LZ4B200_decompress_frames accepts, plus FLG bit 4 (block checksums), bit 2 (content checksum) or
+ * both; linked blocks, dictID and skippable frames stay LZ4B200_ERR_UNSUPPORTED.  On a frame without checksum flags the
+ * result, bytes and consumed length are LZ4B200_decompress_frames's, whatever skipChecksums.
+ *   - With bit 4, every block, compressed or stored raw, is followed by 4 checksum bytes; with bit 2, the EndMark is
+ *     followed by 4.  They belong to the chain: a frame that ends inside one is LZ4B200_ERR_FRAME, and d_consumed[f]
+ *     counts them.
+ *   - skipChecksums == 0: a block checksum is XXH32(seed 0) of the block's payload as stored (the compressed bytes, or
+ *     a stored-raw block's bytes), the content checksum XXH32(seed 0) of the frame's decoded content.  A mismatch gives
+ *     LZ4B200_ERR_CHECKSUM, in LZ4F_decompress's order: a compressed block's checksum before its decode (decode
+ *     failure, room, content size), a stored-raw block's after its room and content size, and the content checksum
+ *     after the content-size check at the end of the frame.  The header checksum stays LZ4B200_ERR_FRAME.
+ *   - skipChecksums != 0 (LZ4F_decompressOptions_t.skipChecksums): the fields are parsed but not compared, and the call
+ *     issues exactly the launches of LZ4B200_decompress_frames.  (The reference's LZ4F_decompress still compares a
+ *     compressed block's checksum under skipChecksums, lz4frame.c:1871-1883; this call compares none.)
+ *
+ * Reads: besides the readable padding of the frames, the content checksum reads each passing frame's decoded bytes in
+ * aligned 16-byte granules, every one of which holds at least one byte of [dst_f, dst_f + d_result[f]).
+ *
+ * Cost: XXH32 is serial within each of its four lanes, so one thread hashes one block (the block checksums) and one
+ * thread one frame's whole content (the content checksum).  The call is built for batches of many frames: a single large
+ * frame's content checksum runs at one thread's speed (DESIGN section 3.11 has the measured rate), and skipChecksums is
+ * the way around it.  Kernel launches: those of LZ4B200_decompress_frames, plus 2 when skipChecksums == 0.
+ */
+#define LZ4B200_ERR_CHECKSUM (-7)   /* per-frame result: a block checksum or the content checksum does not match */
+LZ4B200_API int LZ4B200_decompress_frames_checksummed(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
+                                                      void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
+                                                      int64_t* d_result, int64_t* d_consumed,
+                                                      int64_t nFrames, const int64_t maxBlocks[4], int skipChecksums,
+                                                      void* d_workspace, size_t workspaceBytes, void* stream);
+
+/*
  * Compress nBlocks independent blocks (the batched LZ4_compress_fast; replaces bench.c:464-493 and
  * lz4frame.c:1046-1055).
  *   block i input : d_src + i*srcStride, size (d_srcSize ? d_srcSize[i] : srcSize)

@@ -180,6 +180,23 @@ def decompress_frames(comp, offsets, sizes, capacities, max_blocks, out=None, ou
     Returns (out, results, consumed): results[f] is LZ4B200_decompressFrame_host's return value for frame f (decoded
     bytes or a negative error code), consumed[f] the frame's length when its header and chain are valid, else 0.
     """
+    return _decompress_frames("LZ4B200_decompress_frames", (), comp, offsets, sizes, capacities, max_blocks, out,
+                              out_offsets, results, consumed, workspace, stream)
+
+
+def decompress_frames_checksummed(comp, offsets, sizes, capacities, max_blocks, skip_checksums=False, out=None,
+                                  out_offsets=None, results=None, consumed=None, workspace=None, stream=None):
+    """decompress_frames for frames that may carry XXH32 block and content checksums
+    (LZ4B200_decompress_frames_checksummed): same arguments, workspace and results, and a mismatching checksum gives
+    LZ4B200_ERR_CHECKSUM (-7).  skip_checksums: parse the checksum fields without comparing them.  One thread hashes a
+    frame's whole content, so the content check of a single large frame runs at one thread's speed."""
+    return _decompress_frames("LZ4B200_decompress_frames_checksummed", (1 if skip_checksums else 0,), comp, offsets,
+                              sizes, capacities, max_blocks, out, out_offsets, results, consumed, workspace, stream)
+
+
+def _decompress_frames(entry, mode_args, comp, offsets, sizes, capacities, max_blocks, out, out_offsets, results,
+                       consumed, workspace, stream):
+    """the body of both frame calls: entry is the C function, mode_args what it takes after maxBlocks"""
     lib = _lib.load()
     _need_cuda(comp, offsets, sizes, capacities, out, out_offsets, results, consumed)
     assert comp.dtype == torch.uint8 and offsets.dtype == torch.int64 and sizes.dtype == torch.int64
@@ -202,11 +219,10 @@ def decompress_frames(comp, offsets, sizes, capacities, max_blocks, out=None, ou
             results = torch.empty(n, dtype=torch.int64, device=comp.device)
         if consumed is None:
             consumed = torch.empty(n, dtype=torch.int64, device=comp.device)
-    rc = lib.LZ4B200_decompress_frames(comp.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), out.data_ptr(),
-                                       out_offsets.data_ptr(), capacities.data_ptr(), results.data_ptr(),
-                                       consumed.data_ptr(), n, budget, workspace.data_ptr(), workspace.numel(),
-                                       st.cuda_stream)
-    _lib.check(rc, "LZ4B200_decompress_frames")
+    rc = getattr(lib, entry)(comp.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), out.data_ptr(),
+                             out_offsets.data_ptr(), capacities.data_ptr(), results.data_ptr(), consumed.data_ptr(), n,
+                             budget, *mode_args, workspace.data_ptr(), workspace.numel(), st.cuda_stream)
+    _lib.check(rc, entry)
     return out, results, consumed
 
 

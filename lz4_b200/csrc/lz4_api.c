@@ -306,14 +306,15 @@ size_t LZ4B200_decompress_frames_workspace_bytes(int64_t nFrames, const int64_t 
     return frames_plan(nFrames, maxBlocks, &p) ? p.bytes : 0;
 }
 
-/* index -> per class: scan (phase 1) -> verdict -> per class: expand (phase 2) -> raw blocks.  Every class decodes its
- * whole table (maxBlocks[c] entries, unused ones with size 0) at the uniform capacity of its block size, the capacity
- * lz4frame.c:1901-1904 and LZ4B200_decompressFrame_host decode with. */
-int LZ4B200_decompress_frames(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
-                              void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
-                              int64_t* d_result, int64_t* d_consumed,
-                              int64_t nFrames, const int64_t maxBlocks[4],
-                              void* d_workspace, size_t workspaceBytes, void* stream)
+/* index -> per class: scan (phase 1) -> [block checksums] -> verdict -> per class: expand (phase 2) -> raw blocks ->
+ * [content checksums].  Every class decodes its whole table (maxBlocks[c] entries, unused ones with size 0) at the
+ * uniform capacity of its block size, the capacity lz4frame.c:1901-1904 and LZ4B200_decompressFrame_host decode with.
+ * mode: FC_SUMS_* (lz4_frame_core.h); the bracketed steps run under FC_SUMS_VERIFY only. */
+static int decompress_frames_mode(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
+                                  void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
+                                  int64_t* d_result, int64_t* d_consumed,
+                                  int64_t nFrames, const int64_t maxBlocks[4], int mode,
+                                  void* d_workspace, size_t workspaceBytes, void* stream)
 {
     frames_plan_t p;
     lz4k_frames_args a;
@@ -331,12 +332,16 @@ int LZ4B200_decompress_frames(const void* d_src, const int64_t* d_srcOff, const 
     a.result = d_result; a.consumed = d_consumed; a.nFrames = nFrames;
     for (c = 0; c < 4; c++) { a.maxBlocks[c] = maxBlocks[c]; a.tabBase[c] = p.tabBase[c]; }
     a.nEntries = p.nEntries;
+    a.mode = mode;
     a.frames = ws + p.frames;
     a.tabSrcOff = (int64_t*)(ws + p.srcOff); a.tabDstOff = (int64_t*)(ws + p.dstOff);
     a.tabSrcSize = (int32_t*)(ws + p.srcSize); a.tabOutSize = (int32_t*)(ws + p.outSize); a.tabRawLen = (int32_t*)(ws + p.rawLen);
 
     if ((rc = launched(lz4k_launch_frames_index(&a, stream), "lz4k_launch_frames_index")) != LZ4B200_OK) return rc;
     for (ph = 1; ph <= 2; ph++) {
+        if (ph == 2 && mode == FC_SUMS_VERIFY &&
+            (rc = launched(lz4k_launch_frames_block_sums(&a, stream), "lz4k_launch_frames_block_sums")) != LZ4B200_OK)
+            return rc;
         if (ph == 2 && (rc = launched(lz4k_launch_frames_verdict(&a, stream), "lz4k_launch_frames_verdict")) != LZ4B200_OK)
             return rc;
         for (c = 0; c < 4; c++) {
@@ -348,7 +353,30 @@ int LZ4B200_decompress_frames(const void* d_src, const int64_t* d_srcOff, const 
             if (rc != LZ4B200_OK) return rc;
         }
     }
-    return launched(lz4k_launch_frames_raw(&a, stream), "lz4k_launch_frames_raw");
+    if ((rc = launched(lz4k_launch_frames_raw(&a, stream), "lz4k_launch_frames_raw")) != LZ4B200_OK) return rc;
+    if (mode == FC_SUMS_VERIFY) return launched(lz4k_launch_frames_content_sums(&a, stream), "lz4k_launch_frames_content_sums");
+    return LZ4B200_OK;
+}
+
+int LZ4B200_decompress_frames(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
+                              void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
+                              int64_t* d_result, int64_t* d_consumed,
+                              int64_t nFrames, const int64_t maxBlocks[4],
+                              void* d_workspace, size_t workspaceBytes, void* stream)
+{
+    return decompress_frames_mode(d_src, d_srcOff, d_srcSize, d_dst, d_dstOff, d_dstCap, d_result, d_consumed, nFrames,
+                                  maxBlocks, FC_SUMS_REJECT, d_workspace, workspaceBytes, stream);
+}
+
+int LZ4B200_decompress_frames_checksummed(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
+                                          void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
+                                          int64_t* d_result, int64_t* d_consumed,
+                                          int64_t nFrames, const int64_t maxBlocks[4], int skipChecksums,
+                                          void* d_workspace, size_t workspaceBytes, void* stream)
+{
+    return decompress_frames_mode(d_src, d_srcOff, d_srcSize, d_dst, d_dstOff, d_dstCap, d_result, d_consumed, nFrames,
+                                  maxBlocks, skipChecksums ? FC_SUMS_SKIP : FC_SUMS_VERIFY, d_workspace, workspaceBytes,
+                                  stream);
 }
 
 /* the encode launch arguments, every block size included (a split launch narrows minSize .. maxSize) */
@@ -893,7 +921,7 @@ int64_t LZ4B200_compressFrame_host(const void* h_src, int64_t srcSize, void* h_d
     dst[op++] = (uint8_t)((1u << 6) | (1u << 5) | ((contentSizeFlag ? 1u : 0u) << 3));   /* version 01, B.Indep */
     dst[op++] = (uint8_t)((uint32_t)bsid << 4);
     if (contentSizeFlag) { int i; for (i = 0; i < 8; i++) dst[op++] = (uint8_t)((uint64_t)srcSize >> (8 * i)); }
-    dst[op] = (uint8_t)(fc_xxh32_short(dst + 4, (size_t)(op - 4), 0) >> 8);
+    dst[op] = (uint8_t)(fc_xxh32(dst + 4, (uint64_t)(op - 4), 0) >> 8);
     op++;
 
     nFull = srcSize / bs;
@@ -970,13 +998,13 @@ int64_t LZ4B200_decompressFrame_host(const void* h_src, int64_t srcSize, void* h
     fc_header_t hdr;
     int isRaw, step;
     if (!h_src || (!h_dst && dstCapacity > 0)) return LZ4B200_ERR_ARG;
-    if ((step = fc_frame_header(src, srcSize, dstCapacity, &hdr)) != LZ4B200_OK) return step;   /* lz4frame.c:1340-1425 */
+    if ((step = fc_frame_header(src, srcSize, dstCapacity, FC_SUMS_REJECT, &hdr)) != LZ4B200_OK) return step;   /* lz4frame.c:1340-1425 */
     contentSize = hdr.contentSize;
     bs = fc_block_bytes(hdr.bsid);
 
     /* walk the chain of block headers (serial, O(#blocks)), lz4frame.c:1729-1758 */
     ip = hdr.hdrLen;
-    while ((step = fc_next_block(src, srcSize, bs, &ip, &at, &sz, &isRaw)) == 1) {
+    while ((step = fc_next_block(src, srcSize, bs, 0, &ip, &at, &sz, &isRaw)) == 1) {
         if (nBlocks == capBlocks) {
             int64_t* o2; int32_t* c2; uint8_t* r2;
             capBlocks = capBlocks ? capBlocks * 2 : 1024;

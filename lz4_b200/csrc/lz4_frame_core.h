@@ -1,7 +1,7 @@
 /*
- * lz4_frame_core.h -- the rules of an LZ4 frame of independent blocks, in one place: the header checks and the header
- * checksum (LZ4F_decodeHeader, lz4frame.c:1340-1425), the chain of block headers (lz4frame.c:1729-1758) and the verdict
- * on the decoded blocks.  LZ4B200_decompressFrame_host (lz4_api.c, compiled as C99) and the batched frame decode
+ * lz4_frame_core.h -- the rules of an LZ4 frame of independent blocks, in one place: XXH32, the header checks and the
+ * header checksum (LZ4F_decodeHeader, lz4frame.c:1340-1425), the chain of block headers with its checksum fields
+ * (lz4frame.c:1729-1758) and the verdict on the decoded blocks and their checksums.  LZ4B200_decompressFrame_host (lz4_api.c, compiled as C99) and the batched frame decode
  * (lz4_kernels.cu, CUDA) both decide with these functions; tests/emul/frame_emul.cpp runs the batched call's index passes
  * on the host from the same text.  No CUDA runtime calls, no allocation.
  */
@@ -28,17 +28,49 @@ FC_FN uint32_t fc_rd_le32(const uint8_t* p)
 
 FC_FN uint32_t fc_rotl32(uint32_t x, int r) { return (x << r) | (x >> (32 - r)); }
 
-/* XXH32 of a short message (len < 16), as published in the xxHash specification; the frame header checksum is its second
- * byte (lz4frame.c:781-809: HC = (XXH32(descriptor, 0) >> 8) & 0xFF). */
-FC_FN uint32_t fc_xxh32_short(const uint8_t* p, size_t len, uint32_t seed)
+/* XXH32, as published in the xxHash specification (https://github.com/Cyan4973/xxHash/blob/dev/doc/xxhash_spec.md): the
+ * frame header checksum is the second byte of XXH32(descriptor, 0) (lz4frame.c:781-809), a block checksum XXH32(payload,
+ * 0) and the content checksum XXH32(content, 0).  The kernels of the checksummed frame decode read their stripes their own
+ * way and share the round, the merge and the end with fc_xxh32. */
+#define FC_XXH_P1 2654435761u
+#define FC_XXH_P2 2246822519u
+#define FC_XXH_P3 3266489917u
+#define FC_XXH_P4 668265263u
+#define FC_XXH_P5 374761393u
+
+FC_FN uint32_t fc_xxh32_round(uint32_t acc, uint32_t lane) { return fc_rotl32(acc + lane * FC_XXH_P2, 13) * FC_XXH_P1; }
+
+/* the four accumulators after the last stripe, folded into one */
+FC_FN uint32_t fc_xxh32_merge(uint32_t v1, uint32_t v2, uint32_t v3, uint32_t v4)
 {
-    const uint32_t P1 = 2654435761u, P2 = 2246822519u, P3 = 3266489917u, P4 = 668265263u, P5 = 374761393u;
-    const uint8_t* end = p + len;
-    uint32_t h = seed + P5 + (uint32_t)len;
-    while (p + 4 <= end) { h += fc_rd_le32(p) * P3; h = fc_rotl32(h, 17) * P4; p += 4; }
-    while (p < end) { h += (uint32_t)(*p) * P5; h = fc_rotl32(h, 11) * P1; p++; }
-    h ^= h >> 15; h *= P2; h ^= h >> 13; h *= P3; h ^= h >> 16;
+    return fc_rotl32(v1, 1) + fc_rotl32(v2, 7) + fc_rotl32(v3, 12) + fc_rotl32(v4, 18);
+}
+
+/* the end of a message of len bytes: h (the merged accumulators, or seed + P5 below 16 bytes), the len & 15 bytes after
+ * the last stripe at p, the avalanche */
+FC_FN uint32_t fc_xxh32_end(uint32_t h, const uint8_t* p, uint64_t len)
+{
+    const uint8_t* end = p + (len & 15);
+    h += (uint32_t)len;
+    while (p + 4 <= end) { h += fc_rd_le32(p) * FC_XXH_P3; h = fc_rotl32(h, 17) * FC_XXH_P4; p += 4; }
+    while (p < end) { h += (uint32_t)(*p) * FC_XXH_P5; h = fc_rotl32(h, 11) * FC_XXH_P1; p++; }
+    h ^= h >> 15; h *= FC_XXH_P2; h ^= h >> 13; h *= FC_XXH_P3; h ^= h >> 16;
     return h;
+}
+
+FC_FN uint32_t fc_xxh32(const uint8_t* p, uint64_t len, uint32_t seed)
+{
+    uint32_t h = seed + FC_XXH_P5;
+    if (len >= 16) {
+        uint32_t v1 = seed + FC_XXH_P1 + FC_XXH_P2, v2 = seed + FC_XXH_P2, v3 = seed, v4 = seed - FC_XXH_P1;
+        const uint8_t* limit = p + (len & ~(uint64_t)15);
+        for (; p < limit; p += 16) {
+            v1 = fc_xxh32_round(v1, fc_rd_le32(p));      v2 = fc_xxh32_round(v2, fc_rd_le32(p + 4));
+            v3 = fc_xxh32_round(v3, fc_rd_le32(p + 8));  v4 = fc_xxh32_round(v4, fc_rd_le32(p + 12));
+        }
+        h = fc_xxh32_merge(v1, v2, v3, v4);
+    }
+    return fc_xxh32_end(h, p, len);
 }
 
 FC_FN int64_t fc_block_bytes(int bsid) { return (int64_t)1 << (8 + 2 * bsid); }   /* 4..7 -> 64 KB..4 MB (lz4frame.c:333-342) */
@@ -47,12 +79,24 @@ typedef struct {
     int64_t contentSize;       /* the header's content size, -1 without one (a field of 2^63 or more reads negative too) */
     int32_t hdrLen;            /* bytes of the header: the first block header starts here */
     int32_t bsid;              /* block size ID, 4 .. 7 */
+    int32_t sums;              /* the checksums the frame carries: FC_BLOCK_SUM | FC_CONTENT_SUM */
 } fc_header_t;
+
+/* what the header rules do with FLG's checksum bits: reject them (LZ4B200_ERR_UNSUPPORTED; the host call and
+ * LZ4B200_decompress_frames), or accept them and skip or verify the checksums (LZ4B200_decompress_frames_checksummed) */
+#define FC_SUMS_REJECT 0
+#define FC_SUMS_SKIP   1
+#define FC_SUMS_VERIFY 2
+
+#define FC_BLOCK_SUM   1           /* FLG bit 4: 4 bytes of XXH32(payload) after every block */
+#define FC_CONTENT_SUM 2           /* FLG bit 2: 4 bytes of XXH32(content) after the EndMark */
+#define FC_VERIFY      4           /* (fc_frame_rec.sums) the call compares them */
 
 /* The verdict on a frame's arguments and header, in the order LZ4B200_decompressFrame_host decides them: LZ4B200_OK (h
  * filled in), LZ4B200_ERR_ARG (srcSize or dstCap negative), LZ4B200_ERR_FRAME (malformed header) or
- * LZ4B200_ERR_UNSUPPORTED (skippable frame, linked blocks, checksums, dictID).  Reads src[0, min(srcSize, 19)). */
-FC_FN int fc_frame_header(const uint8_t* src, int64_t srcSize, int64_t dstCap, fc_header_t* h)
+ * LZ4B200_ERR_UNSUPPORTED (skippable frame, linked blocks, checksums under FC_SUMS_REJECT, dictID).  The header checksum
+ * is checked in every mode (lz4frame.c:1418).  Reads src[0, min(srcSize, 19)). */
+FC_FN int fc_frame_header(const uint8_t* src, int64_t srcSize, int64_t dstCap, int mode, fc_header_t* h)
 {
     uint32_t flg, bd, hdrLen, magic;
     int bsid, i;
@@ -68,9 +112,11 @@ FC_FN int fc_frame_header(const uint8_t* src, int64_t srcSize, int64_t dstCap, f
     bd = src[5];
     bsid = (int)((bd >> 4) & 7);
     if ((bd >> 7) || (bd & 15) || bsid < 4) return LZ4B200_ERR_FRAME;                 /* lz4frame.c:1406-1412 */
-    if ((uint8_t)(fc_xxh32_short(src + 4, hdrLen - 5, 0) >> 8) != src[hdrLen - 1]) return LZ4B200_ERR_FRAME;
+    if ((uint8_t)(fc_xxh32(src + 4, hdrLen - 5, 0) >> 8) != src[hdrLen - 1]) return LZ4B200_ERR_FRAME;
     if (!((flg >> 5) & 1)) return LZ4B200_ERR_UNSUPPORTED;                            /* linked blocks */
-    if (((flg >> 4) & 1) || ((flg >> 2) & 1) || (flg & 1)) return LZ4B200_ERR_UNSUPPORTED;   /* checksums, dictID */
+    if (flg & 1) return LZ4B200_ERR_UNSUPPORTED;                                      /* dictID */
+    h->sums = (((flg >> 4) & 1) ? FC_BLOCK_SUM : 0) | (((flg >> 2) & 1) ? FC_CONTENT_SUM : 0);
+    if (h->sums && mode == FC_SUMS_REJECT) return LZ4B200_ERR_UNSUPPORTED;
     h->contentSize = -1;
     if ((flg >> 3) & 1) {
         uint64_t v = 0;
@@ -83,21 +129,28 @@ FC_FN int fc_frame_header(const uint8_t* src, int64_t srcSize, int64_t dstCap, f
 }
 
 /* One step of the chain of block headers (lz4frame.c:1729-1758) from the block header at *ip, for blocks of at most bs
- * bytes.  Returns 1 for a block (*at: its first byte, *size, *raw: stored raw; *ip moves past it), 0 at the EndMark (*ip
- * moves past it: the frame's length), LZ4B200_ERR_FRAME for a truncated chain or a block above bs (maxBlockSize_invalid,
- * lz4frame.c:1745). */
-FC_FN int fc_next_block(const uint8_t* src, int64_t srcSize, int64_t bs, int64_t* ip, int64_t* at, int64_t* size, int* raw)
+ * bytes in a frame carrying the checksums `sums`.  Returns 1 for a block (*at: its first byte, *size, *raw: stored raw;
+ * *ip moves past it and its checksum), 0 at the EndMark (*ip moves past it and the content checksum: the frame's
+ * length), LZ4B200_ERR_FRAME for a truncated chain -- a checksum field is part of the chain (lz4frame.c:1731, 1751) -- or
+ * a block above bs (maxBlockSize_invalid, lz4frame.c:1745). */
+FC_FN int fc_next_block(const uint8_t* src, int64_t srcSize, int64_t bs, int sums, int64_t* ip, int64_t* at, int64_t* size,
+                        int* raw)
 {
+    const int64_t cs = (sums & FC_BLOCK_SUM) ? 4 : 0;
     uint32_t h;
     int64_t sz;
     if (*ip + 4 > srcSize) return LZ4B200_ERR_FRAME;
     h = fc_rd_le32(src + *ip);
     *ip += 4;
-    if (h == 0) return 0;                                                             /* EndMark */
+    if (h == 0) {                                                                     /* EndMark */
+        if ((sums & FC_CONTENT_SUM) && *ip + 4 > srcSize) return LZ4B200_ERR_FRAME;
+        if (sums & FC_CONTENT_SUM) *ip += 4;
+        return 0;
+    }
     sz = (int64_t)(h & 0x7FFFFFFFu);
-    if (sz > bs || *ip + sz > srcSize) return LZ4B200_ERR_FRAME;
+    if (sz > bs || *ip + sz + cs > srcSize) return LZ4B200_ERR_FRAME;
     *at = *ip; *size = sz; *raw = (int)(h >> 31);
-    *ip += sz;
+    *ip += sz + cs;
     return 1;
 }
 
@@ -111,16 +164,27 @@ FC_FN int fc_block_verdict(int64_t pos, int64_t r, int64_t dstCap, int64_t conte
     return LZ4B200_OK;
 }
 
+/* The same with the outcome of the block's checksum (sumBad: it does not match), where LZ4F_decompress judges it: a
+ * compressed block's before its decode (lz4frame.c:1871-1883), a stored-raw block's after its bytes are placed
+ * (lz4frame.c:1803-1830), so after the room and the content size. */
+FC_FN int fc_block_sum_verdict(int64_t pos, int64_t r, int64_t dstCap, int64_t contentSize, int raw, int sumBad)
+{
+    int v;
+    if (sumBad && !raw) return LZ4B200_ERR_CHECKSUM;
+    v = fc_block_verdict(pos, r, dstCap, contentSize);
+    return (v == LZ4B200_OK && sumBad) ? LZ4B200_ERR_CHECKSUM : v;
+}
+
 /* a frame whose every block passed: its result, total decoded bytes, or LZ4B200_ERR_FRAME when the content size differs
- * (frameSize_wrong) */
+ * (frameSize_wrong, lz4frame.c:1984; the content checksum is judged after it, by the caller) */
 FC_FN int64_t fc_frame_result(int64_t total, int64_t contentSize)
 {
     return (contentSize >= 0 && contentSize != total) ? (int64_t)LZ4B200_ERR_FRAME : total;
 }
 
 /* ---------------------------------------------------------------------------------------------
- * The batched frame decode (LZ4B200_decompress_frames): one record per frame, one table of blocks per class (block size
- * ID 4 + c), and the three steps that run one frame per thread.
+ * The batched frame decode (LZ4B200_decompress_frames and LZ4B200_decompress_frames_checksummed): one record per frame,
+ * one table of blocks per class (block size ID 4 + c), and the three steps that run one frame per thread.
  * ------------------------------------------------------------------------------------------- */
 typedef struct {
     int64_t count;             /* blocks the chain walk saw (at most maxBlocks[cls] + 1) */
@@ -129,34 +193,50 @@ typedef struct {
     int64_t consumed;          /* the frame's length once its chain is walked to the EndMark, else 0 */
     int32_t status;            /* LZ4B200_OK or the frame's error code so far */
     int32_t cls;               /* block size ID - 4 (-1 before the header passed) */
-    int32_t hdrLen, pad;
+    int32_t hdrLen;
+    int32_t sums;              /* fc_header_t.sums, | FC_VERIFY when the call compares them */
 } fc_frame_rec;
 
 typedef struct {               /* a class's block table; entry b of every array belongs to one block */
     int64_t* srcOff;           /* absolute offset of the block's bytes in the call's source */
-    int64_t* dstOff;           /* absolute offset of its decoded bytes in the call's destination (set by the verdict) */
+    int64_t* dstOff;           /* absolute offset of its decoded bytes in the call's destination (set by the verdict);
+                                  before the verdict, under FC_VERIFY, the block checksum's state: FC_SUM_* */
     int32_t* srcSize;          /* bytes the decode gets: 0 for a stored-raw block, so that the scan rejects it */
     int32_t* outSize;          /* the decode's return value; -1 once the verdict has failed the block's frame */
     int32_t* rawLen;           /* a stored-raw block's size, -1 for a compressed block */
 } fc_block_tab;
 
-/* Pass 1 (the index): the header rules, then the chain walk, which stops after maxBlocks[cls] + 1 blocks (the frame is over
- * its budget whatever follows).  src: the frame's first byte. */
-FC_FN void fc_index_frame(const uint8_t* src, int64_t srcSize, int64_t dstCap, const int64_t* maxBlocks, fc_frame_rec* r)
+/* the block checksum's state in a table entry's dstOff before the verdict (FC_VERIFY only; the table is cleared to
+ * FC_SUM_NONE first) */
+#define FC_SUM_NONE    0           /* no checksum to compare, or it matches */
+#define FC_SUM_PENDING 1           /* the fill found one; the block checksum kernel compares it */
+#define FC_SUM_BAD     2           /* it does not match */
+
+/* Pass 1 (the index): the header rules under `mode` (FC_SUMS_*), then the chain walk, which stops after
+ * maxBlocks[cls] + 1 blocks (the frame is over its budget whatever follows).  src: the frame's first byte. */
+FC_FN void fc_index_frame_mode(const uint8_t* src, int64_t srcSize, int64_t dstCap, const int64_t* maxBlocks, int mode,
+                               fc_frame_rec* r)
 {
     fc_header_t h;
     int64_t ip, at, sz, n = 0;
     int raw, s;
-    r->count = 0; r->base = 0; r->contentSize = -1; r->consumed = 0; r->cls = -1; r->hdrLen = 0; r->pad = 0;
-    r->status = fc_frame_header(src, srcSize, dstCap, &h);
+    r->count = 0; r->base = 0; r->contentSize = -1; r->consumed = 0; r->cls = -1; r->hdrLen = 0; r->sums = 0;
+    r->status = fc_frame_header(src, srcSize, dstCap, mode, &h);
     if (r->status != LZ4B200_OK) return;
     r->cls = h.bsid - 4; r->contentSize = h.contentSize; r->hdrLen = h.hdrLen;
+    r->sums = h.sums | ((h.sums && mode == FC_SUMS_VERIFY) ? FC_VERIFY : 0);
     ip = h.hdrLen;
-    while ((s = fc_next_block(src, srcSize, fc_block_bytes(h.bsid), &ip, &at, &sz, &raw)) == 1)
+    while ((s = fc_next_block(src, srcSize, fc_block_bytes(h.bsid), h.sums, &ip, &at, &sz, &raw)) == 1)
         if (++n > maxBlocks[r->cls]) break;
     if (s < 0) { r->status = s; return; }
     r->count = n;
     if (s == 0) r->consumed = ip;
+}
+
+/* pass 1 of LZ4B200_decompress_frames, which rejects checksums */
+FC_FN void fc_index_frame(const uint8_t* src, int64_t srcSize, int64_t dstCap, const int64_t* maxBlocks, fc_frame_rec* r)
+{
+    fc_index_frame_mode(src, srcSize, dstCap, maxBlocks, FC_SUMS_REJECT, r);
 }
 
 /* the blocks frame r puts into its class's exclusive scan (a frame that failed pass 1 puts none) */
@@ -170,35 +250,39 @@ FC_FN void fc_place_frame(fc_frame_rec* r, int64_t base, const int64_t* maxBlock
     if (r->status == LZ4B200_OK && base + r->count > maxBlocks[r->cls]) { r->status = LZ4B200_ERR_LIMIT; r->consumed = 0; }
 }
 
-/* Pass 2 (the fill): walks the chain again and writes the frame's entries of its class's table.  srcOff: the frame's offset
- * in the call's source. */
+/* Pass 2 (the fill): walks the chain again and writes the frame's entries of its class's table, and marks the block
+ * checksums to compare.  srcOff: the frame's offset in the call's source. */
 FC_FN void fc_fill_frame(const uint8_t* src, int64_t srcOff, int64_t srcSize, const fc_frame_rec* r, fc_block_tab t)
 {
     int64_t ip = r->hdrLen, at, sz, b = r->base;
     int raw;
     if (r->status != LZ4B200_OK) return;
-    while (fc_next_block(src, srcSize, fc_block_bytes(r->cls + 4), &ip, &at, &sz, &raw) == 1) {
+    const int mark = (r->sums & FC_VERIFY) && (r->sums & FC_BLOCK_SUM);
+    while (fc_next_block(src, srcSize, fc_block_bytes(r->cls + 4), r->sums, &ip, &at, &sz, &raw) == 1) {
         t.srcOff[b] = srcOff + at;
         t.srcSize[b] = raw ? 0 : (int32_t)sz;
         t.rawLen[b] = raw ? (int32_t)sz : -1;
+        if (mark) t.dstOff[b] = FC_SUM_PENDING;
         b++;
     }
 }
 
-/* The verdict, between the scan and the expand: the block rules in block order on the scanned and the raw sizes, each
- * block's tight offset (dstOff: the frame's), the frame's result and consumed length.  Every block of a frame that fails
- * gets outSize -1 and rawLen -1, so that neither the expand nor the raw copy writes any of its bytes. */
+/* The verdict, between the scan and the expand: the block rules in block order on the scanned and the raw sizes and the
+ * block checksums' outcomes, each block's tight offset (dstOff: the frame's), the frame's result and consumed length.
+ * Every block of a frame that fails gets outSize -1 and rawLen -1, so that neither the expand nor the raw copy writes any
+ * of its bytes.  The content checksum of a frame that passes is judged after its bytes are in place. */
 FC_FN void fc_verdict_frame(const fc_frame_rec* r, int64_t dstOff, int64_t dstCap, fc_block_tab t, int64_t* result,
                             int64_t* consumed)
 {
     int64_t pos = 0, res, k;
     int v = LZ4B200_OK;
+    const int verifyBlocks = (r->sums & FC_VERIFY) && (r->sums & FC_BLOCK_SUM);
     if (consumed) *consumed = r->consumed;
     if (r->status != LZ4B200_OK) { *result = r->status; return; }
     for (k = 0; k < r->count && v == LZ4B200_OK; k++) {
         const int64_t b = r->base + k;
         const int64_t rb = t.rawLen[b] >= 0 ? t.rawLen[b] : t.outSize[b];
-        v = fc_block_verdict(pos, rb, dstCap, r->contentSize);
+        v = fc_block_sum_verdict(pos, rb, dstCap, r->contentSize, t.rawLen[b] >= 0, verifyBlocks && t.dstOff[b] == FC_SUM_BAD);
         t.dstOff[b] = dstOff + pos;
         pos += rb;
     }

@@ -1322,14 +1322,18 @@ __global__ void __launch_bounds__(256) lz4_pack_gather_kernel(const uint8_t* __r
 }
 
 /* =============================================================================================
- * batched frame decode (LZ4B200_decompress_frames): the frame rules of lz4_frame_core.h, one frame per thread, around the
- * decode of every class's block table (lz4k_launch_decode, by the caller)
+ * batched frame decode (LZ4B200_decompress_frames, LZ4B200_decompress_frames_checksummed): the frame rules of
+ * lz4_frame_core.h, one frame per thread, around the decode of every class's block table (lz4k_launch_decode, by the
+ * caller)
  *   index  : pass 1 -- header rules and chain walk, one thread per frame
  *   scan   : one CTA -- per class, the exclusive sum of the block counts in frame order: each frame's base in its class's
  *            table, and LZ4B200_ERR_LIMIT where the budget runs out
  *   fill   : pass 2 -- the chain walked again, the table written (after the table is cleared)
  *   verdict: between the scan and the expand of the blocks -- tight offsets, results, failed frames' blocks dropped
  *   raw    : one CTA per stored-raw block of a frame that passed
+ * and, when the checksummed call verifies (FC_SUMS_VERIFY):
+ *   block sums  : before the verdict, one thread per table entry the fill marked: XXH32 of the block's stored payload
+ *   content sums: after the raw blocks, one thread per frame that passed with a content checksum: XXH32 of its output
  * ============================================================================================= */
 __device__ __forceinline__ fc_block_tab frames_tab(const lz4k_frames_args& a, int cls)
 {
@@ -1341,7 +1345,8 @@ __global__ void __launch_bounds__(128) lz4_frames_index_kernel(lz4k_frames_args 
 {
     const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= a.nFrames) return;
-    fc_index_frame(a.src + a.srcOff[f], a.srcSize[f], a.dstCap[f], a.maxBlocks, static_cast<fc_frame_rec*>(a.frames) + f);
+    fc_index_frame_mode(a.src + a.srcOff[f], a.srcSize[f], a.dstCap[f], a.maxBlocks, a.mode,
+                        static_cast<fc_frame_rec*>(a.frames) + f);
 }
 
 constexpr int kFsThreads = 1024, kFsItems = 4;            /* frames scan: kFsItems consecutive frames per thread */
@@ -1421,6 +1426,91 @@ __global__ void __launch_bounds__(256) lz4_frames_raw_kernel(lz4k_frames_args a)
     }
 }
 
+/* XXH32 by one thread (the rounds of lz4_frame_core.h).  The four accumulators are independent chains, the thread's ILP;
+ * the stripes come from aligned 16-byte loads joined by funnel shifts, kXxU stripes' loads in flight and an L2 prefetch
+ * kXxAhead granules ahead.  Every load, the prefetch included, stays inside an aligned 16-byte granule that holds a byte of
+ * the message: a stripe's second granule is clamped to the message's last, which only the last stripe of an aligned
+ * message reaches (and does not use). */
+constexpr int kXxU = 8, kXxAhead = 256;
+
+template <int WS>          /* the message's start, in 4-byte words into its first granule: lane j is word j + WS of lo:hi */
+__device__ __forceinline__ void xxh_stripe(const uint4& lo, const uint4& hi, uint32_t bs, uint32_t v[4])
+{
+    const uint32_t w[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+    v[0] = fc_xxh32_round(v[0], __funnelshift_r(w[WS], w[WS + 1], bs));
+    v[1] = fc_xxh32_round(v[1], __funnelshift_r(w[WS + 1], w[WS + 2], bs));
+    v[2] = fc_xxh32_round(v[2], __funnelshift_r(w[WS + 2], w[WS + 3], bs));
+    v[3] = fc_xxh32_round(v[3], __funnelshift_r(w[WS + 3], w[WS + 4], bs));
+}
+
+/* stripes 0 .. n - 1 of a message whose granules are g[0 .. gLast], starting bs / 8 bytes into word WS of g[0] */
+template <int WS>
+__device__ __forceinline__ void xxh_stripes(const uint4* g, int64_t n, int64_t gLast, uint32_t bs, uint32_t v[4])
+{
+    uint4 lo = __ldg(g);
+    int64_t k = 0;
+    for (; k + kXxU <= n; k += kXxU) {
+        uint4 hi[kXxU];
+        #pragma unroll
+        for (int u = 0; u < kXxU; u++) hi[u] = __ldg(g + min(k + u + 1, gLast));
+        asm volatile("prefetch.global.L2 [%0];" :: "l"(g + min(k + kXxAhead, gLast)));
+        #pragma unroll
+        for (int u = 0; u < kXxU; u++) xxh_stripe<WS>(u ? hi[u - 1] : lo, hi[u], bs, v);
+        lo = hi[kXxU - 1];
+    }
+    for (; k < n; k++) {
+        const uint4 hi = __ldg(g + min(k + 1, gLast));
+        xxh_stripe<WS>(lo, hi, bs, v);
+        lo = hi;
+    }
+}
+
+/* XXH32(p[0 .. len), 0); the bytes after the last stripe are read one by one (fc_xxh32_end) */
+__device__ uint32_t xxh32_dev(const uint8_t* p, int64_t len)
+{
+    uint32_t h = FC_XXH_P5;
+    const int64_t n = len >> 4;
+    if (n) {
+        uint32_t v[4] = {FC_XXH_P1 + FC_XXH_P2, FC_XXH_P2, 0u, 0u - FC_XXH_P1};
+        const uintptr_t at = reinterpret_cast<uintptr_t>(p);
+        const uint4* g = reinterpret_cast<const uint4*>(at & ~uintptr_t(15));
+        const int64_t gLast = (int64_t)(((at + (uintptr_t)len - 1) >> 4) - (at >> 4));
+        const uint32_t bs = (uint32_t)(at & 3) * 8;
+        switch ((at >> 2) & 3) {
+        case 0: xxh_stripes<0>(g, n, gLast, bs, v); break;
+        case 1: xxh_stripes<1>(g, n, gLast, bs, v); break;
+        case 2: xxh_stripes<2>(g, n, gLast, bs, v); break;
+        default: xxh_stripes<3>(g, n, gLast, bs, v); break;
+        }
+        h = fc_xxh32_merge(v[0], v[1], v[2], v[3]);
+    }
+    return fc_xxh32_end(h, p + (n << 4), (uint64_t)len);
+}
+
+/* one thread per table entry: a block the fill marked FC_SUM_PENDING gets FC_SUM_NONE (its checksum, the 4 bytes after
+ * its stored payload, matches) or FC_SUM_BAD, which the verdict turns into LZ4B200_ERR_CHECKSUM */
+__global__ void __launch_bounds__(128) lz4_frames_block_sum_kernel(lz4k_frames_args a)
+{
+    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= a.nEntries || a.tabDstOff[b] != FC_SUM_PENDING) return;
+    const int64_t n = a.tabRawLen[b] >= 0 ? a.tabRawLen[b] : a.tabSrcSize[b];
+    const uint8_t* p = a.src + a.tabSrcOff[b];
+    a.tabDstOff[b] = xxh32_dev(p, n) == fc_rd_le32(p + n) ? FC_SUM_NONE : FC_SUM_BAD;
+}
+
+/* one thread per frame: a frame that passed and carries a content checksum (the 4 bytes before its end) gets
+ * LZ4B200_ERR_CHECKSUM when XXH32 of its output differs */
+__global__ void __launch_bounds__(128) lz4_frames_content_sum_kernel(lz4k_frames_args a)
+{
+    const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= a.nFrames) return;
+    const fc_frame_rec* r = static_cast<const fc_frame_rec*>(a.frames) + f;
+    const int64_t n = a.result[f];
+    if (!(r->sums & FC_VERIFY) || !(r->sums & FC_CONTENT_SUM) || n < 0) return;
+    if (xxh32_dev(a.dst + a.dstOff[f], n) != fc_rd_le32(a.src + a.srcOff[f] + r->consumed - 4))
+        a.result[f] = LZ4B200_ERR_CHECKSUM;
+}
+
 }  // namespace
 
 /* =============================================================================================
@@ -1463,6 +1553,8 @@ int lz4k_launch_frames_index(const lz4k_frames_args* a, void* stream)
     /* unused entries decode nothing: size 0 (the scan rejects them) and no raw bytes */
     cudaError_t e = cudaMemsetAsync(a->tabSrcSize, 0, (size_t)a->nEntries * sizeof(int32_t), s);
     if (e == cudaSuccess) e = cudaMemsetAsync(a->tabRawLen, 0xFF, (size_t)a->nEntries * sizeof(int32_t), s);
+    /* every entry's block checksum state FC_SUM_NONE, before the fill marks the ones to compare */
+    if (e == cudaSuccess && a->mode == FC_SUMS_VERIFY) e = cudaMemsetAsync(a->tabDstOff, 0, (size_t)a->nEntries * sizeof(int64_t), s);
     if (e != cudaSuccess) return (int)e;
     lz4_frames_fill_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);
     g_launches++;
@@ -1481,6 +1573,20 @@ int lz4k_launch_frames_raw(const lz4k_frames_args* a, void* stream)
     const int64_t cap = (int64_t)device_sms() * 16;
     const int64_t grid = a->nEntries < 1 ? 1 : a->nEntries < cap ? a->nEntries : cap;
     lz4_frames_raw_kernel<<<(unsigned)grid, 256, 0, (cudaStream_t)stream>>>(*a);
+    g_launches++;
+    return (int)cudaGetLastError();
+}
+
+int lz4k_launch_frames_block_sums(const lz4k_frames_args* a, void* stream)
+{
+    lz4_frames_block_sum_kernel<<<a->nEntries < 1 ? 1u : frames_grid(a->nEntries), 128, 0, (cudaStream_t)stream>>>(*a);
+    g_launches++;
+    return (int)cudaGetLastError();
+}
+
+int lz4k_launch_frames_content_sums(const lz4k_frames_args* a, void* stream)
+{
+    lz4_frames_content_sum_kernel<<<frames_grid(a->nFrames), 128, 0, (cudaStream_t)stream>>>(*a);
     g_launches++;
     return (int)cudaGetLastError();
 }

@@ -88,6 +88,7 @@ typedef struct {
     int64_t maxBlocks[4];      /* the budget of every class */
     int64_t tabBase[4];        /* class c's entries of the block table start at tabBase[c] */
     int64_t nEntries;          /* entries of the block table (sum of maxBlocks) */
+    int mode;                  /* FC_SUMS_* (lz4_frame_core.h): the checksum flags rejected, skipped or verified */
     void* frames;              /* fc_frame_rec[nFrames] */
     int64_t* tabSrcOff; int64_t* tabDstOff; int32_t* tabSrcSize; int32_t* tabOutSize; int32_t* tabRawLen;
 } lz4k_frames_args;
@@ -98,6 +99,10 @@ int lz4k_launch_frames_index(const lz4k_frames_args* a, void* stream);
 int lz4k_launch_frames_verdict(const lz4k_frames_args* a, void* stream);
 /* the stored-raw blocks of the frames that passed, to their place */
 int lz4k_launch_frames_raw(const lz4k_frames_args* a, void* stream);
+/* FC_SUMS_VERIFY: every marked block's checksum, before the verdict */
+int lz4k_launch_frames_block_sums(const lz4k_frames_args* a, void* stream);
+/* FC_SUMS_VERIFY: the content checksum of every frame that passed, after the raw blocks */
+int lz4k_launch_frames_content_sums(const lz4k_frames_args* a, void* stream);
 uint64_t lz4k_launch_count(void);
 int lz4k_debug_poison_smem(uint32_t pattern, int lo, int hi, void* stream);   /* developer tool */
 int lz4k_launch_ceiling(const lz4k_decode_args* a, int mode, void* stream);   /* developer tool: skeleton of the rows kernel without the decode */
