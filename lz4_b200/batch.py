@@ -13,6 +13,14 @@ captured into a CUDA graph.  The workspace rule of the calls that need one (the 
   - a phased decode (phases 1 or 2) and any call under stream capture need their own: the expand consumes what its
     scan left in the workspace, which a call in between would overwrite, and a graph keeps the workspace's address,
     which the module's cache may free when it grows.
+
+Every wrapper checks its arguments before it allocates or launches anything (_checked) and raises ValueError when one
+fails: tensors are contiguous CUDA tensors on one device, of the dtype their argument takes, with the elements the call
+reads or writes; strides hold a slot's capacity; ints the C call takes as 32-bit ints fit one.  The launch runs with
+that device current, on `stream` (default: that device's current stream).  What would need a read of device memory is
+not checked, so no wrapper synchronises for it: the values of offsets, sizes, per-block targets and src_sizes (a block
+read or written past its buffer), and whether a frames call's `out` holds what out_offsets and capacities place in it.
+Those are the caller's responsibility.
 """
 import ctypes as C
 
@@ -21,21 +29,77 @@ import torch
 from . import _lib
 
 
-def _stream(stream=None):
-    return stream if stream is not None else torch.cuda.current_stream()
+U8, I32, I64 = torch.uint8, torch.int32, torch.int64
+INT32_MIN, INT32_MAX = -2 ** 31, 2 ** 31 - 1
+ANY = (0, None)                 # an element count _checked accepts: at least 0, no upper limit
+
+
+def _checked(what, stream, tensors, ints=(), strides=()):
+    """The argument check of every wrapper: what the kernels would misread or write past, as far as it shows without
+    reading device memory.  Raises ValueError when a check fails.
+      tensors: (name, tensor or None, dtype, (least, most)): a contiguous CUDA tensor of that dtype with least .. most
+               elements (most None: no limit); a byte buffer's elements are its bytes, whatever its shape.  All given
+               tensors are on one device.
+      ints:    (name, value, lo, hi): a host int the C call takes as a 32-bit int, within lo .. hi
+      strides: (name, stride, capacity): slots `stride` bytes apart, each of `capacity` bytes, do not overlap
+    Returns (device, stream): the tensors' device and the stream to launch on -- `stream` if given (it must be on that
+    device), else the device's current stream."""
+    device = None
+    for name, t, dtype, (least, most) in tensors:
+        if t is None:
+            continue
+        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+            raise ValueError("%s: %s must be a CUDA tensor (got %s)" % (
+                what, name, "one on %s" % t.device if isinstance(t, torch.Tensor) else type(t).__name__))
+        if device is None:
+            device = t.device
+        elif t.device != device:
+            raise ValueError("%s: %s is on %s, the other tensors on %s" % (what, name, t.device, device))
+        if t.dtype != dtype:
+            raise ValueError("%s: %s must be %s (got %s)" % (what, name, dtype, t.dtype))
+        if not t.is_contiguous():
+            raise ValueError("%s: %s must be contiguous" % (what, name))
+        if t.numel() < least or (most is not None and t.numel() > most):
+            raise ValueError("%s: %s has %d elements, the call needs %s" % (
+                what, name, t.numel(), "at least %d" % least if most is None else "%d .. %d" % (least, most)))
+    for name, v, lo, hi in ints:
+        if not lo <= int(v) <= hi:
+            raise ValueError("%s: %s = %d is outside %d .. %d" % (what, name, int(v), lo, hi))
+    for name, stride, cap in strides:
+        if int(stride) < max(int(cap), 0):
+            raise ValueError("%s: %s = %d is below the %d bytes of a slot" % (what, name, int(stride), int(cap)))
+    if stream is None:
+        return device, torch.cuda.current_stream(device)
+    if device is not None and stream.device != device:
+        raise ValueError("%s: the stream is on %s, the tensors on %s" % (what, stream.device, device))
+    return device, stream
+
+
+def _int32(name, v):
+    """an int the C call takes as a 32-bit int, as _checked takes it"""
+    return (name, v, INT32_MIN, INT32_MAX)
+
+
+def _extent(n, stride, cap):
+    """the bytes n slots of `cap` bytes, `stride` apart, span"""
+    return (n - 1) * int(stride) + max(int(cap), 0) if n else 0
+
+
+def _launch(device, what, fn, *args):
+    """one C call with `device` current (the library launches on the current device)"""
+    with torch.cuda.device(device):
+        rc = fn(*args)
+    _lib.check(rc, what)
 
 
 _workspaces = {}        # (device index, stream handle) -> workspace owned by this module (grown on demand)
 
 
 def _workspace(device, nbytes, stream, given, what):
-    """The workspace of one call: `given` if the caller passed one (ValueError when it is smaller than nbytes), else the
-    one this module keeps for (device, stream), allocated on that stream and used on no other.  A call that has to keep
-    its workspace past its return -- under stream capture, or a scan whose expand comes later -- must bring its own."""
+    """The workspace of one call: `given` if the caller passed one (_checked made sure it holds nbytes), else the one
+    this module keeps for (device, stream), allocated on that stream and used on no other.  A call that has to keep its
+    workspace past its return -- under stream capture, or a scan whose expand comes later -- must bring its own."""
     if given is not None:
-        _need_cuda(given)
-        if given.numel() < nbytes:
-            raise ValueError("%s: workspace of %d bytes, the call needs %d" % (what, given.numel(), nbytes))
         return given
     if torch.cuda.is_current_stream_capturing():
         raise ValueError("%s under stream capture needs its own workspace= (the graph would keep a cached one's "
@@ -49,47 +113,58 @@ def _workspace(device, nbytes, stream, given, what):
     return ws
 
 
-def _need_cuda(*ts):
-    for t in ts:
-        if t is not None and not t.is_cuda:
-            raise ValueError("device tensors required (got a CPU tensor)")
-
-
 def compress_bound(n):
     return int(_lib.load().LZ4_compressBound(int(n)))
 
 
-def _decode_outputs(lib, comp, offsets, sizes, out_bytes, per_block, cap, out, out_sizes, workspace, st, what):
-    """out, out_sizes and the workspace of a decode call: the ones given, else new ones on the launch stream (the
-    workspace is sized by LZ4B200_decompress_workspace_bytes_for(n, per_block, cap); see _workspace)"""
-    n = int(sizes.numel())
-    ws_bytes = int(lib.LZ4B200_decompress_workspace_bytes_for(n, int(per_block), int(cap)))
-    workspace = _workspace(comp.device, ws_bytes, st, workspace, what)
+def _decode_outputs(device, n, out_bytes, ws_bytes, out, out_sizes, workspace, st, what):
+    """out, out_sizes and the workspace of a decode call: the ones given, else new ones on the launch stream (see
+    _workspace)"""
+    workspace = _workspace(device, ws_bytes, st, workspace, what)
     with torch.cuda.stream(st):                     # temporaries belong to the stream the kernels run on
         if out is None:
-            out = torch.empty(out_bytes, dtype=torch.uint8, device=comp.device)
+            out = torch.empty(out_bytes, dtype=torch.uint8, device=device)
         if out_sizes is None:
-            out_sizes = torch.empty(n, dtype=torch.int32, device=comp.device)
-    assert offsets.dtype == torch.int64 and sizes.dtype == torch.int32 and comp.dtype == torch.uint8
+            out_sizes = torch.empty(n, dtype=torch.int32, device=device)
     return out, out_sizes, workspace
 
 
-def _compress_layout(src, block_size, room, slots, slot_stride, out_sizes, src_sizes, st):
-    """The blocks of a compress call: ceil(len(src) / block_size) of them, in slots of slot_stride bytes (default: room
-    rounded up to 16).  slots, out_sizes and, for a short last block, the per-block src_sizes are allocated on the launch
-    stream unless given.  Returns (n, stride, slots, out_sizes, src_sizes)."""
-    total = int(src.numel())
-    n = (total + block_size - 1) // block_size if total else 0
+def _decode_tensors(comp, offsets, sizes, n, out, out_bytes, out_sizes, workspace, ws_bytes):
+    """the tensors of a decode call as _checked takes them"""
+    return [("comp", comp, U8, ANY), ("offsets", offsets, I64, (n, None)), ("sizes", sizes, I32, ANY),
+            ("out", out, U8, (out_bytes, None)), ("out_sizes", out_sizes, I32, (n, None)),
+            ("workspace", workspace, U8, (ws_bytes, None))]
+
+
+def _block_count(src, block_size):
+    """ceil(len(src) / block_size): the blocks of a compress call (0 for a block_size _checked rejects)"""
+    total, bs = int(src.numel()) if isinstance(src, torch.Tensor) else 0, int(block_size)
+    return (total + bs - 1) // bs if total and bs > 0 else 0
+
+
+def _compress_layout(what, src, block_size, n, room, slots, slot_stride, out_sizes, src_sizes, stream, tensors=(),
+                     ints=()):
+    """The n blocks of a compress call, in slots of slot_stride bytes (default: room rounded up to 16) of which the
+    kernels write at most `room`.  Checks the call's arguments (_checked; tensors and ints: the call's own besides
+    these), then allocates slots, out_sizes and, for a short last block, the per-block src_sizes on the launch stream
+    unless given.  Returns (device, stream, stride, slots, out_sizes, src_sizes)."""
+    bs = int(block_size)
     stride = int(slot_stride if slot_stride is not None else ((room + 15) // 16) * 16)
+    device, st = _checked(what, stream,
+                          [("src", src, U8, ANY), ("slots", slots, U8, (_extent(n, stride, room), None)),
+                           ("out_sizes", out_sizes, I32, (n, None)), ("src_sizes", src_sizes, I32, (n, n))]
+                          + list(tensors), [("block_size", bs, 1, INT32_MAX)] + list(ints),
+                          [("slot_stride", stride, room)])
+    total = int(src.numel())
     with torch.cuda.stream(st):
         if slots is None:
-            slots = torch.empty(max(n, 1) * stride, dtype=torch.uint8, device=src.device)
+            slots = torch.empty(max(n, 1) * stride, dtype=torch.uint8, device=device)
         if out_sizes is None:
-            out_sizes = torch.empty(max(n, 1), dtype=torch.int32, device=src.device)
-        if src_sizes is None and n and total != n * block_size:
-            src_sizes = torch.full((n,), block_size, dtype=torch.int32, device=src.device)
-            src_sizes[-1] = total - (n - 1) * block_size
-    return n, stride, slots, out_sizes, src_sizes
+            out_sizes = torch.empty(max(n, 1), dtype=torch.int32, device=device)
+        if src_sizes is None and n and total != n * bs:
+            src_sizes = torch.full((n,), bs, dtype=torch.int32, device=device)
+            src_sizes[-1] = total - (n - 1) * bs
+    return device, st, stride, slots, out_sizes, src_sizes
 
 
 def decompress_blocks(comp, offsets, sizes, block_capacity, out=None, out_stride=None, out_sizes=None,
@@ -103,20 +178,22 @@ def decompress_blocks(comp, offsets, sizes, block_capacity, out=None, out_stride
     Returns (out, out_sizes) -- out_sizes[i] is LZ4_decompress_safe's return value.
     """
     lib = _lib.load()
-    _need_cuda(comp, offsets, sizes, out)
     if int(phases) in (1, 2) and workspace is None:
         raise ValueError("decompress_blocks: phases %d needs workspace= (the expand reads what the scan left there)"
                          % int(phases))
     n = int(sizes.numel())
-    stride = int(out_stride if out_stride is not None else block_capacity)
-    st = _stream(stream)
-    out, out_sizes, workspace = _decode_outputs(lib, comp, offsets, sizes, n * stride, 0, block_capacity, out, out_sizes,
-                                                workspace, st, "decompress_blocks")
-    rc = lib.LZ4B200_decompress_blocks_phased(comp.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), out.data_ptr(),
-                                              None, stride, None, int(block_capacity), out_sizes.data_ptr(), n,
-                                              workspace.data_ptr(), workspace.numel(), int(phases),
-                                              st.cuda_stream)
-    _lib.check(rc, "LZ4B200_decompress_blocks")
+    cap = int(block_capacity)
+    stride = int(out_stride if out_stride is not None else cap)
+    ws_bytes = int(lib.LZ4B200_decompress_workspace_bytes_for(n, 0, cap))
+    device, st = _checked("decompress_blocks", stream,
+                          _decode_tensors(comp, offsets, sizes, n, out, _extent(n, stride, cap), out_sizes, workspace,
+                                          ws_bytes),
+                          [_int32("block_capacity", cap)], [("out_stride", stride, cap)])
+    out, out_sizes, workspace = _decode_outputs(device, n, n * stride, ws_bytes, out, out_sizes, workspace, st,
+                                                "decompress_blocks")
+    _launch(device, "LZ4B200_decompress_blocks", lib.LZ4B200_decompress_blocks_phased, comp.data_ptr(),
+            offsets.data_ptr(), sizes.data_ptr(), out.data_ptr(), None, stride, None, cap, out_sizes.data_ptr(), n,
+            workspace.data_ptr(), workspace.numel(), int(phases), st.cuda_stream)
     return out, out_sizes
 
 
@@ -127,31 +204,35 @@ def decompress_blocks_partial(comp, offsets, sizes, target, out=None, out_stride
 
     target: one int for every block, or an int32 device tensor of per-block targets.  Block i is written to
     out[i*out_stride : i*out_stride + out_sizes[i]] (out_stride defaults to the largest target: with per-block targets
-    that reads target.max() on the host, so a captured call passes out_stride).
+    that reads target.max() on the host, so a captured call passes out_stride).  With per-block targets each block's
+    slot is out_stride bytes, so a given out holds len(sizes) * out_stride bytes and no target may exceed out_stride.
     Returns (out, out_sizes) -- out_sizes[i] is LZ4_decompress_safe_partial's return value.
     """
     lib = _lib.load()
     per_block = isinstance(target, torch.Tensor)
-    _need_cuda(comp, offsets, sizes, out, target if per_block else None)
     n = int(sizes.numel())
     if per_block:
-        assert target.dtype == torch.int32 and target.numel() == n
         uniform = 0
         if out_stride is None:
             if torch.cuda.is_current_stream_capturing():
                 raise ValueError("decompress_blocks_partial under stream capture with per-block targets needs out_stride")
-            biggest = int(target.max()) if n else 0
+            biggest = int(target.max()) if target.numel() else 0
     else:
         uniform = biggest = int(target)
     stride = int(out_stride if out_stride is not None else max(biggest, 0))
-    st = _stream(stream)
-    out, out_sizes, workspace = _decode_outputs(lib, comp, offsets, sizes, max(n * stride, 1), per_block, uniform, out,
-                                                out_sizes, workspace, st, "decompress_blocks_partial")
-    rc = lib.LZ4B200_decompress_blocks_partial(comp.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), out.data_ptr(),
-                                               None, stride, target.data_ptr() if per_block else None, uniform,
-                                               out_sizes.data_ptr(), n, workspace.data_ptr(), workspace.numel(),
-                                               st.cuda_stream)
-    _lib.check(rc, "LZ4B200_decompress_blocks_partial")
+    ws_bytes = int(lib.LZ4B200_decompress_workspace_bytes_for(n, int(per_block), uniform))
+    tensors = _decode_tensors(comp, offsets, sizes, n, out, n * stride if per_block else _extent(n, stride, uniform),
+                              out_sizes, workspace, ws_bytes)
+    if per_block:
+        tensors.append(("target", target, I32, (n, n)))
+    device, st = _checked("decompress_blocks_partial", stream, tensors, [_int32("target", uniform)],
+                          [("out_stride", stride, uniform)])
+    out, out_sizes, workspace = _decode_outputs(device, n, max(n * stride, 1), ws_bytes, out, out_sizes, workspace, st,
+                                                "decompress_blocks_partial")
+    _launch(device, "LZ4B200_decompress_blocks_partial", lib.LZ4B200_decompress_blocks_partial, comp.data_ptr(),
+            offsets.data_ptr(), sizes.data_ptr(), out.data_ptr(), None, stride,
+            target.data_ptr() if per_block else None, uniform, out_sizes.data_ptr(), n, workspace.data_ptr(),
+            workspace.numel(), st.cuda_stream)
     return out, out_sizes
 
 
@@ -198,31 +279,32 @@ def _decompress_frames(entry, mode_args, comp, offsets, sizes, capacities, max_b
                        consumed, workspace, stream):
     """the body of both frame calls: entry is the C function, mode_args what it takes after maxBlocks"""
     lib = _lib.load()
-    _need_cuda(comp, offsets, sizes, capacities, out, out_offsets, results, consumed)
-    assert comp.dtype == torch.uint8 and offsets.dtype == torch.int64 and sizes.dtype == torch.int64
-    assert capacities.dtype == torch.int64
     n = int(sizes.numel())
     budget = _budget(max_blocks)
-    st = _stream(stream)
     ws_bytes = int(lib.LZ4B200_decompress_frames_workspace_bytes(n, budget))
     if ws_bytes == 0:
         raise ValueError("decompress_frames: budgets must be 0 .. 2^31 - 1")
-    workspace = _workspace(comp.device, ws_bytes, st, workspace, "decompress_frames")
+    at_least_n = (n, None)
+    device, st = _checked("decompress_frames", stream,
+                          [("comp", comp, U8, ANY), ("offsets", offsets, I64, at_least_n), ("sizes", sizes, I64, ANY),
+                           ("capacities", capacities, I64, (n, n)), ("out", out, U8, ANY),
+                           ("out_offsets", out_offsets, I64, at_least_n), ("results", results, I64, at_least_n),
+                           ("consumed", consumed, I64, at_least_n), ("workspace", workspace, U8, (ws_bytes, None))])
+    workspace = _workspace(device, ws_bytes, st, workspace, "decompress_frames")
     with torch.cuda.stream(st):                     # temporaries belong to the stream the kernels run on
         if out_offsets is None:
             out_offsets = torch.cumsum(capacities, 0) - capacities
         if out is None:
             if torch.cuda.is_current_stream_capturing():
                 raise ValueError("decompress_frames under stream capture needs out=")
-            out = torch.empty(max(int(capacities.sum()) if n else 0, 1), dtype=torch.uint8, device=comp.device)
+            out = torch.empty(max(int(capacities.sum()) if n else 0, 1), dtype=torch.uint8, device=device)
         if results is None:
-            results = torch.empty(n, dtype=torch.int64, device=comp.device)
+            results = torch.empty(n, dtype=torch.int64, device=device)
         if consumed is None:
-            consumed = torch.empty(n, dtype=torch.int64, device=comp.device)
-    rc = getattr(lib, entry)(comp.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), out.data_ptr(),
-                             out_offsets.data_ptr(), capacities.data_ptr(), results.data_ptr(), consumed.data_ptr(), n,
-                             budget, *mode_args, workspace.data_ptr(), workspace.numel(), st.cuda_stream)
-    _lib.check(rc, entry)
+            consumed = torch.empty(n, dtype=torch.int64, device=device)
+    _launch(device, entry, getattr(lib, entry), comp.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), out.data_ptr(),
+            out_offsets.data_ptr(), capacities.data_ptr(), results.data_ptr(), consumed.data_ptr(), n, budget,
+            *mode_args, workspace.data_ptr(), workspace.numel(), st.cuda_stream)
     return out, results, consumed
 
 
@@ -236,17 +318,17 @@ def compress_blocks(src, block_size, acceleration=1, slots=None, slot_stride=Non
     Returns (slots, out_sizes, slot_stride): block i's bytes are slots[i*slot_stride : i*slot_stride+out_sizes[i]].
     """
     lib = _lib.load()
-    _need_cuda(src, slots)
-    cap = int(slot_capacity if slot_capacity is not None else compress_bound(block_size))
-    st = _stream(stream)
-    n, stride, slots, out_sizes, src_sizes = _compress_layout(src, block_size, cap, slots, slot_stride, out_sizes,
-                                                              src_sizes, st)
     if mode not in ("exact", "parallel"):
         raise ValueError("mode must be 'exact' or 'parallel'")
+    cap = int(slot_capacity if slot_capacity is not None else compress_bound(block_size))
+    n = _block_count(src, block_size)
+    device, st, stride, slots, out_sizes, src_sizes = _compress_layout(
+        "compress_blocks", src, block_size, n, cap, slots, slot_stride, out_sizes, src_sizes, stream,
+        ints=[_int32("slot_capacity", cap), _int32("acceleration", acceleration)])
     fn = lib.LZ4B200_compress_blocks if mode == "exact" else lib.LZ4B200_compress_blocks_parallel
-    rc = fn(src.data_ptr(), int(block_size), src_sizes.data_ptr() if src_sizes is not None else None,
-            int(block_size), slots.data_ptr(), stride, cap, int(acceleration), out_sizes.data_ptr(), n, st.cuda_stream)
-    _lib.check(rc, "LZ4B200_compress_blocks")
+    _launch(device, "LZ4B200_compress_blocks", fn, src.data_ptr(), int(block_size),
+            src_sizes.data_ptr() if src_sizes is not None else None, int(block_size), slots.data_ptr(), stride, cap,
+            int(acceleration), out_sizes.data_ptr(), n, st.cuda_stream)
     return slots, out_sizes[:n], stride
 
 
@@ -260,18 +342,25 @@ def compress_blocks_hc(src, block_size, level=9, slots=None, slot_stride=None, s
     Returns (slots, out_sizes, slot_stride): block i's bytes are slots[i*slot_stride : i*slot_stride+out_sizes[i]].
     """
     lib = _lib.load()
-    _need_cuda(src, slots)
     cap = int(slot_capacity if slot_capacity is not None else compress_bound(block_size))
-    st = _stream(stream)
-    n, stride, slots, out_sizes, src_sizes = _compress_layout(src, block_size, cap, slots, slot_stride, out_sizes, None, st)
-    workspace = _workspace(src.device, max(int(lib.LZ4B200_compress_blocks_hc_workspace_bytes(n)), 1), st, workspace,
-                           "compress_blocks_hc")
-    rc = lib.LZ4B200_compress_blocks_hc(src.data_ptr(), int(block_size),
-                                        src_sizes.data_ptr() if src_sizes is not None else None, int(block_size),
-                                        slots.data_ptr(), stride, cap, int(level), out_sizes.data_ptr(), n,
-                                        workspace.data_ptr(), workspace.numel(), st.cuda_stream)
-    _lib.check(rc, "LZ4B200_compress_blocks_hc")
+    n = _block_count(src, block_size)
+    ws_bytes = max(int(lib.LZ4B200_compress_blocks_hc_workspace_bytes(n)), 1)
+    device, st, stride, slots, out_sizes, src_sizes = _compress_layout(
+        "compress_blocks_hc", src, block_size, n, cap, slots, slot_stride, out_sizes, None, stream,
+        [("workspace", workspace, U8, (ws_bytes, None))], [_int32("slot_capacity", cap), _int32("level", level)])
+    workspace = _workspace(device, ws_bytes, st, workspace, "compress_blocks_hc")
+    _launch(device, "LZ4B200_compress_blocks_hc", lib.LZ4B200_compress_blocks_hc, src.data_ptr(), int(block_size),
+            src_sizes.data_ptr() if src_sizes is not None else None, int(block_size), slots.data_ptr(), stride, cap,
+            int(level), out_sizes.data_ptr(), n, workspace.data_ptr(), workspace.numel(), st.cuda_stream)
     return slots, out_sizes[:n], stride
+
+
+def _consumed(consumed, n, device, st):
+    """the consumed counts of a destSize call: the given ones, else new ones on the launch stream"""
+    if consumed is None:
+        with torch.cuda.stream(st):
+            consumed = torch.empty(max(n, 1), dtype=torch.int32, device=device)
+    return consumed
 
 
 def compress_blocks_dest_size(src, block_size, target, acceleration=1, slots=None, slot_stride=None, out_sizes=None,
@@ -283,19 +372,16 @@ def compress_blocks_dest_size(src, block_size, target, acceleration=1, slots=Non
     and hold its first consumed[i] input bytes.
     """
     lib = _lib.load()
-    _need_cuda(src, slots, src_sizes)
     room = max(min(int(target), compress_bound(block_size)), 1)
-    st = _stream(stream)
-    n, stride, slots, out_sizes, src_sizes = _compress_layout(src, block_size, room, slots, slot_stride, out_sizes,
-                                                              src_sizes, st)
-    if consumed is None:
-        with torch.cuda.stream(st):
-            consumed = torch.empty(max(n, 1), dtype=torch.int32, device=src.device)
-    rc = lib.LZ4B200_compress_blocks_destSize(src.data_ptr(), int(block_size),
-                                              src_sizes.data_ptr() if src_sizes is not None else None, int(block_size),
-                                              slots.data_ptr(), stride, int(target), int(acceleration),
-                                              out_sizes.data_ptr(), consumed.data_ptr(), n, st.cuda_stream)
-    _lib.check(rc, "LZ4B200_compress_blocks_destSize")
+    n = _block_count(src, block_size)
+    device, st, stride, slots, out_sizes, src_sizes = _compress_layout(
+        "compress_blocks_dest_size", src, block_size, n, room, slots, slot_stride, out_sizes, src_sizes, stream,
+        [("consumed", consumed, I32, (n, None))], [_int32("target", target), _int32("acceleration", acceleration)])
+    consumed = _consumed(consumed, n, device, st)
+    _launch(device, "LZ4B200_compress_blocks_destSize", lib.LZ4B200_compress_blocks_destSize, src.data_ptr(),
+            int(block_size), src_sizes.data_ptr() if src_sizes is not None else None, int(block_size),
+            slots.data_ptr(), stride, int(target), int(acceleration), out_sizes.data_ptr(), consumed.data_ptr(), n,
+            st.cuda_stream)
     return slots, out_sizes[:n], consumed[:n], stride
 
 
@@ -310,22 +396,19 @@ def compress_blocks_hc_dest_size(src, block_size, target, level=9, slots=None, s
     and hold its first consumed[i] input bytes.
     """
     lib = _lib.load()
-    _need_cuda(src, slots, src_sizes)
     room = max(min(int(target), compress_bound(block_size)), 1)
-    st = _stream(stream)
-    n, stride, slots, out_sizes, src_sizes = _compress_layout(src, block_size, room, slots, slot_stride, out_sizes,
-                                                              src_sizes, st)
-    if consumed is None:
-        with torch.cuda.stream(st):
-            consumed = torch.empty(max(n, 1), dtype=torch.int32, device=src.device)
-    workspace = _workspace(src.device, max(int(lib.LZ4B200_compress_blocks_hc_workspace_bytes(n)), 1), st, workspace,
-                           "compress_blocks_hc_dest_size")
-    rc = lib.LZ4B200_compress_blocks_hc_destSize(src.data_ptr(), int(block_size),
-                                                 src_sizes.data_ptr() if src_sizes is not None else None,
-                                                 int(block_size), slots.data_ptr(), stride, int(target), int(level),
-                                                 out_sizes.data_ptr(), consumed.data_ptr(), n, workspace.data_ptr(),
-                                                 workspace.numel(), st.cuda_stream)
-    _lib.check(rc, "LZ4B200_compress_blocks_hc_destSize")
+    n = _block_count(src, block_size)
+    ws_bytes = max(int(lib.LZ4B200_compress_blocks_hc_workspace_bytes(n)), 1)
+    device, st, stride, slots, out_sizes, src_sizes = _compress_layout(
+        "compress_blocks_hc_dest_size", src, block_size, n, room, slots, slot_stride, out_sizes, src_sizes, stream,
+        [("consumed", consumed, I32, (n, None)), ("workspace", workspace, U8, (ws_bytes, None))],
+        [_int32("target", target), _int32("level", level)])
+    consumed = _consumed(consumed, n, device, st)
+    workspace = _workspace(device, ws_bytes, st, workspace, "compress_blocks_hc_dest_size")
+    _launch(device, "LZ4B200_compress_blocks_hc_destSize", lib.LZ4B200_compress_blocks_hc_destSize, src.data_ptr(),
+            int(block_size), src_sizes.data_ptr() if src_sizes is not None else None, int(block_size),
+            slots.data_ptr(), stride, int(target), int(level), out_sizes.data_ptr(), consumed.data_ptr(), n,
+            workspace.data_ptr(), workspace.numel(), st.cuda_stream)
     return slots, out_sizes[:n], consumed[:n], stride
 
 
@@ -340,17 +423,17 @@ def compress_blocks_hc_opt(src, block_size, level=12, slots=None, slot_stride=No
     Returns (slots, out_sizes, slot_stride): block i's bytes are slots[i*slot_stride : i*slot_stride+out_sizes[i]].
     """
     lib = _lib.load()
-    _need_cuda(src, slots)
     cap = int(slot_capacity if slot_capacity is not None else compress_bound(block_size))
-    st = _stream(stream)
-    n, stride, slots, out_sizes, src_sizes = _compress_layout(src, block_size, cap, slots, slot_stride, out_sizes, None, st)
-    workspace = _workspace(src.device, max(int(lib.LZ4B200_compress_blocks_hc_opt_workspace_bytes(n)), 1), st, workspace,
-                           "compress_blocks_hc_opt")
-    rc = lib.LZ4B200_compress_blocks_hc_opt(src.data_ptr(), int(block_size),
-                                            src_sizes.data_ptr() if src_sizes is not None else None, int(block_size),
-                                            slots.data_ptr(), stride, cap, int(level), out_sizes.data_ptr(), n,
-                                            workspace.data_ptr(), workspace.numel(), st.cuda_stream)
-    _lib.check(rc, "LZ4B200_compress_blocks_hc_opt")
+    n = _block_count(src, block_size)
+    ws_bytes = max(int(lib.LZ4B200_compress_blocks_hc_opt_workspace_bytes(n)), 1)
+    device, st, stride, slots, out_sizes, src_sizes = _compress_layout(
+        "compress_blocks_hc_opt", src, block_size, n, cap, slots, slot_stride, out_sizes, None, stream,
+        [("workspace", workspace, U8, (ws_bytes, None))], [_int32("slot_capacity", cap), _int32("level", level)])
+    workspace = _workspace(device, ws_bytes, st, workspace, "compress_blocks_hc_opt")
+    _launch(device, "LZ4B200_compress_blocks_hc_opt", lib.LZ4B200_compress_blocks_hc_opt, src.data_ptr(),
+            int(block_size), src_sizes.data_ptr() if src_sizes is not None else None, int(block_size),
+            slots.data_ptr(), stride, cap, int(level), out_sizes.data_ptr(), n, workspace.data_ptr(), workspace.numel(),
+            st.cuda_stream)
     return slots, out_sizes[:n], stride
 
 
@@ -364,36 +447,37 @@ def compress_blocks_hc_opt_dest_size(src, block_size, target, level=12, slots=No
     and hold its first consumed[i] input bytes.
     """
     lib = _lib.load()
-    _need_cuda(src, slots, src_sizes)
     room = max(min(int(target), compress_bound(block_size)), 1)
-    st = _stream(stream)
-    n, stride, slots, out_sizes, src_sizes = _compress_layout(src, block_size, room, slots, slot_stride, out_sizes,
-                                                              src_sizes, st)
-    if consumed is None:
-        with torch.cuda.stream(st):
-            consumed = torch.empty(max(n, 1), dtype=torch.int32, device=src.device)
-    workspace = _workspace(src.device, max(int(lib.LZ4B200_compress_blocks_hc_opt_workspace_bytes(n)), 1), st, workspace,
-                           "compress_blocks_hc_opt_dest_size")
-    rc = lib.LZ4B200_compress_blocks_hc_opt_destSize(src.data_ptr(), int(block_size),
-                                                     src_sizes.data_ptr() if src_sizes is not None else None,
-                                                     int(block_size), slots.data_ptr(), stride, int(target), int(level),
-                                                     out_sizes.data_ptr(), consumed.data_ptr(), n, workspace.data_ptr(),
-                                                     workspace.numel(), st.cuda_stream)
-    _lib.check(rc, "LZ4B200_compress_blocks_hc_opt_destSize")
+    n = _block_count(src, block_size)
+    ws_bytes = max(int(lib.LZ4B200_compress_blocks_hc_opt_workspace_bytes(n)), 1)
+    device, st, stride, slots, out_sizes, src_sizes = _compress_layout(
+        "compress_blocks_hc_opt_dest_size", src, block_size, n, room, slots, slot_stride, out_sizes, src_sizes, stream,
+        [("consumed", consumed, I32, (n, None)), ("workspace", workspace, U8, (ws_bytes, None))],
+        [_int32("target", target), _int32("level", level)])
+    consumed = _consumed(consumed, n, device, st)
+    workspace = _workspace(device, ws_bytes, st, workspace, "compress_blocks_hc_opt_dest_size")
+    _launch(device, "LZ4B200_compress_blocks_hc_opt_destSize", lib.LZ4B200_compress_blocks_hc_opt_destSize,
+            src.data_ptr(), int(block_size), src_sizes.data_ptr() if src_sizes is not None else None, int(block_size),
+            slots.data_ptr(), stride, int(target), int(level), out_sizes.data_ptr(), consumed.data_ptr(), n,
+            workspace.data_ptr(), workspace.numel(), st.cuda_stream)
     return slots, out_sizes[:n], consumed[:n], stride
 
 
 def pack_blocks(slots, slot_stride, sizes, header_bytes=0, packed=None, stream=None):
-    """Gather variable-size blocks into one contiguous stream.  Returns (packed, offsets[n+1])."""
+    """Gather variable-size blocks into one contiguous stream.  Returns (packed, offsets[n+1]).
+
+    A given `packed` holds len(sizes) * (slot_stride + header_bytes) bytes: what the gather writes when every size fits
+    its slot (a larger size is the caller's responsibility)."""
     lib = _lib.load()
-    _need_cuda(slots, sizes)
     n = int(sizes.numel())
-    st = _stream(stream)
+    room = n * (int(slot_stride) + int(header_bytes))
+    device, st = _checked("pack_blocks", stream,
+                          [("slots", slots, U8, ANY), ("sizes", sizes, I32, ANY), ("packed", packed, U8, (room, None))],
+                          [_int32("header_bytes", header_bytes)], [("slot_stride", slot_stride, 0)])
     with torch.cuda.stream(st):
-        offsets = torch.empty(n + 1, dtype=torch.int64, device=slots.device)
+        offsets = torch.empty(n + 1, dtype=torch.int64, device=device)
         if packed is None:
-            packed = torch.empty(n * (int(slot_stride) + header_bytes) + 16, dtype=torch.uint8, device=slots.device)
-    rc = lib.LZ4B200_pack_blocks(slots.data_ptr(), int(slot_stride), sizes.data_ptr(), n, packed.data_ptr(),
-                                 offsets.data_ptr(), int(header_bytes), st.cuda_stream)
-    _lib.check(rc, "LZ4B200_pack_blocks")
+            packed = torch.empty(room + 16, dtype=torch.uint8, device=device)
+    _launch(device, "LZ4B200_pack_blocks", lib.LZ4B200_pack_blocks, slots.data_ptr(), int(slot_stride),
+            sizes.data_ptr(), n, packed.data_ptr(), offsets.data_ptr(), int(header_bytes), st.cuda_stream)
     return packed, offsets

@@ -6,6 +6,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
+from .block import _u8
 
 
 class Lz4FrameError(RuntimeError):
@@ -14,13 +15,6 @@ class Lz4FrameError(RuntimeError):
                  -5: "destination too small"}
         super().__init__("%s: %s (%d)" % (what, names.get(int(code), "error"), int(code)))
         self.code = int(code)
-
-
-def _u8(data):
-    if isinstance(data, np.ndarray):
-        assert data.dtype == np.uint8
-        return np.ascontiguousarray(data)
-    return np.frombuffer(bytes(data), dtype=np.uint8)
 
 
 def compress_frame(data, block_size_id=4, level=0, content_size=False):

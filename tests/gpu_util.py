@@ -1,5 +1,6 @@
-"""Helpers shared by the GPU parity tests: device-API decode calls that check what they may not touch, the decode
-route a call takes, and the hostile block corpus of the route tests."""
+"""Helpers shared by the GPU parity tests: a stand-in of the library that records the batch wrappers' calls, device-API
+decode calls that check what they may not touch, the decode route a call takes, and the hostile block corpus of the route
+tests."""
 import hashlib
 
 import numpy as np
@@ -26,6 +27,30 @@ def pack_host_blocks(blocks):
         offs[1:] = np.cumsum(sizes[:-1].astype(np.int64))
     buf = np.frombuffer(b"".join(blocks) + b"\x00" * 16, dtype=np.uint8).copy()
     return buf, offs, sizes
+
+
+class Recorder:
+    """liblz4_b200 as the lz4_b200.batch wrappers see it: the size functions are the library's own, every batch call is
+    recorded as (name, arguments), with the device current at the call in .devices, and returns 0 without touching the
+    device."""
+    SIZES = ("LZ4_compressBound", "LZ4B200_decompress_workspace_bytes_for", "LZ4B200_compress_blocks_hc_workspace_bytes",
+             "LZ4B200_compress_blocks_hc_opt_workspace_bytes", "LZ4B200_decompress_frames_workspace_bytes",
+             "LZ4B200_last_cuda_error")
+
+    def __init__(self, real):
+        self.real, self.calls, self.devices = real, [], []
+
+    def __getattr__(self, name):
+        if name in self.SIZES:
+            return getattr(self.real, name)
+        if not name.startswith("LZ4B200_"):
+            raise AttributeError(name)
+
+        def call(*args):
+            self.calls.append((name, args))
+            self.devices.append(torch.cuda.current_device())
+            return 0
+        return call
 
 
 # ------------------------------------------------------------------------------------------

@@ -9,32 +9,12 @@ wrappers allocate outputs with torch), so they run with the GPU suite."""
 import pytest
 import torch
 
+from gpu_util import Recorder
 from lz4_b200 import _lib, batch
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 BLOCK = 65536
-
-
-class Recorder:
-    """liblz4_b200 as the wrappers see it: the size functions are the library's own, every batch call is recorded as
-    (name, arguments) and returns 0 without touching the device."""
-    SIZES = ("LZ4_compressBound", "LZ4B200_decompress_workspace_bytes_for", "LZ4B200_compress_blocks_hc_workspace_bytes",
-             "LZ4B200_last_cuda_error")
-
-    def __init__(self, real):
-        self.real, self.calls = real, []
-
-    def __getattr__(self, name):
-        if name in self.SIZES:
-            return getattr(self.real, name)
-        if not name.startswith("LZ4B200_"):
-            raise AttributeError(name)
-
-        def call(*args):
-            self.calls.append((name, args))
-            return 0
-        return call
 
 
 # where each recorded call keeps its workspace pointer, its size and its stream (positions in the C prototypes)
