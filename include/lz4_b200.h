@@ -433,6 +433,51 @@ LZ4B200_API int LZ4B200_pack_blocks(const void* d_slots, int64_t slotStride, con
                                     void* d_packed, int64_t* d_outOff, int headerBytes, void* stream);
 
 /*
+ * Compress nBlocks buffers of any sizes at any places in device memory in one call (the tensors of a checkpoint, column
+ * chunks, KV-cache pages, message payloads), with the parse of one of the strided calls above:
+ *   block i input : d_src + d_srcOff[i], n_i = d_srcSize[i] bytes
+ *   block i output: d_dst + d_dstOff[i], capacity cap_i = d_dstCap[i]
+ *   d_outSize[i]  : what the matching one-block call returns, and its bytes:
+ *     LZ4B200_PARSE_FAST     LZ4_compress_fast(src_i, dst_i, n_i, cap_i, param)
+ *     LZ4B200_PARSE_PARALLEL the parallel parse of LZ4B200_compress_blocks_parallel for n_i <= 65 536, and
+ *                            LZ4_compress_fast(src_i, dst_i, n_i, cap_i, param) above, routed as that call routes them
+ *     LZ4B200_PARSE_HC       LZ4_compress_HC(src_i, dst_i, n_i, cap_i, param): levels up to 9 (below 1 reads as 9) by the
+ *                            hash-chain kernel of LZ4B200_compress_blocks_hc, 10 .. 12 (above 12 reads as 12) by the
+ *                            optimal parser of LZ4B200_compress_blocks_hc_opt
+ *   Sizes outside 0 .. LZ4_MAX_INPUT_SIZE, empty blocks and capacities of 0 or below give what those calls give.  Each
+ *   block's capacity alone decides between limited and unlimited output.
+ * Memory: nothing outside [dst_i, dst_i + cap_i) is written, so outputs may abut one another; they must not overlap one
+ * another or any source.  The readable padding is that of the strided call, per block: the 16-byte granules holding a
+ * block's first and last byte for PARSE_PARALLEL, the aligned 4-byte words holding its bytes for PARSE_HC.
+ * Workspace: none for PARSE_FAST and PARSE_PARALLEL (the size function returns 0 and d_workspace may be NULL); for
+ * PARSE_HC what LZ4B200_compress_blocks_hc_workspace_bytes or, at levels 10 and above,
+ * LZ4B200_compress_blocks_hc_opt_workspace_bytes asks for nBlocks.  LZ4B200_compress_blocks_indexed_workspace_bytes
+ * returns 0 for an unknown parse.
+ * Launches: one for PARSE_FAST and PARSE_HC, two for PARSE_PARALLEL (blocks up to 64 KB and above, as
+ * LZ4B200_compress_blocks_parallel with d_srcSize); nBlocks == 0 returns LZ4B200_OK without one.  The call does no host
+ * synchronisation and can be captured into a CUDA graph.  LZ4B200_ERR_ARG: nBlocks < 0, an unknown parse, a NULL
+ * d_srcOff, d_srcSize, d_dstOff, d_dstCap or d_outSize, a PARSE_HC call with a NULL d_workspace, then (with blocks
+ * present) a NULL d_src or d_dst, or a PARSE_HC workspace smaller than the size function asks.
+ */
+#define LZ4B200_PARSE_FAST      0   /* LZ4_compress_fast, byte for byte; param = acceleration (clamped as LZ4_compress_fast) */
+#define LZ4B200_PARSE_PARALLEL  1   /* the parallel parse of LZ4B200_compress_blocks_parallel; param = acceleration */
+#define LZ4B200_PARSE_HC        2   /* LZ4_compress_HC, byte for byte; param = level (< 1 -> 9, > 12 -> 12) */
+LZ4B200_API size_t LZ4B200_compress_blocks_indexed_workspace_bytes(int64_t nBlocks, int parse, int param);
+LZ4B200_API int LZ4B200_compress_blocks_indexed(const void* d_src, const int64_t* d_srcOff, const int32_t* d_srcSize,
+                                                void* d_dst, const int64_t* d_dstOff, const int32_t* d_dstCap,
+                                                int32_t* d_outSize, int64_t nBlocks, int parse, int param,
+                                                void* d_workspace, size_t workspaceBytes, void* stream);
+
+/*
+ * LZ4B200_pack_blocks with block i's slot at d_slots + d_slotOff[i] in place of d_slots + i*slotStride: the same
+ * d_outOff, headers, launches and argument rules, and LZ4B200_ERR_ARG for a NULL d_slotOff with blocks present.  It packs
+ * the output of LZ4B200_compress_blocks_indexed (d_slotOff = its d_dstOff, d_sizes = its d_outSize) into one stream.
+ */
+LZ4B200_API int LZ4B200_pack_blocks_indexed(const void* d_slots, const int64_t* d_slotOff, const int32_t* d_sizes,
+                                            int64_t nBlocks, void* d_packed, int64_t* d_outOff, int headerBytes,
+                                            void* stream);
+
+/*
  * The body of an LZ4 frame of independent blocks, assembled on the device (LZ4F_makeBlock, lz4frame.c:883-908):
  * for every block [LE32 header][payload]; a block whose compressed size d_sizes[i] is 0 (it did not fit size - 1) or
  * not smaller than its source is stored raw (payload = its source bytes from d_src + i*srcStride, bit 31 of the

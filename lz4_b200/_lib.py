@@ -57,6 +57,10 @@ PROTOTYPES = [
                                                           _vp, _sz, _vp]),
     ("LZ4B200_compress_blocks_parallel",C.c_int, [_vp, _i64, _vp, _i32, _vp, _i64, _i32, C.c_int, _vp, _i64, _vp]),
     ("LZ4B200_pack_blocks", C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, C.c_int, _vp]),
+    ("LZ4B200_compress_blocks_indexed_workspace_bytes", _sz, [_i64, C.c_int, C.c_int]),
+    ("LZ4B200_compress_blocks_indexed", C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, C.c_int, C.c_int, _vp, _sz,
+                                                  _vp]),
+    ("LZ4B200_pack_blocks_indexed", C.c_int, [_vp, _vp, _vp, _i64, _vp, _vp, C.c_int, _vp]),
     ("LZ4B200_pack_frame_blocks", C.c_int, [_vp, _i64, _vp, _vp, _i64, _i32, _i32, _i64, _vp, _vp, _vp]),
     ("LZ4B200_peer_copy_async", C.c_int, [_vp, C.c_int, _vp, C.c_size_t, _vp]),
     ("LZ4B200_decompress_blocks_host", C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _i64]),

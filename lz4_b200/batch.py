@@ -463,21 +463,94 @@ def compress_blocks_hc_opt_dest_size(src, block_size, target, level=12, slots=No
     return slots, out_sizes[:n], consumed[:n], stride
 
 
-def pack_blocks(slots, slot_stride, sizes, header_bytes=0, packed=None, stream=None):
+_PARSES = {"fast": 0, "parallel": 1, "hc": 2}     # LZ4B200_PARSE_FAST, _PARALLEL, _HC
+
+
+def compress_buffers(src, offsets, sizes, parse="fast", acceleration=1, level=9, out=None, out_offsets=None,
+                     capacities=None, out_sizes=None, workspace=None, stream=None):
+    """Compress len(sizes) buffers of any sizes at any offsets of src in one call (LZ4B200_compress_blocks_indexed).
+
+    src: u8 device buffer; buffer i = src[offsets[i] : offsets[i]+sizes[i]] (int64 / int32 device tensors).  Buffer i
+    is compressed to out[out_offsets[i] : out_offsets[i]+capacities[i]] (int64 / int32 device tensors), and
+    out_sizes[i] is what the one-block call returns for it:
+      parse "fast":     LZ4_compress_fast(buf_i, out_i, sizes[i], capacities[i], acceleration), byte for byte;
+      parse "parallel": the parallel parse of compress_blocks(mode="parallel") for buffers of up to 64 KB, "fast" above;
+      parse "hc":       LZ4_compress_HC(buf_i, out_i, sizes[i], capacities[i], level) at levels 1 .. 12, byte for byte.
+    capacities defaults to LZ4_compressBound(sizes), computed on the device; out_offsets to the exclusive sum of the
+    capacities (those below 0 count as 0), so the outputs abut; out to their total, which is read on the host, so a
+    captured call passes out.  Whether a given out holds what out_offsets and capacities place in it is the caller's
+    responsibility.  workspace: "hc" only, at least LZ4B200_compress_blocks_indexed_workspace_bytes(n, 2, level) bytes
+    (the module's rule above).  "parallel" reads the 16-byte granules around every buffer, "hc" the aligned 4-byte
+    words around it: that memory must be readable.
+    Returns (out, out_sizes, out_offsets, capacities).
+    """
+    lib = _lib.load()
+    if parse not in _PARSES:
+        raise ValueError("compress_buffers: parse must be 'fast', 'parallel' or 'hc' (got %r)" % (parse,))
+    hc = parse == "hc"
+    param = int(level) if hc else int(acceleration)
+    n = int(sizes.numel())
+    ws_bytes = max(int(lib.LZ4B200_compress_blocks_indexed_workspace_bytes(n, _PARSES[parse], param)), 1) if hc else 0
+    at_least_n = (n, None)
+    device, st = _checked("compress_buffers", stream,
+                          [("src", src, U8, ANY), ("offsets", offsets, I64, at_least_n), ("sizes", sizes, I32, ANY),
+                           ("out", out, U8, ANY), ("out_offsets", out_offsets, I64, at_least_n),
+                           ("capacities", capacities, I32, (n, n)), ("out_sizes", out_sizes, I32, at_least_n),
+                           ("workspace", workspace, U8, (ws_bytes, None))],
+                          [_int32("acceleration", acceleration), _int32("level", level)])
+    if hc:
+        workspace = _workspace(device, ws_bytes, st, workspace, "compress_buffers")
+    with torch.cuda.stream(st):                     # temporaries belong to the stream the kernels run on
+        if capacities is None:                      # LZ4_compressBound: 0 outside 0 .. LZ4_MAX_INPUT_SIZE
+            capacities = torch.where((sizes >= 0) & (sizes <= 0x7E000000), sizes + sizes // 255 + 16,
+                                     torch.zeros_like(sizes))
+        room = capacities.clamp(min=0).to(I64)
+        if out_offsets is None:
+            out_offsets = torch.cumsum(room, 0) - room
+        if out is None:
+            if torch.cuda.is_current_stream_capturing():
+                raise ValueError("compress_buffers under stream capture needs out=")
+            out = torch.empty(max(int(room.sum()) if n else 0, 1), dtype=torch.uint8, device=device)
+        if out_sizes is None:
+            out_sizes = torch.empty(max(n, 1), dtype=torch.int32, device=device)
+    _launch(device, "LZ4B200_compress_blocks_indexed", lib.LZ4B200_compress_blocks_indexed, src.data_ptr(),
+            offsets.data_ptr(), sizes.data_ptr(), out.data_ptr(), out_offsets.data_ptr(), capacities.data_ptr(),
+            out_sizes.data_ptr(), n, _PARSES[parse], param, workspace.data_ptr() if workspace is not None else None,
+            workspace.numel() if workspace is not None else 0, st.cuda_stream)
+    return out, out_sizes[:n], out_offsets, capacities
+
+
+def pack_blocks(slots, slot_stride, sizes, header_bytes=0, packed=None, stream=None, slot_offsets=None):
     """Gather variable-size blocks into one contiguous stream.  Returns (packed, offsets[n+1]).
 
     A given `packed` holds len(sizes) * (slot_stride + header_bytes) bytes: what the gather writes when every size fits
-    its slot (a larger size is the caller's responsibility)."""
+    its slot (a larger size is the caller's responsibility).
+    slot_offsets: an int64 device tensor: block i's slot is slots[slot_offsets[i]:] (LZ4B200_pack_blocks_indexed), as
+    compress_buffers leaves its outputs at out_offsets.  slot_stride may then be None: a given packed is not checked
+    against it, and a new one is sized by the exact total of the sizes, which is read on the host (a captured call
+    passes packed or slot_stride).  With slot_stride given, it bounds every block's size and sizes packed as above."""
     lib = _lib.load()
     n = int(sizes.numel())
-    room = n * (int(slot_stride) + int(header_bytes))
+    indexed = slot_offsets is not None
+    room = n * (int(slot_stride) + int(header_bytes)) if slot_stride is not None or not indexed else None
     device, st = _checked("pack_blocks", stream,
-                          [("slots", slots, U8, ANY), ("sizes", sizes, I32, ANY), ("packed", packed, U8, (room, None))],
-                          [_int32("header_bytes", header_bytes)], [("slot_stride", slot_stride, 0)])
+                          [("slots", slots, U8, ANY), ("sizes", sizes, I32, ANY),
+                           ("packed", packed, U8, (room or 0, None)), ("slot_offsets", slot_offsets, I64, (n, None))],
+                          [_int32("header_bytes", header_bytes)],
+                          [("slot_stride", slot_stride, 0)] if slot_stride is not None else [])
     with torch.cuda.stream(st):
         offsets = torch.empty(n + 1, dtype=torch.int64, device=device)
         if packed is None:
+            if room is None:
+                if torch.cuda.is_current_stream_capturing():
+                    raise ValueError("pack_blocks under stream capture with slot_offsets needs packed= or slot_stride")
+                room = (int(sizes.clamp(min=0).sum(dtype=I64)) if n else 0) + n * int(header_bytes)
             packed = torch.empty(room + 16, dtype=torch.uint8, device=device)
-    _launch(device, "LZ4B200_pack_blocks", lib.LZ4B200_pack_blocks, slots.data_ptr(), int(slot_stride),
-            sizes.data_ptr(), n, packed.data_ptr(), offsets.data_ptr(), int(header_bytes), st.cuda_stream)
+    if indexed:
+        _launch(device, "LZ4B200_pack_blocks_indexed", lib.LZ4B200_pack_blocks_indexed, slots.data_ptr(),
+                slot_offsets.data_ptr(), sizes.data_ptr(), n, packed.data_ptr(), offsets.data_ptr(), int(header_bytes),
+                st.cuda_stream)
+    else:
+        _launch(device, "LZ4B200_pack_blocks", lib.LZ4B200_pack_blocks, slots.data_ptr(), int(slot_stride),
+                sizes.data_ptr(), n, packed.data_ptr(), offsets.data_ptr(), int(header_bytes), st.cuda_stream)
     return packed, offsets

@@ -385,9 +385,9 @@ static lz4k_encode_args encode_args(const void* d_src, int64_t srcStride, const 
                                     int32_t* d_outSize, int64_t nBlocks)
 {
     lz4k_encode_args a;
-    a.src = (const uint8_t*)d_src; a.srcStride = srcStride; a.srcSizeArr = d_srcSize; a.srcSize = srcSize;
-    a.dst = (uint8_t*)d_dst; a.dstStride = dstStride; a.dstCap = dstCap; a.acceleration = acceleration;
-    a.outSize = d_outSize; a.nBlocks = nBlocks; a.minSize = INT32_MIN; a.maxSize = INT32_MAX;
+    a.src = (const uint8_t*)d_src; a.srcOff = NULL; a.srcStride = srcStride; a.srcSizeArr = d_srcSize; a.srcSize = srcSize;
+    a.dst = (uint8_t*)d_dst; a.dstOff = NULL; a.dstStride = dstStride; a.dstCapArr = NULL; a.dstCap = dstCap;
+    a.acceleration = acceleration; a.outSize = d_outSize; a.nBlocks = nBlocks; a.minSize = INT32_MIN; a.maxSize = INT32_MAX;
     return a;
 }
 
@@ -484,24 +484,57 @@ int LZ4B200_compress_blocks_destSize(const void* d_src, int64_t srcStride, const
     return launched(lz4k_launch_encode_dest(&a, d_srcConsumed, stream), "lz4k_launch_encode_dest");
 }
 
+/* the parallel parse stages a whole block in shared memory: blocks above 64 KB take the byte-identical encoder.  With
+ * per-block sizes each block goes by its own size (srcSize is not used): both kernels run, each on its blocks. */
+static int encode_parallel(lz4k_encode_args* a, void* stream)
+{
+    int rc;
+    if (!a->srcSizeArr && a->srcSize <= 65536) return launched(lz4k_launch_encode_par(a, stream), "lz4k_launch_encode_par");
+    if (!a->srcSizeArr) return launched(lz4k_launch_encode(a, stream), "lz4k_launch_encode");
+    a->maxSize = 65536;
+    if ((rc = launched(lz4k_launch_encode_par(a, stream), "lz4k_launch_encode_par")) != LZ4B200_OK) return rc;
+    a->minSize = 65537; a->maxSize = INT32_MAX;
+    return launched(lz4k_launch_encode(a, stream), "lz4k_launch_encode");
+}
+
 int LZ4B200_compress_blocks_parallel(const void* d_src, int64_t srcStride, const int32_t* d_srcSize, int32_t srcSize,
                                      void* d_dst, int64_t dstStride, int32_t dstCap, int acceleration,
                                      int32_t* d_outSize, int64_t nBlocks, void* stream)
 {
     lz4k_encode_args a;
-    int rc;
     if (nBlocks < 0) return LZ4B200_ERR_ARG;
     if (nBlocks == 0) return LZ4B200_OK;
     if (!d_dst || !d_outSize) return LZ4B200_ERR_ARG;
     a = encode_args(d_src, srcStride, d_srcSize, srcSize, d_dst, dstStride, dstCap, acceleration, d_outSize, nBlocks);
-    /* the parallel parse stages a whole block in shared memory: blocks above 64 KB take the byte-identical encoder.  With
-     * per-block sizes each block goes by its own size (srcSize is not used): both kernels run, each on its blocks. */
-    if (!d_srcSize && srcSize <= 65536) return launched(lz4k_launch_encode_par(&a, stream), "lz4k_launch_encode_par");
-    if (!d_srcSize) return launched(lz4k_launch_encode(&a, stream), "lz4k_launch_encode");
-    a.maxSize = 65536;
-    if ((rc = launched(lz4k_launch_encode_par(&a, stream), "lz4k_launch_encode_par")) != LZ4B200_OK) return rc;
-    a.minSize = 65537; a.maxSize = INT32_MAX;
-    return launched(lz4k_launch_encode(&a, stream), "lz4k_launch_encode");
+    return encode_parallel(&a, stream);
+}
+
+/* LZ4B200_compress_blocks_indexed's workspace: the HC or optimal-parser slots of its level, none for the other parses */
+size_t LZ4B200_compress_blocks_indexed_workspace_bytes(int64_t nBlocks, int parse, int param)
+{
+    if (parse != LZ4B200_PARSE_HC) return 0;
+    return param >= 10 ? lz4k_encode_hc_opt_workspace_bytes(nBlocks) : lz4k_encode_hc_workspace_bytes(nBlocks);
+}
+
+int LZ4B200_compress_blocks_indexed(const void* d_src, const int64_t* d_srcOff, const int32_t* d_srcSize,
+                                    void* d_dst, const int64_t* d_dstOff, const int32_t* d_dstCap,
+                                    int32_t* d_outSize, int64_t nBlocks, int parse, int param,
+                                    void* d_workspace, size_t workspaceBytes, void* stream)
+{
+    lz4k_encode_args a;
+    if (nBlocks < 0 || parse < LZ4B200_PARSE_FAST || parse > LZ4B200_PARSE_HC) return LZ4B200_ERR_ARG;
+    if (!d_srcOff || !d_srcSize || !d_dstOff || !d_dstCap || !d_outSize) return LZ4B200_ERR_ARG;
+    if (parse == LZ4B200_PARSE_HC && !d_workspace) return LZ4B200_ERR_ARG;
+    if (nBlocks == 0) return LZ4B200_OK;
+    if (!d_src || !d_dst) return LZ4B200_ERR_ARG;
+    if (workspaceBytes < LZ4B200_compress_blocks_indexed_workspace_bytes(nBlocks, parse, param)) return LZ4B200_ERR_ARG;
+    a = encode_args(d_src, 0, d_srcSize, 0, d_dst, 0, 0, parse == LZ4B200_PARSE_HC ? 0 : param, d_outSize, nBlocks);
+    a.srcOff = d_srcOff; a.dstOff = d_dstOff; a.dstCapArr = d_dstCap;
+    if (parse == LZ4B200_PARSE_FAST) return launched(lz4k_launch_encode(&a, stream), "lz4k_launch_encode");
+    if (parse == LZ4B200_PARSE_PARALLEL) return encode_parallel(&a, stream);
+    if (param >= 10)
+        return launched(lz4k_launch_encode_hc_opt(&a, param, d_workspace, workspaceBytes, stream), "lz4k_launch_encode_hc_opt");
+    return launched(lz4k_launch_encode_hc(&a, param, d_workspace, workspaceBytes, stream), "lz4k_launch_encode_hc");
 }
 
 int LZ4B200_pack_blocks(const void* d_slots, int64_t slotStride, const int32_t* d_sizes, int64_t nBlocks,
@@ -509,8 +542,17 @@ int LZ4B200_pack_blocks(const void* d_slots, int64_t slotStride, const int32_t* 
 {
     if (nBlocks < 0 || !d_outOff || (headerBytes != 0 && headerBytes != 4)) return LZ4B200_ERR_ARG;
     if (nBlocks > 0 && (!d_slots || !d_sizes || !d_packed)) return LZ4B200_ERR_ARG;
-    return launched(lz4k_launch_pack((const uint8_t*)d_slots, slotStride, d_sizes, nBlocks, (uint8_t*)d_packed, d_outOff,
-                                     headerBytes, stream), "lz4k_launch_pack");
+    return launched(lz4k_launch_pack((const uint8_t*)d_slots, NULL, slotStride, d_sizes, nBlocks, (uint8_t*)d_packed,
+                                     d_outOff, headerBytes, stream), "lz4k_launch_pack");
+}
+
+int LZ4B200_pack_blocks_indexed(const void* d_slots, const int64_t* d_slotOff, const int32_t* d_sizes, int64_t nBlocks,
+                                void* d_packed, int64_t* d_outOff, int headerBytes, void* stream)
+{
+    if (nBlocks < 0 || !d_outOff || (headerBytes != 0 && headerBytes != 4)) return LZ4B200_ERR_ARG;
+    if (nBlocks > 0 && (!d_slots || !d_slotOff || !d_sizes || !d_packed)) return LZ4B200_ERR_ARG;
+    return launched(lz4k_launch_pack((const uint8_t*)d_slots, d_slotOff, 0, d_sizes, nBlocks, (uint8_t*)d_packed,
+                                     d_outOff, headerBytes, stream), "lz4k_launch_pack");
 }
 
 int LZ4B200_pack_frame_blocks(const void* d_slots, int64_t slotStride, const int32_t* d_sizes, const void* d_src, int64_t srcStride,

@@ -53,7 +53,7 @@ struct HcOptDevAcc : HcDevAcc {
     __device__ __forceinline__ hc::Opt& opt(int r) const { return op[r]; }
 };
 
-/* One slot's blocks: t, t + slots, ...  FILL: LZ4_compress_HC_destSize with targetDstSize = a.dstCap, which also writes
+/* One slot's blocks: t, t + slots, ...  FILL: LZ4_compress_HC_destSize with targetDstSize = the block's capacity, which also writes
  * srcConsumed[b].  OPT: the optimal parser (levels 10 and up) on slots of kHcOptSlotBytes. */
 template <bool FILL, bool OPT = false>
 __device__ __forceinline__ void hc_slot_blocks(const lz4k_encode_args& a, int32_t* srcConsumed, uint8_t* ws, int64_t t,
@@ -66,8 +66,9 @@ __device__ __forceinline__ void hc_slot_blocks(const lz4k_encode_args& a, int32_
     if constexpr (OPT) acc.op = reinterpret_cast<hc::Opt*>(ws + t * slotBytes + kHcSlotBytes);
     for (int64_t b = t; b < a.nBlocks; b += slots) {
         const int n = a.srcSizeArr ? a.srcSizeArr[b] : a.srcSize;
-        acc.src = a.src + b * a.srcStride;
-        acc.dst = a.dst + b * a.dstStride;
+        const int cap = enc_cap(a, b);
+        acc.src = enc_src(a, b);
+        acc.dst = enc_dst(a, b);
         if (n >= hc::kMinLength && (uint32_t)n <= hc::kMaxInput) {         // shorter blocks never touch the tables
             uint4* h = reinterpret_cast<uint4*>(acc.ht);
             for (int k = 0; k < (int)(kHcHashBytes / sizeof(uint4)); k++) h[k] = make_uint4(0, 0, 0, 0);
@@ -75,17 +76,17 @@ __device__ __forceinline__ void hc_slot_blocks(const lz4k_encode_args& a, int32_
         if constexpr (OPT) {    /* the level 1 .. 9 kernels never see the optimal parser's text */
             if (FILL) {
                 int consumed;
-                a.outSize[b] = hc::hc_compress_block_opt_dest(acc, n, a.dstCap, level, consumed);
+                a.outSize[b] = hc::hc_compress_block_opt_dest(acc, n, cap, level, consumed);
                 srcConsumed[b] = consumed;
             } else {
-                a.outSize[b] = hc::hc_compress_block_opt(acc, n, a.dstCap, level);
+                a.outSize[b] = hc::hc_compress_block_opt(acc, n, cap, level);
             }
         } else if (FILL) {
             int consumed;
-            a.outSize[b] = hc::hc_compress_block_dest(acc, n, a.dstCap, level, consumed);
+            a.outSize[b] = hc::hc_compress_block_dest(acc, n, cap, level, consumed);
             srcConsumed[b] = consumed;
         } else {
-            a.outSize[b] = hc::hc_compress_block(acc, n, a.dstCap, level);
+            a.outSize[b] = hc::hc_compress_block(acc, n, cap, level);
         }
     }
 }

@@ -154,11 +154,11 @@ __global__ void __launch_bounds__(kEpThreads, 2) lz4_encode_par_kernel(lz4k_enco
 #endif
 
     for (int64_t b = blockIdx.x; b < a.nBlocks; b += gridDim.x) {
-        const uint8_t* gsrc = a.src + b * a.srcStride;
-        uint8_t* dst = a.dst + b * a.dstStride;
         const int n = a.srcSizeArr ? a.srcSizeArr[b] : a.srcSize;
-        const int64_t cap = a.dstCap;
         if (n < a.minSize || n > a.maxSize) continue;                 /* another launch's block */
+        const uint8_t* gsrc = enc_src(a, b);
+        uint8_t* dst = enc_dst(a, b);
+        const int64_t cap = enc_cap(a, b);
         if (n <= 0 || n > 65536) {                                    /* n == 0: one token byte (lz4.c:1361-1371); larger blocks are not this kernel's */
             if (tid == 0) { int r = 0; if (n == 0 && cap >= 1) { dst[0] = 0; r = 1; } a.outSize[b] = r; }
             continue;

@@ -1158,27 +1158,40 @@ tail:   /* lz4.c:1302-1329 */
 
 constexpr int kEncodeTableBytes = 16384;    // LZ4_HASHTABLESIZE, lz4.h:157-172 (LZ4_MEMORY_USAGE 14)
 
+/* Block b of an encode call: its source, its output and its capacity.  Every encoder addresses its blocks through these:
+ * strided (i * stride, one capacity) when the call has no tables, else from the offsets and capacities tables. */
+__device__ __forceinline__ const uint8_t* enc_src(const lz4k_encode_args& a, int64_t b)
+{
+    return a.src + (a.srcOff ? a.srcOff[b] : b * a.srcStride);
+}
+__device__ __forceinline__ uint8_t* enc_dst(const lz4k_encode_args& a, int64_t b)
+{
+    return a.dst + (a.dstOff ? a.dstOff[b] : b * a.dstStride);
+}
+__device__ __forceinline__ int enc_cap(const lz4k_encode_args& a, int64_t b) { return a.dstCapArr ? a.dstCapArr[b] : a.dstCap; }
+
 __global__ void __launch_bounds__(32) lz4_encode_kernel(lz4k_encode_args a)
 {
     extern __shared__ uint4 tableMem[];
     const int lane = threadIdx.x;
     uint32_t accel = a.acceleration < 1 ? 1u : (a.acceleration > kAccelMax ? (uint32_t)kAccelMax : (uint32_t)a.acceleration);  // lz4.c:1386-1387
     for (int64_t b = blockIdx.x; b < a.nBlocks; b += gridDim.x) {
-        const uint8_t* src = a.src + b * a.srcStride;
-        uint8_t* dst = a.dst + b * a.dstStride;
         const int n = a.srcSizeArr ? a.srcSizeArr[b] : a.srcSize;
         if (n < a.minSize || n > a.maxSize) continue;                   // another launch's block
+        const uint8_t* src = enc_src(a, b);
+        uint8_t* dst = enc_dst(a, b);
+        const int cap = enc_cap(a, b);                                  // notLimited or limitedOutput: this block's own
         int r;
         if ((uint32_t)n > kMaxInput) {                                  // lz4.c:1360
             r = 0;
         } else if (n == 0) {                                            // lz4.c:1361-1371
-            const bool limited = !(a.dstCap >= 16);
-            if (limited && a.dstCap <= 0) r = 0;
+            const bool limited = !(cap >= 16);
+            if (limited && cap <= 0) r = 0;
             else { if (lane == 0) dst[0] = 0; r = 1; }
         } else if (n < kSmallLimit) {                                   // lz4.c:1389
-            r = encode_block<true>(src, n, dst, a.dstCap, accel, tableMem, lane);
+            r = encode_block<true>(src, n, dst, cap, accel, tableMem, lane);
         } else {
-            r = encode_block<false>(src, n, dst, a.dstCap, accel, tableMem, lane);
+            r = encode_block<false>(src, n, dst, cap, accel, tableMem, lane);
         }
         if (lane == 0) a.outSize[b] = r;
         __syncwarp();
@@ -1196,14 +1209,14 @@ __global__ void __launch_bounds__(32) lz4_encode_dest_kernel(lz4k_encode_args a,
 {
     extern __shared__ uint4 tableMem[];
     const int lane = threadIdx.x;
-    const int target = a.dstCap;
     const uint32_t accel = a.acceleration < 1 ? 1u : (a.acceleration > kAccelMax ? (uint32_t)kAccelMax : (uint32_t)a.acceleration);  // lz4.c:1386-1387
     const uint32_t accelFill = a.acceleration < 1 ? 1u : (a.acceleration > kFillAccelMax ? (uint32_t)kFillAccelMax : (uint32_t)a.acceleration);
     for (int64_t b = blockIdx.x; b < a.nBlocks; b += gridDim.x) {
-        const uint8_t* src = a.src + b * a.srcStride;
-        uint8_t* dst = a.dst + b * a.dstStride;
         const int n = a.srcSizeArr ? a.srcSizeArr[b] : a.srcSize;
         if (n < a.minSize || n > a.maxSize) continue;                   // another launch's block
+        const uint8_t* src = enc_src(a, b);
+        uint8_t* dst = enc_dst(a, b);
+        const int target = enc_cap(a, b);
         const int bound = (uint32_t)n > kMaxInput ? 0 : n + n / 255 + 16;   // LZ4_compressBound
         uint32_t consumed = (uint32_t)n;
         int r;
@@ -1305,7 +1318,9 @@ __global__ void __launch_bounds__(1024) lz4_pack_scan_kernel(const int32_t* __re
     if (threadIdx.x == 0) outOff[n] = carry;
 }
 
-__global__ void __launch_bounds__(256) lz4_pack_gather_kernel(const uint8_t* __restrict__ slots, int64_t slotStride,
+/* block b's slot is slots + slotOff[b], or slots + b * slotStride without the table */
+__global__ void __launch_bounds__(256) lz4_pack_gather_kernel(const uint8_t* __restrict__ slots,
+                                                              const int64_t* __restrict__ slotOff, int64_t slotStride,
                                                               const int32_t* __restrict__ sizes, int64_t n,
                                                               uint8_t* __restrict__ packed, const int64_t* __restrict__ outOff,
                                                               int headerBytes, FrameRule fr)
@@ -1313,7 +1328,7 @@ __global__ void __launch_bounds__(256) lz4_pack_gather_kernel(const uint8_t* __r
     for (int64_t b = blockIdx.x; b < n; b += gridDim.x) {
         bool isRaw;
         const int s = pack_payload(fr, sizes, b, n, isRaw);
-        const uint8_t* from = isRaw ? fr.raw + b * fr.rawStride : slots + b * slotStride;
+        const uint8_t* from = isRaw ? fr.raw + b * fr.rawStride : slots + (slotOff ? slotOff[b] : b * slotStride);
         uint8_t* to = packed + outOff[b];
         const uint32_t hw = (uint32_t)s | (isRaw ? 0x80000000u : 0u);
         if (headerBytes == 4 && threadIdx.x < 4) to[threadIdx.x] = (uint8_t)(hw >> (8 * threadIdx.x));   // lz4frame.c:896-907 LE32
@@ -1524,15 +1539,16 @@ static int device_sms()
     return sms;
 }
 
-static int launch_pack(const uint8_t* slots, int64_t slotStride, const int32_t* sizes, int64_t nBlocks, uint8_t* packed,
-                       int64_t* outOff, int headerBytes, FrameRule fr, cudaStream_t s)
+static int launch_pack(const uint8_t* slots, const int64_t* slotOff, int64_t slotStride, const int32_t* sizes,
+                       int64_t nBlocks, uint8_t* packed, int64_t* outOff, int headerBytes, FrameRule fr, cudaStream_t s)
 {
     lz4_pack_scan_kernel<<<1, 1024, 0, s>>>(sizes, nBlocks, outOff, headerBytes, fr);
     g_launches++;
     if (nBlocks > 0) {
         const int64_t cap = (int64_t)device_sms() * 16;
         int64_t grid = nBlocks < cap ? nBlocks : cap;
-        lz4_pack_gather_kernel<<<(unsigned)grid, 256, 0, s>>>(slots, slotStride, sizes, nBlocks, packed, outOff, headerBytes, fr);
+        lz4_pack_gather_kernel<<<(unsigned)grid, 256, 0, s>>>(slots, slotOff, slotStride, sizes, nBlocks, packed, outOff,
+                                                              headerBytes, fr);
         g_launches++;
     }
     return (int)cudaGetLastError();
@@ -1837,11 +1853,11 @@ int lz4k_launch_encode_hc_opt_dest(const lz4k_encode_args* a, int32_t* srcConsum
     return (int)cudaGetLastError();
 }
 
-int lz4k_launch_pack(const uint8_t* slots, int64_t slotStride, const int32_t* sizes, int64_t nBlocks,
-                     uint8_t* packed, int64_t* outOff, int headerBytes, void* stream)
+int lz4k_launch_pack(const uint8_t* slots, const int64_t* slotOff, int64_t slotStride, const int32_t* sizes,
+                     int64_t nBlocks, uint8_t* packed, int64_t* outOff, int headerBytes, void* stream)
 {
     FrameRule fr; fr.raw = nullptr; fr.rawStride = 0; fr.blockSize = 0; fr.lastSize = 0;
-    return launch_pack(slots, slotStride, sizes, nBlocks, packed, outOff, headerBytes, fr, (cudaStream_t)stream);
+    return launch_pack(slots, slotOff, slotStride, sizes, nBlocks, packed, outOff, headerBytes, fr, (cudaStream_t)stream);
 }
 
 /* frame body: [LE32 header][payload] per block, stored-raw rule applied on the device (src = the blocks' source bytes) */
@@ -1849,7 +1865,7 @@ int lz4k_launch_pack_frame(const uint8_t* slots, int64_t slotStride, const int32
                            int32_t blockSize, int32_t lastSize, int64_t nBlocks, uint8_t* packed, int64_t* outOff, void* stream)
 {
     FrameRule fr; fr.raw = src; fr.rawStride = srcStride; fr.blockSize = blockSize; fr.lastSize = lastSize;
-    return launch_pack(slots, slotStride, sizes, nBlocks, packed, outOff, 4, fr, (cudaStream_t)stream);
+    return launch_pack(slots, nullptr, slotStride, sizes, nBlocks, packed, outOff, 4, fr, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -30,11 +30,14 @@ typedef struct {
 
 typedef struct {
     const uint8_t* src;
+    const int64_t* srcOff;     /* [n] or NULL -> i*srcStride */
     int64_t srcStride;
     const int32_t* srcSizeArr; /* [n] or NULL -> srcSize */
     int32_t srcSize;
     uint8_t* dst;
+    const int64_t* dstOff;     /* [n] or NULL -> i*dstStride */
     int64_t dstStride;
+    const int32_t* dstCapArr;  /* [n] or NULL -> dstCap */
     int32_t dstCap;
     int32_t acceleration;
     int32_t* outSize;
@@ -69,8 +72,9 @@ size_t lz4k_encode_hc_opt_workspace_bytes(int64_t nBlocks);
 int lz4k_launch_encode_hc_opt(const lz4k_encode_args* a, int level, void* workspace, size_t workspaceBytes, void* stream);
 int lz4k_launch_encode_hc_opt_dest(const lz4k_encode_args* a, int32_t* srcConsumed, int level, void* workspace,
                                    size_t workspaceBytes, void* stream);
-int lz4k_launch_pack(const uint8_t* slots, int64_t slotStride, const int32_t* sizes, int64_t nBlocks,
-                     uint8_t* packed, int64_t* outOff, int headerBytes, void* stream);
+/* block i's bytes are at slots + (slotOff ? slotOff[i] : i*slotStride) */
+int lz4k_launch_pack(const uint8_t* slots, const int64_t* slotOff, int64_t slotStride, const int32_t* sizes,
+                     int64_t nBlocks, uint8_t* packed, int64_t* outOff, int headerBytes, void* stream);
 /* the body of an LZ4 frame: [LE32 block header][payload] per block; blocks whose compression did not gain are stored raw */
 int lz4k_launch_pack_frame(const uint8_t* slots, int64_t slotStride, const int32_t* sizes, const uint8_t* src, int64_t srcStride,
                            int32_t blockSize, int32_t lastSize, int64_t nBlocks, uint8_t* packed, int64_t* outOff, void* stream);
