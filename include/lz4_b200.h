@@ -297,6 +297,55 @@ LZ4B200_API int LZ4B200_decompress_frames_checksummed(const void* d_src, const i
                                                       void* d_workspace, size_t workspaceBytes, void* stream);
 
 /*
+ * Write nFrames LZ4 frames from sources in device memory (the batched LZ4F_compressFrame, lz4frame.h:224 /
+ * lz4frame.c:425-498), at every compression level:
+ *   frame f input : d_src + d_srcOff[f], n_f = d_srcSize[f] bytes
+ *   frame f output: d_dst + d_dstOff[f], capacity d_dstCap[f]
+ *   d_result[f]   : in this order, LZ4B200_ERR_ARG (n_f < 0 or d_dstCap[f] < 0), LZ4B200_ERR_DSTSIZE (d_dstCap[f] below
+ *                   LZ4F_compressFrameBound(n_f, &prefs) at the frame's block size ID, 19 + 4 x blocks + n_f + 4: the
+ *                   reference's dstMaxSize_tooSmall), LZ4B200_ERR_LIMIT (below), else the frame's length
+ * With parallel == 0 frame f is, byte for byte, what LZ4F_compressFrame(dst_f, d_dstCap[f], src_f, n_f, &prefs) writes for
+ *   prefs = { frameInfo = { blockSizeID, LZ4F_blockIndependent, noContentChecksum, LZ4F_frame,
+ *                           contentSize = contentSizeFlag ? n_f : 0, dictID 0, noBlockChecksum },
+ *             compressionLevel, autoFlush 1, favorDecSpeed 0 }:
+ * the block size ID (0 means 4, else 4 .. 7) is shrunk per frame as LZ4F_optimalBSID does (lz4frame.c:362-373), so the
+ * frames of one call can fall in different classes; an empty frame has no content-size field (lz4frame.c:445-446); a
+ * block that does not compress into size - 1 bytes is stored raw (LZ4F_makeBlock, lz4frame.c:883-908).  Levels below 2
+ * use LZ4_compress_fast with acceleration -level + 1 for negative levels (below -65 536 as -65 536), 1 otherwise
+ * (lz4frame.c:911-921); levels 2 and up use LZ4_compress_HC_extStateHC_fastReset (lz4frame.c:931-937): 2 .. 9 through
+ * the hash-chain kernel of LZ4B200_compress_blocks_hc, 10 .. 12 (above 12 reads as 12) through the optimal parser.
+ * parallel != 0 (levels below 2 only; LZ4B200_ERR_ARG at the others): every block goes through LZ4B200_PARSE_PARALLEL,
+ * routed by size as LZ4B200_compress_blocks_indexed routes it, with capacity size - 1; the header, block headers,
+ * stored-raw rule, EndMark and results are as above.  The frame is valid and deterministic, not the reference's bytes.
+ *
+ * Memory: only [dst_f, dst_f + d_result[f]) is written, nothing for a failed frame; outputs may abut, and must not overlap
+ * one another, any source or the workspace.  Destinations are byte-aligned anywhere.  With parallel, the 16-byte granules
+ * holding the first and the last byte of every frame's source must be readable (the parse's readable padding); at levels
+ * 2 and up, the aligned 4-byte words holding its bytes.
+ *
+ * The budget: maxBlocks (a host array) bounds the blocks the call compresses from frames of block size ID 4 + c
+ * (maxBlocks[0 .. 3]: 64 KB, 256 KB, 1 MB, 4 MB blocks), the rule of LZ4B200_decompress_frames word for word: a frame
+ * gets LZ4B200_ERR_LIMIT when the blocks of the earlier frames of its class that passed the checks above, plus its own,
+ * exceed maxBlocks[c].  The host sizes everything from it, so the call never synchronises and can be captured into a
+ * CUDA graph.  The workspace (LZ4B200_compress_frames_workspace_bytes; 0 for arguments the call rejects) holds 48 bytes
+ * per frame, 48 per budgeted block, one slot of blockSize - 1 bytes rounded up to 16 per budgeted block -- about as much
+ * memory as the budgeted source -- and, at levels 2 and up, the workspace of LZ4B200_compress_blocks_hc (levels 2 .. 9)
+ * or LZ4B200_compress_blocks_hc_opt (10 and up) for the sum of maxBlocks.
+ *
+ * Kernel launches: 7 (8 with parallel); 5 when every maxBlocks[c] is 0.  nFrames == 0 returns LZ4B200_OK without one.
+ * LZ4B200_ERR_ARG: nFrames < 0, a NULL maxBlocks or an entry outside 0 .. 2^31 - 1, blockSizeID outside {0, 4 .. 7},
+ * parallel with compressionLevel >= 2, then (with frames present) a NULL pointer or a workspace smaller than the size
+ * function asks.
+ */
+LZ4B200_API size_t LZ4B200_compress_frames_workspace_bytes(int64_t nFrames, const int64_t maxBlocks[4], int compressionLevel);
+LZ4B200_API int LZ4B200_compress_frames(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
+                                        void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
+                                        int64_t* d_result, int64_t nFrames,
+                                        int blockSizeID, int compressionLevel, int contentSizeFlag, int parallel,
+                                        const int64_t maxBlocks[4],
+                                        void* d_workspace, size_t workspaceBytes, void* stream);
+
+/*
  * Compress nBlocks independent blocks (the batched LZ4_compress_fast; replaces bench.c:464-493 and
  * lz4frame.c:1046-1055).
  *   block i input : d_src + i*srcStride, size (d_srcSize ? d_srcSize[i] : srcSize)

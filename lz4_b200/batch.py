@@ -308,6 +308,86 @@ def _decompress_frames(entry, mode_args, comp, offsets, sizes, capacities, max_b
     return out, results, consumed
 
 
+def compress_frames_workspace_bytes(n_frames, max_blocks, level=0):
+    """LZ4B200_compress_frames_workspace_bytes: the workspace compress_frames needs (0: arguments it rejects)"""
+    return int(_lib.load().LZ4B200_compress_frames_workspace_bytes(int(n_frames), _budget(max_blocks), int(level)))
+
+
+def _frame_plan(sizes, block_size_id):
+    """(budget, capacities) for frames of these sizes: the blocks of each class, and LZ4B200_compressFrameBound per
+    frame at its optimal block size ID (which is at least the reference's bound).  Reads sizes on the host."""
+    bsid = int(block_size_id) or 4
+    budget, caps = [0, 0, 0, 0], []
+    for n in sizes.tolist():
+        b = 4
+        while b < bsid and n > 1 << (8 + 2 * b):
+            b += 1
+        bs = 1 << (8 + 2 * b)
+        if n >= 0:
+            budget[b - 4] += (n + bs - 1) // bs
+        caps.append(max(int(_lib.load().LZ4B200_compressFrameBound(max(n, 0), b)), 0))
+    return budget, caps
+
+
+def compress_frames(src, offsets, sizes, max_blocks=None, block_size_id=4, level=0, content_size=False, parallel=False,
+                    out=None, out_offsets=None, capacities=None, results=None, workspace=None, stream=None):
+    """Write len(sizes) LZ4 frames from buffers in device memory (LZ4B200_compress_frames): frame f is, byte for byte,
+    LZ4F_compressFrame of src[offsets[f] : offsets[f]+sizes[f]] with independent blocks, no checksums, the block size
+    ID block_size_id (0 or 4 .. 7, shrunk per frame as LZ4F_optimalBSID does), the content size when content_size, and
+    the compression level `level` (levels 2 and up through the HC encoders).  parallel: the parallel parse (levels
+    below 2 only): valid frames, not the reference's bytes.
+
+    offsets, sizes: int64 device tensors.  Frame f is written at out[out_offsets[f]:] with capacities[f] bytes of room
+    (int64 device tensors).  max_blocks: the blocks the call compresses at most from frames of each block size ID 4 .. 7
+    (4 host ints); a frame past its class's budget gets LZ4B200_ERR_LIMIT (-6).  Left as None, max_blocks and
+    capacities are computed from sizes read on the host (capacities: LZ4B200_compressFrameBound per frame), which is a
+    host sync: under stream capture max_blocks, out and capacities must be given.  out_offsets defaults to the
+    exclusive sum of the capacities and out to their total.
+    Returns (out, results): results[f] is the frame's length, or LZ4B200_ERR_ARG (a negative size or capacity),
+    LZ4B200_ERR_DSTSIZE (a capacity below the reference's bound) or LZ4B200_ERR_LIMIT.
+    """
+    lib = _lib.load()
+    n = int(sizes.numel()) if isinstance(sizes, torch.Tensor) else 0
+    capturing = torch.cuda.is_current_stream_capturing()
+    if capturing and (max_blocks is None or out is None or capacities is None):
+        raise ValueError("compress_frames under stream capture needs max_blocks=, out= and capacities= (computing them "
+                         "reads sizes on the host)")
+    at_least_n = (n, None)
+    device, st = _checked("compress_frames", stream,
+                          [("src", src, U8, ANY), ("offsets", offsets, I64, at_least_n), ("sizes", sizes, I64, ANY),
+                           ("out", out, U8, ANY), ("out_offsets", out_offsets, I64, at_least_n),
+                           ("capacities", capacities, I64, (n, n)), ("results", results, I64, at_least_n),
+                           ("workspace", workspace, U8, ANY)],
+                          [_int32("block_size_id", block_size_id), _int32("level", level)])
+    if int(block_size_id) not in (0, 4, 5, 6, 7):
+        raise ValueError("compress_frames: block_size_id must be 0 or 4 .. 7 (got %d)" % int(block_size_id))
+    if parallel and int(level) >= 2:
+        raise ValueError("compress_frames: parallel takes levels below 2 (got %d)" % int(level))
+    plan = _frame_plan(sizes, block_size_id) if max_blocks is None or capacities is None else None
+    budget = _budget(max_blocks if max_blocks is not None else plan[0])
+    ws_bytes = int(lib.LZ4B200_compress_frames_workspace_bytes(n, budget, int(level)))
+    if ws_bytes == 0:
+        raise ValueError("compress_frames: budgets must be 0 .. 2^31 - 1")
+    if workspace is not None and workspace.numel() < ws_bytes:
+        raise ValueError("compress_frames: workspace has %d elements, the call needs at least %d"
+                         % (workspace.numel(), ws_bytes))
+    workspace = _workspace(device, ws_bytes, st, workspace, "compress_frames")
+    with torch.cuda.stream(st):                     # temporaries belong to the stream the kernels run on
+        if capacities is None:
+            capacities = torch.tensor(plan[1], dtype=I64, device=device)
+        if out_offsets is None:
+            out_offsets = torch.cumsum(capacities.clamp(min=0), 0) - capacities.clamp(min=0)
+        if out is None:
+            out = torch.empty(max(int(capacities.clamp(min=0).sum()) if n else 0, 1), dtype=torch.uint8, device=device)
+        if results is None:
+            results = torch.empty(max(n, 1), dtype=torch.int64, device=device)
+    _launch(device, "LZ4B200_compress_frames", lib.LZ4B200_compress_frames, src.data_ptr(), offsets.data_ptr(),
+            sizes.data_ptr(), out.data_ptr(), out_offsets.data_ptr(), capacities.data_ptr(), results.data_ptr(), n,
+            int(block_size_id), int(level), 1 if content_size else 0, 1 if parallel else 0, budget,
+            workspace.data_ptr(), workspace.numel(), st.cuda_stream)
+    return out, results[:n]
+
+
 def compress_blocks(src, block_size, acceleration=1, slots=None, slot_stride=None, slot_capacity=None,
                     out_sizes=None, src_sizes=None, stream=None, mode="exact"):
     """Compress src (u8 device tensor) as ceil(len/block_size) independent blocks.

@@ -565,6 +565,111 @@ int LZ4B200_pack_frame_blocks(const void* d_slots, int64_t slotStride, const int
                     "lz4k_launch_pack_frame");
 }
 
+/* The workspace of LZ4B200_compress_frames, from the budget and the level alone: the frame records, the block table of
+ * every class (entries tabBase[c] .. tabBase[c] + maxBlocks[c] - 1: source offset, size, slot offset, capacity, result,
+ * the pack scan, the place), one slot of blockSize - 1 bytes rounded up to 16 per budgeted block, and for levels 2 and
+ * up the HC encoder's workspace for the whole table.  Regions start on 256 bytes, as in frames_plan. */
+typedef struct {
+    size_t frames, srcOff, srcSize, slotOff, cap, outSize, bodyOff, packOff, slots, hc, hcBytes, bytes;
+    int64_t tabBase[4], slotBase[4], slotStride[4], nEntries;
+} cframes_plan_t;
+
+/* 0 for arguments the call rejects (nFrames < 0, a NULL budget, an entry outside 0 .. FRAMES_MAX_BUDGET) */
+static int cframes_plan(int64_t nFrames, const int64_t* maxBlocks, int level, cframes_plan_t* p)
+{
+    size_t at = 0;
+    int64_t slotBytes = 0;
+    int c;
+    if (nFrames < 0 || !maxBlocks) return 0;
+    p->nEntries = 0;
+    for (c = 0; c < 4; c++) {
+        if (maxBlocks[c] < 0 || maxBlocks[c] > FRAMES_MAX_BUDGET) return 0;
+        p->tabBase[c] = p->nEntries;
+        p->nEntries += maxBlocks[c];
+        p->slotStride[c] = (fc_block_bytes(4 + c) - 1 + 15) & ~(int64_t)15;
+        p->slotBase[c] = slotBytes;
+        slotBytes += maxBlocks[c] * p->slotStride[c];
+    }
+    p->frames = at;  at = up256(at + (size_t)nFrames * sizeof(fc_frame_rec));
+    p->srcOff = at;  at = up256(at + (size_t)p->nEntries * sizeof(int64_t));
+    p->srcSize = at; at = up256(at + (size_t)p->nEntries * sizeof(int32_t));
+    p->slotOff = at; at = up256(at + (size_t)p->nEntries * sizeof(int64_t));
+    p->cap = at;     at = up256(at + (size_t)p->nEntries * sizeof(int32_t));
+    p->outSize = at; at = up256(at + (size_t)p->nEntries * sizeof(int32_t));
+    p->bodyOff = at; at = up256(at + (size_t)(p->nEntries + 1) * sizeof(int64_t));
+    p->packOff = at; at = up256(at + (size_t)p->nEntries * sizeof(int64_t));
+    p->slots = at;   at = up256(at + (size_t)slotBytes);
+    p->hcBytes = level < 2 ? 0 : level >= 10 ? lz4k_encode_hc_opt_workspace_bytes(p->nEntries)
+                                             : lz4k_encode_hc_workspace_bytes(p->nEntries);
+    p->hc = at;      at = up256(at + p->hcBytes);
+    p->bytes = at + 256;
+    return 1;
+}
+
+size_t LZ4B200_compress_frames_workspace_bytes(int64_t nFrames, const int64_t maxBlocks[4], int compressionLevel)
+{
+    cframes_plan_t p;
+    return cframes_plan(nFrames, maxBlocks, compressionLevel, &p) ? p.bytes : 0;
+}
+
+/* index (+ budget scan, fill) -> one encode of the whole table -> pack scan -> headers, places, EndMarks, results ->
+ * gather.  Every block is compressed into its slot with capacity size - 1, as LZ4F_makeBlock does (lz4frame.c:883-908). */
+int LZ4B200_compress_frames(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
+                            void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
+                            int64_t* d_result, int64_t nFrames,
+                            int blockSizeID, int compressionLevel, int contentSizeFlag, int parallel,
+                            const int64_t maxBlocks[4],
+                            void* d_workspace, size_t workspaceBytes, void* stream)
+{
+    cframes_plan_t p;
+    lz4k_cframes_args a;
+    lz4k_encode_args e;
+    uint8_t* ws;
+    int c, rc, accel;
+    if (!cframes_plan(nFrames, maxBlocks, compressionLevel, &p)) return LZ4B200_ERR_ARG;
+    if (blockSizeID == 0) blockSizeID = 4;
+    if (blockSizeID < 4 || blockSizeID > 7) return LZ4B200_ERR_ARG;
+    if (parallel && compressionLevel >= 2) return LZ4B200_ERR_ARG;
+    if (nFrames == 0) return LZ4B200_OK;
+    if (!d_src || !d_srcOff || !d_srcSize || !d_dst || !d_dstOff || !d_dstCap || !d_result || !d_workspace)
+        return LZ4B200_ERR_ARG;
+    if (workspaceBytes < p.bytes) return LZ4B200_ERR_ARG;
+    ws = (uint8_t*)(((uintptr_t)d_workspace + 255) & ~(uintptr_t)255);
+    memset(&a, 0, sizeof a);
+    a.src = (const uint8_t*)d_src; a.srcOff = d_srcOff; a.srcSize = d_srcSize;
+    a.dst = (uint8_t*)d_dst; a.dstOff = d_dstOff; a.dstCap = d_dstCap;
+    a.result = d_result; a.nFrames = nFrames;
+    for (c = 0; c < 4; c++) {
+        a.maxBlocks[c] = maxBlocks[c]; a.tabBase[c] = p.tabBase[c];
+        a.slotBase[c] = p.slotBase[c]; a.slotStride[c] = p.slotStride[c];
+    }
+    a.nEntries = p.nEntries;
+    a.bsid = blockSizeID;
+    a.contentSizeFlag = contentSizeFlag != 0;
+    a.frames = ws + p.frames;
+    a.slots = ws + p.slots;
+    a.tabSrcOff = (int64_t*)(ws + p.srcOff); a.tabSrcSize = (int32_t*)(ws + p.srcSize);
+    a.tabSlotOff = (int64_t*)(ws + p.slotOff); a.tabCap = (int32_t*)(ws + p.cap); a.tabOutSize = (int32_t*)(ws + p.outSize);
+    a.tabBodyOff = (int64_t*)(ws + p.bodyOff); a.tabPackOff = (int64_t*)(ws + p.packOff);
+
+    if ((rc = launched(lz4k_launch_cframes_index(&a, stream), "lz4k_launch_cframes_index")) != LZ4B200_OK) return rc;
+    /* lz4frame.c:911-921: acceleration -level + 1 below level 1 (LZ4_compress_fast clamps it to 65537; this also keeps
+     * -INT_MIN out), LZ4_compress_HC_extStateHC_fastReset from level 2 */
+    accel = compressionLevel >= 0 ? 1 : compressionLevel < -65536 ? 65537 : -compressionLevel + 1;
+    e = encode_args(d_src, 0, a.tabSrcSize, 0, a.slots, 0, 0, accel, a.tabOutSize, p.nEntries);
+    e.srcOff = a.tabSrcOff; e.dstOff = a.tabSlotOff; e.dstCapArr = a.tabCap;
+    if (compressionLevel >= 10)
+        rc = launched(lz4k_launch_encode_hc_opt(&e, compressionLevel, ws + p.hc, p.hcBytes, stream), "lz4k_launch_encode_hc_opt");
+    else if (compressionLevel >= 2)
+        rc = launched(lz4k_launch_encode_hc(&e, compressionLevel, ws + p.hc, p.hcBytes, stream), "lz4k_launch_encode_hc");
+    else if (parallel)
+        rc = encode_parallel(&e, stream);
+    else
+        rc = launched(lz4k_launch_encode(&e, stream), "lz4k_launch_encode");
+    if (rc != LZ4B200_OK) return rc;
+    return launched(lz4k_launch_cframes_assemble(&a, stream), "lz4k_launch_cframes_assemble");
+}
+
 /* ------------------------------------------------------------------------------------------ */
 /* host-buffer batch calls: H2D -> kernels -> D2H, N_PIPE chunks in flight                     */
 /* ------------------------------------------------------------------------------------------ */
@@ -917,19 +1022,6 @@ int LZ4_decompress_safe_usingDict(const char* src, char* dst, int compressedSize
 /* ------------------------------------------------------------------------------------------ */
 static void wr_le32(uint8_t* p, uint32_t v) { p[0] = (uint8_t)v; p[1] = (uint8_t)(v >> 8); p[2] = (uint8_t)(v >> 16); p[3] = (uint8_t)(v >> 24); }
 
-/* LZ4F_optimalBSID, lz4frame.c:362-373 */
-static int frame_optimal_bsid(int requested, int64_t srcSize)
-{
-    int proposed = 4;
-    int64_t maxBlock = 64 * 1024;
-    while (requested > proposed) {
-        if (srcSize <= maxBlock) return proposed;
-        proposed++;
-        maxBlock <<= 2;
-    }
-    return requested;
-}
-
 int64_t LZ4B200_compressFrameBound(int64_t srcSize, int blockSizeID)
 {
     int64_t bs, nBlocks;
@@ -954,17 +1046,9 @@ int64_t LZ4B200_compressFrame_host(const void* h_src, int64_t srcSize, void* h_d
     if (compressionLevel >= 2) return LZ4B200_ERR_UNSUPPORTED;          /* LZ4HC levels (lz4frame.c:952-962) */
     if (dstCapacity < LZ4B200_compressFrameBound(srcSize, blockSizeID)) return LZ4B200_ERR_DSTSIZE;
     accel = compressionLevel < 0 ? -compressionLevel + 1 : 1;           /* lz4frame.c:913 */
-    bsid = frame_optimal_bsid(blockSizeID, srcSize);                     /* lz4frame.c:447 */
+    bsid = fc_optimal_bsid(blockSizeID, srcSize);                        /* lz4frame.c:447 */
     bs = fc_block_bytes(bsid);
-    if (srcSize == 0) contentSizeFlag = 0;                               /* lz4frame.c:445: contentSize = srcSize = 0 -> no field */
-
-    /* frame header, lz4frame.c:781-809 */
-    wr_le32(dst, FC_MAGIC); op = 4;
-    dst[op++] = (uint8_t)((1u << 6) | (1u << 5) | ((contentSizeFlag ? 1u : 0u) << 3));   /* version 01, B.Indep */
-    dst[op++] = (uint8_t)((uint32_t)bsid << 4);
-    if (contentSizeFlag) { int i; for (i = 0; i < 8; i++) dst[op++] = (uint8_t)((uint64_t)srcSize >> (8 * i)); }
-    dst[op] = (uint8_t)(fc_xxh32(dst + 4, (uint64_t)(op - 4), 0) >> 8);
-    op++;
+    op = fc_frame_header_bytes(dst, bsid, contentSizeFlag ? srcSize : 0);   /* lz4frame.c:781-809 */
 
     nFull = srcSize / bs;
     lastSize = srcSize - nFull * bs;

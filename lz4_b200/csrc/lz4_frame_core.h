@@ -3,7 +3,9 @@
  * header checksum (LZ4F_decodeHeader, lz4frame.c:1340-1425), the chain of block headers with its checksum fields
  * (lz4frame.c:1729-1758) and the verdict on the decoded blocks and their checksums.  LZ4B200_decompressFrame_host (lz4_api.c, compiled as C99) and the batched frame decode
  * (lz4_kernels.cu, CUDA) both decide with these functions; tests/emul/frame_emul.cpp runs the batched call's index passes
- * on the host from the same text.  No CUDA runtime calls, no allocation.
+ * on the host from the same text.  The writing side -- optimal block size ID, bound, header bytes and the index passes of
+ * the batched frame encode -- serves LZ4B200_compressFrame_host and LZ4B200_compress_frames the same way
+ * (tests/emul/compress_frames_emul.cpp).  No CUDA runtime calls, no allocation.
  */
 #ifndef LZ4_FRAME_CORE_H
 #define LZ4_FRAME_CORE_H
@@ -74,6 +76,55 @@ FC_FN uint32_t fc_xxh32(const uint8_t* p, uint64_t len, uint32_t seed)
 }
 
 FC_FN int64_t fc_block_bytes(int bsid) { return (int64_t)1 << (8 + 2 * bsid); }   /* 4..7 -> 64 KB..4 MB (lz4frame.c:333-342) */
+
+/* ---------------------------------------------------------------------------------------------
+ * Writing a frame of independent blocks without checksums (LZ4F_compressFrame, lz4frame.c:425-498):
+ * LZ4B200_compressFrame_host and the batched LZ4B200_compress_frames take these rules from here.
+ * ------------------------------------------------------------------------------------------- */
+/* LZ4F_optimalBSID (lz4frame.c:362-373): the smallest block size ID from 4 up to `requested` (4 .. 7) whose blocks hold
+ * srcSize bytes */
+FC_FN int fc_optimal_bsid(int requested, int64_t srcSize)
+{
+    int proposed = 4;
+    int64_t maxBlock = 64 * 1024;
+    while (requested > proposed) {
+        if (srcSize <= maxBlock) return proposed;
+        proposed++;
+        maxBlock <<= 2;
+    }
+    return requested;
+}
+
+/* blocks of a frame of srcSize >= 0 bytes at block size ID bsid: the full ones and a last partial one */
+FC_FN int64_t fc_frame_blocks(int64_t srcSize, int bsid)
+{
+    const int64_t bs = fc_block_bytes(bsid);
+    return srcSize / bs + (srcSize % bs != 0);
+}
+
+/* LZ4F_compressFrameBound (lz4frame.c:406-417 with LZ4F_compressBound_internal, lz4frame.c:376-403) for autoFlush,
+ * independent blocks and no checksums, at the block size ID the frame is written with: the largest header (19 bytes),
+ * a 4-byte header per block, the source, the EndMark.  Saturates at INT64_MAX. */
+FC_FN int64_t fc_frame_bound(int64_t srcSize, int bsid)
+{
+    const int64_t extra = 19 + 4 * fc_frame_blocks(srcSize, bsid) + 4;
+    return srcSize > INT64_MAX - extra ? INT64_MAX : srcSize + extra;
+}
+
+/* The frame header (LZ4F_compressBegin, lz4frame.c:781-809) into h[0 .. 15): magic, FLG (version 01, independent
+ * blocks, the content-size bit), BD, the content size when contentSize > 0 (an empty frame has none, lz4frame.c:445-446),
+ * and the header checksum byte.  Returns its length, 7 or 15. */
+FC_FN int fc_frame_header_bytes(uint8_t* h, int bsid, int64_t contentSize)
+{
+    int n = 6, i;
+    const int withSize = contentSize > 0;
+    h[0] = (uint8_t)FC_MAGIC; h[1] = (uint8_t)(FC_MAGIC >> 8); h[2] = (uint8_t)(FC_MAGIC >> 16); h[3] = (uint8_t)(FC_MAGIC >> 24);
+    h[4] = (uint8_t)((1u << 6) | (1u << 5) | ((withSize ? 1u : 0u) << 3));
+    h[5] = (uint8_t)((uint32_t)bsid << 4);
+    if (withSize) for (i = 0; i < 8; i++) h[n++] = (uint8_t)((uint64_t)contentSize >> (8 * i));
+    h[n] = (uint8_t)(fc_xxh32(h + 4, (uint64_t)(n - 4), 0) >> 8);
+    return n + 1;
+}
 
 typedef struct {
     int64_t contentSize;       /* the header's content size, -1 without one (a field of 2^63 or more reads negative too) */
@@ -290,6 +341,50 @@ FC_FN void fc_verdict_frame(const fc_frame_rec* r, int64_t dstOff, int64_t dstCa
     if (res < 0)
         for (k = 0; k < r->count; k++) { t.outSize[r->base + k] = -1; t.rawLen[r->base + k] = -1; }
     *result = res;
+}
+
+/* ---------------------------------------------------------------------------------------------
+ * The batched frame encode (LZ4B200_compress_frames): the decode's frame record and budget scan (fc_scan_count,
+ * fc_place_frame), with a record that holds the frame's source size in contentSize, and one table of blocks per class.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct {               /* a class's block table; entry b of every array belongs to one block */
+    int64_t* srcOff;           /* absolute offset of the block's source bytes in the call's source */
+    int32_t* srcSize;          /* its size (0 for an unused entry) */
+    int64_t* slotOff;          /* offset of its slot in the call's workspace */
+    int32_t* cap;              /* size - 1: a block that does not compress into fewer bytes than it has is stored raw */
+} fc_cblock_tab;
+
+/* Pass 1 of the encode: the verdict on frame f's arguments and capacity, in LZ4F_compressFrame's order -- LZ4B200_ERR_ARG
+ * (a negative size or capacity), LZ4B200_ERR_DSTSIZE (dstCap below the reference's bound at the frame's optimal block
+ * size ID, dstMaxSize_tooSmall, lz4frame.c:451-452) -- and its class, block count and header length.  bsid: 4 .. 7. */
+FC_FN void fc_cindex_frame(int64_t srcSize, int64_t dstCap, int bsid, int contentSizeFlag, fc_frame_rec* r)
+{
+    int b;
+    r->count = 0; r->base = 0; r->contentSize = srcSize; r->consumed = 0; r->cls = -1; r->hdrLen = 0; r->sums = 0;
+    r->status = LZ4B200_OK;
+    if (srcSize < 0 || dstCap < 0) { r->status = LZ4B200_ERR_ARG; return; }
+    b = fc_optimal_bsid(bsid, srcSize);
+    if (dstCap < fc_frame_bound(srcSize, b)) { r->status = LZ4B200_ERR_DSTSIZE; return; }
+    r->cls = b - 4;
+    r->count = fc_frame_blocks(srcSize, b);
+    r->hdrLen = (contentSizeFlag && srcSize > 0) ? 15 : 7;
+}
+
+/* Pass 2 of the encode: a frame that passed writes its entries of its class's table (t: that class's).  srcOff: the
+ * frame's offset in the call's source; the class's slots are slotStride bytes apart from slotBase. */
+FC_FN void fc_cfill_frame(const fc_frame_rec* r, int64_t srcOff, int64_t slotBase, int64_t slotStride, fc_cblock_tab t)
+{
+    const int64_t bs = fc_block_bytes(r->cls + 4);
+    int64_t k;
+    if (r->status != LZ4B200_OK) return;
+    for (k = 0; k < r->count; k++) {
+        const int64_t b = r->base + k, left = r->contentSize - k * bs;
+        const int32_t sz = (int32_t)(left < bs ? left : bs);
+        t.srcOff[b] = srcOff + k * bs;
+        t.srcSize[b] = sz;
+        t.slotOff[b] = slotBase + b * slotStride;
+        t.cap[b] = sz - 1;
+    }
 }
 
 #endif /* LZ4_FRAME_CORE_H */

@@ -16,6 +16,7 @@
 #include <stdint.h>
 #include <stdlib.h>
 #include <stddef.h>
+#include <string.h>
 #include <atomic>
 #include <mutex>
 #include "lz4_kernels.h"
@@ -1249,14 +1250,18 @@ __global__ void __launch_bounds__(32) lz4_encode_dest_kernel(lz4k_encode_args a,
  * compression did not gain (size 0 = did not fit size-1, or >= its source size) is stored raw -- payload = the
  * source bytes, bit 31 of the LE32 block header set.
  * ============================================================================================= */
-struct FrameRule { const uint8_t* raw; int64_t rawStride; int32_t blockSize, lastSize; };     /* raw == nullptr: plain pack */
+struct FrameRule {             /* raw == nullptr: plain pack */
+    const uint8_t* raw; int64_t rawStride; int32_t blockSize, lastSize;
+    const int64_t* rawOff;     /* [n] or nullptr: block b's source is raw + rawOff[b], rawSize[b] bytes, in place of */
+    const int32_t* rawSize;    /* raw + b * rawStride, blockSize bytes (lastSize for the last) */
+};
 
 __device__ __forceinline__ int pack_payload(const FrameRule& fr, const int32_t* sizes, int64_t b, int64_t n, bool& isRaw)
 {
     const int c = sizes[b];
     isRaw = false;
     if (!fr.raw) return c > 0 ? c : 0;
-    const int sz = (b == n - 1 && fr.lastSize > 0) ? fr.lastSize : fr.blockSize;
+    const int sz = fr.rawSize ? fr.rawSize[b] : (b == n - 1 && fr.lastSize > 0) ? fr.lastSize : fr.blockSize;
     isRaw = (c <= 0 || c >= sz);                                /* lz4frame.c:896-899 */
     return isRaw ? sz : c;
 }
@@ -1318,18 +1323,23 @@ __global__ void __launch_bounds__(1024) lz4_pack_scan_kernel(const int32_t* __re
     if (threadIdx.x == 0) outOff[n] = carry;
 }
 
-/* block b's slot is slots + slotOff[b], or slots + b * slotStride without the table */
+/* block b's slot is slots + slotOff[b], or slots + b * slotStride without the table; it goes to packed + packOff[b] (a
+ * negative entry: nowhere), or packed + outOff[b] without the table */
 __global__ void __launch_bounds__(256) lz4_pack_gather_kernel(const uint8_t* __restrict__ slots,
                                                               const int64_t* __restrict__ slotOff, int64_t slotStride,
                                                               const int32_t* __restrict__ sizes, int64_t n,
                                                               uint8_t* __restrict__ packed, const int64_t* __restrict__ outOff,
-                                                              int headerBytes, FrameRule fr)
+                                                              const int64_t* __restrict__ packOff, int headerBytes,
+                                                              FrameRule fr)
 {
     for (int64_t b = blockIdx.x; b < n; b += gridDim.x) {
+        const int64_t at = packOff ? packOff[b] : outOff[b];
+        if (at < 0) continue;
         bool isRaw;
         const int s = pack_payload(fr, sizes, b, n, isRaw);
-        const uint8_t* from = isRaw ? fr.raw + b * fr.rawStride : slots + (slotOff ? slotOff[b] : b * slotStride);
-        uint8_t* to = packed + outOff[b];
+        const uint8_t* from = isRaw ? fr.raw + (fr.rawOff ? fr.rawOff[b] : b * fr.rawStride)
+                                    : slots + (slotOff ? slotOff[b] : b * slotStride);
+        uint8_t* to = packed + at;
         const uint32_t hw = (uint32_t)s | (isRaw ? 0x80000000u : 0u);
         if (headerBytes == 4 && threadIdx.x < 4) to[threadIdx.x] = (uint8_t)(hw >> (8 * threadIdx.x));   // lz4frame.c:896-907 LE32
         cta_copy(to + headerBytes, from, s);
@@ -1526,6 +1536,54 @@ __global__ void __launch_bounds__(128) lz4_frames_content_sum_kernel(lz4k_frames
         a.result[f] = LZ4B200_ERR_CHECKSUM;
 }
 
+/* =============================================================================================
+ * batched frame encode (LZ4B200_compress_frames): the frame rules of lz4_frame_core.h around one encode of the whole block
+ * table (by the caller) and the pack scan and gather
+ *   index : pass 1 -- one thread per frame: optimal block size ID, block count, header length, argument and capacity
+ *           verdicts; then the frame decode's budget scan (lz4_frames_scan_kernel) on the same records
+ *   fill  : pass 2 -- one thread per frame that passed: its table entries (source, size, slot, capacity size - 1)
+ *   finish: after the pack scan -- one thread per frame: the header, every block's place, the EndMark, the result; the
+ *           gather then writes every block header and payload to its place
+ * ============================================================================================= */
+__device__ __forceinline__ fc_cblock_tab cframes_tab(const lz4k_cframes_args& a, int cls)
+{
+    const int64_t t = a.tabBase[cls];
+    return fc_cblock_tab{a.tabSrcOff + t, a.tabSrcSize + t, a.tabSlotOff + t, a.tabCap + t};
+}
+
+__global__ void __launch_bounds__(128) lz4_cframes_index_kernel(lz4k_cframes_args a)
+{
+    const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= a.nFrames) return;
+    fc_cindex_frame(a.srcSize[f], a.dstCap[f], a.bsid, a.contentSizeFlag, static_cast<fc_frame_rec*>(a.frames) + f);
+}
+
+__global__ void __launch_bounds__(128) lz4_cframes_fill_kernel(lz4k_cframes_args a)
+{
+    const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= a.nFrames) return;
+    const fc_frame_rec* r = static_cast<const fc_frame_rec*>(a.frames) + f;
+    if (r->status != LZ4B200_OK) return;
+    fc_cfill_frame(r, a.srcOff[f], a.slotBase[r->cls], a.slotStride[r->cls], cframes_tab(a, r->cls));
+}
+
+__global__ void __launch_bounds__(128) lz4_cframes_finish_kernel(lz4k_cframes_args a)
+{
+    const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= a.nFrames) return;
+    const fc_frame_rec* r = static_cast<const fc_frame_rec*>(a.frames) + f;
+    if (r->status != LZ4B200_OK) { a.result[f] = r->status; return; }
+    const int64_t first = a.tabBase[r->cls] + r->base, body0 = a.tabBodyOff[first];
+    const int64_t at = a.dstOff[f] + r->hdrLen;
+    for (int64_t k = 0; k < r->count; k++) a.tabPackOff[first + k] = at + a.tabBodyOff[first + k] - body0;
+    const int64_t end = at + a.tabBodyOff[first + r->count] - body0;
+    uint8_t h[15];
+    const int hl = fc_frame_header_bytes(h, r->cls + 4, a.contentSizeFlag ? r->contentSize : 0);
+    for (int i = 0; i < hl; i++) a.dst[a.dstOff[f] + i] = h[i];
+    for (int i = 0; i < 4; i++) a.dst[end + i] = 0;                  /* EndMark, lz4frame.c:1222 */
+    a.result[f] = end + 4 - a.dstOff[f];
+}
+
 }  // namespace
 
 /* =============================================================================================
@@ -1539,18 +1597,25 @@ static int device_sms()
     return sms;
 }
 
+static void launch_pack_gather(const uint8_t* slots, const int64_t* slotOff, int64_t slotStride, const int32_t* sizes,
+                               int64_t nBlocks, uint8_t* packed, const int64_t* outOff, const int64_t* packOff,
+                               int headerBytes, FrameRule fr, cudaStream_t s)
+{
+    if (nBlocks > 0) {
+        const int64_t cap = (int64_t)device_sms() * 16;
+        int64_t grid = nBlocks < cap ? nBlocks : cap;
+        lz4_pack_gather_kernel<<<(unsigned)grid, 256, 0, s>>>(slots, slotOff, slotStride, sizes, nBlocks, packed, outOff,
+                                                              packOff, headerBytes, fr);
+        g_launches++;
+    }
+}
+
 static int launch_pack(const uint8_t* slots, const int64_t* slotOff, int64_t slotStride, const int32_t* sizes,
                        int64_t nBlocks, uint8_t* packed, int64_t* outOff, int headerBytes, FrameRule fr, cudaStream_t s)
 {
     lz4_pack_scan_kernel<<<1, 1024, 0, s>>>(sizes, nBlocks, outOff, headerBytes, fr);
     g_launches++;
-    if (nBlocks > 0) {
-        const int64_t cap = (int64_t)device_sms() * 16;
-        int64_t grid = nBlocks < cap ? nBlocks : cap;
-        lz4_pack_gather_kernel<<<(unsigned)grid, 256, 0, s>>>(slots, slotOff, slotStride, sizes, nBlocks, packed, outOff,
-                                                              headerBytes, fr);
-        g_launches++;
-    }
+    launch_pack_gather(slots, slotOff, slotStride, sizes, nBlocks, packed, outOff, nullptr, headerBytes, fr, s);
     return (int)cudaGetLastError();
 }
 
@@ -1574,6 +1639,43 @@ int lz4k_launch_frames_index(const lz4k_frames_args* a, void* stream)
     if (e != cudaSuccess) return (int)e;
     lz4_frames_fill_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);
     g_launches++;
+    return (int)cudaGetLastError();
+}
+
+/* the frame decode's budget scan on the encode's records */
+int lz4k_launch_cframes_index(const lz4k_cframes_args* a, void* stream)
+{
+    cudaStream_t s = (cudaStream_t)stream;
+    lz4k_frames_args fa;
+    memset(&fa, 0, sizeof fa);
+    fa.nFrames = a->nFrames;
+    fa.frames = a->frames;
+    for (int c = 0; c < 4; c++) fa.maxBlocks[c] = a->maxBlocks[c];
+    lz4_cframes_index_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);
+    lz4_frames_scan_kernel<<<1, kFsThreads, 0, s>>>(fa);
+    g_launches += 2;
+    /* unused entries compress nothing (size 0, capacity 0) and are written nowhere (place -1) */
+    const size_t n = (size_t)a->nEntries;
+    cudaError_t e = cudaMemsetAsync(a->tabSrcOff, 0, n * sizeof(int64_t), s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(a->tabSrcSize, 0, n * sizeof(int32_t), s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(a->tabSlotOff, 0, n * sizeof(int64_t), s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(a->tabCap, 0, n * sizeof(int32_t), s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(a->tabPackOff, 0xFF, n * sizeof(int64_t), s);
+    if (e != cudaSuccess) return (int)e;
+    lz4_cframes_fill_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);
+    g_launches++;
+    return (int)cudaGetLastError();
+}
+
+int lz4k_launch_cframes_assemble(const lz4k_cframes_args* a, void* stream)
+{
+    cudaStream_t s = (cudaStream_t)stream;
+    FrameRule fr;
+    fr.raw = a->src; fr.rawStride = 0; fr.blockSize = 0; fr.lastSize = 0; fr.rawOff = a->tabSrcOff; fr.rawSize = a->tabSrcSize;
+    lz4_pack_scan_kernel<<<1, 1024, 0, s>>>(a->tabOutSize, a->nEntries, a->tabBodyOff, 4, fr);
+    lz4_cframes_finish_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);
+    g_launches += 2;
+    launch_pack_gather(a->slots, a->tabSlotOff, 0, a->tabOutSize, a->nEntries, a->dst, a->tabBodyOff, a->tabPackOff, 4, fr, s);
     return (int)cudaGetLastError();
 }
 
@@ -1856,7 +1958,7 @@ int lz4k_launch_encode_hc_opt_dest(const lz4k_encode_args* a, int32_t* srcConsum
 int lz4k_launch_pack(const uint8_t* slots, const int64_t* slotOff, int64_t slotStride, const int32_t* sizes,
                      int64_t nBlocks, uint8_t* packed, int64_t* outOff, int headerBytes, void* stream)
 {
-    FrameRule fr; fr.raw = nullptr; fr.rawStride = 0; fr.blockSize = 0; fr.lastSize = 0;
+    FrameRule fr; fr.raw = nullptr; fr.rawStride = 0; fr.blockSize = 0; fr.lastSize = 0; fr.rawOff = nullptr; fr.rawSize = nullptr;
     return launch_pack(slots, slotOff, slotStride, sizes, nBlocks, packed, outOff, headerBytes, fr, (cudaStream_t)stream);
 }
 
@@ -1865,6 +1967,7 @@ int lz4k_launch_pack_frame(const uint8_t* slots, int64_t slotStride, const int32
                            int32_t blockSize, int32_t lastSize, int64_t nBlocks, uint8_t* packed, int64_t* outOff, void* stream)
 {
     FrameRule fr; fr.raw = src; fr.rawStride = srcStride; fr.blockSize = blockSize; fr.lastSize = lastSize;
+    fr.rawOff = nullptr; fr.rawSize = nullptr;
     return launch_pack(slots, nullptr, slotStride, sizes, nBlocks, packed, outOff, 4, fr, (cudaStream_t)stream);
 }
 

@@ -107,6 +107,34 @@ int lz4k_launch_frames_raw(const lz4k_frames_args* a, void* stream);
 int lz4k_launch_frames_block_sums(const lz4k_frames_args* a, void* stream);
 /* FC_SUMS_VERIFY: the content checksum of every frame that passed, after the raw blocks */
 int lz4k_launch_frames_content_sums(const lz4k_frames_args* a, void* stream);
+/* the batched frame encode's own steps (lz4_frame_core.h); the encode of the block table between them is the caller's */
+typedef struct {
+    const uint8_t* src;        /* frame f's source is src + srcOff[f], srcSize[f] bytes */
+    const int64_t* srcOff;
+    const int64_t* srcSize;
+    uint8_t* dst;              /* frame f is written at dst + dstOff[f], dstCap[f] bytes of room */
+    const int64_t* dstOff;
+    const int64_t* dstCap;
+    int64_t* result;           /* [nFrames] */
+    int64_t nFrames;
+    int64_t maxBlocks[4];      /* the budget of every class */
+    int64_t tabBase[4];        /* class c's entries of the block table start at tabBase[c] */
+    int64_t nEntries;          /* entries of the block table (sum of maxBlocks) */
+    int bsid;                  /* the requested block size ID, 4 .. 7 */
+    int contentSizeFlag;
+    void* frames;              /* fc_frame_rec[nFrames] */
+    uint8_t* slots;            /* block b is compressed to slots + tabSlotOff[b] */
+    int64_t slotBase[4];       /* class c's slots: slotBase[c] + k * slotStride[c] from `slots` */
+    int64_t slotStride[4];
+    int64_t* tabSrcOff; int32_t* tabSrcSize; int64_t* tabSlotOff; int32_t* tabCap; int32_t* tabOutSize;
+    int64_t* tabBodyOff;       /* [nEntries + 1]: the pack scan of 4 + payload over the table */
+    int64_t* tabPackOff;       /* where block b's header goes in dst, -1 for an unused entry */
+} lz4k_cframes_args;
+
+/* pass 1 (index), the budget scan of the frame decode, then the table cleared and filled (pass 2) */
+int lz4k_launch_cframes_index(const lz4k_cframes_args* a, void* stream);
+/* after the encode (tabOutSize): the pack scan, the frame headers, places, EndMarks and results, then the gather */
+int lz4k_launch_cframes_assemble(const lz4k_cframes_args* a, void* stream);
 uint64_t lz4k_launch_count(void);
 int lz4k_debug_poison_smem(uint32_t pattern, int lo, int hi, void* stream);   /* developer tool */
 int lz4k_launch_ceiling(const lz4k_decode_args* a, int mode, void* stream);   /* developer tool: skeleton of the rows kernel without the decode */
