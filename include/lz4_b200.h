@@ -284,10 +284,10 @@ LZ4B200_API int LZ4B200_decompress_frames(const void* d_src, const int64_t* d_sr
  * Reads: besides the readable padding of the frames, the content checksum reads each passing frame's decoded bytes in
  * aligned 16-byte granules, every one of which holds at least one byte of [dst_f, dst_f + d_result[f]).
  *
- * Cost: XXH32 is serial within each of its four lanes, so one thread hashes one block (the block checksums) and one
- * thread one frame's whole content (the content checksum).  The call is built for batches of many frames: a single large
- * frame's content checksum runs at one thread's speed (DESIGN section 3.11 has the measured rate), and skipChecksums is
- * the way around it.  Kernel launches: those of LZ4B200_decompress_frames, plus 2 when skipChecksums == 0.
+ * Cost: XXH32 is serial within each of its four lanes, so one thread hashes one block (the block checksums); a frame's
+ * content checksum is hashed by one thread when its content is shorter than 256 KiB and otherwise by a warp that stages the
+ * content through shared memory for the lane that hashes it (DESIGN sections 3.11 and 3.14 have the measured rates).
+ * Kernel launches: those of LZ4B200_decompress_frames, plus 2 when skipChecksums == 0.
  */
 #define LZ4B200_ERR_CHECKSUM (-7)   /* per-frame result: a block checksum or the content checksum does not match */
 LZ4B200_API int LZ4B200_decompress_frames_checksummed(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
@@ -344,6 +344,42 @@ LZ4B200_API int LZ4B200_compress_frames(const void* d_src, const int64_t* d_srcO
                                         int blockSizeID, int compressionLevel, int contentSizeFlag, int parallel,
                                         const int64_t maxBlocks[4],
                                         void* d_workspace, size_t workspaceBytes, void* stream);
+
+/*
+ * LZ4B200_compress_frames with XXH32 checksums -- the frames the reference `lz4` tool writes by default (a content
+ * checksum, programs/lz4io.c:223-227) and with --BX (block checksums).  The arguments, levels, parallel parse, budget,
+ * LZ4B200_ERR_LIMIT rule, workspace (LZ4B200_compress_frames_workspace_bytes) and argument errors are those of
+ * LZ4B200_compress_frames; the call never synchronises and can be captured into a CUDA graph.  A nonzero flag means on.
+ *
+ * With parallel == 0 frame f is, byte for byte, what LZ4F_compressFrame writes for the prefs of LZ4B200_compress_frames
+ * with blockChecksumFlag and contentChecksumFlag set as given:
+ *   - FLG bit 4 (block checksums) and bit 2 (content checksum) are set, and the header checksum byte follows from them;
+ *   - with block checksums, every block is followed by the LE32 XXH32(payload, 0) of its stored payload: the compressed
+ *     bytes, or a stored-raw block's source bytes (LZ4F_makeBlock, lz4frame.c:883-908);
+ *   - with a content checksum, the EndMark is followed by the LE32 XXH32(source, 0) (lz4frame.c:1225-1229); an empty
+ *     frame gets XXH32("", 0).
+ * d_result[f] is the frame's length, checksums included.  LZ4B200_ERR_DSTSIZE applies exactly below the reference's
+ * LZ4F_compressFrameBound for those prefs (lz4frame.c:376-417): 19 + (4 + 4 B) x blocks + n_f + 4 + 4 C, with B and C
+ * 1 when the flag is on.  With both flags 0 the call is LZ4B200_compress_frames: the same results, bytes and launches.
+ * With parallel != 0 the frames are valid, and their checksums are those of the bytes written.
+ *
+ * Memory: what LZ4B200_compress_frames writes and reads, and, with either flag on, the aligned 16-byte granules that
+ * hold a byte of a frame's source, which the checksums read whole (at levels below 2 without parallel this is a
+ * readable-padding rule the call without checksums does not have).  The block checksums hash a compressed payload in the
+ * workspace, where the encoder left it, and a stored-raw block's in the source; nothing reads the destination.
+ *
+ * Cost: one thread hashes each block; each frame's content is hashed by one thread when it is shorter than 256 KiB and by
+ * a warp that stages it through shared memory otherwise (DESIGN section 3.14 has the measured rates).  Kernel launches:
+ * those of LZ4B200_compress_frames, plus 1 with block checksums and 1 with a content checksum -- 7, 8 or 9 (8, 9 or 10
+ * with parallel; 5, 6 or 7 when every maxBlocks[c] is 0).
+ */
+LZ4B200_API int LZ4B200_compress_frames_checksummed(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
+                                                    void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
+                                                    int64_t* d_result, int64_t nFrames,
+                                                    int blockSizeID, int compressionLevel, int contentSizeFlag, int parallel,
+                                                    int blockChecksumFlag, int contentChecksumFlag,
+                                                    const int64_t maxBlocks[4],
+                                                    void* d_workspace, size_t workspaceBytes, void* stream);
 
 /*
  * Compress nBlocks independent blocks (the batched LZ4_compress_fast; replaces bench.c:464-493 and

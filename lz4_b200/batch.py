@@ -269,8 +269,9 @@ def decompress_frames_checksummed(comp, offsets, sizes, capacities, max_blocks, 
                                   out_offsets=None, results=None, consumed=None, workspace=None, stream=None):
     """decompress_frames for frames that may carry XXH32 block and content checksums
     (LZ4B200_decompress_frames_checksummed): same arguments, workspace and results, and a mismatching checksum gives
-    LZ4B200_ERR_CHECKSUM (-7).  skip_checksums: parse the checksum fields without comparing them.  One thread hashes a
-    frame's whole content, so the content check of a single large frame runs at one thread's speed."""
+    LZ4B200_ERR_CHECKSUM (-7).  skip_checksums: parse the checksum fields without comparing them.  A frame's content
+    checksum is hashed by one thread below 256 KiB of content and by a warp that stages the content through shared
+    memory from 256 KiB on."""
     return _decompress_frames("LZ4B200_decompress_frames_checksummed", (1 if skip_checksums else 0,), comp, offsets,
                               sizes, capacities, max_blocks, out, out_offsets, results, consumed, workspace, stream)
 
@@ -313,9 +314,10 @@ def compress_frames_workspace_bytes(n_frames, max_blocks, level=0):
     return int(_lib.load().LZ4B200_compress_frames_workspace_bytes(int(n_frames), _budget(max_blocks), int(level)))
 
 
-def _frame_plan(sizes, block_size_id):
+def _frame_plan(sizes, block_size_id, block_checksum=False, content_checksum=False):
     """(budget, capacities) for frames of these sizes: the blocks of each class, and LZ4B200_compressFrameBound per
-    frame at its optimal block size ID (which is at least the reference's bound).  Reads sizes on the host."""
+    frame at its optimal block size ID (which is at least the reference's bound), plus 4 bytes per block with block
+    checksums and 4 per frame with a content checksum.  Reads sizes on the host."""
     bsid = int(block_size_id) or 4
     budget, caps = [0, 0, 0, 0], []
     for n in sizes.tolist():
@@ -323,9 +325,11 @@ def _frame_plan(sizes, block_size_id):
         while b < bsid and n > 1 << (8 + 2 * b):
             b += 1
         bs = 1 << (8 + 2 * b)
+        k = (max(n, 0) + bs - 1) // bs
         if n >= 0:
-            budget[b - 4] += (n + bs - 1) // bs
-        caps.append(max(int(_lib.load().LZ4B200_compressFrameBound(max(n, 0), b)), 0))
+            budget[b - 4] += k
+        caps.append(max(int(_lib.load().LZ4B200_compressFrameBound(max(n, 0), b)), 0)
+                    + (4 * k if block_checksum else 0) + (4 if content_checksum else 0))
     return budget, caps
 
 
@@ -346,32 +350,54 @@ def compress_frames(src, offsets, sizes, max_blocks=None, block_size_id=4, level
     Returns (out, results): results[f] is the frame's length, or LZ4B200_ERR_ARG (a negative size or capacity),
     LZ4B200_ERR_DSTSIZE (a capacity below the reference's bound) or LZ4B200_ERR_LIMIT.
     """
+    return _compress_frames("compress_frames", None, src, offsets, sizes, max_blocks, block_size_id, level,
+                            content_size, parallel, out, out_offsets, capacities, results, workspace, stream)
+
+
+def compress_frames_checksummed(src, offsets, sizes, max_blocks=None, block_size_id=4, level=0, content_size=False,
+                                parallel=False, block_checksum=False, content_checksum=True, out=None, out_offsets=None,
+                                capacities=None, results=None, workspace=None, stream=None):
+    """compress_frames with XXH32 checksums (LZ4B200_compress_frames_checksummed): block_checksum puts the LE32
+    XXH32(payload, 0) after every block, content_checksum the LE32 XXH32(source, 0) after the EndMark, as
+    LZ4F_compressFrame does with blockChecksumFlag and contentChecksumFlag.  The defaults are the `lz4` tool's: a content
+    checksum, no block checksums.  Same arguments, capture rules and results as compress_frames; the default capacities
+    are its bound plus 4 bytes per block with block checksums and 4 per frame with a content checksum, the reference's
+    LZ4F_compressFrameBound for those flags."""
+    return _compress_frames("compress_frames_checksummed", (1 if block_checksum else 0, 1 if content_checksum else 0),
+                            src, offsets, sizes, max_blocks, block_size_id, level, content_size, parallel, out,
+                            out_offsets, capacities, results, workspace, stream)
+
+
+def _compress_frames(name, sums, src, offsets, sizes, max_blocks, block_size_id, level, content_size, parallel, out,
+                     out_offsets, capacities, results, workspace, stream):
+    """the body of compress_frames (sums None) and compress_frames_checksummed (sums: the two flags)"""
     lib = _lib.load()
     n = int(sizes.numel()) if isinstance(sizes, torch.Tensor) else 0
     capturing = torch.cuda.is_current_stream_capturing()
     if capturing and (max_blocks is None or out is None or capacities is None):
-        raise ValueError("compress_frames under stream capture needs max_blocks=, out= and capacities= (computing them "
-                         "reads sizes on the host)")
+        raise ValueError("%s under stream capture needs max_blocks=, out= and capacities= (computing them "
+                         "reads sizes on the host)" % name)
     at_least_n = (n, None)
-    device, st = _checked("compress_frames", stream,
+    device, st = _checked(name, stream,
                           [("src", src, U8, ANY), ("offsets", offsets, I64, at_least_n), ("sizes", sizes, I64, ANY),
                            ("out", out, U8, ANY), ("out_offsets", out_offsets, I64, at_least_n),
                            ("capacities", capacities, I64, (n, n)), ("results", results, I64, at_least_n),
                            ("workspace", workspace, U8, ANY)],
                           [_int32("block_size_id", block_size_id), _int32("level", level)])
     if int(block_size_id) not in (0, 4, 5, 6, 7):
-        raise ValueError("compress_frames: block_size_id must be 0 or 4 .. 7 (got %d)" % int(block_size_id))
+        raise ValueError("%s: block_size_id must be 0 or 4 .. 7 (got %d)" % (name, int(block_size_id)))
     if parallel and int(level) >= 2:
-        raise ValueError("compress_frames: parallel takes levels below 2 (got %d)" % int(level))
-    plan = _frame_plan(sizes, block_size_id) if max_blocks is None or capacities is None else None
+        raise ValueError("%s: parallel takes levels below 2 (got %d)" % (name, int(level)))
+    plan = (_frame_plan(sizes, block_size_id, *(bool(x) for x in (sums or (0, 0))))
+            if max_blocks is None or capacities is None else None)
     budget = _budget(max_blocks if max_blocks is not None else plan[0])
     ws_bytes = int(lib.LZ4B200_compress_frames_workspace_bytes(n, budget, int(level)))
     if ws_bytes == 0:
-        raise ValueError("compress_frames: budgets must be 0 .. 2^31 - 1")
+        raise ValueError("%s: budgets must be 0 .. 2^31 - 1" % name)
     if workspace is not None and workspace.numel() < ws_bytes:
-        raise ValueError("compress_frames: workspace has %d elements, the call needs at least %d"
-                         % (workspace.numel(), ws_bytes))
-    workspace = _workspace(device, ws_bytes, st, workspace, "compress_frames")
+        raise ValueError("%s: workspace has %d elements, the call needs at least %d"
+                         % (name, workspace.numel(), ws_bytes))
+    workspace = _workspace(device, ws_bytes, st, workspace, name)
     with torch.cuda.stream(st):                     # temporaries belong to the stream the kernels run on
         if capacities is None:
             capacities = torch.tensor(plan[1], dtype=I64, device=device)
@@ -381,10 +407,11 @@ def compress_frames(src, offsets, sizes, max_blocks=None, block_size_id=4, level
             out = torch.empty(max(int(capacities.clamp(min=0).sum()) if n else 0, 1), dtype=torch.uint8, device=device)
         if results is None:
             results = torch.empty(max(n, 1), dtype=torch.int64, device=device)
-    _launch(device, "LZ4B200_compress_frames", lib.LZ4B200_compress_frames, src.data_ptr(), offsets.data_ptr(),
-            sizes.data_ptr(), out.data_ptr(), out_offsets.data_ptr(), capacities.data_ptr(), results.data_ptr(), n,
-            int(block_size_id), int(level), 1 if content_size else 0, 1 if parallel else 0, budget,
-            workspace.data_ptr(), workspace.numel(), st.cuda_stream)
+    entry = "LZ4B200_" + name
+    _launch(device, entry, getattr(lib, entry), src.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), out.data_ptr(),
+            out_offsets.data_ptr(), capacities.data_ptr(), results.data_ptr(), n, int(block_size_id), int(level),
+            1 if content_size else 0, 1 if parallel else 0, *(sums or ()), budget, workspace.data_ptr(),
+            workspace.numel(), st.cuda_stream)
     return out, results[:n]
 
 

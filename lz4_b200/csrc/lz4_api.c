@@ -613,13 +613,15 @@ size_t LZ4B200_compress_frames_workspace_bytes(int64_t nFrames, const int64_t ma
 }
 
 /* index (+ budget scan, fill) -> one encode of the whole table -> pack scan -> headers, places, EndMarks, results ->
- * gather.  Every block is compressed into its slot with capacity size - 1, as LZ4F_makeBlock does (lz4frame.c:883-908). */
-int LZ4B200_compress_frames(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
-                            void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
-                            int64_t* d_result, int64_t nFrames,
-                            int blockSizeID, int compressionLevel, int contentSizeFlag, int parallel,
-                            const int64_t maxBlocks[4],
-                            void* d_workspace, size_t workspaceBytes, void* stream)
+ * gather -> [block checksums] -> [content checksums].  Every block is compressed into its slot with capacity size - 1,
+ * as LZ4F_makeBlock does (lz4frame.c:883-908).  sums: FC_BLOCK_SUM | FC_CONTENT_SUM; the bracketed steps run for the
+ * checksums the frames carry. */
+static int compress_frames_sums(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
+                                void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
+                                int64_t* d_result, int64_t nFrames,
+                                int blockSizeID, int compressionLevel, int contentSizeFlag, int parallel, int sums,
+                                const int64_t maxBlocks[4],
+                                void* d_workspace, size_t workspaceBytes, void* stream)
 {
     cframes_plan_t p;
     lz4k_cframes_args a;
@@ -646,6 +648,7 @@ int LZ4B200_compress_frames(const void* d_src, const int64_t* d_srcOff, const in
     a.nEntries = p.nEntries;
     a.bsid = blockSizeID;
     a.contentSizeFlag = contentSizeFlag != 0;
+    a.sums = sums;
     a.frames = ws + p.frames;
     a.slots = ws + p.slots;
     a.tabSrcOff = (int64_t*)(ws + p.srcOff); a.tabSrcSize = (int32_t*)(ws + p.srcSize);
@@ -667,7 +670,38 @@ int LZ4B200_compress_frames(const void* d_src, const int64_t* d_srcOff, const in
     else
         rc = launched(lz4k_launch_encode(&e, stream), "lz4k_launch_encode");
     if (rc != LZ4B200_OK) return rc;
-    return launched(lz4k_launch_cframes_assemble(&a, stream), "lz4k_launch_cframes_assemble");
+    if ((rc = launched(lz4k_launch_cframes_assemble(&a, stream), "lz4k_launch_cframes_assemble")) != LZ4B200_OK) return rc;
+    if ((sums & FC_BLOCK_SUM) &&
+        (rc = launched(lz4k_launch_cframes_block_sums(&a, stream), "lz4k_launch_cframes_block_sums")) != LZ4B200_OK)
+        return rc;
+    if (sums & FC_CONTENT_SUM) return launched(lz4k_launch_cframes_content_sums(&a, stream), "lz4k_launch_cframes_content_sums");
+    return LZ4B200_OK;
+}
+
+int LZ4B200_compress_frames(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
+                            void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
+                            int64_t* d_result, int64_t nFrames,
+                            int blockSizeID, int compressionLevel, int contentSizeFlag, int parallel,
+                            const int64_t maxBlocks[4],
+                            void* d_workspace, size_t workspaceBytes, void* stream)
+{
+    return compress_frames_sums(d_src, d_srcOff, d_srcSize, d_dst, d_dstOff, d_dstCap, d_result, nFrames, blockSizeID,
+                                compressionLevel, contentSizeFlag, parallel, 0, maxBlocks, d_workspace, workspaceBytes,
+                                stream);
+}
+
+int LZ4B200_compress_frames_checksummed(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
+                                        void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
+                                        int64_t* d_result, int64_t nFrames,
+                                        int blockSizeID, int compressionLevel, int contentSizeFlag, int parallel,
+                                        int blockChecksumFlag, int contentChecksumFlag,
+                                        const int64_t maxBlocks[4],
+                                        void* d_workspace, size_t workspaceBytes, void* stream)
+{
+    return compress_frames_sums(d_src, d_srcOff, d_srcSize, d_dst, d_dstOff, d_dstCap, d_result, nFrames, blockSizeID,
+                                compressionLevel, contentSizeFlag, parallel,
+                                (blockChecksumFlag ? FC_BLOCK_SUM : 0) | (contentChecksumFlag ? FC_CONTENT_SUM : 0),
+                                maxBlocks, d_workspace, workspaceBytes, stream);
 }
 
 /* ------------------------------------------------------------------------------------------ */

@@ -78,9 +78,12 @@ FC_FN uint32_t fc_xxh32(const uint8_t* p, uint64_t len, uint32_t seed)
 FC_FN int64_t fc_block_bytes(int bsid) { return (int64_t)1 << (8 + 2 * bsid); }   /* 4..7 -> 64 KB..4 MB (lz4frame.c:333-342) */
 
 /* ---------------------------------------------------------------------------------------------
- * Writing a frame of independent blocks without checksums (LZ4F_compressFrame, lz4frame.c:425-498):
- * LZ4B200_compressFrame_host and the batched LZ4B200_compress_frames take these rules from here.
+ * Writing a frame of independent blocks (LZ4F_compressFrame, lz4frame.c:425-498): LZ4B200_compressFrame_host (no
+ * checksums) and the batched LZ4B200_compress_frames and LZ4B200_compress_frames_checksummed take these rules from here.
  * ------------------------------------------------------------------------------------------- */
+#define FC_BLOCK_SUM   1           /* FLG bit 4: 4 bytes of XXH32(payload) after every block */
+#define FC_CONTENT_SUM 2           /* FLG bit 2: 4 bytes of XXH32(content) after the EndMark */
+
 /* LZ4F_optimalBSID (lz4frame.c:362-373): the smallest block size ID from 4 up to `requested` (4 .. 7) whose blocks hold
  * srcSize bytes */
 FC_FN int fc_optimal_bsid(int requested, int64_t srcSize)
@@ -102,29 +105,40 @@ FC_FN int64_t fc_frame_blocks(int64_t srcSize, int bsid)
     return srcSize / bs + (srcSize % bs != 0);
 }
 
-/* LZ4F_compressFrameBound (lz4frame.c:406-417 with LZ4F_compressBound_internal, lz4frame.c:376-403) for autoFlush,
- * independent blocks and no checksums, at the block size ID the frame is written with: the largest header (19 bytes),
- * a 4-byte header per block, the source, the EndMark.  Saturates at INT64_MAX. */
-FC_FN int64_t fc_frame_bound(int64_t srcSize, int bsid)
+/* LZ4F_compressFrameBound (lz4frame.c:406-417 with LZ4F_compressBound_internal, lz4frame.c:376-403) for autoFlush and
+ * independent blocks, at the block size ID the frame is written with, for a frame carrying the checksums `sums`
+ * (FC_BLOCK_SUM | FC_CONTENT_SUM): the largest header (19 bytes), a 4-byte header and, with block checksums, a
+ * 4-byte checksum per block, the source, the EndMark and, with a content checksum, its 4 bytes.  Saturates at
+ * INT64_MAX. */
+FC_FN int64_t fc_frame_bound_sums(int64_t srcSize, int bsid, int sums)
 {
-    const int64_t extra = 19 + 4 * fc_frame_blocks(srcSize, bsid) + 4;
+    const int64_t extra = 19 + (4 + ((sums & FC_BLOCK_SUM) ? 4 : 0)) * fc_frame_blocks(srcSize, bsid) + 4 +
+                          ((sums & FC_CONTENT_SUM) ? 4 : 0);
     return srcSize > INT64_MAX - extra ? INT64_MAX : srcSize + extra;
 }
 
+/* the same without checksums */
+FC_FN int64_t fc_frame_bound(int64_t srcSize, int bsid) { return fc_frame_bound_sums(srcSize, bsid, 0); }
+
 /* The frame header (LZ4F_compressBegin, lz4frame.c:781-809) into h[0 .. 15): magic, FLG (version 01, independent
- * blocks, the content-size bit), BD, the content size when contentSize > 0 (an empty frame has none, lz4frame.c:445-446),
- * and the header checksum byte.  Returns its length, 7 or 15. */
-FC_FN int fc_frame_header_bytes(uint8_t* h, int bsid, int64_t contentSize)
+ * blocks, the block checksum bit 4, the content-size bit 3, the content checksum bit 2), BD, the content size when
+ * contentSize > 0 (an empty frame has none, lz4frame.c:445-446), and the header checksum byte.  sums: FC_BLOCK_SUM |
+ * FC_CONTENT_SUM.  Returns its length, 7 or 15. */
+FC_FN int fc_frame_header_sums(uint8_t* h, int bsid, int64_t contentSize, int sums)
 {
     int n = 6, i;
     const int withSize = contentSize > 0;
     h[0] = (uint8_t)FC_MAGIC; h[1] = (uint8_t)(FC_MAGIC >> 8); h[2] = (uint8_t)(FC_MAGIC >> 16); h[3] = (uint8_t)(FC_MAGIC >> 24);
-    h[4] = (uint8_t)((1u << 6) | (1u << 5) | ((withSize ? 1u : 0u) << 3));
+    h[4] = (uint8_t)((1u << 6) | (1u << 5) | (((sums & FC_BLOCK_SUM) ? 1u : 0u) << 4) | ((withSize ? 1u : 0u) << 3) |
+                     (((sums & FC_CONTENT_SUM) ? 1u : 0u) << 2));
     h[5] = (uint8_t)((uint32_t)bsid << 4);
     if (withSize) for (i = 0; i < 8; i++) h[n++] = (uint8_t)((uint64_t)contentSize >> (8 * i));
     h[n] = (uint8_t)(fc_xxh32(h + 4, (uint64_t)(n - 4), 0) >> 8);
     return n + 1;
 }
+
+/* the same without checksums */
+FC_FN int fc_frame_header_bytes(uint8_t* h, int bsid, int64_t contentSize) { return fc_frame_header_sums(h, bsid, contentSize, 0); }
 
 typedef struct {
     int64_t contentSize;       /* the header's content size, -1 without one (a field of 2^63 or more reads negative too) */
@@ -139,8 +153,6 @@ typedef struct {
 #define FC_SUMS_SKIP   1
 #define FC_SUMS_VERIFY 2
 
-#define FC_BLOCK_SUM   1           /* FLG bit 4: 4 bytes of XXH32(payload) after every block */
-#define FC_CONTENT_SUM 2           /* FLG bit 2: 4 bytes of XXH32(content) after the EndMark */
 #define FC_VERIFY      4           /* (fc_frame_rec.sums) the call compares them */
 
 /* The verdict on a frame's arguments and header, in the order LZ4B200_decompressFrame_host decides them: LZ4B200_OK (h
@@ -344,8 +356,9 @@ FC_FN void fc_verdict_frame(const fc_frame_rec* r, int64_t dstOff, int64_t dstCa
 }
 
 /* ---------------------------------------------------------------------------------------------
- * The batched frame encode (LZ4B200_compress_frames): the decode's frame record and budget scan (fc_scan_count,
- * fc_place_frame), with a record that holds the frame's source size in contentSize, and one table of blocks per class.
+ * The batched frame encode (LZ4B200_compress_frames, LZ4B200_compress_frames_checksummed): the decode's frame record
+ * and budget scan (fc_scan_count, fc_place_frame), with a record that holds the frame's source size in contentSize and
+ * the checksums it is written with in sums, and one table of blocks per class.
  * ------------------------------------------------------------------------------------------- */
 typedef struct {               /* a class's block table; entry b of every array belongs to one block */
     int64_t* srcOff;           /* absolute offset of the block's source bytes in the call's source */
@@ -356,18 +369,25 @@ typedef struct {               /* a class's block table; entry b of every array 
 
 /* Pass 1 of the encode: the verdict on frame f's arguments and capacity, in LZ4F_compressFrame's order -- LZ4B200_ERR_ARG
  * (a negative size or capacity), LZ4B200_ERR_DSTSIZE (dstCap below the reference's bound at the frame's optimal block
- * size ID, dstMaxSize_tooSmall, lz4frame.c:451-452) -- and its class, block count and header length.  bsid: 4 .. 7. */
-FC_FN void fc_cindex_frame(int64_t srcSize, int64_t dstCap, int bsid, int contentSizeFlag, fc_frame_rec* r)
+ * size ID for the checksums `sums`, dstMaxSize_tooSmall, lz4frame.c:451-452) -- and its class, block count, header
+ * length and checksums (r->sums).  bsid: 4 .. 7. */
+FC_FN void fc_cindex_frame_sums(int64_t srcSize, int64_t dstCap, int bsid, int contentSizeFlag, int sums, fc_frame_rec* r)
 {
     int b;
-    r->count = 0; r->base = 0; r->contentSize = srcSize; r->consumed = 0; r->cls = -1; r->hdrLen = 0; r->sums = 0;
+    r->count = 0; r->base = 0; r->contentSize = srcSize; r->consumed = 0; r->cls = -1; r->hdrLen = 0; r->sums = sums;
     r->status = LZ4B200_OK;
     if (srcSize < 0 || dstCap < 0) { r->status = LZ4B200_ERR_ARG; return; }
     b = fc_optimal_bsid(bsid, srcSize);
-    if (dstCap < fc_frame_bound(srcSize, b)) { r->status = LZ4B200_ERR_DSTSIZE; return; }
+    if (dstCap < fc_frame_bound_sums(srcSize, b, sums)) { r->status = LZ4B200_ERR_DSTSIZE; return; }
     r->cls = b - 4;
     r->count = fc_frame_blocks(srcSize, b);
     r->hdrLen = (contentSizeFlag && srcSize > 0) ? 15 : 7;
+}
+
+/* pass 1 of LZ4B200_compress_frames, which writes no checksums */
+FC_FN void fc_cindex_frame(int64_t srcSize, int64_t dstCap, int bsid, int contentSizeFlag, fc_frame_rec* r)
+{
+    fc_cindex_frame_sums(srcSize, dstCap, bsid, contentSizeFlag, 0, r);
 }
 
 /* Pass 2 of the encode: a frame that passed writes its entries of its class's table (t: that class's).  srcOff: the

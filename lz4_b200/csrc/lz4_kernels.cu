@@ -1292,8 +1292,10 @@ __device__ __forceinline__ void cta_copy(uint8_t* to, const uint8_t* from, int s
     for (int k = head + (body << 4) + threadIdx.x; k < s; k += blockDim.x) to[k] = from[k];
 }
 
+/* outOff[i] = the sum of headerBytes + payload + trailerBytes over the entries before i; outOff[n] = the total */
 __global__ void __launch_bounds__(1024) lz4_pack_scan_kernel(const int32_t* __restrict__ sizes, int64_t n,
-                                                             int64_t* __restrict__ outOff, int headerBytes, FrameRule fr)
+                                                             int64_t* __restrict__ outOff, int headerBytes,
+                                                             int trailerBytes, FrameRule fr)
 {
     __shared__ int64_t warpSums[32];
     __shared__ int64_t carry;
@@ -1303,7 +1305,7 @@ __global__ void __launch_bounds__(1024) lz4_pack_scan_kernel(const int32_t* __re
     for (int64_t base = 0; base < n; base += 1024) {
         int64_t i = base + threadIdx.x;
         int64_t v = 0;
-        if (i < n) { bool isRaw; v = pack_payload(fr, sizes, i, n, isRaw) + headerBytes; }
+        if (i < n) { bool isRaw; v = pack_payload(fr, sizes, i, n, isRaw) + headerBytes + trailerBytes; }
         int64_t x = v;
         for (int d = 1; d < 32; d <<= 1) { int64_t y = __shfl_up_sync(kFull, x, d); if (lane >= d) x += y; }
         if (lane == 31) warpSums[wid] = x;
@@ -1358,7 +1360,8 @@ __global__ void __launch_bounds__(256) lz4_pack_gather_kernel(const uint8_t* __r
  *   raw    : one CTA per stored-raw block of a frame that passed
  * and, when the checksummed call verifies (FC_SUMS_VERIFY):
  *   block sums  : before the verdict, one thread per table entry the fill marked: XXH32 of the block's stored payload
- *   content sums: after the raw blocks, one thread per frame that passed with a content checksum: XXH32 of its output
+ *   content sums: after the raw blocks, content_hash over the frames that passed with a content checksum: XXH32 of
+ *                 their output
  * ============================================================================================= */
 __device__ __forceinline__ fc_block_tab frames_tab(const lz4k_frames_args& a, int cls)
 {
@@ -1512,6 +1515,130 @@ __device__ uint32_t xxh32_dev(const uint8_t* p, int64_t len)
     return fc_xxh32_end(h, p + (n << 4), (uint64_t)len);
 }
 
+/* XXH32(p[0 .. len), 0) by one warp, for long messages: the lanes stream the message's aligned 16-byte granules into a
+ * ring of kXsRing chunks of kXsChunk granules in shared memory with cp.async (kXsRing - 1 chunks in flight), and lane 0
+ * runs the four accumulators over the staged granules -- xxh_stripe's funnel-shift join, then fc_xxh32_merge and
+ * fc_xxh32_end -- while the next chunks arrive.  A single thread's loads bound xxh32_dev to about one DRAM round trip per
+ * 128 bytes; here the hash's own dependency chain bounds the rate.  Every load stays inside an aligned 16-byte granule
+ * that holds a byte of the message.  All 32 lanes call it with the same message; the digest is lane 0's. */
+constexpr int kXsChunk = 64, kXsRing = 8;            /* 1 KB chunks, 7 in flight: 8 KB per warp */
+/* The content-checksum kernels ask for half of the SM's unified L1 / shared memory as shared memory (4 CTAs of 32 KB):
+ * the other half stays L1 for the one-lane path, whose 16-byte loads reuse each 128-byte line eight times.  With the
+ * driver's own choice the carveout grows with the CTAs that fit and the one-lane path loses its lines (DESIGN 3.14). */
+constexpr int kXsCarveoutPct = 50;
+constexpr int kXsWarps = 4;                          /* warps per CTA of the content-checksum kernels */
+constexpr int64_t kXsLongWarps = 4096;               /* at most this many warps look for long messages */
+
+__device__ __forceinline__ void cp_async16(void* smem, const void* gmem)
+{
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem)), "l"(gmem) : "memory");
+}
+
+/* the stripes whose second granule is staged at s[i0 .. iEnd) (stripe k's second granule is granule k + 1), eight
+ * granules read ahead of their rounds, so that the shared-memory loads stay off the accumulators' chains */
+template <int WS>
+__device__ __forceinline__ void xxh_staged_chunk(const uint4* s, int i0, int iEnd, uint32_t bs, uint4& lo, uint32_t v[4])
+{
+    int i = i0;
+    for (; i + 8 <= iEnd; i += 8) {
+        uint4 hi[8];
+        #pragma unroll
+        for (int u = 0; u < 8; u++) hi[u] = s[i + u];
+        #pragma unroll
+        for (int u = 0; u < 8; u++) xxh_stripe<WS>(u ? hi[u - 1] : lo, hi[u], bs, v);
+        lo = hi[7];
+    }
+    for (; i < iEnd; i++) {
+        const uint4 hi = s[i];
+        xxh_stripe<WS>(lo, hi, bs, v);
+        lo = hi;
+    }
+}
+
+__device__ uint32_t xxh32_staged(const uint8_t* p, int64_t len, uint4* ring)
+{
+    const int lane = threadIdx.x & 31;
+    const uintptr_t at = reinterpret_cast<uintptr_t>(p);
+    const uint4* g = reinterpret_cast<const uint4*>(at & ~uintptr_t(15));
+    const int64_t n = len >> 4;                                     /* stripes */
+    const int64_t gLast = (int64_t)(((at + (uintptr_t)len - 1) >> 4) - (at >> 4));
+    const int64_t gUse = n < gLast ? n : gLast;                     /* the granules the stripes read: 0 .. gUse */
+    const int64_t chunks = n / kXsChunk + 1;                        /* chunk c stages granules c * kXsChunk + i */
+    const uint32_t bs = (uint32_t)(at & 3) * 8;
+    const int ws = (int)((at >> 2) & 3);
+    uint32_t v[4] = {FC_XXH_P1 + FC_XXH_P2, FC_XXH_P2, 0u, 0u - FC_XXH_P1};
+    uint4 lo = make_uint4(0, 0, 0, 0);
+    auto issue = [&](int64_t c) {                                   /* one commit group per chunk, empty past the end */
+        if (c < chunks) {
+            uint4* slot = ring + (c % kXsRing) * kXsChunk;
+            #pragma unroll
+            for (int i = lane; i < kXsChunk; i += 32)
+                if (c * kXsChunk + i <= gUse) cp_async16(slot + i, g + c * kXsChunk + i);
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    };
+    for (int c = 0; c < kXsRing - 1; c++) issue(c);
+    for (int64_t c = 0; c < chunks; c++) {
+        asm volatile("cp.async.wait_group %0;" ::"n"(kXsRing - 2) : "memory");    /* this lane's part of chunk c */
+        __syncwarp();               /* every lane's part of chunk c is staged, and lane 0 is done with chunk c - 1 */
+        issue(c + kXsRing - 1);     /* into chunk c - 1's slot */
+        if (lane == 0) {
+            const uint4* sl = ring + (c % kXsRing) * kXsChunk;
+            const int64_t left = n + 1 - c * kXsChunk;              /* second granules up to granule n */
+            const int iEnd = left < kXsChunk ? (int)left : kXsChunk;
+            int i0 = 0;
+            if (c == 0) { lo = sl[0]; i0 = 1; }
+            switch (ws) {
+            case 0: xxh_staged_chunk<0>(sl, i0, iEnd, bs, lo, v); break;
+            case 1: xxh_staged_chunk<1>(sl, i0, iEnd, bs, lo, v); break;
+            case 2: xxh_staged_chunk<2>(sl, i0, iEnd, bs, lo, v); break;
+            default: xxh_staged_chunk<3>(sl, i0, iEnd, bs, lo, v); break;
+            }
+        }
+    }
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    __syncwarp();
+    return fc_xxh32_end(n ? fc_xxh32_merge(v[0], v[1], v[2], v[3]) : FC_XXH_P5, p + (n << 4), (uint64_t)len);
+}
+
+/* Messages from this length on are hashed by a warp (xxh32_staged), shorter ones by one lane each (xxh32_dev): on an
+ * H100 the two take the same time for batches of 256 KB messages, and the warp is faster from there on (DESIGN section
+ * 3.14). */
+#ifndef LZ4K_XXH_STAGED_MIN
+#define LZ4K_XXH_STAGED_MIN (256 << 10)
+#endif
+constexpr int64_t kXsMin = LZ4K_XXH_STAGED_MIN;
+
+__host__ __device__ constexpr int64_t xs_long_warps(int64_t n) { return n < kXsLongWarps ? n : kXsLongWarps; }
+
+/* The content hash of n messages in one launch of xs_grid(n) CTAs of kXsWarps warps: first ceil(n / 32) "short" warps,
+ * in which lane i of warp j hashes message 32j + i if it is shorter than kXsMin, then xs_long_warps(n) "long" warps, in
+ * which warp k stages messages k, k + xs_long_warps(n), ... that are long and skips the others.  msg(f, &p, &len) says
+ * whether message f is to be hashed and where it is; done(f, h) takes its digest. */
+template <class Msg, class Done>
+__device__ __forceinline__ void content_hash(int64_t n, Msg msg, Done done)
+{
+    __shared__ uint4 ring[kXsWarps][kXsRing * kXsChunk];
+    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nShort = (n + 31) >> 5;
+    const uint8_t* p;
+    int64_t len;
+    if (warp < nShort) {
+        const int64_t f = warp * 32 + (threadIdx.x & 31);
+        if (f < n && msg(f, &p, &len) && len < kXsMin) done(f, xxh32_dev(p, len));
+        return;
+    }
+    for (int64_t f = warp - nShort; f < n; f += xs_long_warps(n)) {       /* the same f in the whole warp */
+        if (!msg(f, &p, &len) || len < kXsMin) continue;
+        const uint32_t h = xxh32_staged(p, len, ring[threadIdx.x >> 5]);
+        if ((threadIdx.x & 31) == 0) done(f, h);
+    }
+}
+
+__host__ __device__ constexpr int64_t xs_grid(int64_t n)
+{
+    return ((n + 31) / 32 + xs_long_warps(n) + kXsWarps - 1) / kXsWarps;
+}
+
 /* one thread per table entry: a block the fill marked FC_SUM_PENDING gets FC_SUM_NONE (its checksum, the 4 bytes after
  * its stored payload, matches) or FC_SUM_BAD, which the verdict turns into LZ4B200_ERR_CHECKSUM */
 __global__ void __launch_bounds__(128) lz4_frames_block_sum_kernel(lz4k_frames_args a)
@@ -1523,27 +1650,35 @@ __global__ void __launch_bounds__(128) lz4_frames_block_sum_kernel(lz4k_frames_a
     a.tabDstOff[b] = xxh32_dev(p, n) == fc_rd_le32(p + n) ? FC_SUM_NONE : FC_SUM_BAD;
 }
 
-/* one thread per frame: a frame that passed and carries a content checksum (the 4 bytes before its end) gets
+/* content_hash over the frames: a frame that passed and carries a content checksum (the 4 bytes before its end) gets
  * LZ4B200_ERR_CHECKSUM when XXH32 of its output differs */
-__global__ void __launch_bounds__(128) lz4_frames_content_sum_kernel(lz4k_frames_args a)
+__global__ void __launch_bounds__(32 * kXsWarps) lz4_frames_content_sum_kernel(lz4k_frames_args a)
 {
-    const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (f >= a.nFrames) return;
-    const fc_frame_rec* r = static_cast<const fc_frame_rec*>(a.frames) + f;
-    const int64_t n = a.result[f];
-    if (!(r->sums & FC_VERIFY) || !(r->sums & FC_CONTENT_SUM) || n < 0) return;
-    if (xxh32_dev(a.dst + a.dstOff[f], n) != fc_rd_le32(a.src + a.srcOff[f] + r->consumed - 4))
-        a.result[f] = LZ4B200_ERR_CHECKSUM;
+    content_hash(a.nFrames,
+        [&](int64_t f, const uint8_t** p, int64_t* len) {
+            const fc_frame_rec* r = static_cast<const fc_frame_rec*>(a.frames) + f;
+            *p = a.dst + a.dstOff[f];
+            *len = a.result[f];
+            return (r->sums & FC_VERIFY) && (r->sums & FC_CONTENT_SUM) && *len >= 0;
+        },
+        [&](int64_t f, uint32_t h) {
+            const fc_frame_rec* r = static_cast<const fc_frame_rec*>(a.frames) + f;
+            if (h != fc_rd_le32(a.src + a.srcOff[f] + r->consumed - 4)) a.result[f] = LZ4B200_ERR_CHECKSUM;
+        });
 }
 
 /* =============================================================================================
- * batched frame encode (LZ4B200_compress_frames): the frame rules of lz4_frame_core.h around one encode of the whole block
- * table (by the caller) and the pack scan and gather
+ * batched frame encode (LZ4B200_compress_frames, LZ4B200_compress_frames_checksummed): the frame rules of
+ * lz4_frame_core.h around one encode of the whole block table (by the caller) and the pack scan and gather
  *   index : pass 1 -- one thread per frame: optimal block size ID, block count, header length, argument and capacity
  *           verdicts; then the frame decode's budget scan (lz4_frames_scan_kernel) on the same records
  *   fill  : pass 2 -- one thread per frame that passed: its table entries (source, size, slot, capacity size - 1)
  *   finish: after the pack scan -- one thread per frame: the header, every block's place, the EndMark, the result; the
  *           gather then writes every block header and payload to its place
+ * and, with checksums (a.sums):
+ *   block sums  : one thread per placed table entry: XXH32 of the block's payload, read from its slot (or, stored raw,
+ *                 from the source), into the 4 bytes after the payload
+ *   content sums: content_hash over the frames that passed: XXH32 of the source, into the 4 bytes after the EndMark
  * ============================================================================================= */
 __device__ __forceinline__ fc_cblock_tab cframes_tab(const lz4k_cframes_args& a, int cls)
 {
@@ -1551,11 +1686,25 @@ __device__ __forceinline__ fc_cblock_tab cframes_tab(const lz4k_cframes_args& a,
     return fc_cblock_tab{a.tabSrcOff + t, a.tabSrcSize + t, a.tabSlotOff + t, a.tabCap + t};
 }
 
+/* the pack's frame rule over the block table: a block is stored raw from the source when its encode did not gain */
+__host__ __device__ inline FrameRule cframes_rule(const lz4k_cframes_args& a)
+{
+    FrameRule fr;
+    fr.raw = a.src; fr.rawStride = 0; fr.blockSize = 0; fr.lastSize = 0; fr.rawOff = a.tabSrcOff; fr.rawSize = a.tabSrcSize;
+    return fr;
+}
+
+__device__ __forceinline__ void st_le32(uint8_t* p, uint32_t v)
+{
+    for (int i = 0; i < 4; i++) p[i] = (uint8_t)(v >> (8 * i));
+}
+
 __global__ void __launch_bounds__(128) lz4_cframes_index_kernel(lz4k_cframes_args a)
 {
     const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= a.nFrames) return;
-    fc_cindex_frame(a.srcSize[f], a.dstCap[f], a.bsid, a.contentSizeFlag, static_cast<fc_frame_rec*>(a.frames) + f);
+    fc_cindex_frame_sums(a.srcSize[f], a.dstCap[f], a.bsid, a.contentSizeFlag, a.sums,
+                         static_cast<fc_frame_rec*>(a.frames) + f);
 }
 
 __global__ void __launch_bounds__(128) lz4_cframes_fill_kernel(lz4k_cframes_args a)
@@ -1567,6 +1716,8 @@ __global__ void __launch_bounds__(128) lz4_cframes_fill_kernel(lz4k_cframes_args
     fc_cfill_frame(r, a.srcOff[f], a.slotBase[r->cls], a.slotStride[r->cls], cframes_tab(a, r->cls));
 }
 
+/* the pack scan counted 4 + payload (+ 4 with block checksums) per entry, so the EndMark follows the last block's
+ * checksum; a content checksum takes the 4 bytes after it */
 __global__ void __launch_bounds__(128) lz4_cframes_finish_kernel(lz4k_cframes_args a)
 {
     const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1578,10 +1729,34 @@ __global__ void __launch_bounds__(128) lz4_cframes_finish_kernel(lz4k_cframes_ar
     for (int64_t k = 0; k < r->count; k++) a.tabPackOff[first + k] = at + a.tabBodyOff[first + k] - body0;
     const int64_t end = at + a.tabBodyOff[first + r->count] - body0;
     uint8_t h[15];
-    const int hl = fc_frame_header_bytes(h, r->cls + 4, a.contentSizeFlag ? r->contentSize : 0);
+    const int hl = fc_frame_header_sums(h, r->cls + 4, a.contentSizeFlag ? r->contentSize : 0, r->sums);
     for (int i = 0; i < hl; i++) a.dst[a.dstOff[f] + i] = h[i];
     for (int i = 0; i < 4; i++) a.dst[end + i] = 0;                  /* EndMark, lz4frame.c:1222 */
-    a.result[f] = end + 4 - a.dstOff[f];
+    a.result[f] = end + 4 + ((r->sums & FC_CONTENT_SUM) ? 4 : 0) - a.dstOff[f];
+}
+
+/* LZ4F_makeBlock's block checksum (lz4frame.c:904-907): XXH32(payload, 0) after the payload of every placed entry */
+__global__ void __launch_bounds__(128) lz4_cframes_block_sum_kernel(lz4k_cframes_args a)
+{
+    const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= a.nEntries) return;
+    if (a.tabPackOff[b] < 0) return;
+    bool isRaw;
+    const int s = pack_payload(cframes_rule(a), a.tabOutSize, b, a.nEntries, isRaw);
+    const uint32_t h = xxh32_dev(isRaw ? a.src + a.tabSrcOff[b] : a.slots + a.tabSlotOff[b], s);
+    st_le32(a.dst + a.tabPackOff[b] + 4 + s, h);
+}
+
+/* the content checksum (lz4frame.c:1225-1229): XXH32(source, 0) after the EndMark of every frame that passed */
+__global__ void __launch_bounds__(32 * kXsWarps) lz4_cframes_content_sum_kernel(lz4k_cframes_args a)
+{
+    content_hash(a.nFrames,
+        [&](int64_t f, const uint8_t** p, int64_t* len) {
+            *p = a.src + a.srcOff[f];
+            *len = a.srcSize[f];
+            return static_cast<const fc_frame_rec*>(a.frames)[f].status == LZ4B200_OK;
+        },
+        [&](int64_t f, uint32_t h) { st_le32(a.dst + a.dstOff[f] + a.result[f] - 4, h); });
 }
 
 }  // namespace
@@ -1613,7 +1788,7 @@ static void launch_pack_gather(const uint8_t* slots, const int64_t* slotOff, int
 static int launch_pack(const uint8_t* slots, const int64_t* slotOff, int64_t slotStride, const int32_t* sizes,
                        int64_t nBlocks, uint8_t* packed, int64_t* outOff, int headerBytes, FrameRule fr, cudaStream_t s)
 {
-    lz4_pack_scan_kernel<<<1, 1024, 0, s>>>(sizes, nBlocks, outOff, headerBytes, fr);
+    lz4_pack_scan_kernel<<<1, 1024, 0, s>>>(sizes, nBlocks, outOff, headerBytes, 0, fr);
     g_launches++;
     launch_pack_gather(slots, slotOff, slotStride, sizes, nBlocks, packed, outOff, nullptr, headerBytes, fr, s);
     return (int)cudaGetLastError();
@@ -1670,12 +1845,31 @@ int lz4k_launch_cframes_index(const lz4k_cframes_args* a, void* stream)
 int lz4k_launch_cframes_assemble(const lz4k_cframes_args* a, void* stream)
 {
     cudaStream_t s = (cudaStream_t)stream;
-    FrameRule fr;
-    fr.raw = a->src; fr.rawStride = 0; fr.blockSize = 0; fr.lastSize = 0; fr.rawOff = a->tabSrcOff; fr.rawSize = a->tabSrcSize;
-    lz4_pack_scan_kernel<<<1, 1024, 0, s>>>(a->tabOutSize, a->nEntries, a->tabBodyOff, 4, fr);
+    const FrameRule fr = cframes_rule(*a);
+    lz4_pack_scan_kernel<<<1, 1024, 0, s>>>(a->tabOutSize, a->nEntries, a->tabBodyOff, 4, (a->sums & FC_BLOCK_SUM) ? 4 : 0, fr);
     lz4_cframes_finish_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);
     g_launches += 2;
     launch_pack_gather(a->slots, a->tabSlotOff, 0, a->tabOutSize, a->nEntries, a->dst, a->tabBodyOff, a->tabPackOff, 4, fr, s);
+    return (int)cudaGetLastError();
+}
+
+int lz4k_launch_cframes_block_sums(const lz4k_cframes_args* a, void* stream)
+{
+    lz4_cframes_block_sum_kernel<<<a->nEntries < 1 ? 1u : frames_grid(a->nEntries), 128, 0, (cudaStream_t)stream>>>(*a);
+    g_launches++;
+    return (int)cudaGetLastError();
+}
+
+static void xs_carveout(const void* kernel)
+{
+    cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, kXsCarveoutPct);
+}
+
+int lz4k_launch_cframes_content_sums(const lz4k_cframes_args* a, void* stream)
+{
+    xs_carveout((const void*)lz4_cframes_content_sum_kernel);
+    lz4_cframes_content_sum_kernel<<<(unsigned)xs_grid(a->nFrames), 32 * kXsWarps, 0, (cudaStream_t)stream>>>(*a);
+    g_launches++;
     return (int)cudaGetLastError();
 }
 
@@ -1704,7 +1898,8 @@ int lz4k_launch_frames_block_sums(const lz4k_frames_args* a, void* stream)
 
 int lz4k_launch_frames_content_sums(const lz4k_frames_args* a, void* stream)
 {
-    lz4_frames_content_sum_kernel<<<frames_grid(a->nFrames), 128, 0, (cudaStream_t)stream>>>(*a);
+    xs_carveout((const void*)lz4_frames_content_sum_kernel);
+    lz4_frames_content_sum_kernel<<<(unsigned)xs_grid(a->nFrames), 32 * kXsWarps, 0, (cudaStream_t)stream>>>(*a);
     g_launches++;
     return (int)cudaGetLastError();
 }

@@ -122,12 +122,13 @@ typedef struct {
     int64_t nEntries;          /* entries of the block table (sum of maxBlocks) */
     int bsid;                  /* the requested block size ID, 4 .. 7 */
     int contentSizeFlag;
+    int sums;                  /* the checksums every frame is written with: FC_BLOCK_SUM | FC_CONTENT_SUM */
     void* frames;              /* fc_frame_rec[nFrames] */
     uint8_t* slots;            /* block b is compressed to slots + tabSlotOff[b] */
     int64_t slotBase[4];       /* class c's slots: slotBase[c] + k * slotStride[c] from `slots` */
     int64_t slotStride[4];
     int64_t* tabSrcOff; int32_t* tabSrcSize; int64_t* tabSlotOff; int32_t* tabCap; int32_t* tabOutSize;
-    int64_t* tabBodyOff;       /* [nEntries + 1]: the pack scan of 4 + payload over the table */
+    int64_t* tabBodyOff;       /* [nEntries + 1]: the pack scan of 4 + payload (+ 4 with block checksums) over the table */
     int64_t* tabPackOff;       /* where block b's header goes in dst, -1 for an unused entry */
 } lz4k_cframes_args;
 
@@ -135,6 +136,10 @@ typedef struct {
 int lz4k_launch_cframes_index(const lz4k_cframes_args* a, void* stream);
 /* after the encode (tabOutSize): the pack scan, the frame headers, places, EndMarks and results, then the gather */
 int lz4k_launch_cframes_assemble(const lz4k_cframes_args* a, void* stream);
+/* FC_BLOCK_SUM, after the assembly: the block checksums, one thread per placed table entry */
+int lz4k_launch_cframes_block_sums(const lz4k_cframes_args* a, void* stream);
+/* FC_CONTENT_SUM, after the assembly: the content checksum of every frame that passed, in one launch */
+int lz4k_launch_cframes_content_sums(const lz4k_cframes_args* a, void* stream);
 uint64_t lz4k_launch_count(void);
 int lz4k_debug_poison_smem(uint32_t pattern, int lo, int hi, void* stream);   /* developer tool */
 int lz4k_launch_ceiling(const lz4k_decode_args* a, int mode, void* stream);   /* developer tool: skeleton of the rows kernel without the decode */
