@@ -297,6 +297,78 @@ LZ4B200_API int LZ4B200_decompress_frames_checksummed(const void* d_src, const i
                                                       void* d_workspace, size_t workspaceBytes, void* stream);
 
 /*
+ * Decode nFiles whole .lz4 files that are already in device memory, as `lz4 -d -c` decodes each of them piped to its
+ * standard input (LZ4IO_decompressSrcFile and selectDecoder, lz4io.c:2349-2436).  "File" is the bytes of one .lz4 file:
+ *   file f input : d_src + d_srcOff[f], d_srcSize[f] bytes
+ *   file f output: d_dst + d_dstOff[f], d_dstCap[f] bytes of room
+ * A file is a sequence of units, read from offset p with r bytes left:
+ *   - r == 0 ends the file (an empty file decodes to 0 bytes); 1 <= r < 4 is LZ4B200_ERR_FRAME;
+ *   - magic 0x184D2204, an LZ4 frame: the rules of LZ4B200_decompress_frames_checksummed, unchanged -- header, chain,
+ *     block and content checksums (skipChecksums as there: `lz4 -d --no-frame-crc`), stored-raw blocks, content size,
+ *     LZ4B200_ERR_UNSUPPORTED for linked blocks and dictID.  The unit ends after its EndMark and content checksum; a frame
+ *     cut short is LZ4B200_ERR_FRAME;
+ *   - magic 0x184D2A50 .. 0x184D2A5F, a skippable frame: an LE32 size, then that many bytes; it decodes to nothing.
+ *     Fewer than 8 bytes, or a size that runs past the file's end, is LZ4B200_ERR_FRAME (`lz4 -d` on a pipe);
+ *   - magic 0x184C2102, a legacy stream (`lz4 -l`): words w, each followed by a block of w compressed bytes decoded as
+ *     LZ4_decompress_safe(block, out, w, 8 MiB), the blocks' output back to back.  The unit ends with the file or at a
+ *     word above LZ4_COMPRESSBOUND(8 MiB) = 8 421 520, which is the next unit's magic.  1 .. 3 bytes where a word is due,
+ *     a block cut short, or a block that fails to decode (w == 0 included) is LZ4B200_ERR_FRAME;
+ *   - any other magic is LZ4B200_ERR_FRAME, at the start of a file or after other units.
+ * Results:
+ *   d_result[f]  : the file's decoded size, or the code of its first failing unit in file order: LZ4B200_ERR_ARG (a
+ *                  negative size, or a negative room when decoding), LZ4B200_ERR_FRAME, LZ4B200_ERR_UNSUPPORTED,
+ *                  LZ4B200_ERR_DSTSIZE (the unit's bytes do not fit the room left after the units before it),
+ *                  LZ4B200_ERR_CHECKSUM or LZ4B200_ERR_LIMIT (below).  Inside one LZ4 frame the order is the frames call's.
+ *   d_consumed[f]: (may be NULL) d_srcSize[f] on success, else the offset in the file of the failing unit's first byte
+ *                  (0 for LZ4B200_ERR_ARG)
+ *   d_prefix[f]  : (may be NULL) the decoded bytes of the units before the failing unit; d_result[f] on success
+ * On success [dst_f, dst_f + d_result[f]) holds what `lz4 -d` writes; on failure [dst_f, dst_f + d_prefix[f]) holds the
+ * output of the units before the failing one, a prefix of what `lz4 -d` writes before it fails, and the bytes after it
+ * are unspecified.  Nothing is written outside [dst_f, dst_f + d_dstCap[f]); output regions must not overlap.  Readable
+ * padding: 16 bytes before and after every file.
+ *
+ * The budget: maxUnits bounds the units the call takes (LZ4 frames, skippable frames and legacy streams over all files),
+ * maxBlocks[c] the blocks of class c: maxBlocks[0 .. 3] the blocks of frames of block size ID 4 + c (64 KB .. 4 MB),
+ * maxBlocks[4] legacy blocks.  Units and blocks are counted in file order, then in unit order.  A unit whose index
+ * reaches maxUnits, or whose blocks with those of the earlier units of its class exceed maxBlocks[c], gets
+ * LZ4B200_ERR_LIMIT, after its own header errors and its chain errors within maxBlocks[c] + 1 blocks (the frames calls'
+ * rule).  A file's walk stops at its first unit that fails its header or chain rules or stops short on its budget, and
+ * after maxUnits + 1 units, which bounds the work a file of tiny skippable frames can cause; only the units it took are
+ * counted.  Results do not depend on scheduling.  The host plans every step from the budget and the call never
+ * synchronises, so it can be captured into a CUDA graph.
+ *
+ * sizeOnly != 0: d_dst, d_dstOff and d_dstCap may be NULL and are not read, the room is unlimited and no byte is written.
+ * The results are the decoded sizes; block checksums are still verified unless skipChecksums, content checksums are not
+ * compared (no bytes are produced).  The allocate-then-decode companion for files without a content size, which is how
+ * `lz4` writes them by default.
+ *
+ * Deviations from `lz4 -d`: linked blocks and dictID are LZ4B200_ERR_UNSUPPORTED (`lz4 -d` decodes them); under
+ * skipChecksums a compressed block's checksum is not compared (the frames call's rule); a skippable frame that runs past
+ * the end is LZ4B200_ERR_FRAME (the pipe behaviour, not the seekable file's); the pass-through of non-LZ4 input
+ * (`lz4 -dcf`) is not offered.
+ *
+ * Kernel launches: 4 (the walk, the unit scan, the unit records, the fold), plus, when maxUnits > 0: 3 (the frame
+ * decode's budget scan and table fill, the totals); the phases of LZ4B200_decompress_blocks_phased for every class with
+ * a budget (3 for maxBlocks[0] and 4 for each of maxBlocks[1 .. 4], or only the scans when sizeOnly: 1 and 2); 1 for the
+ * block checksums unless skipChecksums; and, unless sizeOnly, 3 (place, verdict, raw blocks) and 1
+ * for the content checksums unless skipChecksums.  nFiles == 0 returns LZ4B200_OK without one.
+ * LZ4B200_ERR_ARG: nFiles < 0, a NULL maxBlocks, maxUnits or a budget entry outside 0 .. 2^31 - 1; then, with files
+ * present, a NULL d_src, d_srcOff, d_srcSize, d_result or d_workspace, a NULL d_dst, d_dstOff or d_dstCap unless
+ * sizeOnly, or a workspace smaller than LZ4B200_decompress_files_workspace_bytes asks (0 for arguments the call
+ * rejects).  The workspace is that of LZ4B200_decompress_frames for maxUnits frames with a fifth class of 8 MiB blocks
+ * (about 2 x 8 MiB per budgeted legacy block, the tiles kernel's marks), plus 40 bytes per unit and 32 per file.
+ */
+#define LZ4B200_FILE_CLASSES 5   /* maxBlocks[0..3]: frame blocks of 64 KB .. 4 MB (block size ID 4 + c); [4]: legacy 8 MiB blocks */
+LZ4B200_API size_t LZ4B200_decompress_files_workspace_bytes(int64_t nFiles, int64_t maxUnits,
+                                                            const int64_t maxBlocks[LZ4B200_FILE_CLASSES]);
+LZ4B200_API int LZ4B200_decompress_files(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
+                                         void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
+                                         int64_t* d_result, int64_t* d_consumed, int64_t* d_prefix,
+                                         int64_t nFiles, int64_t maxUnits, const int64_t maxBlocks[LZ4B200_FILE_CLASSES],
+                                         int skipChecksums, int sizeOnly,
+                                         void* d_workspace, size_t workspaceBytes, void* stream);
+
+/*
  * Write nFrames LZ4 frames from sources in device memory (the batched LZ4F_compressFrame, lz4frame.h:224 /
  * lz4frame.c:425-498), at every compression level:
  *   frame f input : d_src + d_srcOff[f], n_f = d_srcSize[f] bytes

@@ -44,6 +44,9 @@ PROTOTYPES = [
     ("LZ4B200_decompress_frames", C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, C.POINTER(_i64), _vp, _sz, _vp]),
     ("LZ4B200_decompress_frames_checksummed", C.c_int,
      [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, C.POINTER(_i64), C.c_int, _vp, _sz, _vp]),
+    ("LZ4B200_decompress_files_workspace_bytes", _sz, [_i64, _i64, C.POINTER(_i64)]),
+    ("LZ4B200_decompress_files", C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, C.POINTER(_i64),
+                                           C.c_int, C.c_int, _vp, _sz, _vp]),
     ("LZ4B200_compress_frames_workspace_bytes", _sz, [_i64, C.POINTER(_i64), C.c_int]),
     ("LZ4B200_compress_frames", C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, C.c_int, C.c_int, C.c_int, C.c_int,
                                           C.POINTER(_i64), _vp, _sz, _vp]),

@@ -309,6 +309,88 @@ def _decompress_frames(entry, mode_args, comp, offsets, sizes, capacities, max_b
     return out, results, consumed
 
 
+def _file_budget(max_blocks):
+    """the per-class budget of the file calls (64 KB, 256 KB, 1 MB, 4 MB frame blocks, 8 MiB legacy blocks)"""
+    mb = [int(x) for x in max_blocks]
+    if len(mb) != 5:
+        raise ValueError("max_blocks: one budget per block size ID 4 .. 7 and one for legacy blocks (5 values)")
+    return (C.c_int64 * 5)(*mb)
+
+
+def decompress_files_workspace_bytes(n_files, max_units, max_blocks):
+    """LZ4B200_decompress_files_workspace_bytes: the workspace decompress_files and decompressed_file_sizes need (0:
+    arguments they reject)"""
+    return int(_lib.load().LZ4B200_decompress_files_workspace_bytes(int(n_files), int(max_units),
+                                                                     _file_budget(max_blocks)))
+
+
+def decompress_files(comp, offsets, sizes, capacities, max_units, max_blocks, skip_checksums=False, out=None,
+                     out_offsets=None, results=None, consumed=None, prefix=None, workspace=None, stream=None):
+    """Decode len(sizes) whole .lz4 files held in device memory as `lz4 -d` decodes them (LZ4B200_decompress_files):
+    LZ4 frames one after another, skippable frames and `lz4 -l` legacy streams.
+
+    comp: u8[*] device buffer; file f = comp[offsets[f] : offsets[f]+sizes[f]] (int64 device tensors), with 16 readable
+    bytes before and after it.  File f decodes to out[out_offsets[f] : out_offsets[f]+capacities[f]] (int64 device
+    tensors); out_offsets defaults to the exclusive sum of capacities, and out to their total (read on the host: a
+    captured call passes out).  max_units: the units (frames, skippable frames, legacy streams) the call takes over all
+    files; max_blocks: its blocks per class (5 host ints: frame blocks of block size ID 4 .. 7, legacy blocks).
+    skip_checksums: `lz4 -d --no-frame-crc`.
+    Returns (out, results, consumed, prefix): results[f] the decoded size or the code of the file's first failing unit,
+    consumed[f] sizes[f] or that unit's offset, prefix[f] the decoded bytes of the units before it."""
+    return _decompress_files(False, comp, offsets, sizes, capacities, max_units, max_blocks, skip_checksums, out,
+                             out_offsets, results, consumed, prefix, workspace, stream)
+
+
+def decompressed_file_sizes(comp, offsets, sizes, max_units, max_blocks, skip_checksums=False, results=None,
+                            consumed=None, prefix=None, workspace=None, stream=None):
+    """The size-only pass of decompress_files (sizeOnly): the same results with unlimited room and no byte written --
+    the decoded size of every file, block checksums verified unless skipped, content checksums not compared.
+    Returns (results, consumed, prefix)."""
+    return _decompress_files(True, comp, offsets, sizes, None, max_units, max_blocks, skip_checksums, None, None,
+                             results, consumed, prefix, workspace, stream)[1:]
+
+
+def _decompress_files(size_only, comp, offsets, sizes, capacities, max_units, max_blocks, skip_checksums, out,
+                      out_offsets, results, consumed, prefix, workspace, stream):
+    lib = _lib.load()
+    what = "decompressed_file_sizes" if size_only else "decompress_files"
+    n = int(sizes.numel()) if isinstance(sizes, torch.Tensor) else 0
+    budget = _file_budget(max_blocks)
+    ws_bytes = int(lib.LZ4B200_decompress_files_workspace_bytes(n, int(max_units), budget))
+    if ws_bytes == 0:
+        raise ValueError("%s: max_units and the budgets must be 0 .. 2^31 - 1" % what)
+    at_least_n = (n, None)
+    device, st = _checked(what, stream,
+                          [("comp", comp, U8, ANY), ("offsets", offsets, I64, at_least_n), ("sizes", sizes, I64, ANY),
+                           ("capacities", capacities, I64, (n, n)), ("out", out, U8, ANY),
+                           ("out_offsets", out_offsets, I64, at_least_n), ("results", results, I64, at_least_n),
+                           ("consumed", consumed, I64, at_least_n), ("prefix", prefix, I64, at_least_n),
+                           ("workspace", workspace, U8, (ws_bytes, None))])
+    if not size_only and capacities is None:
+        raise ValueError("%s: capacities must be a CUDA tensor" % what)
+    workspace = _workspace(device, ws_bytes, st, workspace, what)
+    with torch.cuda.stream(st):                     # temporaries belong to the stream the kernels run on
+        if not size_only:
+            if out_offsets is None:
+                out_offsets = torch.cumsum(capacities, 0) - capacities
+            if out is None:
+                if torch.cuda.is_current_stream_capturing():
+                    raise ValueError("%s under stream capture needs out=" % what)
+                out = torch.empty(max(int(capacities.sum()) if n else 0, 1), dtype=torch.uint8, device=device)
+        if results is None:
+            results = torch.empty(n, dtype=torch.int64, device=device)
+        if consumed is None:
+            consumed = torch.empty(n, dtype=torch.int64, device=device)
+        if prefix is None:
+            prefix = torch.empty(n, dtype=torch.int64, device=device)
+    ptr = (lambda t: t.data_ptr() if t is not None else None)
+    _launch(device, "LZ4B200_decompress_files", lib.LZ4B200_decompress_files, comp.data_ptr(), offsets.data_ptr(),
+            sizes.data_ptr(), ptr(out), ptr(out_offsets), ptr(capacities), results.data_ptr(), consumed.data_ptr(),
+            prefix.data_ptr(), n, int(max_units), budget, 1 if skip_checksums else 0, 1 if size_only else 0,
+            workspace.data_ptr(), workspace.numel(), st.cuda_stream)
+    return out, results, consumed, prefix
+
+
 def compress_frames_workspace_bytes(n_frames, max_blocks, level=0):
     """LZ4B200_compress_frames_workspace_bytes: the workspace compress_frames needs (0: arguments it rejects)"""
     return int(_lib.load().LZ4B200_compress_frames_workspace_bytes(int(n_frames), _budget(max_blocks), int(level)))

@@ -264,26 +264,29 @@ int LZ4B200_decompress_blocks_partial(const void* d_src, const int64_t* d_srcOff
 /* The workspace of LZ4B200_decompress_frames, from the budget alone: the frame records, the block table of every class
  * (entries tabBase[c] .. tabBase[c] + maxBlocks[c] - 1), then one decode workspace per class with a budget, each the
  * size that gives the class's uniform capacity its own route (LZ4B200_decompress_workspace_bytes_for(maxBlocks[c], 0,
- * block size)).  Regions start on 256 bytes from a base rounded up to 256 (the 256 bytes of slack in `bytes`). */
+ * fc_class_bytes(c))).  Regions start on 256 bytes from a base rounded up to 256 (the 256 bytes of slack in `bytes`).
+ * The frames calls plan 4 classes, LZ4B200_decompress_files all FC_CLASSES (class 4: legacy blocks); it puts its own
+ * regions after these, from `end`. */
 #define FRAMES_MAX_BUDGET 0x7FFFFFFF
 typedef struct {
-    size_t frames, srcOff, dstOff, srcSize, outSize, rawLen, decode[4], decodeBytes[4], bytes;
-    int64_t tabBase[4], nEntries;
+    size_t frames, srcOff, dstOff, srcSize, outSize, rawLen, decode[FC_CLASSES], decodeBytes[FC_CLASSES], end, bytes;
+    int64_t maxBlocks[FC_CLASSES], tabBase[FC_CLASSES], nEntries;
 } frames_plan_t;
 
 static size_t up256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 /* 0 for arguments the call rejects (nFrames < 0, a NULL budget, an entry outside 0 .. FRAMES_MAX_BUDGET) */
-static int frames_plan(int64_t nFrames, const int64_t* maxBlocks, frames_plan_t* p)
+static int frames_plan(int64_t nFrames, const int64_t* maxBlocks, int classes, frames_plan_t* p)
 {
     size_t at = 0;
     int c;
     if (nFrames < 0 || !maxBlocks) return 0;
     p->nEntries = 0;
-    for (c = 0; c < 4; c++) {
-        if (maxBlocks[c] < 0 || maxBlocks[c] > FRAMES_MAX_BUDGET) return 0;
+    for (c = 0; c < FC_CLASSES; c++) {
+        p->maxBlocks[c] = c < classes ? maxBlocks[c] : 0;
+        if (p->maxBlocks[c] < 0 || p->maxBlocks[c] > FRAMES_MAX_BUDGET) return 0;
         p->tabBase[c] = p->nEntries;
-        p->nEntries += maxBlocks[c];
+        p->nEntries += p->maxBlocks[c];
     }
     p->frames = at;  at = up256(at + (size_t)nFrames * sizeof(fc_frame_rec));
     p->srcOff = at;  at = up256(at + (size_t)p->nEntries * sizeof(int64_t));
@@ -291,11 +294,12 @@ static int frames_plan(int64_t nFrames, const int64_t* maxBlocks, frames_plan_t*
     p->srcSize = at; at = up256(at + (size_t)p->nEntries * sizeof(int32_t));
     p->outSize = at; at = up256(at + (size_t)p->nEntries * sizeof(int32_t));
     p->rawLen = at;  at = up256(at + (size_t)p->nEntries * sizeof(int32_t));
-    for (c = 0; c < 4; c++) {
-        p->decodeBytes[c] = maxBlocks[c] ? lz4k_decode_workspace_bytes(maxBlocks[c], 0, (int32_t)fc_block_bytes(4 + c), SIZE_MAX) : 0;
+    for (c = 0; c < FC_CLASSES; c++) {
+        p->decodeBytes[c] = p->maxBlocks[c] ? lz4k_decode_workspace_bytes(p->maxBlocks[c], 0, (int32_t)fc_class_bytes(c), SIZE_MAX) : 0;
         p->decode[c] = at;
         at = up256(at + p->decodeBytes[c]);
     }
+    p->end = at;
     p->bytes = at + 256;
     return 1;
 }
@@ -303,7 +307,39 @@ static int frames_plan(int64_t nFrames, const int64_t* maxBlocks, frames_plan_t*
 size_t LZ4B200_decompress_frames_workspace_bytes(int64_t nFrames, const int64_t maxBlocks[4])
 {
     frames_plan_t p;
-    return frames_plan(nFrames, maxBlocks, &p) ? p.bytes : 0;
+    return frames_plan(nFrames, maxBlocks, 4, &p) ? p.bytes : 0;
+}
+
+/* the frame decode's arguments on the planned workspace ws (aligned to 256) */
+static void frames_args(lz4k_frames_args* a, const frames_plan_t* p, uint8_t* ws, int mode)
+{
+    int c;
+    for (c = 0; c < FC_CLASSES; c++) { a->maxBlocks[c] = p->maxBlocks[c]; a->tabBase[c] = p->tabBase[c]; }
+    a->nEntries = p->nEntries;
+    a->mode = mode;
+    a->frames = ws + p->frames;
+    a->tabSrcOff = (int64_t*)(ws + p->srcOff); a->tabDstOff = (int64_t*)(ws + p->dstOff);
+    a->tabSrcSize = (int32_t*)(ws + p->srcSize); a->tabOutSize = (int32_t*)(ws + p->outSize); a->tabRawLen = (int32_t*)(ws + p->rawLen);
+}
+
+/* one phase (1: scan, 2: expand) of the decode of every class's table with a budget, at the class's uniform capacity
+ * on its planned workspace (the launches of LZ4B200_decompress_blocks_phased; the scans read no destination, which
+ * LZ4B200_decompress_files does not have when it only sizes) */
+static int frames_decode_phase(const lz4k_frames_args* a, const frames_plan_t* p, uint8_t* ws, int ph, void* stream)
+{
+    lz4k_decode_args d;
+    int c, rc;
+    for (c = 0; c < FC_CLASSES; c++) {
+        const int64_t t = p->tabBase[c];
+        if (!p->maxBlocks[c]) continue;
+        memset(&d, 0, sizeof d);
+        d.src = a->src; d.srcOff = a->tabSrcOff + t; d.srcSize = a->tabSrcSize + t;
+        d.dst = a->dst; d.dstOff = a->tabDstOff + t; d.dstCap = (int32_t)fc_class_bytes(c);
+        d.outSize = a->tabOutSize + t; d.nBlocks = p->maxBlocks[c];
+        d.workspace = ws + p->decode[c]; d.workspaceBytes = p->decodeBytes[c];
+        if ((rc = launched(lz4k_launch_decode(&d, ph, 0, stream), "lz4k_launch_decode")) != LZ4B200_OK) return rc;
+    }
+    return LZ4B200_OK;
 }
 
 /* index -> per class: scan (phase 1) -> [block checksums] -> verdict -> per class: expand (phase 2) -> raw blocks ->
@@ -319,8 +355,8 @@ static int decompress_frames_mode(const void* d_src, const int64_t* d_srcOff, co
     frames_plan_t p;
     lz4k_frames_args a;
     uint8_t* ws;
-    int c, ph, rc;
-    if (!frames_plan(nFrames, maxBlocks, &p)) return LZ4B200_ERR_ARG;
+    int ph, rc;
+    if (!frames_plan(nFrames, maxBlocks, 4, &p)) return LZ4B200_ERR_ARG;
     if (nFrames == 0) return LZ4B200_OK;
     if (!d_src || !d_srcOff || !d_srcSize || !d_dst || !d_dstOff || !d_dstCap || !d_result || !d_workspace)
         return LZ4B200_ERR_ARG;
@@ -330,12 +366,7 @@ static int decompress_frames_mode(const void* d_src, const int64_t* d_srcOff, co
     a.src = (const uint8_t*)d_src; a.srcOff = d_srcOff; a.srcSize = d_srcSize;
     a.dst = (uint8_t*)d_dst; a.dstOff = d_dstOff; a.dstCap = d_dstCap;
     a.result = d_result; a.consumed = d_consumed; a.nFrames = nFrames;
-    for (c = 0; c < 4; c++) { a.maxBlocks[c] = maxBlocks[c]; a.tabBase[c] = p.tabBase[c]; }
-    a.nEntries = p.nEntries;
-    a.mode = mode;
-    a.frames = ws + p.frames;
-    a.tabSrcOff = (int64_t*)(ws + p.srcOff); a.tabDstOff = (int64_t*)(ws + p.dstOff);
-    a.tabSrcSize = (int32_t*)(ws + p.srcSize); a.tabOutSize = (int32_t*)(ws + p.outSize); a.tabRawLen = (int32_t*)(ws + p.rawLen);
+    frames_args(&a, &p, ws, mode);
 
     if ((rc = launched(lz4k_launch_frames_index(&a, stream), "lz4k_launch_frames_index")) != LZ4B200_OK) return rc;
     for (ph = 1; ph <= 2; ph++) {
@@ -344,14 +375,7 @@ static int decompress_frames_mode(const void* d_src, const int64_t* d_srcOff, co
             return rc;
         if (ph == 2 && (rc = launched(lz4k_launch_frames_verdict(&a, stream), "lz4k_launch_frames_verdict")) != LZ4B200_OK)
             return rc;
-        for (c = 0; c < 4; c++) {
-            const int64_t t = p.tabBase[c];
-            if (!maxBlocks[c]) continue;
-            rc = LZ4B200_decompress_blocks_phased(d_src, a.tabSrcOff + t, a.tabSrcSize + t, d_dst, a.tabDstOff + t, 0, NULL,
-                                                  (int32_t)fc_block_bytes(4 + c), a.tabOutSize + t, maxBlocks[c],
-                                                  ws + p.decode[c], p.decodeBytes[c], ph, stream);
-            if (rc != LZ4B200_OK) return rc;
-        }
+        if ((rc = frames_decode_phase(&a, &p, ws, ph, stream)) != LZ4B200_OK) return rc;
     }
     if ((rc = launched(lz4k_launch_frames_raw(&a, stream), "lz4k_launch_frames_raw")) != LZ4B200_OK) return rc;
     if (mode == FC_SUMS_VERIFY) return launched(lz4k_launch_frames_content_sums(&a, stream), "lz4k_launch_frames_content_sums");
@@ -377,6 +401,92 @@ int LZ4B200_decompress_frames_checksummed(const void* d_src, const int64_t* d_sr
     return decompress_frames_mode(d_src, d_srcOff, d_srcSize, d_dst, d_dstOff, d_dstCap, d_result, d_consumed, nFrames,
                                   maxBlocks, skipChecksums ? FC_SUMS_SKIP : FC_SUMS_VERIFY, d_workspace, workspaceBytes,
                                   stream);
+}
+
+/* The workspace of LZ4B200_decompress_files: the frame decode's plan for maxUnits unit records and all FC_CLASSES
+ * classes, then the file records and the units' source offsets, lengths, places, rooms and results. */
+typedef struct {
+    frames_plan_t f;
+    size_t files, uSrcOff, uSrcSize, uDstOff, uDstCap, uResult, bytes;
+} files_plan_t;
+
+/* 0 for arguments the call rejects (nFiles < 0, maxUnits or a budget entry outside 0 .. FRAMES_MAX_BUDGET, a NULL
+ * budget) */
+static int files_plan(int64_t nFiles, int64_t maxUnits, const int64_t* maxBlocks, files_plan_t* p)
+{
+    size_t at, u;
+    if (nFiles < 0 || maxUnits < 0 || maxUnits > FRAMES_MAX_BUDGET) return 0;
+    if (!frames_plan(maxUnits, maxBlocks, FC_CLASSES, &p->f)) return 0;
+    u = (size_t)maxUnits * sizeof(int64_t);
+    at = p->f.end;
+    p->files = at;    at = up256(at + (size_t)nFiles * sizeof(fc_file_rec));
+    p->uSrcOff = at;  at = up256(at + u);
+    p->uSrcSize = at; at = up256(at + u);
+    p->uDstOff = at;  at = up256(at + u);
+    p->uDstCap = at;  at = up256(at + u);
+    p->uResult = at;  at = up256(at + u);
+    p->bytes = at + 256;
+    return 1;
+}
+
+size_t LZ4B200_decompress_files_workspace_bytes(int64_t nFiles, int64_t maxUnits, const int64_t maxBlocks[LZ4B200_FILE_CLASSES])
+{
+    files_plan_t p;
+    return files_plan(nFiles, maxUnits, maxBlocks, &p) ? p.bytes : 0;
+}
+
+/* files index -> files scan -> files fill -> frames scan and fill on the units -> per class: scan (phase 1) -> [block
+ * checksums] -> totals, then either the fold (sizeOnly) or place -> verdict -> per class: expand (phase 2) -> raw blocks
+ * -> [content checksums] -> fold.  The unit steps are skipped when maxUnits is 0. */
+int LZ4B200_decompress_files(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
+                             void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
+                             int64_t* d_result, int64_t* d_consumed, int64_t* d_prefix,
+                             int64_t nFiles, int64_t maxUnits, const int64_t maxBlocks[LZ4B200_FILE_CLASSES],
+                             int skipChecksums, int sizeOnly,
+                             void* d_workspace, size_t workspaceBytes, void* stream)
+{
+    files_plan_t p;
+    lz4k_files_args a;
+    uint8_t* ws;
+    int rc;
+    const int mode = skipChecksums ? FC_SUMS_SKIP : FC_SUMS_VERIFY;
+    if (!files_plan(nFiles, maxUnits, maxBlocks, &p)) return LZ4B200_ERR_ARG;
+    if (nFiles == 0) return LZ4B200_OK;
+    if (!d_src || !d_srcOff || !d_srcSize || !d_result || !d_workspace) return LZ4B200_ERR_ARG;
+    if (!sizeOnly && (!d_dst || !d_dstOff || !d_dstCap)) return LZ4B200_ERR_ARG;
+    if (workspaceBytes < p.bytes) return LZ4B200_ERR_ARG;
+    ws = (uint8_t*)(((uintptr_t)d_workspace + 255) & ~(uintptr_t)255);
+    memset(&a, 0, sizeof a);
+    a.srcOff = d_srcOff; a.srcSize = d_srcSize;
+    a.dstOff = sizeOnly ? NULL : d_dstOff; a.dstCap = sizeOnly ? NULL : d_dstCap;
+    a.result = d_result; a.consumed = d_consumed; a.prefix = d_prefix;
+    a.nFiles = nFiles; a.maxUnits = maxUnits; a.sizeOnly = sizeOnly != 0;
+    a.files = ws + p.files;
+    a.u.src = (const uint8_t*)d_src; a.u.dst = sizeOnly ? NULL : (uint8_t*)d_dst;
+    a.u.srcOff = (const int64_t*)(ws + p.uSrcOff); a.u.srcSize = (const int64_t*)(ws + p.uSrcSize);
+    a.u.dstOff = (const int64_t*)(ws + p.uDstOff); a.u.dstCap = (const int64_t*)(ws + p.uDstCap);
+    a.u.result = (int64_t*)(ws + p.uResult); a.u.consumed = NULL; a.u.nFrames = maxUnits;
+    frames_args(&a.u, &p.f, ws, mode);
+
+    if ((rc = launched(lz4k_launch_files_index(&a, stream), "lz4k_launch_files_index")) != LZ4B200_OK) return rc;
+    if (maxUnits) {
+        if ((rc = frames_decode_phase(&a.u, &p.f, ws, 1, stream)) != LZ4B200_OK) return rc;
+        if (mode == FC_SUMS_VERIFY &&
+            (rc = launched(lz4k_launch_frames_block_sums(&a.u, stream), "lz4k_launch_frames_block_sums")) != LZ4B200_OK)
+            return rc;
+        if ((rc = launched(lz4k_launch_files_totals(&a, stream), "lz4k_launch_files_totals")) != LZ4B200_OK) return rc;
+        if (!sizeOnly) {
+            if ((rc = launched(lz4k_launch_files_place(&a, stream), "lz4k_launch_files_place")) != LZ4B200_OK) return rc;
+            if ((rc = launched(lz4k_launch_frames_verdict(&a.u, stream), "lz4k_launch_frames_verdict")) != LZ4B200_OK)
+                return rc;
+            if ((rc = frames_decode_phase(&a.u, &p.f, ws, 2, stream)) != LZ4B200_OK) return rc;
+            if ((rc = launched(lz4k_launch_frames_raw(&a.u, stream), "lz4k_launch_frames_raw")) != LZ4B200_OK) return rc;
+            if (mode == FC_SUMS_VERIFY &&
+                (rc = launched(lz4k_launch_frames_content_sums(&a.u, stream), "lz4k_launch_frames_content_sums")) != LZ4B200_OK)
+                return rc;
+        }
+    }
+    return launched(lz4k_launch_files_fold(&a, stream), "lz4k_launch_files_fold");
 }
 
 /* the encode launch arguments, every block size included (a split launch narrows minSize .. maxSize) */

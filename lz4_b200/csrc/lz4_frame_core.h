@@ -5,7 +5,9 @@
  * (lz4_kernels.cu, CUDA) both decide with these functions; tests/emul/frame_emul.cpp runs the batched call's index passes
  * on the host from the same text.  The writing side -- optimal block size ID, bound, header bytes and the index passes of
  * the batched frame encode -- serves LZ4B200_compressFrame_host and LZ4B200_compress_frames the same way
- * (tests/emul/compress_frames_emul.cpp).  No CUDA runtime calls, no allocation.
+ * (tests/emul/compress_frames_emul.cpp).  The file layer of LZ4B200_decompress_files -- the units of a .lz4 file, their
+ * placement and the fold of their results -- sits on the frame decode's rules (tests/emul/decompress_files_emul.cpp).
+ * No CUDA runtime calls, no allocation.
  */
 #ifndef LZ4_FRAME_CORE_H
 #define LZ4_FRAME_CORE_H
@@ -22,6 +24,7 @@
 
 #define FC_MAGIC           0x184D2204u     /* lz4frame.c: LZ4F_MAGICNUMBER */
 #define FC_MAGIC_SKIPPABLE 0x184D2A50u     /* .. LZ4F_MAGIC_SKIPPABLE_START */
+#define FC_MAGIC_LEGACY    0x184C2102u     /* lz4io.c: LEGACY_MAGICNUMBER, the `lz4 -l` format */
 
 FC_FN uint32_t fc_rd_le32(const uint8_t* p)
 {
@@ -76,6 +79,16 @@ FC_FN uint32_t fc_xxh32(const uint8_t* p, uint64_t len, uint32_t seed)
 }
 
 FC_FN int64_t fc_block_bytes(int bsid) { return (int64_t)1 << (8 + 2 * bsid); }   /* 4..7 -> 64 KB..4 MB (lz4frame.c:333-342) */
+
+/* The block classes of the batched decode: 0 .. 3 hold frame blocks of block size ID 4 + c, class 4 the blocks of a
+ * legacy stream (LZ4B200_decompress_files only; the frames calls give it a budget of 0). */
+#define FC_CLASSES      5
+#define FC_LEGACY_CLASS 4
+#define FC_LEGACY_BLOCK (8 << 20)          /* lz4io.c: LEGACY_BLOCKSIZE, the capacity a legacy block decodes with */
+#define FC_LEGACY_BOUND 8421520            /* LZ4_COMPRESSBOUND(8 MiB): a larger block word ends a legacy unit */
+
+/* the uniform capacity the blocks of class cls decode with */
+FC_FN int64_t fc_class_bytes(int cls) { return cls == FC_LEGACY_CLASS ? FC_LEGACY_BLOCK : fc_block_bytes(4 + cls); }
 
 /* ---------------------------------------------------------------------------------------------
  * Writing a frame of independent blocks (LZ4F_compressFrame, lz4frame.c:425-498): LZ4B200_compressFrame_host (no
@@ -217,6 +230,31 @@ FC_FN int fc_next_block(const uint8_t* src, int64_t srcSize, int64_t bs, int sum
     return 1;
 }
 
+/* One step of a legacy unit's chain (LZ4IO_decodeLegacyStream, lz4io.c:1836-1883) from the block word at *ip: 0 when the
+ * unit ends -- no bytes left, or a word above FC_LEGACY_BOUND, which is the next unit's magic (*ip stays on it) -- 1 for
+ * a block of that many compressed bytes (*at, *size; *ip moves past it), LZ4B200_ERR_FRAME for 1 .. 3 bytes left or a
+ * block cut short.  A block of 0 bytes is a block: its decode fails. */
+FC_FN int fc_next_legacy_block(const uint8_t* src, int64_t srcSize, int64_t* ip, int64_t* at, int64_t* size)
+{
+    uint32_t w;
+    if (*ip == srcSize) return 0;
+    if (*ip + 4 > srcSize) return LZ4B200_ERR_FRAME;
+    w = fc_rd_le32(src + *ip);
+    if (w > FC_LEGACY_BOUND) return 0;
+    if (*ip + 4 + (int64_t)w > srcSize) return LZ4B200_ERR_FRAME;
+    *at = *ip + 4; *size = (int64_t)w;
+    *ip += 4 + (int64_t)w;
+    return 1;
+}
+
+/* the chain step of a block of class cls: a frame's (fc_next_block) or a legacy unit's, whose blocks are never raw */
+FC_FN int fc_next_class_block(const uint8_t* src, int64_t srcSize, int cls, int sums, int64_t* ip, int64_t* at,
+                              int64_t* size, int* raw)
+{
+    if (cls == FC_LEGACY_CLASS) { *raw = 0; return fc_next_legacy_block(src, srcSize, ip, at, size); }
+    return fc_next_block(src, srcSize, fc_block_bytes(4 + cls), sums, ip, at, size, raw);
+}
+
 /* The verdict on one decoded block: r = its decoded size (a stored-raw block's size; negative: it failed to decode),
  * written at pos of a frame with dstCap bytes of room.  Decode failure, then the room, then the content size. */
 FC_FN int fc_block_verdict(int64_t pos, int64_t r, int64_t dstCap, int64_t contentSize)
@@ -255,7 +293,8 @@ typedef struct {
     int64_t contentSize;       /* as fc_header_t */
     int64_t consumed;          /* the frame's length once its chain is walked to the EndMark, else 0 */
     int32_t status;            /* LZ4B200_OK or the frame's error code so far */
-    int32_t cls;               /* block size ID - 4 (-1 before the header passed) */
+    int32_t cls;               /* block size ID - 4 (-1 before the header passed, and for a skippable frame);
+                                  FC_LEGACY_CLASS for a legacy unit of LZ4B200_decompress_files */
     int32_t hdrLen;
     int32_t sums;              /* fc_header_t.sums, | FC_VERIFY when the call compares them */
 } fc_frame_rec;
@@ -275,25 +314,36 @@ typedef struct {               /* a class's block table; entry b of every array 
 #define FC_SUM_PENDING 1           /* the fill found one; the block checksum kernel compares it */
 #define FC_SUM_BAD     2           /* it does not match */
 
-/* Pass 1 (the index): the header rules under `mode` (FC_SUMS_*), then the chain walk, which stops after
- * maxBlocks[cls] + 1 blocks (the frame is over its budget whatever follows).  src: the frame's first byte. */
-FC_FN void fc_index_frame_mode(const uint8_t* src, int64_t srcSize, int64_t dstCap, const int64_t* maxBlocks, int mode,
-                               fc_frame_rec* r)
+/* The chain walk of pass 1 from the end of r's header (r->cls, hdrLen and sums set), which stops after maxBlocks[cls] + 1
+ * blocks (the frame is over its budget whatever follows): r->count, and r->consumed once the chain ends. */
+FC_FN void fc_walk_chain(const uint8_t* src, int64_t srcSize, const int64_t* maxBlocks, fc_frame_rec* r)
 {
-    fc_header_t h;
-    int64_t ip, at, sz, n = 0;
+    int64_t ip = r->hdrLen, at, sz, n = 0;
     int raw, s;
-    r->count = 0; r->base = 0; r->contentSize = -1; r->consumed = 0; r->cls = -1; r->hdrLen = 0; r->sums = 0;
-    r->status = fc_frame_header(src, srcSize, dstCap, mode, &h);
-    if (r->status != LZ4B200_OK) return;
-    r->cls = h.bsid - 4; r->contentSize = h.contentSize; r->hdrLen = h.hdrLen;
-    r->sums = h.sums | ((h.sums && mode == FC_SUMS_VERIFY) ? FC_VERIFY : 0);
-    ip = h.hdrLen;
-    while ((s = fc_next_block(src, srcSize, fc_block_bytes(h.bsid), h.sums, &ip, &at, &sz, &raw)) == 1)
+    while ((s = fc_next_class_block(src, srcSize, r->cls, r->sums, &ip, &at, &sz, &raw)) == 1)
         if (++n > maxBlocks[r->cls]) break;
     if (s < 0) { r->status = s; return; }
     r->count = n;
     if (s == 0) r->consumed = ip;
+}
+
+FC_FN void fc_clear_rec(fc_frame_rec* r)
+{
+    r->count = 0; r->base = 0; r->contentSize = -1; r->consumed = 0; r->cls = -1; r->hdrLen = 0; r->sums = 0;
+    r->status = LZ4B200_OK;
+}
+
+/* Pass 1 (the index): the header rules under `mode` (FC_SUMS_*), then the chain walk.  src: the frame's first byte. */
+FC_FN void fc_index_frame_mode(const uint8_t* src, int64_t srcSize, int64_t dstCap, const int64_t* maxBlocks, int mode,
+                               fc_frame_rec* r)
+{
+    fc_header_t h;
+    fc_clear_rec(r);
+    r->status = fc_frame_header(src, srcSize, dstCap, mode, &h);
+    if (r->status != LZ4B200_OK) return;
+    r->cls = h.bsid - 4; r->contentSize = h.contentSize; r->hdrLen = h.hdrLen;
+    r->sums = h.sums | ((h.sums && mode == FC_SUMS_VERIFY) ? FC_VERIFY : 0);
+    fc_walk_chain(src, srcSize, maxBlocks, r);
 }
 
 /* pass 1 of LZ4B200_decompress_frames, which rejects checksums */
@@ -319,9 +369,9 @@ FC_FN void fc_fill_frame(const uint8_t* src, int64_t srcOff, int64_t srcSize, co
 {
     int64_t ip = r->hdrLen, at, sz, b = r->base;
     int raw;
-    if (r->status != LZ4B200_OK) return;
+    if (r->status != LZ4B200_OK || r->cls < 0) return;
     const int mark = (r->sums & FC_VERIFY) && (r->sums & FC_BLOCK_SUM);
-    while (fc_next_block(src, srcSize, fc_block_bytes(r->cls + 4), r->sums, &ip, &at, &sz, &raw) == 1) {
+    while (fc_next_class_block(src, srcSize, r->cls, r->sums, &ip, &at, &sz, &raw) == 1) {
         t.srcOff[b] = srcOff + at;
         t.srcSize[b] = raw ? 0 : (int32_t)sz;
         t.rawLen[b] = raw ? (int32_t)sz : -1;
@@ -353,6 +403,141 @@ FC_FN void fc_verdict_frame(const fc_frame_rec* r, int64_t dstOff, int64_t dstCa
     if (res < 0)
         for (k = 0; k < r->count; k++) { t.outSize[r->base + k] = -1; t.rawLen[r->base + k] = -1; }
     *result = res;
+}
+
+/* ---------------------------------------------------------------------------------------------
+ * The batched file decode (LZ4B200_decompress_files): a .lz4 file is a sequence of units -- LZ4 frames, skippable frames
+ * and legacy streams -- read as `lz4 -d` reads its standard input (selectDecoder, lz4io.c:2349-2405).  Every unit gets a
+ * fc_frame_rec and runs through the frame decode's steps as a frame of its own; the steps below give the units their
+ * records, their places in their file's output, and fold their results into one per file.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct {
+    int64_t units;             /* units the walk took (at most maxUnits + 1), the one that failed pass 1 included */
+    int64_t base;              /* the index of the file's first unit in the call's unit order (files, then units) */
+    int64_t overOff;           /* the offset of the file's first unit at index maxUnits or above (set by the fill) */
+    int32_t status;            /* LZ4B200_ERR_ARG (a negative size or room), else the pass-1 status of the last unit */
+    int32_t pad;
+} fc_file_rec;
+
+/* Pass 1 of the unit at src, rem >= 1 bytes before the file's end: the record fc_index_frame_mode gives an LZ4 frame
+ * (consumed 0: its chain was cut short by the budget), a record of no blocks for a skippable frame, a legacy unit of
+ * class FC_LEGACY_CLASS walked as a chain, or LZ4B200_ERR_FRAME for fewer than 4 bytes, a skippable frame that runs
+ * past the end (lz4io.c:2384-2391 on a pipe) and any other magic. */
+FC_FN void fc_next_unit(const uint8_t* src, int64_t rem, const int64_t* maxBlocks, int mode, fc_frame_rec* r)
+{
+    uint32_t magic;
+    fc_clear_rec(r);
+    r->status = LZ4B200_ERR_FRAME;
+    if (rem < 4) return;
+    magic = fc_rd_le32(src);
+    if (magic == FC_MAGIC) { fc_index_frame_mode(src, rem, 0, maxBlocks, mode, r); return; }
+    if ((magic & 0xFFFFFFF0u) == FC_MAGIC_SKIPPABLE) {
+        if (rem < 8 || 8 + (int64_t)fc_rd_le32(src + 4) > rem) return;
+        r->status = LZ4B200_OK;
+        r->consumed = 8 + (int64_t)fc_rd_le32(src + 4);
+        return;
+    }
+    if (magic != FC_MAGIC_LEGACY) return;
+    r->status = LZ4B200_OK;
+    r->cls = FC_LEGACY_CLASS;
+    r->hdrLen = 4;
+    fc_walk_chain(src, rem, maxBlocks, r);
+}
+
+/* The walk of one file (srcSize bytes, dstCap of room; dstCap 0 when the call only sizes): unit after unit until the
+ * end, a unit that fails pass 1 or stops short on its budget, or maxUnits + 1 units -- the file is then over the unit
+ * budget whatever follows. */
+FC_FN void fc_index_file(const uint8_t* src, int64_t srcSize, int64_t dstCap, int64_t maxUnits, const int64_t* maxBlocks,
+                         int mode, fc_file_rec* f)
+{
+    fc_frame_rec r;
+    int64_t p = 0;
+    f->units = 0; f->base = 0; f->overOff = 0; f->status = LZ4B200_OK; f->pad = 0;
+    if (srcSize < 0 || dstCap < 0) { f->status = LZ4B200_ERR_ARG; return; }
+    while (p < srcSize && f->units <= maxUnits) {
+        fc_next_unit(src + p, srcSize - p, maxBlocks, mode, &r);
+        f->units++;
+        if (r.status != LZ4B200_OK || r.consumed == 0) { f->status = r.status; return; }
+        p += r.consumed;
+    }
+}
+
+/* After the scan of the unit counts (f->base): the walk again, writing the record, absolute source offset and length
+ * (the rest of the file for a unit whose end pass 1 did not reach) of every unit below index maxUnits. */
+FC_FN void fc_fill_file(const uint8_t* src, int64_t srcOff, int64_t srcSize, int64_t maxUnits, const int64_t* maxBlocks,
+                        int mode, fc_file_rec* f, fc_frame_rec* units, int64_t* uSrcOff, int64_t* uSrcSize)
+{
+    int64_t p = 0, k;
+    for (k = 0; k < f->units; k++) {
+        const int64_t u = f->base + k;
+        if (u >= maxUnits) { f->overOff = p; return; }
+        fc_next_unit(src + p, srcSize - p, maxBlocks, mode, &units[u]);
+        uSrcOff[u] = srcOff + p;
+        uSrcSize[u] = units[u].consumed ? units[u].consumed : srcSize - p;
+        p += units[u].consumed;
+    }
+}
+
+/* A unit's totals, after the scans of its blocks (and their checksums): the verdict of fc_verdict_frame with unlimited
+ * room and no placement -- its decoded size, or its error code.  The content checksum is not part of it. */
+FC_FN int64_t fc_totals_frame(const fc_frame_rec* r, fc_block_tab t)
+{
+    int64_t pos = 0, k;
+    int v = LZ4B200_OK;
+    const int verifyBlocks = (r->sums & FC_VERIFY) && (r->sums & FC_BLOCK_SUM);
+    if (r->status != LZ4B200_OK) return r->status;
+    for (k = 0; k < r->count && v == LZ4B200_OK; k++) {
+        const int64_t b = r->base + k;
+        const int64_t rb = t.rawLen[b] >= 0 ? t.rawLen[b] : t.outSize[b];
+        v = fc_block_sum_verdict(pos, rb, INT64_MAX, r->contentSize, t.rawLen[b] >= 0, verifyBlocks && t.dstOff[b] == FC_SUM_BAD);
+        pos += rb < 0 ? 0 : rb;
+    }
+    return v != LZ4B200_OK ? (int64_t)v : fc_frame_result(pos, r->contentSize);
+}
+
+/* The placement of a file's units (dstOff, dstCap: the file's), before the verdict: every recorded unit gets the next
+ * free byte of the file's output and the room left, until the first whose totals fail or do not fit -- the verdict
+ * gives it its code in the frame order.  The units after it get room -1, so that the verdict fails them before any of
+ * their bytes is placed. */
+FC_FN void fc_place_file(const fc_file_rec* f, int64_t dstOff, int64_t dstCap, int64_t maxUnits, const int64_t* totals,
+                         int64_t* uDstOff, int64_t* uDstCap)
+{
+    int64_t pos = 0, k;
+    int failed = 0;
+    for (k = 0; k < f->units && f->base + k < maxUnits; k++) {
+        const int64_t u = f->base + k, t = totals[u];
+        uDstOff[u] = dstOff + pos;
+        uDstCap[u] = failed ? -1 : dstCap - pos;
+        if (failed) continue;
+        if (t < 0 || t > dstCap - pos) failed = 1;
+        else pos += t;
+    }
+}
+
+/* The fold: the file's result (decoded bytes, or the code of its first failing unit in file order), consumed (srcSize,
+ * or that unit's offset) and prefix (the decoded bytes of the units before it).  uResult: every recorded unit's result
+ * (the verdict's, or its totals when the call only sizes).  A unit at index maxUnits or above has no record: it fails
+ * pass 1 with its own code (the walk's last unit), else it is LZ4B200_ERR_LIMIT. */
+FC_FN void fc_fold_file(const fc_file_rec* f, int64_t srcOff, int64_t srcSize, int64_t maxUnits, const int64_t* uResult,
+                        const int64_t* uSrcOff, int64_t* result, int64_t* consumed, int64_t* prefix)
+{
+    int64_t pos = 0, at = srcSize, res = 0, k;
+    if (f->status == LZ4B200_ERR_ARG) { res = LZ4B200_ERR_ARG; at = 0; }
+    for (k = 0; k < f->units && res >= 0; k++) {
+        const int64_t u = f->base + k;
+        if (u >= maxUnits) {
+            res = (k + 1 == f->units && f->status != LZ4B200_OK) ? (int64_t)f->status : (int64_t)LZ4B200_ERR_LIMIT;
+            at = f->overOff;
+        } else if (uResult[u] < 0) {
+            res = uResult[u];
+            at = uSrcOff[u] - srcOff;
+        } else {
+            pos += uResult[u];
+        }
+    }
+    *result = res < 0 ? res : pos;
+    if (consumed) *consumed = at;
+    if (prefix) *prefix = pos;
 }
 
 /* ---------------------------------------------------------------------------------------------

@@ -1381,50 +1381,50 @@ constexpr int kFsThreads = 1024, kFsItems = 4;            /* frames scan: kFsIte
 
 __global__ void __launch_bounds__(kFsThreads) lz4_frames_scan_kernel(lz4k_frames_args a)
 {
-    __shared__ int64_t warpSums[4][32];
-    __shared__ int64_t carry[4];
+    __shared__ int64_t warpSums[FC_CLASSES][32];
+    __shared__ int64_t carry[FC_CLASSES];
     fc_frame_rec* rec = static_cast<fc_frame_rec*>(a.frames);
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    if (threadIdx.x < 4) carry[threadIdx.x] = 0;
+    if (threadIdx.x < FC_CLASSES) carry[threadIdx.x] = 0;
     __syncthreads();
     for (int64_t base = 0; base < a.nFrames; base += kFsThreads * kFsItems) {
         const int64_t f0 = base + (int64_t)threadIdx.x * kFsItems;
-        int64_t v[4] = {0, 0, 0, 0}, x[4];
+        int64_t v[FC_CLASSES] = {0, 0, 0, 0, 0}, x[FC_CLASSES];
         #pragma unroll
         for (int i = 0; i < kFsItems; i++) {
             if (f0 + i >= a.nFrames) break;
             const int64_t n = fc_scan_count(&rec[f0 + i]);
             const int cls = rec[f0 + i].cls;
             #pragma unroll
-            for (int c = 0; c < 4; c++) v[c] += cls == c ? n : 0;
+            for (int c = 0; c < FC_CLASSES; c++) v[c] += cls == c ? n : 0;
         }
         #pragma unroll
-        for (int c = 0; c < 4; c++) {
+        for (int c = 0; c < FC_CLASSES; c++) {
             x[c] = v[c];
             for (int d = 1; d < 32; d <<= 1) { const int64_t y = __shfl_up_sync(kFull, x[c], d); if (lane >= d) x[c] += y; }
             if (lane == 31) warpSums[c][wid] = x[c];
         }
         __syncthreads();
-        if (wid < 4) {                                        /* warp c scans class c's warp sums */
+        if (wid < FC_CLASSES) {                               /* warp c scans class c's warp sums */
             int64_t s = warpSums[wid][lane];
             for (int d = 1; d < 32; d <<= 1) { const int64_t y = __shfl_up_sync(kFull, s, d); if (lane >= d) s += y; }
             warpSums[wid][lane] = s;
         }
         __syncthreads();
-        int64_t pre[4];
+        int64_t pre[FC_CLASSES];
         #pragma unroll
-        for (int c = 0; c < 4; c++) pre[c] = carry[c] + (wid ? warpSums[c][wid - 1] : 0) + x[c] - v[c];
+        for (int c = 0; c < FC_CLASSES; c++) pre[c] = carry[c] + (wid ? warpSums[c][wid - 1] : 0) + x[c] - v[c];
         #pragma unroll
         for (int i = 0; i < kFsItems; i++) {
             if (f0 + i >= a.nFrames) break;
             fc_frame_rec* r = &rec[f0 + i];
             const int64_t n = fc_scan_count(r);
             #pragma unroll
-            for (int c = 0; c < 4; c++)
+            for (int c = 0; c < FC_CLASSES; c++)
                 if (r->cls == c) { fc_place_frame(r, pre[c], a.maxBlocks); pre[c] += n; }
         }
         __syncthreads();                                      /* every thread has read carry */
-        if (threadIdx.x == kFsThreads - 1) for (int c = 0; c < 4; c++) carry[c] = pre[c];
+        if (threadIdx.x == kFsThreads - 1) for (int c = 0; c < FC_CLASSES; c++) carry[c] = pre[c];
         __syncthreads();
     }
 }
@@ -1668,6 +1668,91 @@ __global__ void __launch_bounds__(32 * kXsWarps) lz4_frames_content_sum_kernel(l
 }
 
 /* =============================================================================================
+ * batched file decode (LZ4B200_decompress_files): the file rules of lz4_frame_core.h around the frame decode's steps,
+ * which take every unit of every file as a frame of their own (lz4k_files_args.u)
+ *   index : one thread per file -- the walk of its units (fc_index_file)
+ *   scan  : one CTA -- the exclusive sum of the unit counts in file order: each file's first unit index
+ *   fill  : one thread per file -- the walk again, a record per unit below the unit budget (fc_fill_file); then the
+ *           frame decode's budget scan and table fill on the unit records
+ *   totals: after the scans of the blocks -- one thread per unit: its decoded size or error with unlimited room
+ *   place : one thread per file -- each unit's place and room, the units after the first failure given room -1
+ *   fold  : last, one thread per file -- result, consumed and prefix from the unit results
+ * ============================================================================================= */
+__global__ void __launch_bounds__(128) lz4_files_index_kernel(lz4k_files_args a)
+{
+    const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= a.nFiles) return;
+    fc_index_file(a.u.src + a.srcOff[f], a.srcSize[f], a.sizeOnly ? 0 : a.dstCap[f], a.maxUnits, a.u.maxBlocks, a.u.mode,
+                  static_cast<fc_file_rec*>(a.files) + f);
+}
+
+__global__ void __launch_bounds__(kFsThreads) lz4_files_scan_kernel(lz4k_files_args a)
+{
+    __shared__ int64_t warpSums[32];
+    __shared__ int64_t carry;
+    fc_file_rec* rec = static_cast<fc_file_rec*>(a.files);
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    if (threadIdx.x == 0) carry = 0;
+    __syncthreads();
+    for (int64_t base = 0; base < a.nFiles; base += kFsThreads * kFsItems) {
+        const int64_t f0 = base + (int64_t)threadIdx.x * kFsItems;
+        int64_t v = 0;
+        #pragma unroll
+        for (int i = 0; i < kFsItems; i++) if (f0 + i < a.nFiles) v += rec[f0 + i].units;
+        int64_t x = v;
+        for (int d = 1; d < 32; d <<= 1) { const int64_t y = __shfl_up_sync(kFull, x, d); if (lane >= d) x += y; }
+        if (lane == 31) warpSums[wid] = x;
+        __syncthreads();
+        if (wid == 0) {
+            int64_t t = warpSums[lane];
+            for (int d = 1; d < 32; d <<= 1) { const int64_t y = __shfl_up_sync(kFull, t, d); if (lane >= d) t += y; }
+            warpSums[lane] = t;
+        }
+        __syncthreads();
+        int64_t pre = carry + (wid ? warpSums[wid - 1] : 0) + x - v;
+        #pragma unroll
+        for (int i = 0; i < kFsItems; i++)
+            if (f0 + i < a.nFiles) { rec[f0 + i].base = pre; pre += rec[f0 + i].units; }
+        __syncthreads();                                      /* every thread has read carry */
+        if (threadIdx.x == kFsThreads - 1) carry = pre;
+        __syncthreads();
+    }
+}
+
+__global__ void __launch_bounds__(128) lz4_files_fill_kernel(lz4k_files_args a)
+{
+    const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= a.nFiles) return;
+    fc_fill_file(a.u.src + a.srcOff[f], a.srcOff[f], a.srcSize[f], a.maxUnits, a.u.maxBlocks, a.u.mode,
+                 static_cast<fc_file_rec*>(a.files) + f, static_cast<fc_frame_rec*>(a.u.frames),
+                 const_cast<int64_t*>(a.u.srcOff), const_cast<int64_t*>(a.u.srcSize));
+}
+
+__global__ void __launch_bounds__(128) lz4_files_totals_kernel(lz4k_files_args a)
+{
+    const int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (u >= a.u.nFrames) return;
+    const fc_frame_rec* r = static_cast<const fc_frame_rec*>(a.u.frames) + u;
+    a.u.result[u] = fc_totals_frame(r, frames_tab(a.u, r->cls));
+}
+
+__global__ void __launch_bounds__(128) lz4_files_place_kernel(lz4k_files_args a)
+{
+    const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= a.nFiles) return;
+    fc_place_file(static_cast<const fc_file_rec*>(a.files) + f, a.dstOff[f], a.dstCap[f], a.maxUnits, a.u.result,
+                  const_cast<int64_t*>(a.u.dstOff), const_cast<int64_t*>(a.u.dstCap));
+}
+
+__global__ void __launch_bounds__(128) lz4_files_fold_kernel(lz4k_files_args a)
+{
+    const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= a.nFiles) return;
+    fc_fold_file(static_cast<const fc_file_rec*>(a.files) + f, a.srcOff[f], a.srcSize[f], a.maxUnits, a.u.result,
+                 a.u.srcOff, a.result + f, a.consumed ? a.consumed + f : nullptr, a.prefix ? a.prefix + f : nullptr);
+}
+
+/* =============================================================================================
  * batched frame encode (LZ4B200_compress_frames, LZ4B200_compress_frames_checksummed): the frame rules of
  * lz4_frame_core.h around one encode of the whole block table (by the caller) and the pack scan and gather
  *   index : pass 1 -- one thread per frame: optimal block size ID, block count, header length, argument and capacity
@@ -1800,19 +1885,65 @@ uint64_t lz4k_launch_count(void) { return g_launches.load(); }
 
 static unsigned frames_grid(int64_t n) { return (unsigned)((n + 127) / 128); }
 
-int lz4k_launch_frames_index(const lz4k_frames_args* a, void* stream)
+/* the budget scan, then the table cleared and filled, on index records already in a->frames */
+static cudaError_t frames_tables(const lz4k_frames_args* a, cudaStream_t s)
 {
-    cudaStream_t s = (cudaStream_t)stream;
-    lz4_frames_index_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);
     lz4_frames_scan_kernel<<<1, kFsThreads, 0, s>>>(*a);
-    g_launches += 2;
+    g_launches++;
     /* unused entries decode nothing: size 0 (the scan rejects them) and no raw bytes */
     cudaError_t e = cudaMemsetAsync(a->tabSrcSize, 0, (size_t)a->nEntries * sizeof(int32_t), s);
     if (e == cudaSuccess) e = cudaMemsetAsync(a->tabRawLen, 0xFF, (size_t)a->nEntries * sizeof(int32_t), s);
     /* every entry's block checksum state FC_SUM_NONE, before the fill marks the ones to compare */
     if (e == cudaSuccess && a->mode == FC_SUMS_VERIFY) e = cudaMemsetAsync(a->tabDstOff, 0, (size_t)a->nEntries * sizeof(int64_t), s);
-    if (e != cudaSuccess) return (int)e;
+    if (e != cudaSuccess) return e;
     lz4_frames_fill_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);
+    g_launches++;
+    return cudaGetLastError();
+}
+
+int lz4k_launch_frames_index(const lz4k_frames_args* a, void* stream)
+{
+    cudaStream_t s = (cudaStream_t)stream;
+    lz4_frames_index_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);
+    g_launches++;
+    return (int)frames_tables(a, s);
+}
+
+/* Records of units past the last file's stay 0xFF bytes: status -1 and class -1, which every later step passes over.
+ * Without unit records (maxUnits 0) only the files' own steps run. */
+int lz4k_launch_files_index(const lz4k_files_args* a, void* stream)
+{
+    cudaStream_t s = (cudaStream_t)stream;
+    const unsigned grid = frames_grid(a->nFiles);
+    lz4_files_index_kernel<<<grid, 128, 0, s>>>(*a);
+    lz4_files_scan_kernel<<<1, kFsThreads, 0, s>>>(*a);
+    g_launches += 2;
+    if (a->maxUnits) {
+        const cudaError_t e = cudaMemsetAsync(a->u.frames, 0xFF, (size_t)a->maxUnits * sizeof(fc_frame_rec), s);
+        if (e != cudaSuccess) return (int)e;
+    }
+    lz4_files_fill_kernel<<<grid, 128, 0, s>>>(*a);
+    g_launches++;
+    return a->maxUnits ? (int)frames_tables(&a->u, s) : (int)cudaGetLastError();
+}
+
+int lz4k_launch_files_totals(const lz4k_files_args* a, void* stream)
+{
+    lz4_files_totals_kernel<<<frames_grid(a->maxUnits), 128, 0, (cudaStream_t)stream>>>(*a);
+    g_launches++;
+    return (int)cudaGetLastError();
+}
+
+int lz4k_launch_files_place(const lz4k_files_args* a, void* stream)
+{
+    lz4_files_place_kernel<<<frames_grid(a->nFiles), 128, 0, (cudaStream_t)stream>>>(*a);
+    g_launches++;
+    return (int)cudaGetLastError();
+}
+
+int lz4k_launch_files_fold(const lz4k_files_args* a, void* stream)
+{
+    lz4_files_fold_kernel<<<frames_grid(a->nFiles), 128, 0, (cudaStream_t)stream>>>(*a);
     g_launches++;
     return (int)cudaGetLastError();
 }

@@ -89,8 +89,8 @@ typedef struct {
     int64_t* result;           /* [nFrames] */
     int64_t* consumed;         /* [nFrames] or NULL */
     int64_t nFrames;
-    int64_t maxBlocks[4];      /* the budget of every class */
-    int64_t tabBase[4];        /* class c's entries of the block table start at tabBase[c] */
+    int64_t maxBlocks[5];      /* the budget of every class (FC_CLASSES; the frames calls give class 4 none) */
+    int64_t tabBase[5];        /* class c's entries of the block table start at tabBase[c] */
     int64_t nEntries;          /* entries of the block table (sum of maxBlocks) */
     int mode;                  /* FC_SUMS_* (lz4_frame_core.h): the checksum flags rejected, skipped or verified */
     void* frames;              /* fc_frame_rec[nFrames] */
@@ -107,6 +107,32 @@ int lz4k_launch_frames_raw(const lz4k_frames_args* a, void* stream);
 int lz4k_launch_frames_block_sums(const lz4k_frames_args* a, void* stream);
 /* FC_SUMS_VERIFY: the content checksum of every frame that passed, after the raw blocks */
 int lz4k_launch_frames_content_sums(const lz4k_frames_args* a, void* stream);
+/* the batched file decode's own steps (lz4_frame_core.h): its units run through the frame decode's steps as the frames
+ * of `u`, whose per-frame tables (srcOff, srcSize, dstOff, dstCap, result) are the units' own, in the workspace */
+typedef struct {
+    const int64_t* srcOff;     /* file f is u.src + srcOff[f], srcSize[f] bytes */
+    const int64_t* srcSize;
+    const int64_t* dstOff;     /* file f decodes to u.dst + dstOff[f], dstCap[f] bytes of room (NULL when sizing) */
+    const int64_t* dstCap;
+    int64_t* result;           /* [nFiles] */
+    int64_t* consumed;         /* [nFiles] or NULL */
+    int64_t* prefix;           /* [nFiles] or NULL */
+    int64_t nFiles;
+    int64_t maxUnits;          /* records of u (u.nFrames) */
+    int sizeOnly;
+    void* files;               /* fc_file_rec[nFiles] */
+    lz4k_frames_args u;
+} lz4k_files_args;
+
+/* the walk of every file, the scan of the unit counts, the unit records (fill), then the frame decode's budget scan and
+ * table fill on them (as lz4k_launch_frames_index) */
+int lz4k_launch_files_index(const lz4k_files_args* a, void* stream);
+/* after the scans of the blocks (and the block checksums): every unit's totals into u.result */
+int lz4k_launch_files_totals(const lz4k_files_args* a, void* stream);
+/* after the totals: every unit's place and room (u.dstOff, u.dstCap); the frame verdict follows */
+int lz4k_launch_files_place(const lz4k_files_args* a, void* stream);
+/* last: every file's result, consumed and prefix from the unit results */
+int lz4k_launch_files_fold(const lz4k_files_args* a, void* stream);
 /* the batched frame encode's own steps (lz4_frame_core.h); the encode of the block table between them is the caller's */
 typedef struct {
     const uint8_t* src;        /* frame f's source is src + srcOff[f], srcSize[f] bytes */
