@@ -454,6 +454,50 @@ LZ4B200_API int LZ4B200_compress_frames_checksummed(const void* d_src, const int
                                                     void* d_workspace, size_t workspaceBytes, void* stream);
 
 /*
+ * Write nFiles `lz4 -l` legacy streams -- the format the reference tool's help calls "Linux kernel compression" -- from
+ * sources in device memory, at every compression level (LZ4IO_compressLegacy_internal, programs/lz4io.c:766-910):
+ *   file f input : d_src + d_srcOff[f], n_f = d_srcSize[f] bytes
+ *   file f output: d_dst + d_dstOff[f], capacity d_dstCap[f]
+ *   d_result[f]  : in this order, LZ4B200_ERR_ARG (n_f < 0 or d_dstCap[f] < 0), LZ4B200_ERR_DSTSIZE (d_dstCap[f] below
+ *                  LZ4B200_compressLegacyBound(n_f)), LZ4B200_ERR_LIMIT (below), else the stream's length
+ * File f's output is, byte for byte, what `lz4 -l -c -<level>` (`--fast=N` for level -N) writes for src_f piped to its
+ * standard input: the LE32 magic 0x184C2102, then for every 8 MiB chunk of the source (the last one may be short) the LE32
+ * compressed size and the compressed block.  There is no EndMark, no checksum and no stored-raw block: an incompressible
+ * chunk is written compressed, larger than its input.  An empty source gives the 4-byte magic alone.  The level mapping is
+ * the tool's, not LZ4B200_compress_frames's: levels below 3 use LZ4_compress_fast with acceleration -level for negative
+ * levels (above 65 537 as 65 537; --fast=N is acceleration N, where a frame gets N + 1) and 1 otherwise, so level 2 is
+ * the fast parse; levels 3 and up use LZ4_compress_HC (above 12 read as 12): 3 .. 9 through the hash-chain kernel of
+ * LZ4B200_compress_blocks_hc, 10 .. 12 through the optimal parser.  Every chunk is compressed with capacity
+ * LZ4_compressBound(chunk), as the tool's room of LZ4_compressBound(8 MiB) + 4 never limits it.  No parallel parse is
+ * offered: it takes blocks of at most 64 KB, and every chunk but a short last one is 8 MiB.
+ *
+ * LZ4B200_compressLegacyBound(n) = 4 + the sum over the chunks of 4 + LZ4_compressBound(chunk); the tool has no capacity
+ * of its own, so LZ4B200_ERR_DSTSIZE follows LZ4B200_compress_frames's convention: it is decided before encoding.  Only
+ * [dst_f, dst_f + d_result[f]) is written, nothing for a failed file; outputs may abut, and must not overlap one another,
+ * any source or the workspace.  Destinations are byte-aligned anywhere.  Readable padding is that of the encoder that
+ * runs: at levels 3 and up, the aligned 4-byte words holding a source's bytes.
+ *
+ * The budget: maxBlocks bounds the 8 MiB chunks the call compresses, with LZ4B200_compress_frames's rule word for word
+ * over one class: a file gets LZ4B200_ERR_LIMIT when the chunks of the earlier files that passed the checks above, plus
+ * its own, exceed maxBlocks.  The host sizes everything from it, so the call never synchronises and can be captured into
+ * a CUDA graph.  The workspace (LZ4B200_compress_legacy_workspace_bytes; 0 for arguments the call rejects) holds 48 bytes
+ * per file, 48 per budgeted chunk, a slot of LZ4_compressBound(8 MiB) per budgeted chunk and, at levels 3 and up, the
+ * workspace of LZ4B200_compress_blocks_hc (levels 3 .. 9) or LZ4B200_compress_blocks_hc_opt (10 and up) for maxBlocks
+ * blocks.
+ *
+ * Cost: one warp parses each chunk at the fast levels, one thread at levels 3 and up, so a single large file is few
+ * lanes of work; DESIGN section 3.16 has the measured times.  Kernel launches: 7; 5 when maxBlocks is 0.  nFiles == 0
+ * returns LZ4B200_OK without one.  LZ4B200_ERR_ARG: nFiles < 0 or maxBlocks outside 0 .. 2^31 - 1, then (with files
+ * present) a NULL pointer or a workspace smaller than the size function asks.
+ */
+LZ4B200_API int64_t LZ4B200_compressLegacyBound(int64_t srcSize);      /* LZ4B200_ERR_ARG for srcSize < 0 */
+LZ4B200_API size_t LZ4B200_compress_legacy_workspace_bytes(int64_t nFiles, int64_t maxBlocks, int compressionLevel);
+LZ4B200_API int LZ4B200_compress_legacy(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
+                                        void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
+                                        int64_t* d_result, int64_t nFiles, int compressionLevel, int64_t maxBlocks,
+                                        void* d_workspace, size_t workspaceBytes, void* stream);
+
+/*
  * Compress nBlocks independent blocks (the batched LZ4_compress_fast; replaces bench.c:464-493 and
  * lz4frame.c:1046-1055).
  *   block i input : d_src + i*srcStride, size (d_srcSize ? d_srcSize[i] : srcSize)

@@ -52,6 +52,9 @@ PROTOTYPES = [
                                           C.POINTER(_i64), _vp, _sz, _vp]),
     ("LZ4B200_compress_frames_checksummed", C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, C.c_int, C.c_int, C.c_int,
                                                       C.c_int, C.c_int, C.c_int, C.POINTER(_i64), _vp, _sz, _vp]),
+    ("LZ4B200_compressLegacyBound", _i64, [_i64]),
+    ("LZ4B200_compress_legacy_workspace_bytes", _sz, [_i64, _i64, C.c_int]),
+    ("LZ4B200_compress_legacy", C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, C.c_int, _i64, _vp, _sz, _vp]),
     ("LZ4B200_compress_blocks", C.c_int, [_vp, _i64, _vp, _i32, _vp, _i64, _i32, C.c_int, _vp, _i64, _vp]),
     ("LZ4B200_compress_blocks_destSize", C.c_int, [_vp, _i64, _vp, _i32, _vp, _i64, _i32, C.c_int, _vp, _vp, _i64, _vp]),
     ("LZ4B200_compress_blocks_hc_workspace_bytes", _sz, [_i64]),

@@ -497,6 +497,75 @@ def _compress_frames(name, sums, src, offsets, sizes, max_blocks, block_size_id,
     return out, results[:n]
 
 
+LEGACY_BLOCK = 8 << 20          # the chunk an `lz4 -l` stream compresses at a time
+
+
+def legacy_bound(n):
+    """LZ4B200_compressLegacyBound: the longest `lz4 -l` stream of n bytes, 4 + the sum over its 8 MiB chunks of 4 +
+    LZ4_compressBound(chunk) (LZ4B200_ERR_ARG for n < 0)"""
+    return int(_lib.load().LZ4B200_compressLegacyBound(int(n)))
+
+
+def compress_legacy_workspace_bytes(n_files, max_blocks, level=1):
+    """LZ4B200_compress_legacy_workspace_bytes: the workspace compress_legacy needs (0: arguments it rejects)"""
+    return int(_lib.load().LZ4B200_compress_legacy_workspace_bytes(int(n_files), int(max_blocks), int(level)))
+
+
+def compress_legacy(src, offsets, sizes, max_blocks=None, level=1, out=None, out_offsets=None, capacities=None,
+                    results=None, workspace=None, stream=None):
+    """Write len(sizes) `lz4 -l` legacy streams from buffers in device memory (LZ4B200_compress_legacy): stream f is,
+    byte for byte, what `lz4 -l -c -<level>` (`--fast=N` for level -N) writes for src[offsets[f] : offsets[f]+sizes[f]]
+    piped to its standard input -- the magic, then per 8 MiB chunk its LE32 compressed size and block.  The level
+    mapping is the tool's: below 3 the fast parse (acceleration -level for negative levels), 3 and up LZ4_compress_HC.
+
+    offsets, sizes: int64 device tensors.  Stream f is written at out[out_offsets[f]:] with capacities[f] bytes of room
+    (int64 device tensors).  max_blocks: the 8 MiB chunks the call compresses at most (a host int); a file past it gets
+    LZ4B200_ERR_LIMIT (-6).  Left as None, max_blocks and capacities are computed from sizes read on the host
+    (capacities: legacy_bound per file), which is a host sync: under stream capture max_blocks, out and capacities must
+    be given.  out_offsets defaults to the exclusive sum of the capacities and out to their total.
+    Returns (out, results): results[f] is the stream's length, or LZ4B200_ERR_ARG (a negative size or capacity),
+    LZ4B200_ERR_DSTSIZE (a capacity below legacy_bound) or LZ4B200_ERR_LIMIT.
+    """
+    name = "compress_legacy"
+    lib = _lib.load()
+    n = int(sizes.numel()) if isinstance(sizes, torch.Tensor) else 0
+    if torch.cuda.is_current_stream_capturing() and (max_blocks is None or out is None or capacities is None):
+        raise ValueError("%s under stream capture needs max_blocks=, out= and capacities= (computing them "
+                         "reads sizes on the host)" % name)
+    at_least_n = (n, None)
+    device, st = _checked(name, stream,
+                          [("src", src, U8, ANY), ("offsets", offsets, I64, at_least_n), ("sizes", sizes, I64, ANY),
+                           ("out", out, U8, ANY), ("out_offsets", out_offsets, I64, at_least_n),
+                           ("capacities", capacities, I64, (n, n)), ("results", results, I64, at_least_n),
+                           ("workspace", workspace, U8, ANY)],
+                          [_int32("level", level)])
+    if max_blocks is None or capacities is None:
+        host_sizes = sizes.tolist()
+        need = sum((s + LEGACY_BLOCK - 1) // LEGACY_BLOCK for s in host_sizes if s >= 0)
+        caps = [max(legacy_bound(max(s, 0)), 0) for s in host_sizes]
+    budget = int(max_blocks) if max_blocks is not None else need
+    ws_bytes = compress_legacy_workspace_bytes(n, budget, level)
+    if ws_bytes == 0:
+        raise ValueError("%s: max_blocks must be 0 .. 2^31 - 1 (got %d)" % (name, budget))
+    if workspace is not None and workspace.numel() < ws_bytes:
+        raise ValueError("%s: workspace has %d elements, the call needs at least %d"
+                         % (name, workspace.numel(), ws_bytes))
+    workspace = _workspace(device, ws_bytes, st, workspace, name)
+    with torch.cuda.stream(st):                     # temporaries belong to the stream the kernels run on
+        if capacities is None:
+            capacities = torch.tensor(caps, dtype=I64, device=device)
+        if out_offsets is None:
+            out_offsets = torch.cumsum(capacities.clamp(min=0), 0) - capacities.clamp(min=0)
+        if out is None:
+            out = torch.empty(max(int(capacities.clamp(min=0).sum()) if n else 0, 1), dtype=torch.uint8, device=device)
+        if results is None:
+            results = torch.empty(max(n, 1), dtype=torch.int64, device=device)
+    _launch(device, "LZ4B200_" + name, lib.LZ4B200_compress_legacy, src.data_ptr(), offsets.data_ptr(),
+            sizes.data_ptr(), out.data_ptr(), out_offsets.data_ptr(), capacities.data_ptr(), results.data_ptr(), n,
+            int(level), budget, workspace.data_ptr(), workspace.numel(), st.cuda_stream)
+    return out, results[:n]
+
+
 def compress_blocks(src, block_size, acceleration=1, slots=None, slot_stride=None, slot_capacity=None,
                     out_sizes=None, src_sizes=None, stream=None, mode="exact"):
     """Compress src (u8 device tensor) as ceil(len/block_size) independent blocks.

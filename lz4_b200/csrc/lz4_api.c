@@ -675,28 +675,31 @@ int LZ4B200_pack_frame_blocks(const void* d_slots, int64_t slotStride, const int
                     "lz4k_launch_pack_frame");
 }
 
-/* The workspace of LZ4B200_compress_frames, from the budget and the level alone: the frame records, the block table of
+/* The workspace of the frame-encode calls (LZ4B200_compress_frames, LZ4B200_compress_frames_checksummed,
+ * LZ4B200_compress_legacy), from the budget of every class and the encode alone: the frame records, the block table of
  * every class (entries tabBase[c] .. tabBase[c] + maxBlocks[c] - 1: source offset, size, slot offset, capacity, result,
- * the pack scan, the place), one slot of blockSize - 1 bytes rounded up to 16 per budgeted block, and for levels 2 and
- * up the HC encoder's workspace for the whole table.  Regions start on 256 bytes, as in frames_plan. */
+ * the pack scan, the place), one slot per budgeted block -- blockSize - 1 bytes for a frame block, LZ4_compressBound(8 MiB)
+ * for a legacy block, rounded up to 16 -- and, when the encode is an HC one (hcLevel > 0), the HC encoder's workspace for
+ * the whole table.  Regions start on 256 bytes, as in frames_plan. */
 typedef struct {
     size_t frames, srcOff, srcSize, slotOff, cap, outSize, bodyOff, packOff, slots, hc, hcBytes, bytes;
-    int64_t tabBase[4], slotBase[4], slotStride[4], nEntries;
+    int64_t tabBase[FC_CLASSES], slotBase[FC_CLASSES], slotStride[FC_CLASSES], nEntries;
 } cframes_plan_t;
 
-/* 0 for arguments the call rejects (nFrames < 0, a NULL budget, an entry outside 0 .. FRAMES_MAX_BUDGET) */
-static int cframes_plan(int64_t nFrames, const int64_t* maxBlocks, int level, cframes_plan_t* p)
+/* 0 for arguments the call rejects (nFrames < 0, a NULL budget, an entry outside 0 .. FRAMES_MAX_BUDGET).  maxBlocks:
+ * FC_CLASSES entries. */
+static int cframes_plan(int64_t nFrames, const int64_t* maxBlocks, int hcLevel, cframes_plan_t* p)
 {
     size_t at = 0;
     int64_t slotBytes = 0;
     int c;
     if (nFrames < 0 || !maxBlocks) return 0;
     p->nEntries = 0;
-    for (c = 0; c < 4; c++) {
+    for (c = 0; c < FC_CLASSES; c++) {
         if (maxBlocks[c] < 0 || maxBlocks[c] > FRAMES_MAX_BUDGET) return 0;
         p->tabBase[c] = p->nEntries;
         p->nEntries += maxBlocks[c];
-        p->slotStride[c] = (fc_block_bytes(4 + c) - 1 + 15) & ~(int64_t)15;
+        p->slotStride[c] = ((c == FC_LEGACY_CLASS ? FC_LEGACY_BOUND : fc_block_bytes(4 + c) - 1) + 15) & ~(int64_t)15;
         p->slotBase[c] = slotBytes;
         slotBytes += maxBlocks[c] * p->slotStride[c];
     }
@@ -709,39 +712,69 @@ static int cframes_plan(int64_t nFrames, const int64_t* maxBlocks, int level, cf
     p->bodyOff = at; at = up256(at + (size_t)(p->nEntries + 1) * sizeof(int64_t));
     p->packOff = at; at = up256(at + (size_t)p->nEntries * sizeof(int64_t));
     p->slots = at;   at = up256(at + (size_t)slotBytes);
-    p->hcBytes = level < 2 ? 0 : level >= 10 ? lz4k_encode_hc_opt_workspace_bytes(p->nEntries)
-                                             : lz4k_encode_hc_workspace_bytes(p->nEntries);
+    p->hcBytes = hcLevel <= 0 ? 0 : hcLevel >= 10 ? lz4k_encode_hc_opt_workspace_bytes(p->nEntries)
+                                                  : lz4k_encode_hc_workspace_bytes(p->nEntries);
     p->hc = at;      at = up256(at + p->hcBytes);
     p->bytes = at + 256;
     return 1;
 }
 
+/* The frames calls' budget over FC_CLASSES in mb: theirs for block size IDs 4 .. 7, none for legacy blocks (NULL stays
+ * NULL, for cframes_plan to reject) */
+static const int64_t* cframes_budget(const int64_t* maxBlocks, int64_t mb[FC_CLASSES])
+{
+    int c;
+    if (!maxBlocks) return NULL;
+    for (c = 0; c < 4; c++) mb[c] = maxBlocks[c];
+    mb[FC_LEGACY_CLASS] = 0;
+    return mb;
+}
+
+/* The encode of a frame-writing call at `level` (lz4frame.c:911-937): *hcLevel 0 and LZ4_compress_fast with acceleration
+ * -level + 1 below level 1 (LZ4_compress_fast clamps it to 65537; this also keeps -INT_MIN out) below level 2, else
+ * LZ4_compress_HC_extStateHC_fastReset at *hcLevel = level */
+static void frames_levels(int level, int* hcLevel, int* accel)
+{
+    *hcLevel = level >= 2 ? level : 0;
+    *accel = level >= 0 ? 1 : level < -65536 ? 65537 : -level + 1;
+}
+
+/* The encode of `lz4 -l` at `level` (lz4io.c:788-837): below 3, LZ4_compress_fast with acceleration -level for negative
+ * levels and 0, read as 1, otherwise (above 65537 as 65537); from 3 on, LZ4_compress_HC at *hcLevel = level (above 12
+ * read as 12) */
+static void legacy_levels(int level, int* hcLevel, int* accel)
+{
+    *hcLevel = level >= 3 ? level : 0;
+    *accel = level >= 0 ? 1 : level < -65537 ? 65537 : -level;
+}
+
 size_t LZ4B200_compress_frames_workspace_bytes(int64_t nFrames, const int64_t maxBlocks[4], int compressionLevel)
 {
     cframes_plan_t p;
-    return cframes_plan(nFrames, maxBlocks, compressionLevel, &p) ? p.bytes : 0;
+    int64_t mb[FC_CLASSES];
+    int hcLevel, accel;
+    frames_levels(compressionLevel, &hcLevel, &accel);
+    return cframes_plan(nFrames, cframes_budget(maxBlocks, mb), hcLevel, &p) ? p.bytes : 0;
 }
 
-/* index (+ budget scan, fill) -> one encode of the whole table -> pack scan -> headers, places, EndMarks, results ->
- * gather -> [block checksums] -> [content checksums].  Every block is compressed into its slot with capacity size - 1,
- * as LZ4F_makeBlock does (lz4frame.c:883-908).  sums: FC_BLOCK_SUM | FC_CONTENT_SUM; the bracketed steps run for the
- * checksums the frames carry. */
-static int compress_frames_sums(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
-                                void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
-                                int64_t* d_result, int64_t nFrames,
-                                int blockSizeID, int compressionLevel, int contentSizeFlag, int parallel, int sums,
-                                const int64_t maxBlocks[4],
-                                void* d_workspace, size_t workspaceBytes, void* stream)
+/* The body of the frame-writing calls: index (+ budget scan, fill) -> one encode of the whole table -> pack scan ->
+ * headers, places, EndMarks, results -> gather -> [block checksums] -> [content checksums].  A frame block is compressed
+ * into its slot with capacity size - 1, as LZ4F_makeBlock does (lz4frame.c:883-908); a legacy block with capacity
+ * LZ4_compressBound(size).  legacy: `lz4 -l` streams (blockSizeID, contentSizeFlag, parallel and sums unused).  sums:
+ * FC_BLOCK_SUM | FC_CONTENT_SUM; the bracketed steps run for the checksums the frames carry.  maxBlocks: FC_CLASSES
+ * entries; hcLevel, accel: the encode (frames_levels, legacy_levels). */
+static int cframes_run(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
+                       void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
+                       int64_t* d_result, int64_t nFrames, const int64_t* maxBlocks, int legacy,
+                       int blockSizeID, int contentSizeFlag, int parallel, int sums, int hcLevel, int accel,
+                       void* d_workspace, size_t workspaceBytes, void* stream)
 {
     cframes_plan_t p;
     lz4k_cframes_args a;
     lz4k_encode_args e;
     uint8_t* ws;
-    int c, rc, accel;
-    if (!cframes_plan(nFrames, maxBlocks, compressionLevel, &p)) return LZ4B200_ERR_ARG;
-    if (blockSizeID == 0) blockSizeID = 4;
-    if (blockSizeID < 4 || blockSizeID > 7) return LZ4B200_ERR_ARG;
-    if (parallel && compressionLevel >= 2) return LZ4B200_ERR_ARG;
+    int c, rc;
+    if (!cframes_plan(nFrames, maxBlocks, hcLevel, &p)) return LZ4B200_ERR_ARG;
     if (nFrames == 0) return LZ4B200_OK;
     if (!d_src || !d_srcOff || !d_srcSize || !d_dst || !d_dstOff || !d_dstCap || !d_result || !d_workspace)
         return LZ4B200_ERR_ARG;
@@ -751,11 +784,12 @@ static int compress_frames_sums(const void* d_src, const int64_t* d_srcOff, cons
     a.src = (const uint8_t*)d_src; a.srcOff = d_srcOff; a.srcSize = d_srcSize;
     a.dst = (uint8_t*)d_dst; a.dstOff = d_dstOff; a.dstCap = d_dstCap;
     a.result = d_result; a.nFrames = nFrames;
-    for (c = 0; c < 4; c++) {
+    for (c = 0; c < FC_CLASSES; c++) {
         a.maxBlocks[c] = maxBlocks[c]; a.tabBase[c] = p.tabBase[c];
         a.slotBase[c] = p.slotBase[c]; a.slotStride[c] = p.slotStride[c];
     }
     a.nEntries = p.nEntries;
+    a.legacy = legacy;
     a.bsid = blockSizeID;
     a.contentSizeFlag = contentSizeFlag != 0;
     a.sums = sums;
@@ -766,15 +800,12 @@ static int compress_frames_sums(const void* d_src, const int64_t* d_srcOff, cons
     a.tabBodyOff = (int64_t*)(ws + p.bodyOff); a.tabPackOff = (int64_t*)(ws + p.packOff);
 
     if ((rc = launched(lz4k_launch_cframes_index(&a, stream), "lz4k_launch_cframes_index")) != LZ4B200_OK) return rc;
-    /* lz4frame.c:911-921: acceleration -level + 1 below level 1 (LZ4_compress_fast clamps it to 65537; this also keeps
-     * -INT_MIN out), LZ4_compress_HC_extStateHC_fastReset from level 2 */
-    accel = compressionLevel >= 0 ? 1 : compressionLevel < -65536 ? 65537 : -compressionLevel + 1;
     e = encode_args(d_src, 0, a.tabSrcSize, 0, a.slots, 0, 0, accel, a.tabOutSize, p.nEntries);
     e.srcOff = a.tabSrcOff; e.dstOff = a.tabSlotOff; e.dstCapArr = a.tabCap;
-    if (compressionLevel >= 10)
-        rc = launched(lz4k_launch_encode_hc_opt(&e, compressionLevel, ws + p.hc, p.hcBytes, stream), "lz4k_launch_encode_hc_opt");
-    else if (compressionLevel >= 2)
-        rc = launched(lz4k_launch_encode_hc(&e, compressionLevel, ws + p.hc, p.hcBytes, stream), "lz4k_launch_encode_hc");
+    if (hcLevel >= 10)
+        rc = launched(lz4k_launch_encode_hc_opt(&e, hcLevel, ws + p.hc, p.hcBytes, stream), "lz4k_launch_encode_hc_opt");
+    else if (hcLevel > 0)
+        rc = launched(lz4k_launch_encode_hc(&e, hcLevel, ws + p.hc, p.hcBytes, stream), "lz4k_launch_encode_hc");
     else if (parallel)
         rc = encode_parallel(&e, stream);
     else
@@ -786,6 +817,25 @@ static int compress_frames_sums(const void* d_src, const int64_t* d_srcOff, cons
         return rc;
     if (sums & FC_CONTENT_SUM) return launched(lz4k_launch_cframes_content_sums(&a, stream), "lz4k_launch_cframes_content_sums");
     return LZ4B200_OK;
+}
+
+/* the two frames calls: their own argument rules, then the body with their budget and levels */
+static int compress_frames_sums(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
+                                void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
+                                int64_t* d_result, int64_t nFrames,
+                                int blockSizeID, int compressionLevel, int contentSizeFlag, int parallel, int sums,
+                                const int64_t maxBlocks[4],
+                                void* d_workspace, size_t workspaceBytes, void* stream)
+{
+    int64_t mb[FC_CLASSES];
+    int hcLevel, accel;
+    if (blockSizeID == 0) blockSizeID = 4;
+    if (blockSizeID < 4 || blockSizeID > 7) return LZ4B200_ERR_ARG;
+    if (parallel && compressionLevel >= 2) return LZ4B200_ERR_ARG;
+    frames_levels(compressionLevel, &hcLevel, &accel);
+    return cframes_run(d_src, d_srcOff, d_srcSize, d_dst, d_dstOff, d_dstCap, d_result, nFrames,
+                       cframes_budget(maxBlocks, mb), 0, blockSizeID, contentSizeFlag, parallel, sums, hcLevel, accel,
+                       d_workspace, workspaceBytes, stream);
 }
 
 int LZ4B200_compress_frames(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
@@ -812,6 +862,41 @@ int LZ4B200_compress_frames_checksummed(const void* d_src, const int64_t* d_srcO
                                 compressionLevel, contentSizeFlag, parallel,
                                 (blockChecksumFlag ? FC_BLOCK_SUM : 0) | (contentChecksumFlag ? FC_CONTENT_SUM : 0),
                                 maxBlocks, d_workspace, workspaceBytes, stream);
+}
+
+int64_t LZ4B200_compressLegacyBound(int64_t srcSize)
+{
+    return srcSize < 0 ? LZ4B200_ERR_ARG : fc_legacy_bound(srcSize);
+}
+
+/* the legacy call's budget over FC_CLASSES in mb: maxBlocks legacy blocks, no frame blocks */
+static const int64_t* legacy_budget(int64_t maxBlocks, int64_t mb[FC_CLASSES])
+{
+    int c;
+    for (c = 0; c < 4; c++) mb[c] = 0;
+    mb[FC_LEGACY_CLASS] = maxBlocks;
+    return mb;
+}
+
+size_t LZ4B200_compress_legacy_workspace_bytes(int64_t nFiles, int64_t maxBlocks, int compressionLevel)
+{
+    cframes_plan_t p;
+    int64_t mb[FC_CLASSES];
+    int hcLevel, accel;
+    legacy_levels(compressionLevel, &hcLevel, &accel);
+    return cframes_plan(nFiles, legacy_budget(maxBlocks, mb), hcLevel, &p) ? p.bytes : 0;
+}
+
+int LZ4B200_compress_legacy(const void* d_src, const int64_t* d_srcOff, const int64_t* d_srcSize,
+                            void* d_dst, const int64_t* d_dstOff, const int64_t* d_dstCap,
+                            int64_t* d_result, int64_t nFiles, int compressionLevel, int64_t maxBlocks,
+                            void* d_workspace, size_t workspaceBytes, void* stream)
+{
+    int64_t mb[FC_CLASSES];
+    int hcLevel, accel;
+    legacy_levels(compressionLevel, &hcLevel, &accel);
+    return cframes_run(d_src, d_srcOff, d_srcSize, d_dst, d_dstOff, d_dstCap, d_result, nFiles,
+                       legacy_budget(maxBlocks, mb), 1, 0, 0, 0, 0, hcLevel, accel, d_workspace, workspaceBytes, stream);
 }
 
 /* ------------------------------------------------------------------------------------------ */

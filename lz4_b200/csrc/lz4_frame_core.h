@@ -7,7 +7,8 @@
  * the batched frame encode -- serves LZ4B200_compressFrame_host and LZ4B200_compress_frames the same way
  * (tests/emul/compress_frames_emul.cpp).  The file layer of LZ4B200_decompress_files -- the units of a .lz4 file, their
  * placement and the fold of their results -- sits on the frame decode's rules (tests/emul/decompress_files_emul.cpp).
- * No CUDA runtime calls, no allocation.
+ * The legacy stream's writing rules serve LZ4B200_compress_legacy through the frame encode's passes
+ * (tests/emul/compress_legacy_emul.cpp).  No CUDA runtime calls, no allocation.
  */
 #ifndef LZ4_FRAME_CORE_H
 #define LZ4_FRAME_CORE_H
@@ -80,11 +81,12 @@ FC_FN uint32_t fc_xxh32(const uint8_t* p, uint64_t len, uint32_t seed)
 
 FC_FN int64_t fc_block_bytes(int bsid) { return (int64_t)1 << (8 + 2 * bsid); }   /* 4..7 -> 64 KB..4 MB (lz4frame.c:333-342) */
 
-/* The block classes of the batched decode: 0 .. 3 hold frame blocks of block size ID 4 + c, class 4 the blocks of a
- * legacy stream (LZ4B200_decompress_files only; the frames calls give it a budget of 0). */
+/* The block classes of the batched decode and encode: 0 .. 3 hold frame blocks of block size ID 4 + c, class 4 the blocks
+ * of a legacy stream (LZ4B200_decompress_files and LZ4B200_compress_legacy; the frames calls give it a budget of 0). */
 #define FC_CLASSES      5
 #define FC_LEGACY_CLASS 4
-#define FC_LEGACY_BLOCK (8 << 20)          /* lz4io.c: LEGACY_BLOCKSIZE, the capacity a legacy block decodes with */
+#define FC_LEGACY_BLOCK (8 << 20)          /* lz4io.c: LEGACY_BLOCKSIZE, the capacity a legacy block decodes with and
+                                              the chunk the tool compresses */
 #define FC_LEGACY_BOUND 8421520            /* LZ4_COMPRESSBOUND(8 MiB): a larger block word ends a legacy unit */
 
 /* the uniform capacity the blocks of class cls decode with */
@@ -541,16 +543,27 @@ FC_FN void fc_fold_file(const fc_file_rec* f, int64_t srcOff, int64_t srcSize, i
 }
 
 /* ---------------------------------------------------------------------------------------------
- * The batched frame encode (LZ4B200_compress_frames, LZ4B200_compress_frames_checksummed): the decode's frame record
- * and budget scan (fc_scan_count, fc_place_frame), with a record that holds the frame's source size in contentSize and
- * the checksums it is written with in sums, and one table of blocks per class.
+ * The batched frame encode (LZ4B200_compress_frames, LZ4B200_compress_frames_checksummed, and LZ4B200_compress_legacy
+ * in class FC_LEGACY_CLASS): the decode's frame record and budget scan (fc_scan_count, fc_place_frame), with a record
+ * that holds the frame's source size in contentSize and the checksums it is written with in sums, and one table of
+ * blocks per class.
  * ------------------------------------------------------------------------------------------- */
 typedef struct {               /* a class's block table; entry b of every array belongs to one block */
     int64_t* srcOff;           /* absolute offset of the block's source bytes in the call's source */
     int32_t* srcSize;          /* its size (0 for an unused entry) */
     int64_t* slotOff;          /* offset of its slot in the call's workspace */
-    int32_t* cap;              /* size - 1: a block that does not compress into fewer bytes than it has is stored raw */
+    int32_t* cap;              /* a frame block's size - 1 (one that does not compress into fewer bytes than it has is
+                                  stored raw), a legacy block's LZ4_compressBound(size) */
 } fc_cblock_tab;
+
+/* The record of an encode's pass 1 before its verdicts: the source size in contentSize, the checksums in sums; 0 for a
+ * negative size or capacity (LZ4B200_ERR_ARG), else 1 */
+FC_FN int fc_cclear_rec(int64_t srcSize, int64_t dstCap, int sums, fc_frame_rec* r)
+{
+    r->count = 0; r->base = 0; r->contentSize = srcSize; r->consumed = 0; r->cls = -1; r->hdrLen = 0; r->sums = sums;
+    r->status = (srcSize < 0 || dstCap < 0) ? LZ4B200_ERR_ARG : LZ4B200_OK;
+    return r->status == LZ4B200_OK;
+}
 
 /* Pass 1 of the encode: the verdict on frame f's arguments and capacity, in LZ4F_compressFrame's order -- LZ4B200_ERR_ARG
  * (a negative size or capacity), LZ4B200_ERR_DSTSIZE (dstCap below the reference's bound at the frame's optimal block
@@ -559,9 +572,7 @@ typedef struct {               /* a class's block table; entry b of every array 
 FC_FN void fc_cindex_frame_sums(int64_t srcSize, int64_t dstCap, int bsid, int contentSizeFlag, int sums, fc_frame_rec* r)
 {
     int b;
-    r->count = 0; r->base = 0; r->contentSize = srcSize; r->consumed = 0; r->cls = -1; r->hdrLen = 0; r->sums = sums;
-    r->status = LZ4B200_OK;
-    if (srcSize < 0 || dstCap < 0) { r->status = LZ4B200_ERR_ARG; return; }
+    if (!fc_cclear_rec(srcSize, dstCap, sums, r)) return;
     b = fc_optimal_bsid(bsid, srcSize);
     if (dstCap < fc_frame_bound_sums(srcSize, b, sums)) { r->status = LZ4B200_ERR_DSTSIZE; return; }
     r->cls = b - 4;
@@ -575,11 +586,48 @@ FC_FN void fc_cindex_frame(int64_t srcSize, int64_t dstCap, int bsid, int conten
     fc_cindex_frame_sums(srcSize, dstCap, bsid, contentSizeFlag, 0, r);
 }
 
+/* ---------------------------------------------------------------------------------------------
+ * Writing an `lz4 -l` legacy stream (LZ4IO_compressLegacy_internal, lz4io.c:766-910): the LE32 magic FC_MAGIC_LEGACY,
+ * then for every FC_LEGACY_BLOCK chunk of the source (the last one may be short) the LE32 compressed size and the
+ * compressed block.  No EndMark, no checksum, no stored-raw block: an incompressible chunk is written compressed, larger
+ * than it is.  An empty source gives the magic alone (lz4io.c:729-731).  LZ4B200_compress_legacy runs the frame
+ * encode's steps with these rules in class FC_LEGACY_CLASS.
+ * ------------------------------------------------------------------------------------------- */
+
+/* LZ4_compressBound of a chunk of n <= FC_LEGACY_BLOCK bytes: the capacity the tool compresses it with never limits it
+ * (lz4io.c:886), so its bytes are those at this capacity */
+FC_FN int32_t fc_legacy_cap(int32_t n) { return n + n / 255 + 16; }
+
+/* the chunks of a source of n >= 0 bytes */
+FC_FN int64_t fc_legacy_blocks(int64_t n) { return n / FC_LEGACY_BLOCK + (n % FC_LEGACY_BLOCK != 0); }
+
+/* The longest stream of a source of n >= 0 bytes: 4 + the sum over its chunks of 4 + LZ4_compressBound(chunk).
+ * Saturates at INT64_MAX. */
+FC_FN int64_t fc_legacy_bound(int64_t n)
+{
+    const int64_t last = n % FC_LEGACY_BLOCK;
+    const int64_t extra = 4 + (n / FC_LEGACY_BLOCK) * (4 + FC_LEGACY_BOUND - FC_LEGACY_BLOCK) +
+                          (last ? 4 + fc_legacy_cap((int32_t)last) - last : 0);
+    return n > INT64_MAX - extra ? INT64_MAX : n + extra;
+}
+
+/* Pass 1 of the legacy encode: LZ4B200_ERR_ARG (a negative size or capacity), LZ4B200_ERR_DSTSIZE (dstCap below
+ * fc_legacy_bound), else class FC_LEGACY_CLASS, the chunk count and the 4-byte magic as the header. */
+FC_FN void fc_lindex_file(int64_t srcSize, int64_t dstCap, fc_frame_rec* r)
+{
+    if (!fc_cclear_rec(srcSize, dstCap, 0, r)) return;
+    if (dstCap < fc_legacy_bound(srcSize)) { r->status = LZ4B200_ERR_DSTSIZE; return; }
+    r->cls = FC_LEGACY_CLASS;
+    r->count = fc_legacy_blocks(srcSize);
+    r->hdrLen = 4;
+}
+
 /* Pass 2 of the encode: a frame that passed writes its entries of its class's table (t: that class's).  srcOff: the
- * frame's offset in the call's source; the class's slots are slotStride bytes apart from slotBase. */
+ * frame's offset in the call's source; the class's slots are slotStride bytes apart from slotBase.  A frame block's
+ * capacity is size - 1, a legacy block's LZ4_compressBound(size) (fc_legacy_cap). */
 FC_FN void fc_cfill_frame(const fc_frame_rec* r, int64_t srcOff, int64_t slotBase, int64_t slotStride, fc_cblock_tab t)
 {
-    const int64_t bs = fc_block_bytes(r->cls + 4);
+    const int64_t bs = fc_class_bytes(r->cls);
     int64_t k;
     if (r->status != LZ4B200_OK) return;
     for (k = 0; k < r->count; k++) {
@@ -588,7 +636,7 @@ FC_FN void fc_cfill_frame(const fc_frame_rec* r, int64_t srcOff, int64_t slotBas
         t.srcOff[b] = srcOff + k * bs;
         t.srcSize[b] = sz;
         t.slotOff[b] = slotBase + b * slotStride;
-        t.cap[b] = sz - 1;
+        t.cap[b] = r->cls == FC_LEGACY_CLASS ? fc_legacy_cap(sz) : sz - 1;
     }
 }
 

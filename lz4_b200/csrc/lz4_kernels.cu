@@ -1753,13 +1753,17 @@ __global__ void __launch_bounds__(128) lz4_files_fold_kernel(lz4k_files_args a)
 }
 
 /* =============================================================================================
- * batched frame encode (LZ4B200_compress_frames, LZ4B200_compress_frames_checksummed): the frame rules of
- * lz4_frame_core.h around one encode of the whole block table (by the caller) and the pack scan and gather
+ * batched frame encode (LZ4B200_compress_frames, LZ4B200_compress_frames_checksummed) and legacy encode
+ * (LZ4B200_compress_legacy): the rules of lz4_frame_core.h around one encode of the whole block table (by the caller)
+ * and the pack scan and gather
  *   index : pass 1 -- one thread per frame: optimal block size ID, block count, header length, argument and capacity
- *           verdicts; then the frame decode's budget scan (lz4_frames_scan_kernel) on the same records
- *   fill  : pass 2 -- one thread per frame that passed: its table entries (source, size, slot, capacity size - 1)
- *   finish: after the pack scan -- one thread per frame: the header, every block's place, the EndMark, the result; the
- *           gather then writes every block header and payload to its place
+ *           verdicts (legacy: its own kernel, the chunk count in class FC_LEGACY_CLASS); then the frame decode's budget
+ *           scan (lz4_frames_scan_kernel) on the same records
+ *   fill  : pass 2 -- one thread per frame that passed: its table entries (source, size, slot, capacity size - 1, or
+ *           LZ4_compressBound(size) for a legacy block)
+ *   finish: after the pack scan -- one thread per frame: the header, every block's place, the EndMark, the result
+ *           (legacy: its own kernel, the magic, the places and the result); the gather then writes every block header
+ *           and payload to its place
  * and, with checksums (a.sums):
  *   block sums  : one thread per placed table entry: XXH32 of the block's payload, read from its slot (or, stored raw,
  *                 from the source), into the 4 bytes after the payload
@@ -1771,11 +1775,13 @@ __device__ __forceinline__ fc_cblock_tab cframes_tab(const lz4k_cframes_args& a,
     return fc_cblock_tab{a.tabSrcOff + t, a.tabSrcSize + t, a.tabSlotOff + t, a.tabCap + t};
 }
 
-/* the pack's frame rule over the block table: a block is stored raw from the source when its encode did not gain */
+/* the pack's rule over the block table: a frame block is stored raw from the source when its encode did not gain; a
+ * legacy block never is (the plain rule: its encode always fits LZ4_compressBound) */
 __host__ __device__ inline FrameRule cframes_rule(const lz4k_cframes_args& a)
 {
     FrameRule fr;
-    fr.raw = a.src; fr.rawStride = 0; fr.blockSize = 0; fr.lastSize = 0; fr.rawOff = a.tabSrcOff; fr.rawSize = a.tabSrcSize;
+    fr.raw = a.legacy ? nullptr : a.src;
+    fr.rawStride = 0; fr.blockSize = 0; fr.lastSize = 0; fr.rawOff = a.tabSrcOff; fr.rawSize = a.tabSrcSize;
     return fr;
 }
 
@@ -1792,6 +1798,13 @@ __global__ void __launch_bounds__(128) lz4_cframes_index_kernel(lz4k_cframes_arg
                          static_cast<fc_frame_rec*>(a.frames) + f);
 }
 
+__global__ void __launch_bounds__(128) lz4_clegacy_index_kernel(lz4k_cframes_args a)
+{
+    const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= a.nFrames) return;
+    fc_lindex_file(a.srcSize[f], a.dstCap[f], static_cast<fc_frame_rec*>(a.frames) + f);
+}
+
 __global__ void __launch_bounds__(128) lz4_cframes_fill_kernel(lz4k_cframes_args a)
 {
     const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1799,6 +1812,16 @@ __global__ void __launch_bounds__(128) lz4_cframes_fill_kernel(lz4k_cframes_args
     const fc_frame_rec* r = static_cast<const fc_frame_rec*>(a.frames) + f;
     if (r->status != LZ4B200_OK) return;
     fc_cfill_frame(r, a.srcOff[f], a.slotBase[r->cls], a.slotStride[r->cls], cframes_tab(a, r->cls));
+}
+
+/* the places of frame f's blocks, packed from the end of its header on, for the gather (tabPackOff); returns the end of
+ * its last block in dst */
+__device__ __forceinline__ int64_t cframes_place(const lz4k_cframes_args& a, int64_t f, const fc_frame_rec* r)
+{
+    const int64_t first = a.tabBase[r->cls] + r->base, body0 = a.tabBodyOff[first];
+    const int64_t at = a.dstOff[f] + r->hdrLen;
+    for (int64_t k = 0; k < r->count; k++) a.tabPackOff[first + k] = at + a.tabBodyOff[first + k] - body0;
+    return at + a.tabBodyOff[first + r->count] - body0;
 }
 
 /* the pack scan counted 4 + payload (+ 4 with block checksums) per entry, so the EndMark follows the last block's
@@ -1809,15 +1832,24 @@ __global__ void __launch_bounds__(128) lz4_cframes_finish_kernel(lz4k_cframes_ar
     if (f >= a.nFrames) return;
     const fc_frame_rec* r = static_cast<const fc_frame_rec*>(a.frames) + f;
     if (r->status != LZ4B200_OK) { a.result[f] = r->status; return; }
-    const int64_t first = a.tabBase[r->cls] + r->base, body0 = a.tabBodyOff[first];
-    const int64_t at = a.dstOff[f] + r->hdrLen;
-    for (int64_t k = 0; k < r->count; k++) a.tabPackOff[first + k] = at + a.tabBodyOff[first + k] - body0;
-    const int64_t end = at + a.tabBodyOff[first + r->count] - body0;
+    const int64_t end = cframes_place(a, f, r);
     uint8_t h[15];
     const int hl = fc_frame_header_sums(h, r->cls + 4, a.contentSizeFlag ? r->contentSize : 0, r->sums);
     for (int i = 0; i < hl; i++) a.dst[a.dstOff[f] + i] = h[i];
     for (int i = 0; i < 4; i++) a.dst[end + i] = 0;                  /* EndMark, lz4frame.c:1222 */
     a.result[f] = end + 4 + ((r->sums & FC_CONTENT_SUM) ? 4 : 0) - a.dstOff[f];
+}
+
+/* a legacy stream: the magic, then its blocks (lz4io.c:858-864); it ends with its last block */
+__global__ void __launch_bounds__(128) lz4_clegacy_finish_kernel(lz4k_cframes_args a)
+{
+    const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= a.nFrames) return;
+    const fc_frame_rec* r = static_cast<const fc_frame_rec*>(a.frames) + f;
+    if (r->status != LZ4B200_OK) { a.result[f] = r->status; return; }
+    const int64_t end = cframes_place(a, f, r);
+    st_le32(a.dst + a.dstOff[f], FC_MAGIC_LEGACY);
+    a.result[f] = end - a.dstOff[f];
 }
 
 /* LZ4F_makeBlock's block checksum (lz4frame.c:904-907): XXH32(payload, 0) after the payload of every placed entry */
@@ -1956,8 +1988,9 @@ int lz4k_launch_cframes_index(const lz4k_cframes_args* a, void* stream)
     memset(&fa, 0, sizeof fa);
     fa.nFrames = a->nFrames;
     fa.frames = a->frames;
-    for (int c = 0; c < 4; c++) fa.maxBlocks[c] = a->maxBlocks[c];
-    lz4_cframes_index_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);
+    for (int c = 0; c < FC_CLASSES; c++) fa.maxBlocks[c] = a->maxBlocks[c];
+    if (a->legacy) lz4_clegacy_index_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);
+    else lz4_cframes_index_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);
     lz4_frames_scan_kernel<<<1, kFsThreads, 0, s>>>(fa);
     g_launches += 2;
     /* unused entries compress nothing (size 0, capacity 0) and are written nowhere (place -1) */
@@ -1978,7 +2011,8 @@ int lz4k_launch_cframes_assemble(const lz4k_cframes_args* a, void* stream)
     cudaStream_t s = (cudaStream_t)stream;
     const FrameRule fr = cframes_rule(*a);
     lz4_pack_scan_kernel<<<1, 1024, 0, s>>>(a->tabOutSize, a->nEntries, a->tabBodyOff, 4, (a->sums & FC_BLOCK_SUM) ? 4 : 0, fr);
-    lz4_cframes_finish_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);
+    if (a->legacy) lz4_clegacy_finish_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);
+    else lz4_cframes_finish_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);
     g_launches += 2;
     launch_pack_gather(a->slots, a->tabSlotOff, 0, a->tabOutSize, a->nEntries, a->dst, a->tabBodyOff, a->tabPackOff, 4, fr, s);
     return (int)cudaGetLastError();

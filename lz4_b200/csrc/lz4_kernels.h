@@ -133,7 +133,8 @@ int lz4k_launch_files_totals(const lz4k_files_args* a, void* stream);
 int lz4k_launch_files_place(const lz4k_files_args* a, void* stream);
 /* last: every file's result, consumed and prefix from the unit results */
 int lz4k_launch_files_fold(const lz4k_files_args* a, void* stream);
-/* the batched frame encode's own steps (lz4_frame_core.h); the encode of the block table between them is the caller's */
+/* the batched frame and legacy encode's own steps (lz4_frame_core.h); the encode of the block table between them is the
+ * caller's */
 typedef struct {
     const uint8_t* src;        /* frame f's source is src + srcOff[f], srcSize[f] bytes */
     const int64_t* srcOff;
@@ -143,16 +144,18 @@ typedef struct {
     const int64_t* dstCap;
     int64_t* result;           /* [nFrames] */
     int64_t nFrames;
-    int64_t maxBlocks[4];      /* the budget of every class */
-    int64_t tabBase[4];        /* class c's entries of the block table start at tabBase[c] */
+    int64_t maxBlocks[5];      /* the budget of every class (FC_CLASSES; the frames calls give class 4 none, the legacy
+                                  call classes 0 .. 3 none) */
+    int64_t tabBase[5];        /* class c's entries of the block table start at tabBase[c] */
     int64_t nEntries;          /* entries of the block table (sum of maxBlocks) */
-    int bsid;                  /* the requested block size ID, 4 .. 7 */
+    int legacy;                /* `lz4 -l` legacy streams (LZ4B200_compress_legacy) instead of frames */
+    int bsid;                  /* the requested block size ID, 4 .. 7 (frames) */
     int contentSizeFlag;
     int sums;                  /* the checksums every frame is written with: FC_BLOCK_SUM | FC_CONTENT_SUM */
     void* frames;              /* fc_frame_rec[nFrames] */
     uint8_t* slots;            /* block b is compressed to slots + tabSlotOff[b] */
-    int64_t slotBase[4];       /* class c's slots: slotBase[c] + k * slotStride[c] from `slots` */
-    int64_t slotStride[4];
+    int64_t slotBase[5];       /* class c's slots: slotBase[c] + k * slotStride[c] from `slots` */
+    int64_t slotStride[5];
     int64_t* tabSrcOff; int32_t* tabSrcSize; int64_t* tabSlotOff; int32_t* tabCap; int32_t* tabOutSize;
     int64_t* tabBodyOff;       /* [nEntries + 1]: the pack scan of 4 + payload (+ 4 with block checksums) over the table */
     int64_t* tabPackOff;       /* where block b's header goes in dst, -1 for an unused entry */
@@ -160,7 +163,8 @@ typedef struct {
 
 /* pass 1 (index), the budget scan of the frame decode, then the table cleared and filled (pass 2) */
 int lz4k_launch_cframes_index(const lz4k_cframes_args* a, void* stream);
-/* after the encode (tabOutSize): the pack scan, the frame headers, places, EndMarks and results, then the gather */
+/* after the encode (tabOutSize): the pack scan, the frame headers, places, EndMarks and results (legacy: the magic, the
+ * places and the results), then the gather */
 int lz4k_launch_cframes_assemble(const lz4k_cframes_args* a, void* stream);
 /* FC_BLOCK_SUM, after the assembly: the block checksums, one thread per placed table entry */
 int lz4k_launch_cframes_block_sums(const lz4k_cframes_args* a, void* stream);
