@@ -709,6 +709,33 @@ LZ4B200_API int LZ4B200_compress_blocks_host(const void* h_src, int64_t srcStrid
                                              void* h_dst, int64_t dstStride, int32_t dstCap, int acceleration,
                                              int32_t* h_outSize, int64_t nBlocks);
 
+/*
+ * Decode nFiles whole .lz4 files in host memory, as LZ4B200_decompress_files (section 2) decodes them in device memory,
+ * with no budget and no workspace: file f is h_src + h_srcOff[f], h_srcSize[f] bytes, and decodes to h_dst +
+ * h_dstOff[f] with h_dstCap[f] bytes of room.
+ *   h_result[f], h_consumed[f], h_prefix[f] (the last two optional): what LZ4B200_decompress_files returns for the same
+ *   files with a budget that covers them all -- the same grammar, unit order, error order inside a frame, skipChecksums
+ *   and sizeOnly rules and the same deviations from `lz4 -d` -- so never LZ4B200_ERR_LIMIT.
+ * On success [dst_f, dst_f + result) holds what `lz4 -d` writes; on failure [dst_f, dst_f + prefix) holds the output of
+ * the units before the failing one.  Nothing outside [dst_f, dst_f + cap_f) is written.  sizeOnly != 0: no byte is
+ * written and h_dst, h_dstOff and h_dstCap may be NULL.  Host regions must not overlap each other or the source; no
+ * readable padding is needed (the call stages the bytes itself).
+ * The files are walked on the host and their blocks cut into groups of at most 64 MiB of decode capacity (one block at
+ * least; small files share a group, a large frame spans many).  Each group goes through the device on one of the
+ * pipeline's streams -- its source pieces up, one decode per block class, the block checksums, its output assembled in
+ * file order, the content hashes (a frame's hash state carried from group to group in device memory), its bytes down --
+ * with four groups in flight, so device memory is bounded by the pipeline, not by the files.  DESIGN section 3.17.
+ * Returns LZ4B200_OK, LZ4B200_ERR_ARG (nFiles < 0; with files, a NULL h_src, h_srcOff, h_srcSize or h_result, or a NULL
+ * h_dst, h_dstOff or h_dstCap unless sizeOnly; or host memory for the walk ran out, which LZ4B200_last_cuda_error()
+ * then says) or LZ4B200_ERR_CUDA (no device
+ * included: there is no CPU fallback).  nFiles == 0 returns LZ4B200_OK without touching the device.  Synchronous; one
+ * host-buffer call runs at a time.
+ */
+LZ4B200_API int LZ4B200_decompress_files_host(const void* h_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
+                                              void* h_dst, const int64_t* h_dstOff, const int64_t* h_dstCap,
+                                              int64_t* h_result, int64_t* h_consumed, int64_t* h_prefix,
+                                              int64_t nFiles, int skipChecksums, int sizeOnly);
+
 /* ---------------------------------------------------------------------------------------------
  * 4. Frame layer (SURVEY.md section 8 f-1): one-shot LZ4 frames of INDEPENDENT blocks, host buffers.
  *    The container logic (header, block headers, EndMark) runs on the host, every block goes through

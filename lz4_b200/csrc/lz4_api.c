@@ -9,6 +9,7 @@
 #include "../../include/lz4_b200.h"
 #include "lz4_kernels.h"
 #include "lz4_frame_core.h"
+#include "lz4_files_plan.h"
 
 #include <cuda_runtime_api.h>
 #include <pthread.h>
@@ -1428,4 +1429,292 @@ int64_t LZ4B200_decompressFrame_host(const void* h_src, int64_t srcSize, void* h
 done:
     free(off); free(csz); free(raw); free(rets);
     return result;
+}
+
+/* ------------------------------------------------------------------------------------------ */
+/* whole .lz4 files over host buffers: LZ4B200_decompress_files's results, pipelined in groups  */
+/* ------------------------------------------------------------------------------------------ */
+/* The content hash of a frame whose blocks span groups is carried in device memory from one group's carry kernel to the
+ * next group's: group g writes slot g % FH_CARRIES of the ring and group g + 1 reads it after g's event.  Group
+ * g + FH_CARRIES writes the same slot only after its pipeline slot, last used by group g + 1, is idle. */
+#define FH_CARRIES (N_PIPE + 1)
+#define FH_GAP     (64 << 10)   /* source pieces at most this far apart in h_src go over in one copy */
+/* A group is retired (its results read, its bytes sent down) FH_LAG groups after it is issued, so that the copies down
+ * of the groups before it run beside its kernels and the copies up of the groups after it.  Its slot is taken again
+ * N_PIPE groups after it: FH_LAG < N_PIPE. */
+#define FH_LAG     (N_PIPE - 1)
+static struct { int ready; cudaEvent_t hashed[N_PIPE]; void* carry; } g_fh;
+
+static int fh_init(void)
+{
+    int rc = LZ4B200_OK, i;
+    if (g_fh.ready) return rc;
+    for (i = 0; i < N_PIPE; i++) CU(cudaEventCreateWithFlags(&g_fh.hashed[i], cudaEventDisableTiming));
+    CU(cudaMalloc(&g_fh.carry, FH_CARRIES * sizeof(fc_xxh32_state)));
+    g_fh.ready = 1;
+done:
+    return rc;
+}
+
+/* A group's table in its slot (the host copy pinned, the device copy the kernels use), for n blocks and nSegs segments:
+ * [srcOff, gatherOff, dstOff: i64 n | segments | srcSize, rawLen, ord, sum: i32 n] go up, [sum, outSize: i32 n |
+ * segBad: i32 nSegs] come back, [blockSize: i32 n | blockFrom: i64 n | blockOff: i64 n + 1] stay on the device. */
+typedef struct { size_t srcOff, gatherOff, dstOff, segs, srcSize, rawLen, ord, sum, outSize, segBad, blockSize, blockFrom, blockOff, bytes; } fh_tab_t;
+
+static fh_tab_t fh_tab(int64_t n, int64_t nSegs)
+{
+    fh_tab_t t;
+    const size_t w8 = (size_t)n * 8, w4 = (size_t)n * 4;
+    t.srcOff = 0; t.gatherOff = w8; t.dstOff = 2 * w8; t.segs = 3 * w8;
+    t.srcSize = t.segs + (size_t)nSegs * sizeof(lz4k_hash_seg);
+    t.rawLen = t.srcSize + w4; t.ord = t.rawLen + w4; t.sum = t.ord + w4; t.outSize = t.sum + w4; t.segBad = t.outSize + w4;
+    t.blockSize = t.segBad + (size_t)nSegs * 4;
+    t.blockFrom = (t.blockSize + w4 + 7) & ~(size_t)7;
+    t.blockOff = t.blockFrom + w8;
+    t.bytes = t.blockOff + w8 + 8;
+    return t;
+}
+
+/* what the host keeps of a group in flight: its blocks and segments (the rest is in its slot's pinned table) */
+typedef struct { int64_t first, end, nSegs; } fh_group_t;
+
+/* Issue group gr on slot s (group index g): the table, the source pieces, the decode per class, the block checksums,
+ * and unless sizeOnly the assembly and the content hash; then the results back to the pinned table. */
+static int fh_issue(const fp_plan* p, const uint8_t* src, int64_t g, slot_t* s, fh_group_t* gr, int sizeOnly, int verify,
+                    int64_t* copies)
+{
+    const int64_t n = gr->end - gr->first;
+    const int hash = verify && !sizeOnly;               /* the content checksums (none when the call only sizes) */
+    int64_t nc[FC_CLASSES] = {0, 0, 0, 0, 0}, cb[FC_CLASSES], fill[FC_CLASSES], k, e, nSegs = 0, nCopies = 0;
+    int64_t slotBytes = 0, inBytes = 0, at;
+    size_t wsBytes = 0;
+    int c, rc = LZ4B200_OK, anySum = 0, carry = 0;
+    fh_tab_t t;
+    uint8_t* h;
+    uint8_t* d;
+    lz4k_group_args a;
+    lz4k_hash_seg* seg;
+    /* the classes, their slots, the segments and the source pieces */
+    for (k = gr->first; k < gr->end; k++) nc[(int)p->blocks[k].cls]++;
+    for (c = 0, at = 0; c < FC_CLASSES; c++) {
+        cb[c] = at; fill[c] = at; at += nc[c];
+        slotBytes += nc[c] * fc_class_bytes(c);
+        if (nc[c]) {
+            const size_t w = lz4k_decode_workspace_bytes(nc[c], 0, (int32_t)fc_class_bytes(c), SIZE_MAX);
+            if (w > wsBytes) wsBytes = w;
+        }
+    }
+    for (k = gr->first; k < gr->end; k++) {
+        const fp_unit* u = &p->units[p->blocks[k].unit];
+        if (hash && fp_content(u) && (k == gr->first || p->blocks[k - 1].unit != p->blocks[k].unit)) nSegs++;
+    }
+    /* pieces: [hostOff, devOff, bytes] triples in `copies` (room for one per block), staged after the slots */
+    for (k = gr->first; k < gr->end; k++) {
+        const fp_block* b = &p->blocks[k];
+        const int64_t lo = b->srcOff, hi = b->srcOff + b->size + b->sumBytes;
+        int64_t* cp = nCopies ? copies + 3 * (nCopies - 1) : NULL;
+        if (cp && lo >= cp[0] && lo <= cp[0] + cp[2] + FH_GAP) { if (hi > cp[0] + cp[2]) cp[2] = hi - cp[0]; }
+        else { cp = copies + 3 * nCopies++; cp[0] = lo; cp[2] = hi - lo; }
+    }
+    at = sizeOnly ? 0 : (slotBytes + 255) & ~(int64_t)255;              /* (the scan alone writes no slot) */
+    for (k = 0; k < nCopies; k++) { copies[3 * k + 1] = at; at = (at + copies[3 * k + 2] + 15) & ~(int64_t)15; }
+    inBytes = at;
+    t = fh_tab(n, nSegs);
+    if ((rc = slot_take(s, 0, (size_t)inBytes, wsBytes, sizeOnly ? 0 : (size_t)slotBytes, t.bytes)) != LZ4B200_OK)
+        return rc;
+    h = (uint8_t*)s->h_tab.p;
+    seg = (lz4k_hash_seg*)(h + t.segs);
+    gr->nSegs = 0;
+    /* the table: entries by class, blocks in file order */
+    {
+        int64_t* srcOff = (int64_t*)(h + t.srcOff);
+        int64_t* gatherOff = (int64_t*)(h + t.gatherOff);
+        int64_t* dstOff = (int64_t*)(h + t.dstOff);
+        int32_t* srcSize = (int32_t*)(h + t.srcSize);
+        int32_t* rawLen = (int32_t*)(h + t.rawLen);
+        int32_t* ord = (int32_t*)(h + t.ord);
+        int32_t* sum = (int32_t*)(h + t.sum);
+        int64_t slotAt[FC_CLASSES], piece = 0, u = -1;
+        for (c = 0, at = 0; c < FC_CLASSES; c++) { slotAt[c] = at; at += nc[c] * fc_class_bytes(c); }
+        for (k = gr->first; k < gr->end; k++) {
+            const fp_block* b = &p->blocks[k];
+            const int64_t* cp;
+            while (!(b->srcOff >= copies[3 * piece] && b->srcOff < copies[3 * piece] + copies[3 * piece + 2] + 1)) piece++;
+            cp = copies + 3 * piece;
+            e = fill[(int)b->cls]++;
+            ord[k - gr->first] = (int32_t)e;
+            srcOff[e] = cp[1] + (b->srcOff - cp[0]);
+            dstOff[e] = slotAt[(int)b->cls] + (e - cb[(int)b->cls]) * fc_class_bytes(b->cls);
+            gatherOff[e] = b->raw ? srcOff[e] : dstOff[e];
+            srcSize[e] = b->raw ? 0 : b->size;
+            rawLen[e] = b->raw ? b->size : -1;
+            sum[e] = (verify && b->verify) ? FC_SUM_PENDING : FC_SUM_NONE;
+            anySum |= verify && b->verify;
+            if (b->unit != u) {
+                const fp_unit* un = &p->units[b->unit];
+                u = b->unit;
+                if (hash && fp_content(un)) {
+                    lz4k_hash_seg* q = &seg[gr->nSegs++];
+                    q->first = (int32_t)(k - gr->first);
+                    q->end = (int32_t)(k - gr->first + 1);
+                    q->expected = un->contentSum;
+                    q->flags = (un->r.base < gr->first ? LZ4K_SEG_CONTINUES : 0) |
+                               (un->r.base + un->r.count <= gr->end ? LZ4K_SEG_ENDS : 0);
+                    if (q->flags != LZ4K_SEG_ENDS) carry = 1;
+                }
+            } else if (hash && fp_content(&p->units[u])) {
+                seg[gr->nSegs - 1].end++;
+            }
+        }
+    }
+    /* up: the table and the pieces */
+    d = (uint8_t*)s->d_tab.p;
+    CU(cudaMemcpyAsync(d, h, t.outSize, cudaMemcpyHostToDevice, s->stream));
+    for (k = 0; k < nCopies; k++)
+        CU(cudaMemcpyAsync((uint8_t*)s->out.p + copies[3 * k + 1], src + copies[3 * k], (size_t)copies[3 * k + 2],
+                           cudaMemcpyHostToDevice, s->stream));
+    memset(&a, 0, sizeof a);
+    a.base = (uint8_t*)s->out.p; a.packed = (uint8_t*)s->pack.p; a.n = n;
+    a.srcOff = (const int64_t*)(d + t.srcOff); a.gatherOff = (const int64_t*)(d + t.gatherOff);
+    a.srcSize = (const int32_t*)(d + t.srcSize); a.rawLen = (const int32_t*)(d + t.rawLen);
+    a.ord = (const int32_t*)(d + t.ord); a.sum = (int32_t*)(d + t.sum); a.outSize = (const int32_t*)(d + t.outSize);
+    a.blockSize = (int32_t*)(d + t.blockSize); a.blockFrom = (int64_t*)(d + t.blockFrom); a.blockOff = (int64_t*)(d + t.blockOff);
+    a.segs = (const lz4k_hash_seg*)(d + t.segs); a.nSegs = gr->nSegs; a.segBad = (int32_t*)(d + t.segBad);
+    a.carryIn = (const fc_xxh32_state*)g_fh.carry + (g + FH_CARRIES - 1) % FH_CARRIES;
+    a.carryOut = (fc_xxh32_state*)g_fh.carry + g % FH_CARRIES;
+    /* the decode of every class at its uniform capacity (the scan alone when sizing) */
+    for (c = 0; c < FC_CLASSES; c++) {
+        lz4k_decode_args dd;
+        if (!nc[c]) continue;
+        memset(&dd, 0, sizeof dd);
+        dd.src = a.base; dd.srcOff = a.srcOff + cb[c]; dd.srcSize = a.srcSize + cb[c];
+        dd.dst = a.base; dd.dstOff = (const int64_t*)(d + t.dstOff) + cb[c]; dd.dstCap = (int32_t)fc_class_bytes(c);
+        dd.outSize = (int32_t*)(d + t.outSize) + cb[c]; dd.nBlocks = nc[c];
+        dd.workspace = s->ws.p; dd.workspaceBytes = s->ws.cap;
+        if ((rc = launched(lz4k_launch_decode(&dd, sizeOnly ? 1 : 3, 0, s->stream), "lz4k_launch_decode")) != LZ4B200_OK)
+            return rc;
+    }
+    if (anySum && (rc = launched(lz4k_launch_group_block_sums(&a, s->stream), "lz4k_launch_group_block_sums")) != LZ4B200_OK)
+        return rc;
+    if (!sizeOnly) {
+        if ((rc = launched(lz4k_launch_group_assemble(&a, s->stream), "lz4k_launch_group_assemble")) != LZ4B200_OK) return rc;
+        if (gr->nSegs) {
+            if (seg[0].flags & LZ4K_SEG_CONTINUES)       /* after the group before: its carry kernel left the state */
+                CU(cudaStreamWaitEvent(s->stream, g_fh.hashed[(g + N_PIPE - 1) % N_PIPE], 0));
+            if ((rc = launched(lz4k_launch_group_content(&a, carry, s->stream), "lz4k_launch_group_content")) != LZ4B200_OK)
+                return rc;
+            if (!(seg[gr->nSegs - 1].flags & LZ4K_SEG_ENDS)) CU(cudaEventRecord(g_fh.hashed[g % N_PIPE], s->stream));
+        }
+    }
+    /* down: the block checksums' outcomes, the decode's results and the segments' */
+    CU(cudaMemcpyAsync(h + t.sum, d + t.sum, t.blockSize - t.sum, cudaMemcpyDeviceToHost, s->stream));
+done:
+    return rc;
+}
+
+/* Retire the group gr that ran on slot s: its results into the plan, then (unless sizeOnly) its bytes from the slot's
+ * packed output to each file's running position, one copy per run of bytes contiguous on both sides, clipped to the
+ * file's room and stopping at the file's first block that failed to decode. */
+static int fh_retire(fp_plan* p, slot_t* s, const fh_group_t* gr, int sizeOnly, uint8_t* dst, const int64_t* dstOff,
+                     const int64_t* dstCap, int64_t* filePos, uint8_t* fileStop)
+{
+    const int64_t n = gr->end - gr->first;
+    const fh_tab_t t = fh_tab(n, gr->nSegs);
+    int64_t k, pos = 0, runDev = 0, runLen = 0;
+    uint8_t* runHost = NULL;
+    const uint8_t* h;
+    const int32_t *ord, *sum, *out, *segBad;
+    const lz4k_hash_seg* seg;
+    int rc = slot_wait(s);
+    if (rc != LZ4B200_OK) return rc;
+    h = (const uint8_t*)s->h_tab.p;
+    ord = (const int32_t*)(h + t.ord); sum = (const int32_t*)(h + t.sum); out = (const int32_t*)(h + t.outSize);
+    segBad = (const int32_t*)(h + t.segBad); seg = (const lz4k_hash_seg*)(h + t.segs);
+    for (k = 0; k < n; k++) {
+        p->outSize[gr->first + k] = out[ord[k]];
+        p->sumState[gr->first + k] = sum[ord[k]] == FC_SUM_BAD ? FC_SUM_BAD : FC_SUM_NONE;
+    }
+    for (k = 0; k < gr->nSegs; k++)
+        if (seg[k].flags & LZ4K_SEG_ENDS) p->contentBad[p->blocks[gr->first + seg[k].first].unit] = segBad[k] != 0;
+    if (sizeOnly) return rc;
+    for (k = 0; k < n; k++) {
+        const fp_block* b = &p->blocks[gr->first + k];
+        const int64_t f = p->units[b->unit].file;
+        const int64_t sz = b->raw ? b->size : out[ord[k]] > 0 ? out[ord[k]] : 0;
+        if (!fileStop[f]) {
+            if (!b->raw && out[ord[k]] < 0) fileStop[f] = 1;
+            else {
+                const int64_t room = dstCap[f] - filePos[f], w = sz < room ? sz : room > 0 ? room : 0;
+                uint8_t* to = dst + dstOff[f] + filePos[f];
+                if (w > 0) {
+                    if (runLen && runDev + runLen == pos && runHost + runLen == to) runLen += w;
+                    else {
+                        if (runLen) CU(cudaMemcpyAsync(runHost, (uint8_t*)s->pack.p + runDev, (size_t)runLen, cudaMemcpyDeviceToHost, s->stream));
+                        runDev = pos; runHost = to; runLen = w;
+                    }
+                }
+                if (w < sz) fileStop[f] = 1;
+                filePos[f] += sz;
+            }
+        }
+        pos += sz;
+    }
+    if (runLen) CU(cudaMemcpyAsync(runHost, (uint8_t*)s->pack.p + runDev, (size_t)runLen, cudaMemcpyDeviceToHost, s->stream));
+done:
+    return rc;
+}
+
+/* LZ4B200_ERR_ARG, with LZ4B200_last_cuda_error() saying that the host's memory ran out (under the host lock) */
+static int out_of_host_memory(void)
+{
+    snprintf(g_cuda_error, sizeof(g_cuda_error), "LZ4B200_decompress_files_host: out of host memory");
+    return LZ4B200_ERR_ARG;
+}
+
+/* walk (host) -> per group, N_PIPE in flight: issue group g, then retire group g - FH_LAG -> fold (host) */
+int LZ4B200_decompress_files_host(const void* h_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
+                                  void* h_dst, const int64_t* h_dstOff, const int64_t* h_dstCap,
+                                  int64_t* h_result, int64_t* h_consumed, int64_t* h_prefix,
+                                  int64_t nFiles, int skipChecksums, int sizeOnly)
+{
+    const int verify = !skipChecksums;
+    fp_plan p;
+    fh_group_t grs[N_PIPE];
+    int64_t *copies = NULL, *filePos = NULL, first, g, nGroups = 0;
+    uint8_t* fileStop = NULL;
+    int rc;
+    if (nFiles < 0) return LZ4B200_ERR_ARG;
+    if (nFiles == 0) return LZ4B200_OK;
+    if (!h_src || !h_srcOff || !h_srcSize || !h_result) return LZ4B200_ERR_ARG;
+    if (!sizeOnly && (!h_dst || !h_dstOff || !h_dstCap)) return LZ4B200_ERR_ARG;
+    memset(&p, 0, sizeof p);
+    if ((rc = host_begin()) != LZ4B200_OK) goto done;
+    if ((rc = fh_init()) != LZ4B200_OK) goto done;
+    if (!fp_build((const uint8_t*)h_src, h_srcOff, h_srcSize, sizeOnly ? NULL : h_dstCap, nFiles,
+                  verify ? FC_SUMS_VERIFY : FC_SUMS_SKIP, &p)) { rc = out_of_host_memory(); goto done; }
+    copies = (int64_t*)malloc((size_t)(p.nBlocks ? p.nBlocks : 1) * 3 * sizeof(int64_t));
+    filePos = (int64_t*)calloc((size_t)nFiles, sizeof(int64_t));
+    fileStop = (uint8_t*)calloc((size_t)nFiles, 1);
+    if (!copies || !filePos || !fileStop) { rc = out_of_host_memory(); goto done; }
+    for (first = 0; first < p.nBlocks; nGroups++) first = fp_group_end(&p, first, CHUNK_OUT_BYTES);
+    for (g = 0, first = 0; g < nGroups + FH_LAG; g++) {
+        if (g < nGroups) {
+            fh_group_t* gr = &grs[g % N_PIPE];
+            gr->first = first;
+            gr->end = fp_group_end(&p, first, CHUNK_OUT_BYTES);
+            first = gr->end;
+            if ((rc = fh_issue(&p, (const uint8_t*)h_src, g, &g_ctx.slot[g % N_PIPE], gr, sizeOnly, verify, copies)) != LZ4B200_OK)
+                goto done;
+        }
+        if (g >= FH_LAG && (rc = fh_retire(&p, &g_ctx.slot[(g - FH_LAG) % N_PIPE], &grs[(g - FH_LAG) % N_PIPE], sizeOnly,
+                                           (uint8_t*)h_dst, h_dstOff, h_dstCap, filePos, fileStop)) != LZ4B200_OK)
+            goto done;
+    }
+    /* every group has retired: the results are in the plan (the last copies down may still run) */
+    if (!fp_fold(&p, h_srcSize, sizeOnly ? NULL : h_dstCap, h_result, h_consumed, h_prefix)) rc = out_of_host_memory();
+done:
+    rc = host_end(rc);
+    fp_free(&p);
+    free(copies); free(filePos); free(fileStop);
+    return rc;
 }

@@ -79,6 +79,48 @@ FC_FN uint32_t fc_xxh32(const uint8_t* p, uint64_t len, uint32_t seed)
     return fc_xxh32_end(h, p, len);
 }
 
+/* XXH32 with seed 0 over a message that arrives in pieces (LZ4B200_decompress_files_host: a frame's content spans the
+ * groups of its blocks): the four accumulators, the bytes taken so far and the 0 .. 15 bytes after the last full
+ * stripe.  fc_xxh32_digest after any split of the message into fc_xxh32_update calls equals fc_xxh32(message, 0). */
+typedef struct {
+    uint32_t v[4];
+    uint32_t tailLen;          /* bytes in tail: total & 15 */
+    uint64_t total;
+    uint8_t tail[16];
+} fc_xxh32_state;
+
+FC_FN void fc_xxh32_init(fc_xxh32_state* s)
+{
+    s->v[0] = FC_XXH_P1 + FC_XXH_P2; s->v[1] = FC_XXH_P2; s->v[2] = 0; s->v[3] = 0u - FC_XXH_P1;
+    s->tailLen = 0; s->total = 0;
+}
+
+FC_FN void fc_xxh32_stripe(uint32_t v[4], const uint8_t* p)
+{
+    v[0] = fc_xxh32_round(v[0], fc_rd_le32(p));      v[1] = fc_xxh32_round(v[1], fc_rd_le32(p + 4));
+    v[2] = fc_xxh32_round(v[2], fc_rd_le32(p + 8));  v[3] = fc_xxh32_round(v[3], fc_rd_le32(p + 12));
+}
+
+FC_FN void fc_xxh32_update(fc_xxh32_state* s, const uint8_t* p, uint64_t len)
+{
+    const uint8_t* end = p + len;
+    s->total += len;
+    if (s->tailLen) {                                                      /* complete the stripe the tail began */
+        while (s->tailLen < 16 && p < end) s->tail[s->tailLen++] = *p++;
+        if (s->tailLen < 16) return;
+        fc_xxh32_stripe(s->v, s->tail);
+        s->tailLen = 0;
+    }
+    for (; end - p >= 16; p += 16) fc_xxh32_stripe(s->v, p);
+    while (p < end) s->tail[s->tailLen++] = *p++;
+}
+
+FC_FN uint32_t fc_xxh32_digest(const fc_xxh32_state* s)
+{
+    const uint32_t h = s->total >= 16 ? fc_xxh32_merge(s->v[0], s->v[1], s->v[2], s->v[3]) : FC_XXH_P5;
+    return fc_xxh32_end(h, s->tail, s->total);
+}
+
 FC_FN int64_t fc_block_bytes(int bsid) { return (int64_t)1 << (8 + 2 * bsid); }   /* 4..7 -> 64 KB..4 MB (lz4frame.c:333-342) */
 
 /* The block classes of the batched decode and encode: 0 .. 3 hold frame blocks of block size ID 4 + c, class 4 the blocks

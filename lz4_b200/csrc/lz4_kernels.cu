@@ -1555,7 +1555,8 @@ __device__ __forceinline__ void xxh_staged_chunk(const uint4* s, int i0, int iEn
     }
 }
 
-__device__ uint32_t xxh32_staged(const uint8_t* p, int64_t len, uint4* ring)
+/* the stripes of p[0 .. len) run from the accumulators v (lane 0's v holds the result) */
+__device__ __forceinline__ void xxh32_staged_stripes(const uint8_t* p, int64_t len, uint4* ring, uint32_t v[4])
 {
     const int lane = threadIdx.x & 31;
     const uintptr_t at = reinterpret_cast<uintptr_t>(p);
@@ -1566,7 +1567,6 @@ __device__ uint32_t xxh32_staged(const uint8_t* p, int64_t len, uint4* ring)
     const int64_t chunks = n / kXsChunk + 1;                        /* chunk c stages granules c * kXsChunk + i */
     const uint32_t bs = (uint32_t)(at & 3) * 8;
     const int ws = (int)((at >> 2) & 3);
-    uint32_t v[4] = {FC_XXH_P1 + FC_XXH_P2, FC_XXH_P2, 0u, 0u - FC_XXH_P1};
     uint4 lo = make_uint4(0, 0, 0, 0);
     auto issue = [&](int64_t c) {                                   /* one commit group per chunk, empty past the end */
         if (c < chunks) {
@@ -1598,6 +1598,13 @@ __device__ uint32_t xxh32_staged(const uint8_t* p, int64_t len, uint4* ring)
     }
     asm volatile("cp.async.wait_group 0;" ::: "memory");
     __syncwarp();
+}
+
+__device__ uint32_t xxh32_staged(const uint8_t* p, int64_t len, uint4* ring)
+{
+    const int64_t n = len >> 4;
+    uint32_t v[4] = {FC_XXH_P1 + FC_XXH_P2, FC_XXH_P2, 0u, 0u - FC_XXH_P1};
+    xxh32_staged_stripes(p, len, ring, v);
     return fc_xxh32_end(n ? fc_xxh32_merge(v[0], v[1], v[2], v[3]) : FC_XXH_P5, p + (n << 4), (uint64_t)len);
 }
 
@@ -1750,6 +1757,100 @@ __global__ void __launch_bounds__(128) lz4_files_fold_kernel(lz4k_files_args a)
     if (f >= a.nFiles) return;
     fc_fold_file(static_cast<const fc_file_rec*>(a.files) + f, a.srcOff[f], a.srcSize[f], a.maxUnits, a.u.result,
                  a.u.srcOff, a.result + f, a.consumed ? a.consumed + f : nullptr, a.prefix ? a.prefix + f : nullptr);
+}
+
+/* =============================================================================================
+ * one group of the host-buffer file decode (LZ4B200_decompress_files_host): the host walks the files and cuts their
+ * blocks into groups; per group, around the decode of its table (one launch per class, by the caller):
+ *   block sums: content_hash over the entries marked FC_SUM_PENDING: XXH32 of the staged stored bytes
+ *   sizes     : one thread per block, in file order -- its output size and the place of its bytes: its decode slot
+ *               or, stored raw, its staged bytes
+ *   scan      : lz4_pack_scan_kernel over the sizes: each block's place in the group's output
+ *   gather    : lz4_pack_gather_kernel from those places
+ *   hash      : content_hash over the segments that start and end their frame in the group
+ *   carry     : one warp for each of the first and the last segment when it continues a frame from the group before
+ *               (the state that group's carry left) or leaves it open for the next (the state the next one reads)
+ * ============================================================================================= */
+__device__ __forceinline__ bool seg_carried(const lz4k_hash_seg& g)
+{
+    return (g.flags & LZ4K_SEG_CONTINUES) || !(g.flags & LZ4K_SEG_ENDS);
+}
+
+__device__ __forceinline__ int64_t group_stored(const lz4k_group_args& a, int64_t e)
+{
+    return a.rawLen[e] >= 0 ? a.rawLen[e] : a.srcSize[e];
+}
+
+__global__ void __launch_bounds__(32 * kXsWarps) lz4_group_block_sum_kernel(lz4k_group_args a)
+{
+    content_hash(a.n,
+        [&](int64_t e, const uint8_t** p, int64_t* len) {
+            *p = a.base + a.srcOff[e];
+            *len = group_stored(a, e);
+            return a.sum[e] == FC_SUM_PENDING;
+        },
+        [&](int64_t e, uint32_t h) {
+            const int64_t n = group_stored(a, e);
+            a.sum[e] = h == fc_rd_le32(a.base + a.srcOff[e] + n) ? FC_SUM_NONE : FC_SUM_BAD;
+        });
+}
+
+/* one thread per block: its output size and where its bytes are, in file order, for the pack scan and gather */
+__global__ void __launch_bounds__(128) lz4_group_sizes_kernel(lz4k_group_args a)
+{
+    const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= a.n) return;
+    const int32_t e = a.ord[k], o = a.outSize[e];
+    a.blockSize[k] = a.rawLen[e] >= 0 ? a.rawLen[e] : o > 0 ? o : 0;
+    a.blockFrom[k] = a.gatherOff[e];
+}
+
+__global__ void __launch_bounds__(32 * kXsWarps) lz4_group_hash_kernel(lz4k_group_args a)
+{
+    content_hash(a.nSegs,
+        [&](int64_t s, const uint8_t** p, int64_t* len) {
+            const lz4k_hash_seg g = a.segs[s];
+            *p = a.packed + a.blockOff[g.first];
+            *len = a.blockOff[g.end] - a.blockOff[g.first];
+            return !seg_carried(g);
+        },
+        [&](int64_t s, uint32_t h) { a.segBad[s] = h != a.segs[s].expected; });
+}
+
+/* Warp 0 takes the first segment, warp 1 the last (when there are two or more), if it is carried: the state it
+ * continues (or a fresh one), the bytes that complete its tail (every lane alike), the stripes by the warp
+ * (xxh32_staged_stripes, lane 0's accumulators broadcast), the bytes after them into the tail; then lane 0 compares the
+ * digest or leaves the state for the next group. */
+__global__ void __launch_bounds__(64) lz4_group_carry_kernel(lz4k_group_args a)
+{
+    __shared__ uint4 ring[2][kXsRing * kXsChunk];
+    const int w = threadIdx.x >> 5;
+    if (w == 1 && a.nSegs < 2) return;
+    const int64_t s = w == 0 ? 0 : a.nSegs - 1;
+    const lz4k_hash_seg g = a.segs[s];
+    if (!seg_carried(g)) return;
+    const uint8_t* p = a.packed + a.blockOff[g.first];
+    const int64_t len = a.blockOff[g.end] - a.blockOff[g.first];
+    fc_xxh32_state st;
+    if (g.flags & LZ4K_SEG_CONTINUES) st = *static_cast<const fc_xxh32_state*>(a.carryIn);
+    else fc_xxh32_init(&st);
+    int64_t k = 0;
+    if (st.tailLen) {
+        k = 16 - (int64_t)st.tailLen < len ? 16 - (int64_t)st.tailLen : len;
+        fc_xxh32_update(&st, p, (uint64_t)k);
+    }
+    const int64_t body = (len - k) & ~(int64_t)15;
+    if (body) {
+        xxh32_staged_stripes(p + k, body, ring[w], st.v);
+        #pragma unroll
+        for (int i = 0; i < 4; i++) st.v[i] = __shfl_sync(kFull, st.v[i], 0);
+        st.total += (uint64_t)body;
+    }
+    fc_xxh32_update(&st, p + k + body, (uint64_t)(len - k - body));
+    if ((threadIdx.x & 31) == 0) {
+        if (g.flags & LZ4K_SEG_ENDS) a.segBad[s] = fc_xxh32_digest(&st) != g.expected;
+        else *static_cast<fc_xxh32_state*>(a.carryOut) = st;
+    }
 }
 
 /* =============================================================================================
@@ -1977,6 +2078,34 @@ int lz4k_launch_files_fold(const lz4k_files_args* a, void* stream)
 {
     lz4_files_fold_kernel<<<frames_grid(a->nFiles), 128, 0, (cudaStream_t)stream>>>(*a);
     g_launches++;
+    return (int)cudaGetLastError();
+}
+
+static void xs_carveout(const void* kernel);
+
+int lz4k_launch_group_block_sums(const lz4k_group_args* a, void* stream)
+{
+    xs_carveout((const void*)lz4_group_block_sum_kernel);
+    lz4_group_block_sum_kernel<<<(unsigned)xs_grid(a->n), 32 * kXsWarps, 0, (cudaStream_t)stream>>>(*a);
+    g_launches++;
+    return (int)cudaGetLastError();
+}
+
+int lz4k_launch_group_assemble(const lz4k_group_args* a, void* stream)
+{
+    cudaStream_t s = (cudaStream_t)stream;
+    lz4_group_sizes_kernel<<<frames_grid(a->n), 128, 0, s>>>(*a);
+    g_launches++;
+    return launch_pack(a->base, a->blockFrom, 0, a->blockSize, a->n, a->packed, a->blockOff, 0, FrameRule{}, s);
+}
+
+int lz4k_launch_group_content(const lz4k_group_args* a, int carry, void* stream)
+{
+    cudaStream_t s = (cudaStream_t)stream;
+    xs_carveout((const void*)lz4_group_hash_kernel);
+    lz4_group_hash_kernel<<<(unsigned)xs_grid(a->nSegs), 32 * kXsWarps, 0, s>>>(*a);
+    g_launches++;
+    if (carry) { lz4_group_carry_kernel<<<1, 64, 0, s>>>(*a); g_launches++; }
     return (int)cudaGetLastError();
 }
 

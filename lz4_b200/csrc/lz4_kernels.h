@@ -133,6 +133,46 @@ int lz4k_launch_files_totals(const lz4k_files_args* a, void* stream);
 int lz4k_launch_files_place(const lz4k_files_args* a, void* stream);
 /* last: every file's result, consumed and prefix from the unit results */
 int lz4k_launch_files_fold(const lz4k_files_args* a, void* stream);
+/* The steps of one group of LZ4B200_decompress_files_host around the decode of its blocks (one lz4k_launch_decode per
+ * class, by the caller).  A group is a run of consecutive blocks of the call's files; its table lists them by class
+ * (entry e), and ord gives the entry of the k-th block in file order.  A hash segment is a run of blocks of one frame
+ * that carries a content checksum. */
+#define LZ4K_SEG_CONTINUES 1   /* the frame began in an earlier group: the hash starts from the carried state */
+#define LZ4K_SEG_ENDS      2   /* the frame's last block is in this group: the digest is compared */
+typedef struct {
+    int32_t first, end;        /* blocks [first, end) of the group, in file order */
+    uint32_t expected;         /* the content checksum the frame carries */
+    int32_t flags;             /* LZ4K_SEG_* */
+} lz4k_hash_seg;
+
+typedef struct {
+    uint8_t* base;             /* the decode's slots and the staged source bytes, in one buffer */
+    uint8_t* packed;           /* the group's output, block after block in file order */
+    int64_t n;                 /* blocks */
+    const int64_t* srcOff;     /* [n] entry e's stored bytes at base + srcOff[e] */
+    const int64_t* gatherOff;  /* [n] its output: base + gatherOff[e] (its decode slot, or its stored bytes if raw) */
+    const int32_t* srcSize;    /* [n] stored bytes given to the decode (0 for a stored-raw block) */
+    const int32_t* rawLen;     /* [n] a stored-raw block's size, -1 for a compressed one */
+    const int32_t* ord;        /* [n] the entry of block k */
+    int32_t* sum;              /* [n] FC_SUM_PENDING: the block checksum to compare; the kernel writes NONE or BAD */
+    const int32_t* outSize;    /* [n] the decode's results */
+    int32_t* blockSize;        /* [n] output bytes of block k: its rawLen, or its decoded size (0 if it failed) */
+    int64_t* blockFrom;        /* [n] block k's output before the gather: base + the gatherOff of its entry */
+    int64_t* blockOff;         /* [n + 1] where block k goes in packed; blockOff[n] = the group's output bytes */
+    const lz4k_hash_seg* segs; /* [nSegs], in file order */
+    int64_t nSegs;
+    int32_t* segBad;           /* [nSegs] 1 where a segment that ends the frame does not match */
+    const void* carryIn;       /* fc_xxh32_state of the frame the first segment continues */
+    void* carryOut;            /* .. of the frame the last segment leaves open */
+} lz4k_group_args;
+
+/* every block checksum marked FC_SUM_PENDING, over the staged stored bytes */
+int lz4k_launch_group_block_sums(const lz4k_group_args* a, void* stream);
+/* after the decode: each block's output size and place in file order, their scan (the pack scan), the gather into
+ * packed (the pack gather) */
+int lz4k_launch_group_assemble(const lz4k_group_args* a, void* stream);
+/* after the assembly: the content hash of every segment; carry: a segment continues or leaves its frame open */
+int lz4k_launch_group_content(const lz4k_group_args* a, int carry, void* stream);
 /* the batched frame and legacy encode's own steps (lz4_frame_core.h); the encode of the block table between them is the
  * caller's */
 typedef struct {

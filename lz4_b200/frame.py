@@ -1,6 +1,7 @@
 """One-shot LZ4 frames of independent blocks (SURVEY.md section 8 f-1): the Python face of
 LZ4B200_compressFrame_host / LZ4B200_decompressFrame_host (the roles of LZ4F_compressFrame,
-lz4frame.h:224, and of a one-shot LZ4F_decompress, lz4frame.h:470)."""
+lz4frame.h:224, and of a one-shot LZ4F_decompress, lz4frame.h:470), and of LZ4B200_decompress_files_host:
+whole .lz4 files in host memory decoded as `lz4 -d` decodes them."""
 import ctypes as C
 
 import numpy as np
@@ -12,7 +13,7 @@ from .block import _u8
 class Lz4FrameError(RuntimeError):
     def __init__(self, code, what):
         names = {-1: "bad argument", -2: "CUDA error", -3: "malformed frame", -4: "unsupported frame feature",
-                 -5: "destination too small"}
+                 -5: "destination too small", -6: "over the call's budget", -7: "checksum mismatch"}
         super().__init__("%s: %s (%d)" % (what, names.get(int(code), "error"), int(code)))
         self.code = int(code)
 
@@ -40,3 +41,81 @@ def decompress_frame(frame, capacity):
     if r < 0:
         raise Lz4FrameError(r, "LZ4B200_decompressFrame_host")
     return dst[:r].tobytes()
+
+
+def _i64(name, v):
+    v = int(v)
+    if not -2 ** 63 <= v < 2 ** 63:
+        raise ValueError("%s = %d does not fit an int64" % (name, v))
+    return v
+
+
+def _files_call(src, offs, sizes, caps, skip_checksums, size_only):
+    """one LZ4B200_decompress_files_host call: (results, consumed, prefixes, output or None)"""
+    lib = _lib.load()
+    n = len(offs)
+    i64 = lambda a: np.ascontiguousarray(a, dtype=np.int64)
+    offs, sizes = i64(offs), i64(sizes)
+    res, con, pre = (np.zeros(n, dtype=np.int64) for _ in range(3))
+    out = dst_offs = caps_a = None
+    if not size_only:
+        caps_a = i64(caps)
+        dst_offs = np.zeros(n, dtype=np.int64)
+        room = np.maximum(caps_a, 0)
+        dst_offs[1:] = np.cumsum(room)[:-1]
+        out = np.empty(max(int(room.sum()), 1), dtype=np.uint8)
+    ptr = lambda a: a.ctypes.data if a is not None else None
+    rc = int(lib.LZ4B200_decompress_files_host(src.ctypes.data, offs.ctypes.data, sizes.ctypes.data, ptr(out),
+                                               ptr(dst_offs), ptr(caps_a), res.ctypes.data, con.ctypes.data,
+                                               pre.ctypes.data, n, 1 if skip_checksums else 0, 1 if size_only else 0))
+    if rc < 0:
+        raise Lz4FrameError(rc, "LZ4B200_decompress_files_host")
+    return res.tolist(), con.tolist(), pre.tolist(), (out, dst_offs)
+
+
+def decompress_files(datas, capacities=None, skip_checksums=False, size_only=False):
+    """Decode whole .lz4 files (concatenated frames, skippable frames, `lz4 -l` legacy streams) from host memory, as
+    LZ4B200_decompress_files_host does.  Per file: (result, consumed, prefix, data) -- result the decoded size or the
+    file's error code, consumed the failing unit's offset (the file's size on success), prefix the bytes decoded before
+    it, and data the decoded bytes (the prefix's bytes on failure; None with size_only).  capacities: each file's room;
+    None runs the size-only pass first and gives each file its decoded size, so that every result is the one at
+    unlimited room."""
+    parts = [_u8(d) for d in datas]
+    n = len(parts)
+    sizes = [len(p) for p in parts]
+    offs = np.zeros(n, dtype=np.int64)
+    if n:
+        offs[1:] = np.cumsum(sizes)[:-1]
+    src = np.concatenate(parts) if n and sum(sizes) else np.zeros(1, dtype=np.uint8)
+    if capacities is not None:
+        capacities = [_i64("capacity", c) for c in capacities]
+        if len(capacities) != n:
+            raise ValueError("capacities has %d values for %d files" % (len(capacities), n))
+    if size_only:
+        res, con, pre, _ = _files_call(src, offs, sizes, None, skip_checksums, True)
+        return [(r, c, p, None) for r, c, p in zip(res, con, pre)]
+    sized = None
+    if capacities is None:
+        # the size-only pass at unlimited room: a file that fails there is given its prefix as room, so that the
+        # decoding pass finds the content checksums of the units before the failing one, and keeps the size-only
+        # pass's answer when it fails at that same unit
+        sized = _files_call(src, offs, sizes, None, skip_checksums, True)
+        capacities = [r if r >= 0 else p for r, p in zip(sized[0], sized[2])]
+    res, con, pre, (out, dst_offs) = _files_call(src, offs, sizes, capacities, skip_checksums, False)
+    got = []
+    for k in range(n):
+        r, c, p = res[k], con[k], pre[k]
+        if sized is not None and sized[0][k] < 0 and r < 0 and c == sized[1][k]:
+            r, c, p = sized[0][k], sized[1][k], sized[2][k]
+        o = int(dst_offs[k])
+        got.append((r, c, p, out[o:o + (r if r >= 0 else p)].tobytes()))
+    return got
+
+
+def decompress_file(data, capacity=None, skip_checksums=False):
+    """One whole .lz4 file from host memory: its decoded bytes, or Lz4FrameError with the file's code.  capacity=None
+    sizes the output with the size-only pass first."""
+    (r, _, _, b), = decompress_files([data], None if capacity is None else [capacity], skip_checksums)
+    if r < 0:
+        raise Lz4FrameError(r, "LZ4B200_decompress_files_host")
+    return b
