@@ -736,6 +736,53 @@ LZ4B200_API int LZ4B200_decompress_files_host(const void* h_src, const int64_t* 
                                               int64_t* h_result, int64_t* h_consumed, int64_t* h_prefix,
                                               int64_t nFiles, int skipChecksums, int sizeOnly);
 
+/*
+ * Write nFiles whole .lz4 files from host memory, as LZ4B200_compress_frames_checksummed (frames) and
+ * LZ4B200_compress_legacy (`lz4 -l` streams) write them in device memory, with no budget, no workspace and no stream:
+ * file f is h_src + h_srcOff[f], h_srcSize[f] bytes, and is written to h_dst + h_dstOff[f] with h_dstCap[f] bytes of
+ * room.
+ *   h_result[f]: what the device call returns for the same file with the same arguments and a budget that covers every
+ *   file -- the file's length, or LZ4B200_ERR_ARG (a negative size or capacity), or LZ4B200_ERR_DSTSIZE, in the device
+ *   call's order; never LZ4B200_ERR_LIMIT.  The bytes are the device call's, so with parallel == 0 they are the reference
+ *   tool's: `lz4 -c -<level> [-B4..7] [--BX] [--no-frame-crc] [--content-size]` and `lz4 -l -c -<level>`.  Each call
+ *   keeps the device call's level mapping: level 2 is lz4mid's HC parse for a frame and the fast parse for a legacy
+ *   stream.
+ * LZ4B200_ERR_DSTSIZE is decided before encoding, against the device call's bound: LZ4B200_compressFrameBound_checksummed
+ * for frames (capacity == bound succeeds, bound - 1 fails; LZ4B200_compressFrameBound, which has no checksums and some
+ * slack, is not this threshold), LZ4B200_compressLegacyBound for legacy streams.  Only [dst_f, dst_f + h_result[f]) is
+ * written, nothing for a failed file.  Host regions must not overlap each other or the source; no readable padding is
+ * needed (the call stages the bytes itself, 16-byte aligned with slack).
+ * The files' blocks are cut into groups of at most G source bytes (LZ4B200_HOST_WRITE_MB, default 512 MiB) and B blocks
+ * (2 048 at HC levels, 65 536 otherwise), one block at least; small files share a group, a large file spans many.  Each
+ * group goes through the device on one of the pipeline's four streams -- its source pieces up, one encode, the body
+ * assembled with stored-raw blocks and block checksums, the content checksums (a frame's hash state carried from group to
+ * group in device memory), its offsets down -- and its body goes to each file's place when it retires; the host writes
+ * headers, EndMarks and digests.  Device memory held at most, over the four slots: 4 x (the staged source, 2 G + 16 B;
+ * the encode's slots, G + G/255 + 32 B; the body, G + G/255 + 24 B; the table, 56 B + 8; at HC levels the HC
+ * workspace, 256 KB x B at levels 2 .. 9 and 320 KB x B at 10 .. 12; each buffer rounded up by at most 1 MiB + 16
+ * bytes), plus 5 x 40 bytes of carried hash state, where G stands for the larger of G and the largest block.  The slots
+ * are shared with the other host-buffer calls and kept between calls.
+ * DESIGN section 3.18.
+ * Returns LZ4B200_OK, LZ4B200_ERR_ARG (nFiles < 0; for frames blockSizeID outside {0, 4 .. 7}, 0 meaning 4, or parallel
+ * with compressionLevel >= 2; then, with files, a NULL pointer; or host memory for the plan ran out, which
+ * LZ4B200_last_cuda_error() then says) or LZ4B200_ERR_CUDA (no device included: there is no CPU fallback).  nFiles == 0
+ * returns LZ4B200_OK without touching the device.  Synchronous; one host-buffer call runs at a time.
+ */
+LZ4B200_API int LZ4B200_compress_frames_host(const void* h_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
+                                             void* h_dst, const int64_t* h_dstOff, const int64_t* h_dstCap,
+                                             int64_t* h_result, int64_t nFiles,
+                                             int blockSizeID, int compressionLevel, int contentSizeFlag, int parallel,
+                                             int blockChecksumFlag, int contentChecksumFlag);
+LZ4B200_API int LZ4B200_compress_legacy_host(const void* h_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
+                                             void* h_dst, const int64_t* h_dstOff, const int64_t* h_dstCap,
+                                             int64_t* h_result, int64_t nFiles, int compressionLevel);
+/* The capacity below which LZ4B200_compress_frames_checksummed and LZ4B200_compress_frames_host give a frame of srcSize
+ * bytes LZ4B200_ERR_DSTSIZE: LZ4F_compressFrameBound for the checksums at the frame's own block size ID (blockSizeID
+ * shrunk as LZ4F_optimalBSID does), 19 + (4 + 4 B) x blocks + srcSize + 4 + 4 C.  LZ4B200_ERR_ARG for srcSize < 0 or
+ * blockSizeID outside {0, 4 .. 7}. */
+LZ4B200_API int64_t LZ4B200_compressFrameBound_checksummed(int64_t srcSize, int blockSizeID, int blockChecksumFlag,
+                                                           int contentChecksumFlag);
+
 /* ---------------------------------------------------------------------------------------------
  * 4. Frame layer (SURVEY.md section 8 f-1): one-shot LZ4 frames of INDEPENDENT blocks, host buffers.
  *    The container logic (header, block headers, EndMark) runs on the host, every block goes through

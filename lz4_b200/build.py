@@ -21,7 +21,8 @@ HEADERS = [os.path.join(CSRC, "lz4_kernels.h"), os.path.join(CSRC, "lz4_rows_cor
            os.path.join(CSRC, "lz4_scan_split.h"), os.path.join(CSRC, "lz4_encode_par.cuh"),
            os.path.join(CSRC, "lz4_decode_plan.h"), os.path.join(CSRC, "lz4_hc_core.h"),
            os.path.join(CSRC, "lz4_encode_hc.cuh"), os.path.join(CSRC, "lz4_frame_core.h"),
-           os.path.join(CSRC, "lz4_files_plan.h"), os.path.join(ROOT, "include", "lz4_b200.h")]
+           os.path.join(CSRC, "lz4_files_plan.h"), os.path.join(CSRC, "lz4_cfiles_plan.h"),
+           os.path.join(ROOT, "include", "lz4_b200.h")]
 
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17",

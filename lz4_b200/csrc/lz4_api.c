@@ -10,6 +10,7 @@
 #include "lz4_kernels.h"
 #include "lz4_frame_core.h"
 #include "lz4_files_plan.h"
+#include "lz4_cfiles_plan.h"
 
 #include <cuda_runtime_api.h>
 #include <pthread.h>
@@ -758,6 +759,17 @@ size_t LZ4B200_compress_frames_workspace_bytes(int64_t nFrames, const int64_t ma
     return cframes_plan(nFrames, cframes_budget(maxBlocks, mb), hcLevel, &p) ? p.bytes : 0;
 }
 
+/* The encode of a frame-writing call's block table e at hcLevel / e->acceleration (frames_levels, legacy_levels): the
+ * optimal parser, the HC parse, the parallel parse routed by block size, or the fast parse.  hc: hcBytes of workspace. */
+static int encode_table(lz4k_encode_args* e, int hcLevel, int parallel, void* hc, size_t hcBytes, void* stream)
+{
+    if (hcLevel >= 10)
+        return launched(lz4k_launch_encode_hc_opt(e, hcLevel, hc, hcBytes, stream), "lz4k_launch_encode_hc_opt");
+    if (hcLevel > 0) return launched(lz4k_launch_encode_hc(e, hcLevel, hc, hcBytes, stream), "lz4k_launch_encode_hc");
+    if (parallel) return encode_parallel(e, stream);
+    return launched(lz4k_launch_encode(e, stream), "lz4k_launch_encode");
+}
+
 /* The body of the frame-writing calls: index (+ budget scan, fill) -> one encode of the whole table -> pack scan ->
  * headers, places, EndMarks, results -> gather -> [block checksums] -> [content checksums].  A frame block is compressed
  * into its slot with capacity size - 1, as LZ4F_makeBlock does (lz4frame.c:883-908); a legacy block with capacity
@@ -803,15 +815,7 @@ static int cframes_run(const void* d_src, const int64_t* d_srcOff, const int64_t
     if ((rc = launched(lz4k_launch_cframes_index(&a, stream), "lz4k_launch_cframes_index")) != LZ4B200_OK) return rc;
     e = encode_args(d_src, 0, a.tabSrcSize, 0, a.slots, 0, 0, accel, a.tabOutSize, p.nEntries);
     e.srcOff = a.tabSrcOff; e.dstOff = a.tabSlotOff; e.dstCapArr = a.tabCap;
-    if (hcLevel >= 10)
-        rc = launched(lz4k_launch_encode_hc_opt(&e, hcLevel, ws + p.hc, p.hcBytes, stream), "lz4k_launch_encode_hc_opt");
-    else if (hcLevel > 0)
-        rc = launched(lz4k_launch_encode_hc(&e, hcLevel, ws + p.hc, p.hcBytes, stream), "lz4k_launch_encode_hc");
-    else if (parallel)
-        rc = encode_parallel(&e, stream);
-    else
-        rc = launched(lz4k_launch_encode(&e, stream), "lz4k_launch_encode");
-    if (rc != LZ4B200_OK) return rc;
+    if ((rc = encode_table(&e, hcLevel, parallel, ws + p.hc, p.hcBytes, stream)) != LZ4B200_OK) return rc;
     if ((rc = launched(lz4k_launch_cframes_assemble(&a, stream), "lz4k_launch_cframes_assemble")) != LZ4B200_OK) return rc;
     if ((sums & FC_BLOCK_SUM) &&
         (rc = launched(lz4k_launch_cframes_block_sums(&a, stream), "lz4k_launch_cframes_block_sums")) != LZ4B200_OK)
@@ -868,6 +872,16 @@ int LZ4B200_compress_frames_checksummed(const void* d_src, const int64_t* d_srcO
 int64_t LZ4B200_compressLegacyBound(int64_t srcSize)
 {
     return srcSize < 0 ? LZ4B200_ERR_ARG : fc_legacy_bound(srcSize);
+}
+
+int64_t LZ4B200_compressFrameBound_checksummed(int64_t srcSize, int blockSizeID, int blockChecksumFlag,
+                                               int contentChecksumFlag)
+{
+    if (srcSize < 0) return LZ4B200_ERR_ARG;
+    if (blockSizeID == 0) blockSizeID = 4;
+    if (blockSizeID < 4 || blockSizeID > 7) return LZ4B200_ERR_ARG;
+    return fc_frame_bound_sums(srcSize, fc_optimal_bsid(blockSizeID, srcSize),
+                               (blockChecksumFlag ? FC_BLOCK_SUM : 0) | (contentChecksumFlag ? FC_CONTENT_SUM : 0));
 }
 
 /* the legacy call's budget over FC_CLASSES in mb: maxBlocks legacy blocks, no frame blocks */
@@ -1665,9 +1679,9 @@ done:
 }
 
 /* LZ4B200_ERR_ARG, with LZ4B200_last_cuda_error() saying that the host's memory ran out (under the host lock) */
-static int out_of_host_memory(void)
+static int out_of_host_memory(const char* call)
 {
-    snprintf(g_cuda_error, sizeof(g_cuda_error), "LZ4B200_decompress_files_host: out of host memory");
+    snprintf(g_cuda_error, sizeof(g_cuda_error), "%s: out of host memory", call);
     return LZ4B200_ERR_ARG;
 }
 
@@ -1691,11 +1705,11 @@ int LZ4B200_decompress_files_host(const void* h_src, const int64_t* h_srcOff, co
     if ((rc = host_begin()) != LZ4B200_OK) goto done;
     if ((rc = fh_init()) != LZ4B200_OK) goto done;
     if (!fp_build((const uint8_t*)h_src, h_srcOff, h_srcSize, sizeOnly ? NULL : h_dstCap, nFiles,
-                  verify ? FC_SUMS_VERIFY : FC_SUMS_SKIP, &p)) { rc = out_of_host_memory(); goto done; }
+                  verify ? FC_SUMS_VERIFY : FC_SUMS_SKIP, &p)) { rc = out_of_host_memory(__func__); goto done; }
     copies = (int64_t*)malloc((size_t)(p.nBlocks ? p.nBlocks : 1) * 3 * sizeof(int64_t));
     filePos = (int64_t*)calloc((size_t)nFiles, sizeof(int64_t));
     fileStop = (uint8_t*)calloc((size_t)nFiles, 1);
-    if (!copies || !filePos || !fileStop) { rc = out_of_host_memory(); goto done; }
+    if (!copies || !filePos || !fileStop) { rc = out_of_host_memory(__func__); goto done; }
     for (first = 0; first < p.nBlocks; nGroups++) first = fp_group_end(&p, first, CHUNK_OUT_BYTES);
     for (g = 0, first = 0; g < nGroups + FH_LAG; g++) {
         if (g < nGroups) {
@@ -1711,10 +1725,286 @@ int LZ4B200_decompress_files_host(const void* h_src, const int64_t* h_srcOff, co
             goto done;
     }
     /* every group has retired: the results are in the plan (the last copies down may still run) */
-    if (!fp_fold(&p, h_srcSize, sizeOnly ? NULL : h_dstCap, h_result, h_consumed, h_prefix)) rc = out_of_host_memory();
+    if (!fp_fold(&p, h_srcSize, sizeOnly ? NULL : h_dstCap, h_result, h_consumed, h_prefix))
+        rc = out_of_host_memory(__func__);
 done:
     rc = host_end(rc);
     fp_free(&p);
     free(copies); free(filePos); free(fileStop);
     return rc;
+}
+
+/* ------------------------------------------------------------------------------------------ */
+/* whole .lz4 files written from host buffers: LZ4B200_compress_frames_checksummed's and       */
+/* LZ4B200_compress_legacy's bytes, pipelined in groups                                        */
+/* ------------------------------------------------------------------------------------------ */
+/* Source bytes per group (G).  One warp encodes one block, so a group costs about one block's encode whatever its size
+ * until the SMs fill, and the rate grows with G: DESIGN section 3.18 has the sweep that chose the default.
+ * LZ4B200_HOST_WRITE_MB overrides it (developer knob for tests/perf), read once per process. */
+#define CW_DEFAULT_MB 512
+/* Blocks per group (B): at HC levels each block holds an HC workspace slot of 256 KB (320 KB for the optimal parser),
+ * so B bounds that workspace; the other parses need no workspace and B only bounds the group's table. */
+#define CW_HC_BLOCKS  2048
+#define CW_BLOCKS     65536
+
+static int64_t write_group_bytes(void)
+{
+    static int64_t v = 0;
+    if (v == 0) {
+        const char* e = getenv("LZ4B200_HOST_WRITE_MB");
+        long mb = e ? atol(e) : 0;
+        v = (int64_t)((mb >= 1 && mb <= 4096) ? mb : CW_DEFAULT_MB) << 20;
+    }
+    return v;
+}
+
+/* A group's table in its slot, for n blocks and nSegs segments: [srcOff, slotOff: i64 n | segments | srcSize, cap: i32 n]
+ * go up, [outSize: i32 n] stays on the device, [bodyOff: i64 n + 1 | digest: u32 nSegs] come back. */
+typedef struct { size_t srcOff, slotOff, segs, srcSize, cap, outSize, bodyOff, digest, bytes; } cw_tab_t;
+
+static cw_tab_t cw_tab(int64_t n, int64_t nSegs)
+{
+    cw_tab_t t;
+    const size_t w8 = (size_t)n * 8, w4 = (size_t)n * 4;
+    t.srcOff = 0; t.slotOff = w8; t.segs = 2 * w8;
+    t.srcSize = t.segs + (size_t)nSegs * sizeof(lz4k_wseg);
+    t.cap = t.srcSize + w4; t.outSize = t.cap + w4;
+    t.bodyOff = (t.outSize + w4 + 7) & ~(size_t)7;
+    t.digest = t.bodyOff + w8 + 8;
+    t.bytes = t.digest + (size_t)nSegs * 4;
+    return t;
+}
+
+/* the encode of a writer call: its parse and level, and the checksums its frames carry (none for legacy streams) */
+typedef struct { int hcLevel, accel, parallel, sums; } cw_enc_t;
+
+static int64_t up16(int64_t x) { return (x + 15) & ~(int64_t)15; }
+
+/* Issue group gr on slot s (group index g): the table and the source pieces up, the encode, the body, the block
+ * checksums, the content checksums; then the body's offsets and the digests back to the pinned table. */
+static int cw_issue(const cp_plan* p, const uint8_t* src, int64_t g, slot_t* s, fh_group_t* gr, const cw_enc_t* c,
+                    int64_t* copies)
+{
+    const int64_t n = gr->end - gr->first, G = write_group_bytes();
+    const int hash = !p->legacy && (c->sums & FC_CONTENT_SUM);
+    int64_t k, f = -1, nCopies = 0, gaps = 0, nSegs = 0, slotBytes = 0, packBytes = 0, at;
+    size_t hcBytes = 0;
+    int rc = LZ4B200_OK, carry = 0;
+    cw_tab_t t;
+    uint8_t *h, *d;
+    lz4k_wseg* seg;
+    lz4k_encode_args e;
+    lz4k_wgroup_args a;
+    /* pieces: [hostOff, devOff, bytes] triples, coalesced across gaps of at most FH_GAP while the group's gaps stay
+     * within G, so that the staged bytes stay within 2 G (plus alignment) */
+    for (k = gr->first; k < gr->end; k++) {
+        const int64_t lo = p->srcOff[k], hi = lo + p->size[k];
+        int64_t* cp = nCopies ? copies + 3 * (nCopies - 1) : NULL;
+        const int64_t gap = cp ? lo - (cp[0] + cp[2]) : 0;
+        if (cp && lo >= cp[0] && gap <= FH_GAP && gaps + (gap > 0 ? gap : 0) <= G) {
+            if (gap > 0) gaps += gap;
+            if (hi > cp[0] + cp[2]) cp[2] = hi - cp[0];
+        } else {
+            cp = copies + 3 * nCopies++; cp[0] = lo; cp[2] = hi - lo;
+        }
+        slotBytes += up16(p->cap[k]);
+        packBytes += 8 + (p->legacy ? p->cap[k] : p->size[k]);
+        if (hash && p->file[k] != f) { nSegs++; f = p->file[k]; }
+    }
+    for (k = 0, at = 0; k < nCopies; k++) { copies[3 * k + 1] = at; at = up16(at + copies[3 * k + 2]); }
+    if (c->hcLevel > 0) hcBytes = c->hcLevel >= 10 ? lz4k_encode_hc_opt_workspace_bytes(n) : lz4k_encode_hc_workspace_bytes(n);
+    t = cw_tab(n, nSegs);
+    if ((rc = slot_take(s, (size_t)at, (size_t)slotBytes, hcBytes, (size_t)packBytes, t.bytes)) != LZ4B200_OK) return rc;
+    h = (uint8_t*)s->h_tab.p;
+    d = (uint8_t*)s->d_tab.p;
+    seg = (lz4k_wseg*)(h + t.segs);
+    gr->nSegs = 0;
+    /* the table: blocks in file order, each frame's blocks one segment */
+    {
+        int64_t* srcOff = (int64_t*)(h + t.srcOff);
+        int64_t* slotOff = (int64_t*)(h + t.slotOff);
+        int32_t* srcSize = (int32_t*)(h + t.srcSize);
+        int32_t* cap = (int32_t*)(h + t.cap);
+        int64_t piece = 0;
+        for (k = gr->first, at = 0, f = -1; k < gr->end; k++) {
+            const int64_t i = k - gr->first;
+            const int64_t* cp;
+            while (!(p->srcOff[k] >= copies[3 * piece] && p->srcOff[k] + p->size[k] <= copies[3 * piece] + copies[3 * piece + 2]))
+                piece++;
+            cp = copies + 3 * piece;
+            srcOff[i] = cp[1] + (p->srcOff[k] - cp[0]);
+            srcSize[i] = p->size[k];
+            cap[i] = p->cap[k];
+            slotOff[i] = at;
+            at += up16(p->cap[k]);
+            if (!hash) continue;
+            if (p->file[k] != f) {
+                const fc_frame_rec* r = &p->files[p->file[k]];
+                lz4k_wseg* q = &seg[gr->nSegs++];
+                f = p->file[k];
+                q->off = srcOff[i]; q->len = 0; q->pad = 0;
+                q->flags = (k > r->base ? LZ4K_SEG_CONTINUES : 0) | (r->base + r->count <= gr->end ? LZ4K_SEG_ENDS : 0);
+                if (q->flags != LZ4K_SEG_ENDS) carry = 1;
+            }
+            seg[gr->nSegs - 1].len += p->size[k];            /* a file's blocks lie together in one piece */
+        }
+    }
+    /* up: the table and the pieces */
+    CU(cudaMemcpyAsync(d, h, t.outSize, cudaMemcpyHostToDevice, s->stream));
+    for (k = 0; k < nCopies; k++)
+        CU(cudaMemcpyAsync((uint8_t*)s->in.p + copies[3 * k + 1], src + copies[3 * k], (size_t)copies[3 * k + 2],
+                           cudaMemcpyHostToDevice, s->stream));
+    /* the encode of every block into its slot at its capacity */
+    e = encode_args(s->in.p, 0, (const int32_t*)(d + t.srcSize), 0, s->out.p, 0, 0, c->accel, (int32_t*)(d + t.outSize), n);
+    e.srcOff = (const int64_t*)(d + t.srcOff); e.dstOff = (const int64_t*)(d + t.slotOff); e.dstCapArr = (const int32_t*)(d + t.cap);
+    if ((rc = encode_table(&e, c->hcLevel, c->parallel, s->ws.p, s->ws.cap, s->stream)) != LZ4B200_OK) return rc;
+    /* the body, the block checksums, the content checksums */
+    memset(&a, 0, sizeof a);
+    a.src = (const uint8_t*)s->in.p; a.slots = (const uint8_t*)s->out.p; a.packed = (uint8_t*)s->pack.p; a.n = n;
+    a.srcOff = e.srcOff; a.srcSize = e.srcSizeArr; a.slotOff = e.dstOff; a.outSize = e.outSize;
+    a.bodyOff = (int64_t*)(d + t.bodyOff);
+    a.legacy = p->legacy;
+    a.blockSums = !p->legacy && (c->sums & FC_BLOCK_SUM);
+    a.segs = (const lz4k_wseg*)(d + t.segs); a.nSegs = gr->nSegs; a.digest = (uint32_t*)(d + t.digest);
+    a.carryIn = (const fc_xxh32_state*)g_fh.carry + (g + FH_CARRIES - 1) % FH_CARRIES;
+    a.carryOut = (fc_xxh32_state*)g_fh.carry + g % FH_CARRIES;
+    if ((rc = launched(lz4k_launch_wgroup_body(&a, s->stream), "lz4k_launch_wgroup_body")) != LZ4B200_OK) return rc;
+    if (gr->nSegs) {
+        if (seg[0].flags & LZ4K_SEG_CONTINUES)           /* after the group before: its carry kernel left the state */
+            CU(cudaStreamWaitEvent(s->stream, g_fh.hashed[(g + N_PIPE - 1) % N_PIPE], 0));
+        if ((rc = launched(lz4k_launch_wgroup_content(&a, carry, s->stream), "lz4k_launch_wgroup_content")) != LZ4B200_OK)
+            return rc;
+        if (!(seg[gr->nSegs - 1].flags & LZ4K_SEG_ENDS)) CU(cudaEventRecord(g_fh.hashed[g % N_PIPE], s->stream));
+    }
+    /* down: the body's offsets and the digests */
+    CU(cudaMemcpyAsync(h + t.bodyOff, d + t.bodyOff, t.bytes - t.bodyOff, cudaMemcpyDeviceToHost, s->stream));
+done:
+    return rc;
+}
+
+/* File f's end at byte pos of its output at: a frame's EndMark and, with the content checksum, its digest; returns the
+ * file's length */
+static int64_t cw_end(const cp_plan* p, int64_t f, uint8_t* at, int64_t pos, uint32_t digest)
+{
+    if (p->legacy) return pos;
+    wr_le32(at + pos, 0);
+    if (p->files[f].sums & FC_CONTENT_SUM) { wr_le32(at + pos + 4, digest); return pos + 8; }
+    return pos + 4;
+}
+
+/* Retire the group gr that ran on slot s: its body from the slot's packed buffer to each file's running position, one
+ * copy per run of bytes contiguous on both sides, and the end of every file whose last block it holds. */
+static int cw_retire(const cp_plan* p, slot_t* s, const fh_group_t* gr, uint8_t* dst, const int64_t* dstOff,
+                     int64_t* filePos, int64_t* result)
+{
+    const int64_t n = gr->end - gr->first;
+    const cw_tab_t t = cw_tab(n, gr->nSegs);
+    int64_t k, f = -1, sg = -1, runDev = 0, runLen = 0;
+    uint8_t* runHost = NULL;
+    const int64_t* bodyOff;
+    const uint32_t* digest;
+    int rc = slot_wait(s);
+    if (rc != LZ4B200_OK) return rc;
+    bodyOff = (const int64_t*)((const uint8_t*)s->h_tab.p + t.bodyOff);
+    digest = (const uint32_t*)((const uint8_t*)s->h_tab.p + t.digest);
+    for (k = 0; k < n; k++) {
+        const int64_t b = gr->first + k, len = bodyOff[k + 1] - bodyOff[k];
+        const fc_frame_rec* r;
+        uint8_t* to;
+        if (p->file[b] != f) { f = p->file[b]; sg++; }      /* (segment sg, when the frames carry content checksums) */
+        r = &p->files[f];
+        to = dst + dstOff[f] + filePos[f];
+        if (runLen && runDev + runLen == bodyOff[k] && runHost + runLen == to) runLen += len;
+        else {
+            if (runLen) CU(cudaMemcpyAsync(runHost, (uint8_t*)s->pack.p + runDev, (size_t)runLen, cudaMemcpyDeviceToHost, s->stream));
+            runDev = bodyOff[k]; runHost = to; runLen = len;
+        }
+        filePos[f] += len;
+        if (b == r->base + r->count - 1)
+            result[f] = cw_end(p, f, dst + dstOff[f], filePos[f], sg < gr->nSegs ? digest[sg] : 0);
+    }
+    if (runLen) CU(cudaMemcpyAsync(runHost, (uint8_t*)s->pack.p + runDev, (size_t)runLen, cudaMemcpyDeviceToHost, s->stream));
+done:
+    return rc;
+}
+
+/* plan (host: verdicts, headers, empty files) -> per group, N_PIPE in flight: issue group g, then retire group
+ * g - FH_LAG (bodies, EndMarks, digests, results) */
+static int compress_files_host(const char* call, const void* h_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
+                               void* h_dst, const int64_t* h_dstOff, const int64_t* h_dstCap, int64_t* h_result,
+                               int64_t nFiles, int legacy, int bsid, int contentSizeFlag, const cw_enc_t* c)
+{
+    uint8_t* dst = (uint8_t*)h_dst;
+    cp_plan p;
+    fh_group_t grs[N_PIPE];
+    int64_t *copies = NULL, *filePos = NULL, first, g, f, nGroups = 0, maxBlocks = c->hcLevel > 0 ? CW_HC_BLOCKS : CW_BLOCKS;
+    int rc;
+    memset(&p, 0, sizeof p);
+    if ((rc = host_begin()) != LZ4B200_OK) goto done;
+    if ((rc = fh_init()) != LZ4B200_OK) goto done;
+    if (!cp_build(h_srcOff, h_srcSize, h_dstCap, nFiles, legacy, bsid, contentSizeFlag, c->sums, &p)) {
+        rc = out_of_host_memory(call); goto done;
+    }
+    copies = (int64_t*)malloc((size_t)(p.nBlocks ? p.nBlocks : 1) * 3 * sizeof(int64_t));
+    filePos = (int64_t*)calloc((size_t)nFiles, sizeof(int64_t));
+    if (!copies || !filePos) { rc = out_of_host_memory(call); goto done; }
+    for (f = 0; f < nFiles; f++) {                  /* the headers; a file of no blocks ends here */
+        const fc_frame_rec* r = &p.files[f];
+        if (r->status != LZ4B200_OK) { h_result[f] = r->status; continue; }
+        filePos[f] = cp_header(&p, f, dst + h_dstOff[f]);
+        if (r->count == 0) h_result[f] = cw_end(&p, f, dst + h_dstOff[f], filePos[f], fc_xxh32(dst, 0, 0));
+    }
+    for (first = 0; first < p.nBlocks; nGroups++) first = cp_group_end(&p, first, write_group_bytes(), maxBlocks);
+    for (g = 0, first = 0; g < nGroups + FH_LAG; g++) {
+        if (g < nGroups) {
+            fh_group_t* gr = &grs[g % N_PIPE];
+            gr->first = first;
+            gr->end = cp_group_end(&p, first, write_group_bytes(), maxBlocks);
+            first = gr->end;
+            if ((rc = cw_issue(&p, (const uint8_t*)h_src, g, &g_ctx.slot[g % N_PIPE], gr, c, copies)) != LZ4B200_OK) goto done;
+        }
+        if (g >= FH_LAG && (rc = cw_retire(&p, &g_ctx.slot[(g - FH_LAG) % N_PIPE], &grs[(g - FH_LAG) % N_PIPE], dst,
+                                           h_dstOff, filePos, h_result)) != LZ4B200_OK)
+            goto done;
+    }
+done:
+    rc = host_end(rc);                              /* (the last copies down end here) */
+    cp_free(&p);
+    free(copies); free(filePos);
+    return rc;
+}
+
+int LZ4B200_compress_frames_host(const void* h_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
+                                 void* h_dst, const int64_t* h_dstOff, const int64_t* h_dstCap,
+                                 int64_t* h_result, int64_t nFiles,
+                                 int blockSizeID, int compressionLevel, int contentSizeFlag, int parallel,
+                                 int blockChecksumFlag, int contentChecksumFlag)
+{
+    cw_enc_t c;
+    if (nFiles < 0) return LZ4B200_ERR_ARG;
+    if (blockSizeID == 0) blockSizeID = 4;
+    if (blockSizeID < 4 || blockSizeID > 7) return LZ4B200_ERR_ARG;
+    if (parallel && compressionLevel >= 2) return LZ4B200_ERR_ARG;
+    if (nFiles == 0) return LZ4B200_OK;
+    if (!h_src || !h_srcOff || !h_srcSize || !h_dst || !h_dstOff || !h_dstCap || !h_result) return LZ4B200_ERR_ARG;
+    frames_levels(compressionLevel, &c.hcLevel, &c.accel);
+    c.parallel = parallel != 0;
+    c.sums = (blockChecksumFlag ? FC_BLOCK_SUM : 0) | (contentChecksumFlag ? FC_CONTENT_SUM : 0);
+    return compress_files_host(__func__, h_src, h_srcOff, h_srcSize, h_dst, h_dstOff, h_dstCap,
+                               h_result, nFiles, 0, blockSizeID, contentSizeFlag, &c);
+}
+
+int LZ4B200_compress_legacy_host(const void* h_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
+                                 void* h_dst, const int64_t* h_dstOff, const int64_t* h_dstCap,
+                                 int64_t* h_result, int64_t nFiles, int compressionLevel)
+{
+    cw_enc_t c;
+    if (nFiles < 0) return LZ4B200_ERR_ARG;
+    if (nFiles == 0) return LZ4B200_OK;
+    if (!h_src || !h_srcOff || !h_srcSize || !h_dst || !h_dstOff || !h_dstCap || !h_result) return LZ4B200_ERR_ARG;
+    legacy_levels(compressionLevel, &c.hcLevel, &c.accel);
+    c.parallel = 0;
+    c.sums = 0;
+    return compress_files_host(__func__, h_src, h_srcOff, h_srcSize, h_dst, h_dstOff, h_dstCap,
+                               h_result, nFiles, 1, 0, 0, &c);
 }

@@ -1977,6 +1977,80 @@ __global__ void __launch_bounds__(32 * kXsWarps) lz4_cframes_content_sum_kernel(
         [&](int64_t f, uint32_t h) { st_le32(a.dst + a.dstOff[f] + a.result[f] - 4, h); });
 }
 
+/* =============================================================================================
+ * one group of the host-buffer file writers (LZ4B200_compress_frames_host, LZ4B200_compress_legacy_host): the host plans
+ * the files and cuts their blocks into groups; per group, after the encode of its blocks (by the caller):
+ *   scan, gather: the pack scan and gather with the frame rule over the staged source (legacy: the plain rule)
+ *   block sums  : content_hash over the blocks: XXH32 of each payload where it lies, into the 4 bytes after it
+ *   hash        : content_hash over the segments that start and end their frame in the group: XXH32 of the source
+ *   carry       : lz4_group_carry_kernel's steps on the first and the last segment when carried, over the source, the
+ *                 digest stored where the frame ends
+ * ============================================================================================= */
+__host__ __device__ inline FrameRule wgroup_rule(const lz4k_wgroup_args& a)
+{
+    FrameRule fr;
+    fr.raw = a.legacy ? nullptr : a.src;
+    fr.rawStride = 0; fr.blockSize = 0; fr.lastSize = 0; fr.rawOff = a.srcOff; fr.rawSize = a.srcSize;
+    return fr;
+}
+
+__global__ void __launch_bounds__(32 * kXsWarps) lz4_wgroup_block_sum_kernel(lz4k_wgroup_args a)
+{
+    content_hash(a.n,
+        [&](int64_t k, const uint8_t** p, int64_t* len) {
+            bool isRaw;
+            *len = pack_payload(wgroup_rule(a), a.outSize, k, a.n, isRaw);
+            *p = isRaw ? a.src + a.srcOff[k] : a.slots + a.slotOff[k];
+            return true;
+        },
+        [&](int64_t k, uint32_t h) { st_le32(a.packed + a.bodyOff[k + 1] - 4, h); });
+}
+
+__global__ void __launch_bounds__(32 * kXsWarps) lz4_wgroup_hash_kernel(lz4k_wgroup_args a)
+{
+    content_hash(a.nSegs,
+        [&](int64_t s, const uint8_t** p, int64_t* len) {
+            *p = a.src + a.segs[s].off;
+            *len = a.segs[s].len;
+            return a.segs[s].flags == LZ4K_SEG_ENDS;
+        },
+        [&](int64_t s, uint32_t h) { a.digest[s] = h; });
+}
+
+/* lz4_group_carry_kernel's steps, kept apart so that the decode's kernel stays as it is: warp 0 takes the first
+ * segment, warp 1 the last, if it is carried; then lane 0 stores the digest or leaves the state for the next group. */
+__global__ void __launch_bounds__(64) lz4_wgroup_carry_kernel(lz4k_wgroup_args a)
+{
+    __shared__ uint4 ring[2][kXsRing * kXsChunk];
+    const int w = threadIdx.x >> 5;
+    if (w == 1 && a.nSegs < 2) return;
+    const int64_t s = w == 0 ? 0 : a.nSegs - 1;
+    const lz4k_wseg g = a.segs[s];
+    if (g.flags == LZ4K_SEG_ENDS) return;
+    const uint8_t* p = a.src + g.off;
+    const int64_t len = g.len;
+    fc_xxh32_state st;
+    if (g.flags & LZ4K_SEG_CONTINUES) st = *static_cast<const fc_xxh32_state*>(a.carryIn);
+    else fc_xxh32_init(&st);
+    int64_t k = 0;
+    if (st.tailLen) {
+        k = 16 - (int64_t)st.tailLen < len ? 16 - (int64_t)st.tailLen : len;
+        fc_xxh32_update(&st, p, (uint64_t)k);
+    }
+    const int64_t body = (len - k) & ~(int64_t)15;
+    if (body) {
+        xxh32_staged_stripes(p + k, body, ring[w], st.v);
+        #pragma unroll
+        for (int i = 0; i < 4; i++) st.v[i] = __shfl_sync(kFull, st.v[i], 0);
+        st.total += (uint64_t)body;
+    }
+    fc_xxh32_update(&st, p + k + body, (uint64_t)(len - k - body));
+    if ((threadIdx.x & 31) == 0) {
+        if (g.flags & LZ4K_SEG_ENDS) a.digest[s] = fc_xxh32_digest(&st);
+        else *static_cast<fc_xxh32_state*>(a.carryOut) = st;
+    }
+}
+
 }  // namespace
 
 /* =============================================================================================
@@ -2106,6 +2180,31 @@ int lz4k_launch_group_content(const lz4k_group_args* a, int carry, void* stream)
     lz4_group_hash_kernel<<<(unsigned)xs_grid(a->nSegs), 32 * kXsWarps, 0, s>>>(*a);
     g_launches++;
     if (carry) { lz4_group_carry_kernel<<<1, 64, 0, s>>>(*a); g_launches++; }
+    return (int)cudaGetLastError();
+}
+
+int lz4k_launch_wgroup_body(const lz4k_wgroup_args* a, void* stream)
+{
+    cudaStream_t s = (cudaStream_t)stream;
+    const FrameRule fr = wgroup_rule(*a);
+    lz4_pack_scan_kernel<<<1, 1024, 0, s>>>(a->outSize, a->n, a->bodyOff, 4, a->blockSums ? 4 : 0, fr);
+    g_launches++;
+    launch_pack_gather(a->slots, a->slotOff, 0, a->outSize, a->n, a->packed, a->bodyOff, nullptr, 4, fr, s);
+    if (a->blockSums) {
+        xs_carveout((const void*)lz4_wgroup_block_sum_kernel);
+        lz4_wgroup_block_sum_kernel<<<(unsigned)xs_grid(a->n), 32 * kXsWarps, 0, s>>>(*a);
+        g_launches++;
+    }
+    return (int)cudaGetLastError();
+}
+
+int lz4k_launch_wgroup_content(const lz4k_wgroup_args* a, int carry, void* stream)
+{
+    cudaStream_t s = (cudaStream_t)stream;
+    xs_carveout((const void*)lz4_wgroup_hash_kernel);
+    lz4_wgroup_hash_kernel<<<(unsigned)xs_grid(a->nSegs), 32 * kXsWarps, 0, s>>>(*a);
+    g_launches++;
+    if (carry) { lz4_wgroup_carry_kernel<<<1, 64, 0, s>>>(*a); g_launches++; }
     return (int)cudaGetLastError();
 }
 

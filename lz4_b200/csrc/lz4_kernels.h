@@ -173,6 +173,39 @@ int lz4k_launch_group_block_sums(const lz4k_group_args* a, void* stream);
 int lz4k_launch_group_assemble(const lz4k_group_args* a, void* stream);
 /* after the assembly: the content hash of every segment; carry: a segment continues or leaves its frame open */
 int lz4k_launch_group_content(const lz4k_group_args* a, int carry, void* stream);
+/* The steps of one group of LZ4B200_compress_frames_host and LZ4B200_compress_legacy_host after the encode of its blocks
+ * (by the caller).  A group is a run of consecutive blocks of the call's files, in file order; a hash segment is the run
+ * of one frame's blocks in the group, whose source bytes lie together in the staged source. */
+typedef struct {
+    int64_t off, len;          /* the segment's source bytes: src + off, len bytes */
+    int32_t flags;             /* LZ4K_SEG_*: CONTINUES a frame begun in the group before, ENDS its frame here */
+    int32_t pad;
+} lz4k_wseg;
+
+typedef struct {
+    const uint8_t* src;        /* the group's staged source */
+    const uint8_t* slots;      /* the encode's output */
+    uint8_t* packed;           /* the group's body: [LE32 header][payload]([LE32 block checksum]) per block */
+    int64_t n;                 /* blocks */
+    const int64_t* srcOff;     /* [n] block k's source: src + srcOff[k], srcSize[k] bytes */
+    const int32_t* srcSize;
+    const int64_t* slotOff;    /* [n] its encode: slots + slotOff[k], outSize[k] bytes */
+    const int32_t* outSize;
+    int64_t* bodyOff;          /* [n + 1] where block k goes in packed; bodyOff[n] = the group's body bytes */
+    int legacy;                /* legacy chunks: never stored raw */
+    int blockSums;             /* a block checksum follows every payload */
+    const lz4k_wseg* segs;     /* [nSegs], in file order */
+    int64_t nSegs;
+    uint32_t* digest;          /* [nSegs] the content checksum of every frame that ends in the group */
+    const void* carryIn;       /* fc_xxh32_state of the frame the first segment continues */
+    void* carryOut;            /* .. of the frame the last segment leaves open */
+} lz4k_wgroup_args;
+
+/* the body: the pack scan (4-byte header, a 4-byte trailer with block checksums) and the gather, frame blocks that did
+ * not gain stored raw from the staged source; then the block checksums */
+int lz4k_launch_wgroup_body(const lz4k_wgroup_args* a, void* stream);
+/* the content checksums of the segments; carry: a segment continues or leaves its frame open */
+int lz4k_launch_wgroup_content(const lz4k_wgroup_args* a, int carry, void* stream);
 /* the batched frame and legacy encode's own steps (lz4_frame_core.h); the encode of the block table between them is the
  * caller's */
 typedef struct {

@@ -1,13 +1,14 @@
 """One-shot LZ4 frames of independent blocks (SURVEY.md section 8 f-1): the Python face of
 LZ4B200_compressFrame_host / LZ4B200_decompressFrame_host (the roles of LZ4F_compressFrame,
-lz4frame.h:224, and of a one-shot LZ4F_decompress, lz4frame.h:470), and of LZ4B200_decompress_files_host:
-whole .lz4 files in host memory decoded as `lz4 -d` decodes them."""
+lz4frame.h:224, and of a one-shot LZ4F_decompress, lz4frame.h:470), of LZ4B200_decompress_files_host:
+whole .lz4 files in host memory decoded as `lz4 -d` decodes them, and of LZ4B200_compress_frames_host and
+LZ4B200_compress_legacy_host: whole .lz4 files written from host memory as the `lz4` tool writes them."""
 import ctypes as C
 
 import numpy as np
 
 from . import _lib
-from .block import _u8
+from .block import _c_int, _u8
 
 
 class Lz4FrameError(RuntimeError):
@@ -119,3 +120,64 @@ def decompress_file(data, capacity=None, skip_checksums=False):
     if r < 0:
         raise Lz4FrameError(r, "LZ4B200_decompress_files_host")
     return b
+
+
+# the `lz4` tool's defaults for a frame: -1, 4 MB blocks (-B7), a content checksum, no block checksums, no content size
+_FRAME_DEFAULTS = dict(block_size_id=7, content_size=False, block_checksum=False, content_checksum=True, parallel=False)
+
+
+def compress_files(datas, level=1, block_size_id=7, content_size=False, block_checksum=False, content_checksum=True,
+                   parallel=False, legacy=False):
+    """Write whole .lz4 files from host memory (LZ4B200_compress_frames_host, or LZ4B200_compress_legacy_host with
+    legacy=True): one bytes per input, what `lz4 -c -<level> [-B<id>] [--BX] [--no-frame-crc] [--content-size]` (or
+    `lz4 -l -c -<level>`) writes for it.  The defaults are the tool's, not compress_frame's.  Every output is sized at
+    its bound, so valid input gives no per-file error.  legacy=True with a frame-only argument away from its default
+    raises ValueError."""
+    frame_args = dict(block_size_id=block_size_id, content_size=content_size, block_checksum=block_checksum,
+                      content_checksum=content_checksum, parallel=parallel)
+    if legacy and any(frame_args[k] != v for k, v in _FRAME_DEFAULTS.items()):
+        raise ValueError("legacy streams take no %s" % ", ".join(k for k, v in _FRAME_DEFAULTS.items()
+                                                                  if frame_args[k] != v))
+    lib = _lib.load()
+    level = _c_int("level", level)
+    bsid = _c_int("block_size_id", block_size_id)
+    parts = [_u8(d) for d in datas]
+    n = len(parts)
+    sizes = np.array([len(p) for p in parts], dtype=np.int64)
+    if legacy:
+        caps = [int(lib.LZ4B200_compressLegacyBound(int(k))) for k in sizes]
+    else:
+        caps = [int(lib.LZ4B200_compressFrameBound_checksummed(int(k), bsid, int(bool(block_checksum)),
+                                                               int(bool(content_checksum)))) for k in sizes]
+        if any(c < 0 for c in caps):
+            raise Lz4FrameError(min(caps), "LZ4B200_compressFrameBound_checksummed")
+    caps = np.array(caps, dtype=np.int64)
+    offs = np.zeros(n, dtype=np.int64)
+    dst_offs = np.zeros(n, dtype=np.int64)
+    if n:
+        offs[1:] = np.cumsum(sizes)[:-1]
+        dst_offs[1:] = np.cumsum(caps)[:-1]
+    src = np.concatenate(parts) if n and int(sizes.sum()) else np.zeros(1, dtype=np.uint8)
+    out = np.empty(max(int(caps.sum()), 1), dtype=np.uint8)
+    res = np.zeros(n, dtype=np.int64)
+    if legacy:
+        name = "LZ4B200_compress_legacy_host"
+        rc = int(lib.LZ4B200_compress_legacy_host(src.ctypes.data, offs.ctypes.data, sizes.ctypes.data, out.ctypes.data,
+                                                  dst_offs.ctypes.data, caps.ctypes.data, res.ctypes.data, n, level))
+    else:
+        name = "LZ4B200_compress_frames_host"
+        rc = int(lib.LZ4B200_compress_frames_host(src.ctypes.data, offs.ctypes.data, sizes.ctypes.data, out.ctypes.data,
+                                                  dst_offs.ctypes.data, caps.ctypes.data, res.ctypes.data, n, bsid, level,
+                                                  int(bool(content_size)), int(bool(parallel)),
+                                                  int(bool(block_checksum)), int(bool(content_checksum))))
+    if rc < 0:
+        raise Lz4FrameError(rc, name)
+    for r in res:
+        if r < 0:
+            raise Lz4FrameError(int(r), name)
+    return [out[int(o):int(o) + int(r)].tobytes() for o, r in zip(dst_offs, res)]
+
+
+def compress_file(data, **kwargs):
+    """One whole .lz4 file from host memory: compress_files([data], **kwargs)[0]"""
+    return compress_files([data], **kwargs)[0]
