@@ -1470,19 +1470,91 @@ done:
     return rc;
 }
 
+static int64_t up16(int64_t x) { return (x + 15) & ~(int64_t)15; }
+
+/* Source pieces: [hostOff, devOff, bytes] triples in copies (room for one per block).  A block's bytes [lo, hi) join
+ * the last piece when they begin in it or at most FH_GAP past its end, while the group's gaps stay within budget. */
+static void piece_add(int64_t* copies, int64_t* nCopies, int64_t* gaps, int64_t lo, int64_t hi, int64_t budget)
+{
+    int64_t* cp = *nCopies ? copies + 3 * (*nCopies - 1) : NULL;
+    const int64_t gap = cp ? lo - (cp[0] + cp[2]) : 0;
+    if (cp && lo >= cp[0] && gap <= FH_GAP && *gaps + (gap > 0 ? gap : 0) <= budget) {
+        if (gap > 0) *gaps += gap;
+        if (hi > cp[0] + cp[2]) cp[2] = hi - cp[0];
+    } else {
+        cp = copies + 3 * (*nCopies)++; cp[0] = lo; cp[2] = hi - lo;
+    }
+}
+
+/* where a block's bytes [lo, hi) are staged: the pieces are searched from *piece on, blocks in the order they were
+ * added */
+static int64_t piece_at(const int64_t* copies, int64_t* piece, int64_t lo, int64_t hi)
+{
+    const int64_t* cp = copies + 3 * *piece;
+    while (!(lo >= cp[0] && hi <= cp[0] + cp[2])) cp = copies + 3 * ++*piece;
+    return cp[1] + (lo - cp[0]);
+}
+
+/* segment q begins at block i of the group [first, end), for a frame of the blocks [base, base + count) */
+static void seg_open(lz4k_seg* q, int64_t i, int64_t base, int64_t count, int64_t first, int64_t end)
+{
+    q->first = (int32_t)i; q->end = (int32_t)i + 1; q->pad = 0;
+    q->flags = (base < first ? LZ4K_SEG_CONTINUES : 0) | (base + count <= end ? LZ4K_SEG_ENDS : 0);
+}
+
+/* The content checksums of group g's segments on slot s (seg: their host copy).  Only the first and the last segment
+ * can be carried: the first continues the state the group before left in the ring, after that group's event; the last
+ * leaves its state in the ring for the group after and records the event that group waits on. */
+static int seg_content(slot_t* s, int64_t g, const lz4k_seg* seg, lz4k_seg_args* a)
+{
+    int32_t f0, fl;
+    int rc = LZ4B200_OK;
+    if (!a->nSegs) return rc;
+    f0 = seg[0].flags; fl = seg[a->nSegs - 1].flags;
+    a->carryIn = (const fc_xxh32_state*)g_fh.carry + (g + FH_CARRIES - 1) % FH_CARRIES;
+    a->carryOut = (fc_xxh32_state*)g_fh.carry + g % FH_CARRIES;
+    if (f0 & LZ4K_SEG_CONTINUES) CU(cudaStreamWaitEvent(s->stream, g_fh.hashed[(g + N_PIPE - 1) % N_PIPE], 0));
+    rc = lz4k_launch_seg_content(a, f0 != LZ4K_SEG_ENDS || fl != LZ4K_SEG_ENDS, s->stream);
+    if ((rc = launched(rc, "lz4k_launch_seg_content")) != LZ4B200_OK) return rc;
+    if (!(fl & LZ4K_SEG_ENDS)) CU(cudaEventRecord(g_fh.hashed[g % N_PIPE], s->stream));
+done:
+    return rc;
+}
+
+/* a run of bytes contiguous in slot s's packed buffer and in the host output, copied down in one piece */
+typedef struct { uint8_t* host; int64_t dev, len; } run_t;
+
+static int run_flush(slot_t* s, run_t* r)
+{
+    int rc = LZ4B200_OK;
+    if (r->len) CU(cudaMemcpyAsync(r->host, (uint8_t*)s->pack.p + r->dev, (size_t)r->len, cudaMemcpyDeviceToHost, s->stream));
+    r->len = 0;
+done:
+    return rc;
+}
+
+/* len bytes at dev in the packed buffer to host: they extend the run, or the run goes down and theirs begins */
+static int run_add(slot_t* s, run_t* r, int64_t dev, uint8_t* host, int64_t len)
+{
+    int rc = LZ4B200_OK;
+    if (r->len && r->dev + r->len == dev && r->host + r->len == host) r->len += len;
+    else if ((rc = run_flush(s, r)) == LZ4B200_OK) { r->dev = dev; r->host = host; r->len = len; }
+    return rc;
+}
+
 /* A group's table in its slot (the host copy pinned, the device copy the kernels use), for n blocks and nSegs segments:
  * [srcOff, gatherOff, dstOff: i64 n | segments | srcSize, rawLen, ord, sum: i32 n] go up, [sum, outSize: i32 n |
- * segBad: i32 nSegs] come back, [blockSize: i32 n | blockFrom: i64 n | blockOff: i64 n + 1] stay on the device. */
-typedef struct { size_t srcOff, gatherOff, dstOff, segs, srcSize, rawLen, ord, sum, outSize, segBad, blockSize, blockFrom, blockOff, bytes; } fh_tab_t;
+ * digest: u32 nSegs] come back, [blockSize: i32 n | blockFrom: i64 n | blockOff: i64 n + 1] stay on the device. */
+typedef struct { size_t srcOff, gatherOff, dstOff, segs, srcSize, rawLen, ord, sum, outSize, digest, blockSize, blockFrom, blockOff, bytes; } fh_tab_t;
 
 static fh_tab_t fh_tab(int64_t n, int64_t nSegs)
 {
     fh_tab_t t;
     const size_t w8 = (size_t)n * 8, w4 = (size_t)n * 4;
     t.srcOff = 0; t.gatherOff = w8; t.dstOff = 2 * w8; t.segs = 3 * w8;
-    t.srcSize = t.segs + (size_t)nSegs * sizeof(lz4k_hash_seg);
-    t.rawLen = t.srcSize + w4; t.ord = t.rawLen + w4; t.sum = t.ord + w4; t.outSize = t.sum + w4; t.segBad = t.outSize + w4;
-    t.blockSize = t.segBad + (size_t)nSegs * 4;
+    t.srcSize = t.segs + (size_t)nSegs * sizeof(lz4k_seg);
+    t.rawLen = t.srcSize + w4; t.ord = t.rawLen + w4; t.sum = t.ord + w4; t.outSize = t.sum + w4; t.digest = t.outSize + w4;
+    t.blockSize = t.digest + (size_t)nSegs * 4;
     t.blockFrom = (t.blockSize + w4 + 7) & ~(size_t)7;
     t.blockOff = t.blockFrom + w8;
     t.bytes = t.blockOff + w8 + 8;
@@ -1499,15 +1571,16 @@ static int fh_issue(const fp_plan* p, const uint8_t* src, int64_t g, slot_t* s, 
 {
     const int64_t n = gr->end - gr->first;
     const int hash = verify && !sizeOnly;               /* the content checksums (none when the call only sizes) */
-    int64_t nc[FC_CLASSES] = {0, 0, 0, 0, 0}, cb[FC_CLASSES], fill[FC_CLASSES], k, e, nSegs = 0, nCopies = 0;
+    int64_t nc[FC_CLASSES] = {0, 0, 0, 0, 0}, cb[FC_CLASSES], fill[FC_CLASSES], k, e, nSegs = 0, nCopies = 0, gaps = 0;
     int64_t slotBytes = 0, inBytes = 0, at;
     size_t wsBytes = 0;
-    int c, rc = LZ4B200_OK, anySum = 0, carry = 0;
+    int c, rc = LZ4B200_OK, anySum = 0;
     fh_tab_t t;
     uint8_t* h;
     uint8_t* d;
     lz4k_group_args a;
-    lz4k_hash_seg* seg;
+    lz4k_seg_args sa;
+    lz4k_seg* seg;
     /* the classes, their slots, the segments and the source pieces */
     for (k = gr->first; k < gr->end; k++) nc[(int)p->blocks[k].cls]++;
     for (c = 0, at = 0; c < FC_CLASSES; c++) {
@@ -1522,22 +1595,20 @@ static int fh_issue(const fp_plan* p, const uint8_t* src, int64_t g, slot_t* s, 
         const fp_unit* u = &p->units[p->blocks[k].unit];
         if (hash && fp_content(u) && (k == gr->first || p->blocks[k - 1].unit != p->blocks[k].unit)) nSegs++;
     }
-    /* pieces: [hostOff, devOff, bytes] triples in `copies` (room for one per block), staged after the slots */
+    /* the pieces, staged after the slots; a group of at most CHUNK_OUT_BYTES of 64 KB or larger slots has fewer gaps
+     * of FH_GAP than that, so the budget never binds */
     for (k = gr->first; k < gr->end; k++) {
         const fp_block* b = &p->blocks[k];
-        const int64_t lo = b->srcOff, hi = b->srcOff + b->size + b->sumBytes;
-        int64_t* cp = nCopies ? copies + 3 * (nCopies - 1) : NULL;
-        if (cp && lo >= cp[0] && lo <= cp[0] + cp[2] + FH_GAP) { if (hi > cp[0] + cp[2]) cp[2] = hi - cp[0]; }
-        else { cp = copies + 3 * nCopies++; cp[0] = lo; cp[2] = hi - lo; }
+        piece_add(copies, &nCopies, &gaps, b->srcOff, b->srcOff + b->size + b->sumBytes, CHUNK_OUT_BYTES);
     }
     at = sizeOnly ? 0 : (slotBytes + 255) & ~(int64_t)255;              /* (the scan alone writes no slot) */
-    for (k = 0; k < nCopies; k++) { copies[3 * k + 1] = at; at = (at + copies[3 * k + 2] + 15) & ~(int64_t)15; }
+    for (k = 0; k < nCopies; k++) { copies[3 * k + 1] = at; at = up16(at + copies[3 * k + 2]); }
     inBytes = at;
     t = fh_tab(n, nSegs);
     if ((rc = slot_take(s, 0, (size_t)inBytes, wsBytes, sizeOnly ? 0 : (size_t)slotBytes, t.bytes)) != LZ4B200_OK)
         return rc;
     h = (uint8_t*)s->h_tab.p;
-    seg = (lz4k_hash_seg*)(h + t.segs);
+    seg = (lz4k_seg*)(h + t.segs);
     gr->nSegs = 0;
     /* the table: entries by class, blocks in file order */
     {
@@ -1552,12 +1623,9 @@ static int fh_issue(const fp_plan* p, const uint8_t* src, int64_t g, slot_t* s, 
         for (c = 0, at = 0; c < FC_CLASSES; c++) { slotAt[c] = at; at += nc[c] * fc_class_bytes(c); }
         for (k = gr->first; k < gr->end; k++) {
             const fp_block* b = &p->blocks[k];
-            const int64_t* cp;
-            while (!(b->srcOff >= copies[3 * piece] && b->srcOff < copies[3 * piece] + copies[3 * piece + 2] + 1)) piece++;
-            cp = copies + 3 * piece;
             e = fill[(int)b->cls]++;
             ord[k - gr->first] = (int32_t)e;
-            srcOff[e] = cp[1] + (b->srcOff - cp[0]);
+            srcOff[e] = piece_at(copies, &piece, b->srcOff, b->srcOff + b->size + b->sumBytes);
             dstOff[e] = slotAt[(int)b->cls] + (e - cb[(int)b->cls]) * fc_class_bytes(b->cls);
             gatherOff[e] = b->raw ? srcOff[e] : dstOff[e];
             srcSize[e] = b->raw ? 0 : b->size;
@@ -1567,15 +1635,8 @@ static int fh_issue(const fp_plan* p, const uint8_t* src, int64_t g, slot_t* s, 
             if (b->unit != u) {
                 const fp_unit* un = &p->units[b->unit];
                 u = b->unit;
-                if (hash && fp_content(un)) {
-                    lz4k_hash_seg* q = &seg[gr->nSegs++];
-                    q->first = (int32_t)(k - gr->first);
-                    q->end = (int32_t)(k - gr->first + 1);
-                    q->expected = un->contentSum;
-                    q->flags = (un->r.base < gr->first ? LZ4K_SEG_CONTINUES : 0) |
-                               (un->r.base + un->r.count <= gr->end ? LZ4K_SEG_ENDS : 0);
-                    if (q->flags != LZ4K_SEG_ENDS) carry = 1;
-                }
+                if (hash && fp_content(un))
+                    seg_open(&seg[gr->nSegs++], k - gr->first, un->r.base, un->r.count, gr->first, gr->end);
             } else if (hash && fp_content(&p->units[u])) {
                 seg[gr->nSegs - 1].end++;
             }
@@ -1593,9 +1654,6 @@ static int fh_issue(const fp_plan* p, const uint8_t* src, int64_t g, slot_t* s, 
     a.srcSize = (const int32_t*)(d + t.srcSize); a.rawLen = (const int32_t*)(d + t.rawLen);
     a.ord = (const int32_t*)(d + t.ord); a.sum = (int32_t*)(d + t.sum); a.outSize = (const int32_t*)(d + t.outSize);
     a.blockSize = (int32_t*)(d + t.blockSize); a.blockFrom = (int64_t*)(d + t.blockFrom); a.blockOff = (int64_t*)(d + t.blockOff);
-    a.segs = (const lz4k_hash_seg*)(d + t.segs); a.nSegs = gr->nSegs; a.segBad = (int32_t*)(d + t.segBad);
-    a.carryIn = (const fc_xxh32_state*)g_fh.carry + (g + FH_CARRIES - 1) % FH_CARRIES;
-    a.carryOut = (fc_xxh32_state*)g_fh.carry + g % FH_CARRIES;
     /* the decode of every class at its uniform capacity (the scan alone when sizing) */
     for (c = 0; c < FC_CLASSES; c++) {
         lz4k_decode_args dd;
@@ -1612,13 +1670,10 @@ static int fh_issue(const fp_plan* p, const uint8_t* src, int64_t g, slot_t* s, 
         return rc;
     if (!sizeOnly) {
         if ((rc = launched(lz4k_launch_group_assemble(&a, s->stream), "lz4k_launch_group_assemble")) != LZ4B200_OK) return rc;
-        if (gr->nSegs) {
-            if (seg[0].flags & LZ4K_SEG_CONTINUES)       /* after the group before: its carry kernel left the state */
-                CU(cudaStreamWaitEvent(s->stream, g_fh.hashed[(g + N_PIPE - 1) % N_PIPE], 0));
-            if ((rc = launched(lz4k_launch_group_content(&a, carry, s->stream), "lz4k_launch_group_content")) != LZ4B200_OK)
-                return rc;
-            if (!(seg[gr->nSegs - 1].flags & LZ4K_SEG_ENDS)) CU(cudaEventRecord(g_fh.hashed[g % N_PIPE], s->stream));
-        }
+        memset(&sa, 0, sizeof sa);                        /* the content hash of the output, block after block */
+        sa.base = a.packed; sa.off = a.blockOff; sa.size = a.blockSize;
+        sa.segs = (const lz4k_seg*)(d + t.segs); sa.nSegs = gr->nSegs; sa.digest = (uint32_t*)(d + t.digest);
+        if ((rc = seg_content(s, g, seg, &sa)) != LZ4B200_OK) return rc;
     }
     /* down: the block checksums' outcomes, the decode's results and the segments' */
     CU(cudaMemcpyAsync(h + t.sum, d + t.sum, t.blockSize - t.sum, cudaMemcpyDeviceToHost, s->stream));
@@ -1634,22 +1689,26 @@ static int fh_retire(fp_plan* p, slot_t* s, const fh_group_t* gr, int sizeOnly, 
 {
     const int64_t n = gr->end - gr->first;
     const fh_tab_t t = fh_tab(n, gr->nSegs);
-    int64_t k, pos = 0, runDev = 0, runLen = 0;
-    uint8_t* runHost = NULL;
+    int64_t k, pos = 0;
+    run_t run = {NULL, 0, 0};
     const uint8_t* h;
-    const int32_t *ord, *sum, *out, *segBad;
-    const lz4k_hash_seg* seg;
+    const int32_t *ord, *sum, *out;
+    const uint32_t* digest;
+    const lz4k_seg* seg;
     int rc = slot_wait(s);
     if (rc != LZ4B200_OK) return rc;
     h = (const uint8_t*)s->h_tab.p;
     ord = (const int32_t*)(h + t.ord); sum = (const int32_t*)(h + t.sum); out = (const int32_t*)(h + t.outSize);
-    segBad = (const int32_t*)(h + t.segBad); seg = (const lz4k_hash_seg*)(h + t.segs);
+    digest = (const uint32_t*)(h + t.digest); seg = (const lz4k_seg*)(h + t.segs);
     for (k = 0; k < n; k++) {
         p->outSize[gr->first + k] = out[ord[k]];
         p->sumState[gr->first + k] = sum[ord[k]] == FC_SUM_BAD ? FC_SUM_BAD : FC_SUM_NONE;
     }
     for (k = 0; k < gr->nSegs; k++)
-        if (seg[k].flags & LZ4K_SEG_ENDS) p->contentBad[p->blocks[gr->first + seg[k].first].unit] = segBad[k] != 0;
+        if (seg[k].flags & LZ4K_SEG_ENDS) {
+            const int64_t u = p->blocks[gr->first + seg[k].first].unit;
+            p->contentBad[u] = digest[k] != p->units[u].contentSum;
+        }
     if (sizeOnly) return rc;
     for (k = 0; k < n; k++) {
         const fp_block* b = &p->blocks[gr->first + k];
@@ -1659,23 +1718,14 @@ static int fh_retire(fp_plan* p, slot_t* s, const fh_group_t* gr, int sizeOnly, 
             if (!b->raw && out[ord[k]] < 0) fileStop[f] = 1;
             else {
                 const int64_t room = dstCap[f] - filePos[f], w = sz < room ? sz : room > 0 ? room : 0;
-                uint8_t* to = dst + dstOff[f] + filePos[f];
-                if (w > 0) {
-                    if (runLen && runDev + runLen == pos && runHost + runLen == to) runLen += w;
-                    else {
-                        if (runLen) CU(cudaMemcpyAsync(runHost, (uint8_t*)s->pack.p + runDev, (size_t)runLen, cudaMemcpyDeviceToHost, s->stream));
-                        runDev = pos; runHost = to; runLen = w;
-                    }
-                }
+                if (w > 0 && (rc = run_add(s, &run, pos, dst + dstOff[f] + filePos[f], w)) != LZ4B200_OK) return rc;
                 if (w < sz) fileStop[f] = 1;
                 filePos[f] += sz;
             }
         }
         pos += sz;
     }
-    if (runLen) CU(cudaMemcpyAsync(runHost, (uint8_t*)s->pack.p + runDev, (size_t)runLen, cudaMemcpyDeviceToHost, s->stream));
-done:
-    return rc;
+    return run_flush(s, &run);
 }
 
 /* LZ4B200_ERR_ARG, with LZ4B200_last_cuda_error() saying that the host's memory ran out (under the host lock) */
@@ -1767,7 +1817,7 @@ static cw_tab_t cw_tab(int64_t n, int64_t nSegs)
     cw_tab_t t;
     const size_t w8 = (size_t)n * 8, w4 = (size_t)n * 4;
     t.srcOff = 0; t.slotOff = w8; t.segs = 2 * w8;
-    t.srcSize = t.segs + (size_t)nSegs * sizeof(lz4k_wseg);
+    t.srcSize = t.segs + (size_t)nSegs * sizeof(lz4k_seg);
     t.cap = t.srcSize + w4; t.outSize = t.cap + w4;
     t.bodyOff = (t.outSize + w4 + 7) & ~(size_t)7;
     t.digest = t.bodyOff + w8 + 8;
@@ -1778,8 +1828,6 @@ static cw_tab_t cw_tab(int64_t n, int64_t nSegs)
 /* the encode of a writer call: its parse and level, and the checksums its frames carry (none for legacy streams) */
 typedef struct { int hcLevel, accel, parallel, sums; } cw_enc_t;
 
-static int64_t up16(int64_t x) { return (x + 15) & ~(int64_t)15; }
-
 /* Issue group gr on slot s (group index g): the table and the source pieces up, the encode, the body, the block
  * checksums, the content checksums; then the body's offsets and the digests back to the pinned table. */
 static int cw_issue(const cp_plan* p, const uint8_t* src, int64_t g, slot_t* s, fh_group_t* gr, const cw_enc_t* c,
@@ -1789,24 +1837,16 @@ static int cw_issue(const cp_plan* p, const uint8_t* src, int64_t g, slot_t* s, 
     const int hash = !p->legacy && (c->sums & FC_CONTENT_SUM);
     int64_t k, f = -1, nCopies = 0, gaps = 0, nSegs = 0, slotBytes = 0, packBytes = 0, at;
     size_t hcBytes = 0;
-    int rc = LZ4B200_OK, carry = 0;
+    int rc = LZ4B200_OK;
     cw_tab_t t;
     uint8_t *h, *d;
-    lz4k_wseg* seg;
+    lz4k_seg* seg;
     lz4k_encode_args e;
     lz4k_wgroup_args a;
-    /* pieces: [hostOff, devOff, bytes] triples, coalesced across gaps of at most FH_GAP while the group's gaps stay
-     * within G, so that the staged bytes stay within 2 G (plus alignment) */
+    lz4k_seg_args sa;
+    /* the pieces, with the group's gaps within G, so that the staged bytes stay within 2 G (plus alignment) */
     for (k = gr->first; k < gr->end; k++) {
-        const int64_t lo = p->srcOff[k], hi = lo + p->size[k];
-        int64_t* cp = nCopies ? copies + 3 * (nCopies - 1) : NULL;
-        const int64_t gap = cp ? lo - (cp[0] + cp[2]) : 0;
-        if (cp && lo >= cp[0] && gap <= FH_GAP && gaps + (gap > 0 ? gap : 0) <= G) {
-            if (gap > 0) gaps += gap;
-            if (hi > cp[0] + cp[2]) cp[2] = hi - cp[0];
-        } else {
-            cp = copies + 3 * nCopies++; cp[0] = lo; cp[2] = hi - lo;
-        }
+        piece_add(copies, &nCopies, &gaps, p->srcOff[k], p->srcOff[k] + p->size[k], G);
         slotBytes += up16(p->cap[k]);
         packBytes += 8 + (p->legacy ? p->cap[k] : p->size[k]);
         if (hash && p->file[k] != f) { nSegs++; f = p->file[k]; }
@@ -1817,7 +1857,7 @@ static int cw_issue(const cp_plan* p, const uint8_t* src, int64_t g, slot_t* s, 
     if ((rc = slot_take(s, (size_t)at, (size_t)slotBytes, hcBytes, (size_t)packBytes, t.bytes)) != LZ4B200_OK) return rc;
     h = (uint8_t*)s->h_tab.p;
     d = (uint8_t*)s->d_tab.p;
-    seg = (lz4k_wseg*)(h + t.segs);
+    seg = (lz4k_seg*)(h + t.segs);
     gr->nSegs = 0;
     /* the table: blocks in file order, each frame's blocks one segment */
     {
@@ -1828,11 +1868,7 @@ static int cw_issue(const cp_plan* p, const uint8_t* src, int64_t g, slot_t* s, 
         int64_t piece = 0;
         for (k = gr->first, at = 0, f = -1; k < gr->end; k++) {
             const int64_t i = k - gr->first;
-            const int64_t* cp;
-            while (!(p->srcOff[k] >= copies[3 * piece] && p->srcOff[k] + p->size[k] <= copies[3 * piece] + copies[3 * piece + 2]))
-                piece++;
-            cp = copies + 3 * piece;
-            srcOff[i] = cp[1] + (p->srcOff[k] - cp[0]);
+            srcOff[i] = piece_at(copies, &piece, p->srcOff[k], p->srcOff[k] + p->size[k]);
             srcSize[i] = p->size[k];
             cap[i] = p->cap[k];
             slotOff[i] = at;
@@ -1840,13 +1876,11 @@ static int cw_issue(const cp_plan* p, const uint8_t* src, int64_t g, slot_t* s, 
             if (!hash) continue;
             if (p->file[k] != f) {
                 const fc_frame_rec* r = &p->files[p->file[k]];
-                lz4k_wseg* q = &seg[gr->nSegs++];
                 f = p->file[k];
-                q->off = srcOff[i]; q->len = 0; q->pad = 0;
-                q->flags = (k > r->base ? LZ4K_SEG_CONTINUES : 0) | (r->base + r->count <= gr->end ? LZ4K_SEG_ENDS : 0);
-                if (q->flags != LZ4K_SEG_ENDS) carry = 1;
+                seg_open(&seg[gr->nSegs++], i, r->base, r->count, gr->first, gr->end);
+            } else {
+                seg[gr->nSegs - 1].end++;                    /* a file's blocks lie together in one piece */
             }
-            seg[gr->nSegs - 1].len += p->size[k];            /* a file's blocks lie together in one piece */
         }
     }
     /* up: the table and the pieces */
@@ -1865,17 +1899,11 @@ static int cw_issue(const cp_plan* p, const uint8_t* src, int64_t g, slot_t* s, 
     a.bodyOff = (int64_t*)(d + t.bodyOff);
     a.legacy = p->legacy;
     a.blockSums = !p->legacy && (c->sums & FC_BLOCK_SUM);
-    a.segs = (const lz4k_wseg*)(d + t.segs); a.nSegs = gr->nSegs; a.digest = (uint32_t*)(d + t.digest);
-    a.carryIn = (const fc_xxh32_state*)g_fh.carry + (g + FH_CARRIES - 1) % FH_CARRIES;
-    a.carryOut = (fc_xxh32_state*)g_fh.carry + g % FH_CARRIES;
     if ((rc = launched(lz4k_launch_wgroup_body(&a, s->stream), "lz4k_launch_wgroup_body")) != LZ4B200_OK) return rc;
-    if (gr->nSegs) {
-        if (seg[0].flags & LZ4K_SEG_CONTINUES)           /* after the group before: its carry kernel left the state */
-            CU(cudaStreamWaitEvent(s->stream, g_fh.hashed[(g + N_PIPE - 1) % N_PIPE], 0));
-        if ((rc = launched(lz4k_launch_wgroup_content(&a, carry, s->stream), "lz4k_launch_wgroup_content")) != LZ4B200_OK)
-            return rc;
-        if (!(seg[gr->nSegs - 1].flags & LZ4K_SEG_ENDS)) CU(cudaEventRecord(g_fh.hashed[g % N_PIPE], s->stream));
-    }
+    memset(&sa, 0, sizeof sa);                            /* the content hash of the staged source */
+    sa.base = a.src; sa.off = a.srcOff; sa.size = a.srcSize;
+    sa.segs = (const lz4k_seg*)(d + t.segs); sa.nSegs = gr->nSegs; sa.digest = (uint32_t*)(d + t.digest);
+    if ((rc = seg_content(s, g, seg, &sa)) != LZ4B200_OK) return rc;
     /* down: the body's offsets and the digests */
     CU(cudaMemcpyAsync(h + t.bodyOff, d + t.bodyOff, t.bytes - t.bodyOff, cudaMemcpyDeviceToHost, s->stream));
 done:
@@ -1899,8 +1927,8 @@ static int cw_retire(const cp_plan* p, slot_t* s, const fh_group_t* gr, uint8_t*
 {
     const int64_t n = gr->end - gr->first;
     const cw_tab_t t = cw_tab(n, gr->nSegs);
-    int64_t k, f = -1, sg = -1, runDev = 0, runLen = 0;
-    uint8_t* runHost = NULL;
+    int64_t k, f = -1, sg = -1;
+    run_t run = {NULL, 0, 0};
     const int64_t* bodyOff;
     const uint32_t* digest;
     int rc = slot_wait(s);
@@ -1910,22 +1938,14 @@ static int cw_retire(const cp_plan* p, slot_t* s, const fh_group_t* gr, uint8_t*
     for (k = 0; k < n; k++) {
         const int64_t b = gr->first + k, len = bodyOff[k + 1] - bodyOff[k];
         const fc_frame_rec* r;
-        uint8_t* to;
         if (p->file[b] != f) { f = p->file[b]; sg++; }      /* (segment sg, when the frames carry content checksums) */
         r = &p->files[f];
-        to = dst + dstOff[f] + filePos[f];
-        if (runLen && runDev + runLen == bodyOff[k] && runHost + runLen == to) runLen += len;
-        else {
-            if (runLen) CU(cudaMemcpyAsync(runHost, (uint8_t*)s->pack.p + runDev, (size_t)runLen, cudaMemcpyDeviceToHost, s->stream));
-            runDev = bodyOff[k]; runHost = to; runLen = len;
-        }
+        if ((rc = run_add(s, &run, bodyOff[k], dst + dstOff[f] + filePos[f], len)) != LZ4B200_OK) return rc;
         filePos[f] += len;
         if (b == r->base + r->count - 1)
             result[f] = cw_end(p, f, dst + dstOff[f], filePos[f], sg < gr->nSegs ? digest[sg] : 0);
     }
-    if (runLen) CU(cudaMemcpyAsync(runHost, (uint8_t*)s->pack.p + runDev, (size_t)runLen, cudaMemcpyDeviceToHost, s->stream));
-done:
-    return rc;
+    return run_flush(s, &run);
 }
 
 /* plan (host: verdicts, headers, empty files) -> per group, N_PIPE in flight: issue group g, then retire group

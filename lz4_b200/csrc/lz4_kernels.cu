@@ -1767,15 +1767,8 @@ __global__ void __launch_bounds__(128) lz4_files_fold_kernel(lz4k_files_args a)
  *               or, stored raw, its staged bytes
  *   scan      : lz4_pack_scan_kernel over the sizes: each block's place in the group's output
  *   gather    : lz4_pack_gather_kernel from those places
- *   hash      : content_hash over the segments that start and end their frame in the group
- *   carry     : one warp for each of the first and the last segment when it continues a frame from the group before
- *               (the state that group's carry left) or leaves it open for the next (the state the next one reads)
+ * then the content checksums of its segments over the output (the segment kernels below)
  * ============================================================================================= */
-__device__ __forceinline__ bool seg_carried(const lz4k_hash_seg& g)
-{
-    return (g.flags & LZ4K_SEG_CONTINUES) || !(g.flags & LZ4K_SEG_ENDS);
-}
-
 __device__ __forceinline__ int64_t group_stored(const lz4k_group_args& a, int64_t e)
 {
     return a.rawLen[e] >= 0 ? a.rawLen[e] : a.srcSize[e];
@@ -1805,54 +1798,6 @@ __global__ void __launch_bounds__(128) lz4_group_sizes_kernel(lz4k_group_args a)
     a.blockFrom[k] = a.gatherOff[e];
 }
 
-__global__ void __launch_bounds__(32 * kXsWarps) lz4_group_hash_kernel(lz4k_group_args a)
-{
-    content_hash(a.nSegs,
-        [&](int64_t s, const uint8_t** p, int64_t* len) {
-            const lz4k_hash_seg g = a.segs[s];
-            *p = a.packed + a.blockOff[g.first];
-            *len = a.blockOff[g.end] - a.blockOff[g.first];
-            return !seg_carried(g);
-        },
-        [&](int64_t s, uint32_t h) { a.segBad[s] = h != a.segs[s].expected; });
-}
-
-/* Warp 0 takes the first segment, warp 1 the last (when there are two or more), if it is carried: the state it
- * continues (or a fresh one), the bytes that complete its tail (every lane alike), the stripes by the warp
- * (xxh32_staged_stripes, lane 0's accumulators broadcast), the bytes after them into the tail; then lane 0 compares the
- * digest or leaves the state for the next group. */
-__global__ void __launch_bounds__(64) lz4_group_carry_kernel(lz4k_group_args a)
-{
-    __shared__ uint4 ring[2][kXsRing * kXsChunk];
-    const int w = threadIdx.x >> 5;
-    if (w == 1 && a.nSegs < 2) return;
-    const int64_t s = w == 0 ? 0 : a.nSegs - 1;
-    const lz4k_hash_seg g = a.segs[s];
-    if (!seg_carried(g)) return;
-    const uint8_t* p = a.packed + a.blockOff[g.first];
-    const int64_t len = a.blockOff[g.end] - a.blockOff[g.first];
-    fc_xxh32_state st;
-    if (g.flags & LZ4K_SEG_CONTINUES) st = *static_cast<const fc_xxh32_state*>(a.carryIn);
-    else fc_xxh32_init(&st);
-    int64_t k = 0;
-    if (st.tailLen) {
-        k = 16 - (int64_t)st.tailLen < len ? 16 - (int64_t)st.tailLen : len;
-        fc_xxh32_update(&st, p, (uint64_t)k);
-    }
-    const int64_t body = (len - k) & ~(int64_t)15;
-    if (body) {
-        xxh32_staged_stripes(p + k, body, ring[w], st.v);
-        #pragma unroll
-        for (int i = 0; i < 4; i++) st.v[i] = __shfl_sync(kFull, st.v[i], 0);
-        st.total += (uint64_t)body;
-    }
-    fc_xxh32_update(&st, p + k + body, (uint64_t)(len - k - body));
-    if ((threadIdx.x & 31) == 0) {
-        if (g.flags & LZ4K_SEG_ENDS) a.segBad[s] = fc_xxh32_digest(&st) != g.expected;
-        else *static_cast<fc_xxh32_state*>(a.carryOut) = st;
-    }
-}
-
 /* =============================================================================================
  * batched frame encode (LZ4B200_compress_frames, LZ4B200_compress_frames_checksummed) and legacy encode
  * (LZ4B200_compress_legacy): the rules of lz4_frame_core.h around one encode of the whole block table (by the caller)
@@ -1876,13 +1821,14 @@ __device__ __forceinline__ fc_cblock_tab cframes_tab(const lz4k_cframes_args& a,
     return fc_cblock_tab{a.tabSrcOff + t, a.tabSrcSize + t, a.tabSlotOff + t, a.tabCap + t};
 }
 
-/* the pack's rule over the block table: a frame block is stored raw from the source when its encode did not gain; a
- * legacy block never is (the plain rule: its encode always fits LZ4_compressBound) */
-__host__ __device__ inline FrameRule cframes_rule(const lz4k_cframes_args& a)
+/* the pack's rule over a block table: a frame block is stored raw from its source (src + srcOff[b], srcSize[b] bytes)
+ * when its encode did not gain; a legacy block never is (the plain rule: its encode always fits LZ4_compressBound) */
+__host__ __device__ inline FrameRule frame_rule(int legacy, const uint8_t* src, const int64_t* srcOff,
+                                                const int32_t* srcSize)
 {
     FrameRule fr;
-    fr.raw = a.legacy ? nullptr : a.src;
-    fr.rawStride = 0; fr.blockSize = 0; fr.lastSize = 0; fr.rawOff = a.tabSrcOff; fr.rawSize = a.tabSrcSize;
+    fr.raw = legacy ? nullptr : src;
+    fr.rawStride = 0; fr.blockSize = 0; fr.lastSize = 0; fr.rawOff = srcOff; fr.rawSize = srcSize;
     return fr;
 }
 
@@ -1960,7 +1906,8 @@ __global__ void __launch_bounds__(128) lz4_cframes_block_sum_kernel(lz4k_cframes
     if (b >= a.nEntries) return;
     if (a.tabPackOff[b] < 0) return;
     bool isRaw;
-    const int s = pack_payload(cframes_rule(a), a.tabOutSize, b, a.nEntries, isRaw);
+    const FrameRule fr = frame_rule(a.legacy, a.src, a.tabSrcOff, a.tabSrcSize);
+    const int s = pack_payload(fr, a.tabOutSize, b, a.nEntries, isRaw);
     const uint32_t h = xxh32_dev(isRaw ? a.src + a.tabSrcOff[b] : a.slots + a.tabSlotOff[b], s);
     st_le32(a.dst + a.tabPackOff[b] + 4 + s, h);
 }
@@ -1982,53 +1929,57 @@ __global__ void __launch_bounds__(32 * kXsWarps) lz4_cframes_content_sum_kernel(
  * the files and cuts their blocks into groups; per group, after the encode of its blocks (by the caller):
  *   scan, gather: the pack scan and gather with the frame rule over the staged source (legacy: the plain rule)
  *   block sums  : content_hash over the blocks: XXH32 of each payload where it lies, into the 4 bytes after it
- *   hash        : content_hash over the segments that start and end their frame in the group: XXH32 of the source
- *   carry       : lz4_group_carry_kernel's steps on the first and the last segment when carried, over the source, the
- *                 digest stored where the frame ends
+ * then the content checksums of its segments over the staged source (the segment kernels below)
  * ============================================================================================= */
-__host__ __device__ inline FrameRule wgroup_rule(const lz4k_wgroup_args& a)
-{
-    FrameRule fr;
-    fr.raw = a.legacy ? nullptr : a.src;
-    fr.rawStride = 0; fr.blockSize = 0; fr.lastSize = 0; fr.rawOff = a.srcOff; fr.rawSize = a.srcSize;
-    return fr;
-}
-
 __global__ void __launch_bounds__(32 * kXsWarps) lz4_wgroup_block_sum_kernel(lz4k_wgroup_args a)
 {
     content_hash(a.n,
         [&](int64_t k, const uint8_t** p, int64_t* len) {
             bool isRaw;
-            *len = pack_payload(wgroup_rule(a), a.outSize, k, a.n, isRaw);
+            *len = pack_payload(frame_rule(a.legacy, a.src, a.srcOff, a.srcSize), a.outSize, k, a.n, isRaw);
             *p = isRaw ? a.src + a.srcOff[k] : a.slots + a.slotOff[k];
             return true;
         },
         [&](int64_t k, uint32_t h) { st_le32(a.packed + a.bodyOff[k + 1] - 4, h); });
 }
 
-__global__ void __launch_bounds__(32 * kXsWarps) lz4_wgroup_hash_kernel(lz4k_wgroup_args a)
+/* =============================================================================================
+ * the content checksums of a group's segments, for the file reader and writers
+ *   hash : content_hash over the segments that begin and end their frame in the group
+ *   carry: one warp for each of the first and the last segment when it continues a frame from the group before (the
+ *          state that group's carry left) or leaves it open for the next (the state the next one reads)
+ * ============================================================================================= */
+__device__ __forceinline__ int64_t seg_bytes(const lz4k_seg_args& a, const lz4k_seg& g, const uint8_t** p)
+{
+    *p = a.base + a.off[g.first];
+    return a.off[g.end - 1] + a.size[g.end - 1] - a.off[g.first];
+}
+
+__global__ void __launch_bounds__(32 * kXsWarps) lz4_seg_hash_kernel(lz4k_seg_args a)
 {
     content_hash(a.nSegs,
         [&](int64_t s, const uint8_t** p, int64_t* len) {
-            *p = a.src + a.segs[s].off;
-            *len = a.segs[s].len;
-            return a.segs[s].flags == LZ4K_SEG_ENDS;
+            const lz4k_seg g = a.segs[s];
+            *len = seg_bytes(a, g, p);
+            return g.flags == LZ4K_SEG_ENDS;
         },
         [&](int64_t s, uint32_t h) { a.digest[s] = h; });
 }
 
-/* lz4_group_carry_kernel's steps, kept apart so that the decode's kernel stays as it is: warp 0 takes the first
- * segment, warp 1 the last, if it is carried; then lane 0 stores the digest or leaves the state for the next group. */
-__global__ void __launch_bounds__(64) lz4_wgroup_carry_kernel(lz4k_wgroup_args a)
+/* Warp 0 takes the first segment, warp 1 the last (when there are two or more), if it is carried: the state it
+ * continues (or a fresh one), the bytes that complete its tail (every lane alike), the stripes by the warp
+ * (xxh32_staged_stripes, lane 0's accumulators broadcast), the bytes after them into the tail; then lane 0 stores the
+ * digest or leaves the state for the next group. */
+__global__ void __launch_bounds__(64) lz4_seg_carry_kernel(lz4k_seg_args a)
 {
     __shared__ uint4 ring[2][kXsRing * kXsChunk];
     const int w = threadIdx.x >> 5;
     if (w == 1 && a.nSegs < 2) return;
     const int64_t s = w == 0 ? 0 : a.nSegs - 1;
-    const lz4k_wseg g = a.segs[s];
+    const lz4k_seg g = a.segs[s];
     if (g.flags == LZ4K_SEG_ENDS) return;
-    const uint8_t* p = a.src + g.off;
-    const int64_t len = g.len;
+    const uint8_t* p;
+    const int64_t len = seg_bytes(a, g, &p);
     fc_xxh32_state st;
     if (g.flags & LZ4K_SEG_CONTINUES) st = *static_cast<const fc_xxh32_state*>(a.carryIn);
     else fc_xxh32_init(&st);
@@ -2173,20 +2124,10 @@ int lz4k_launch_group_assemble(const lz4k_group_args* a, void* stream)
     return launch_pack(a->base, a->blockFrom, 0, a->blockSize, a->n, a->packed, a->blockOff, 0, FrameRule{}, s);
 }
 
-int lz4k_launch_group_content(const lz4k_group_args* a, int carry, void* stream)
-{
-    cudaStream_t s = (cudaStream_t)stream;
-    xs_carveout((const void*)lz4_group_hash_kernel);
-    lz4_group_hash_kernel<<<(unsigned)xs_grid(a->nSegs), 32 * kXsWarps, 0, s>>>(*a);
-    g_launches++;
-    if (carry) { lz4_group_carry_kernel<<<1, 64, 0, s>>>(*a); g_launches++; }
-    return (int)cudaGetLastError();
-}
-
 int lz4k_launch_wgroup_body(const lz4k_wgroup_args* a, void* stream)
 {
     cudaStream_t s = (cudaStream_t)stream;
-    const FrameRule fr = wgroup_rule(*a);
+    const FrameRule fr = frame_rule(a->legacy, a->src, a->srcOff, a->srcSize);
     lz4_pack_scan_kernel<<<1, 1024, 0, s>>>(a->outSize, a->n, a->bodyOff, 4, a->blockSums ? 4 : 0, fr);
     g_launches++;
     launch_pack_gather(a->slots, a->slotOff, 0, a->outSize, a->n, a->packed, a->bodyOff, nullptr, 4, fr, s);
@@ -2198,13 +2139,13 @@ int lz4k_launch_wgroup_body(const lz4k_wgroup_args* a, void* stream)
     return (int)cudaGetLastError();
 }
 
-int lz4k_launch_wgroup_content(const lz4k_wgroup_args* a, int carry, void* stream)
+int lz4k_launch_seg_content(const lz4k_seg_args* a, int carry, void* stream)
 {
     cudaStream_t s = (cudaStream_t)stream;
-    xs_carveout((const void*)lz4_wgroup_hash_kernel);
-    lz4_wgroup_hash_kernel<<<(unsigned)xs_grid(a->nSegs), 32 * kXsWarps, 0, s>>>(*a);
+    xs_carveout((const void*)lz4_seg_hash_kernel);
+    lz4_seg_hash_kernel<<<(unsigned)xs_grid(a->nSegs), 32 * kXsWarps, 0, s>>>(*a);
     g_launches++;
-    if (carry) { lz4_wgroup_carry_kernel<<<1, 64, 0, s>>>(*a); g_launches++; }
+    if (carry) { lz4_seg_carry_kernel<<<1, 64, 0, s>>>(*a); g_launches++; }
     return (int)cudaGetLastError();
 }
 
@@ -2237,7 +2178,7 @@ int lz4k_launch_cframes_index(const lz4k_cframes_args* a, void* stream)
 int lz4k_launch_cframes_assemble(const lz4k_cframes_args* a, void* stream)
 {
     cudaStream_t s = (cudaStream_t)stream;
-    const FrameRule fr = cframes_rule(*a);
+    const FrameRule fr = frame_rule(a->legacy, a->src, a->tabSrcOff, a->tabSrcSize);
     lz4_pack_scan_kernel<<<1, 1024, 0, s>>>(a->tabOutSize, a->nEntries, a->tabBodyOff, 4, (a->sums & FC_BLOCK_SUM) ? 4 : 0, fr);
     if (a->legacy) lz4_clegacy_finish_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);
     else lz4_cframes_finish_kernel<<<frames_grid(a->nFrames), 128, 0, s>>>(*a);

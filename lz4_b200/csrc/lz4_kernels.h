@@ -133,18 +133,37 @@ int lz4k_launch_files_totals(const lz4k_files_args* a, void* stream);
 int lz4k_launch_files_place(const lz4k_files_args* a, void* stream);
 /* last: every file's result, consumed and prefix from the unit results */
 int lz4k_launch_files_fold(const lz4k_files_args* a, void* stream);
-/* The steps of one group of LZ4B200_decompress_files_host around the decode of its blocks (one lz4k_launch_decode per
- * class, by the caller).  A group is a run of consecutive blocks of the call's files; its table lists them by class
- * (entry e), and ord gives the entry of the k-th block in file order.  A hash segment is a run of blocks of one frame
- * that carries a content checksum. */
+/* The content checksums of one group of the host-buffer file reader and writers (LZ4B200_decompress_files_host,
+ * LZ4B200_compress_frames_host).  A group is a run of consecutive blocks of the call's files; a segment is the run of
+ * one frame's blocks in the group, when the frame carries a content checksum.  Its blocks' bytes lie back to back:
+ * block k's are base + off[k], size[k] bytes, so a segment's run from base + off[first] to base + off[end - 1] +
+ * size[end - 1]. */
 #define LZ4K_SEG_CONTINUES 1   /* the frame began in an earlier group: the hash starts from the carried state */
-#define LZ4K_SEG_ENDS      2   /* the frame's last block is in this group: the digest is compared */
+#define LZ4K_SEG_ENDS      2   /* the frame's last block is in this group: its digest is written */
 typedef struct {
     int32_t first, end;        /* blocks [first, end) of the group, in file order */
-    uint32_t expected;         /* the content checksum the frame carries */
     int32_t flags;             /* LZ4K_SEG_* */
-} lz4k_hash_seg;
+    int32_t pad;
+} lz4k_seg;
 
+typedef struct {
+    const uint8_t* base;
+    const int64_t* off;        /* [n] block k's bytes: base + off[k], size[k] bytes */
+    const int32_t* size;
+    const lz4k_seg* segs;      /* [nSegs], in file order */
+    int64_t nSegs;
+    uint32_t* digest;          /* [nSegs] the content checksum of every frame that ends in the group */
+    const void* carryIn;       /* fc_xxh32_state of the frame the first segment continues */
+    void* carryOut;            /* .. of the frame the last segment leaves open */
+} lz4k_seg_args;
+
+/* the digest of every segment that begins and ends its frame in the group; carry: the first or the last segment
+ * continues or leaves its frame open */
+int lz4k_launch_seg_content(const lz4k_seg_args* a, int carry, void* stream);
+
+/* The steps of one group of LZ4B200_decompress_files_host around the decode of its blocks (one lz4k_launch_decode per
+ * class, by the caller).  Its table lists the blocks by class (entry e), and ord gives the entry of the k-th block in
+ * file order. */
 typedef struct {
     uint8_t* base;             /* the decode's slots and the staged source bytes, in one buffer */
     uint8_t* packed;           /* the group's output, block after block in file order */
@@ -159,11 +178,6 @@ typedef struct {
     int32_t* blockSize;        /* [n] output bytes of block k: its rawLen, or its decoded size (0 if it failed) */
     int64_t* blockFrom;        /* [n] block k's output before the gather: base + the gatherOff of its entry */
     int64_t* blockOff;         /* [n + 1] where block k goes in packed; blockOff[n] = the group's output bytes */
-    const lz4k_hash_seg* segs; /* [nSegs], in file order */
-    int64_t nSegs;
-    int32_t* segBad;           /* [nSegs] 1 where a segment that ends the frame does not match */
-    const void* carryIn;       /* fc_xxh32_state of the frame the first segment continues */
-    void* carryOut;            /* .. of the frame the last segment leaves open */
 } lz4k_group_args;
 
 /* every block checksum marked FC_SUM_PENDING, over the staged stored bytes */
@@ -171,17 +185,8 @@ int lz4k_launch_group_block_sums(const lz4k_group_args* a, void* stream);
 /* after the decode: each block's output size and place in file order, their scan (the pack scan), the gather into
  * packed (the pack gather) */
 int lz4k_launch_group_assemble(const lz4k_group_args* a, void* stream);
-/* after the assembly: the content hash of every segment; carry: a segment continues or leaves its frame open */
-int lz4k_launch_group_content(const lz4k_group_args* a, int carry, void* stream);
 /* The steps of one group of LZ4B200_compress_frames_host and LZ4B200_compress_legacy_host after the encode of its blocks
- * (by the caller).  A group is a run of consecutive blocks of the call's files, in file order; a hash segment is the run
- * of one frame's blocks in the group, whose source bytes lie together in the staged source. */
-typedef struct {
-    int64_t off, len;          /* the segment's source bytes: src + off, len bytes */
-    int32_t flags;             /* LZ4K_SEG_*: CONTINUES a frame begun in the group before, ENDS its frame here */
-    int32_t pad;
-} lz4k_wseg;
-
+ * (by the caller), in file order. */
 typedef struct {
     const uint8_t* src;        /* the group's staged source */
     const uint8_t* slots;      /* the encode's output */
@@ -194,18 +199,11 @@ typedef struct {
     int64_t* bodyOff;          /* [n + 1] where block k goes in packed; bodyOff[n] = the group's body bytes */
     int legacy;                /* legacy chunks: never stored raw */
     int blockSums;             /* a block checksum follows every payload */
-    const lz4k_wseg* segs;     /* [nSegs], in file order */
-    int64_t nSegs;
-    uint32_t* digest;          /* [nSegs] the content checksum of every frame that ends in the group */
-    const void* carryIn;       /* fc_xxh32_state of the frame the first segment continues */
-    void* carryOut;            /* .. of the frame the last segment leaves open */
 } lz4k_wgroup_args;
 
 /* the body: the pack scan (4-byte header, a 4-byte trailer with block checksums) and the gather, frame blocks that did
  * not gain stored raw from the staged source; then the block checksums */
 int lz4k_launch_wgroup_body(const lz4k_wgroup_args* a, void* stream);
-/* the content checksums of the segments; carry: a segment continues or leaves its frame open */
-int lz4k_launch_wgroup_content(const lz4k_wgroup_args* a, int carry, void* stream);
 /* the batched frame and legacy encode's own steps (lz4_frame_core.h); the encode of the block table between them is the
  * caller's */
 typedef struct {

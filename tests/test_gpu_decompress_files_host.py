@@ -1,8 +1,8 @@
 """LZ4B200_decompress_files_host on the GPU: every file of tests/golden/decompress_files.json in both checksum modes and
 the size-only pass against LZ4B200_decompress_files (with a budget that covers them all) and the Python model, with guard
-bytes around every output region at exact capacity and one byte less; the same corpus and long frames, a legacy stream
-and late corruptions in a child process with 1 MiB groups, so that every pipeline slot is reused and frame, unit and
-file boundaries fall on group edges; at the default group size a 1 GiB frame of 4 MB blocks and one of 64 KB blocks,
+bytes around every output region at exact capacity and one byte less; the same corpus and long frames, a legacy stream,
+late corruptions and a frame of blocks just short of 64 KB in a child process with 1 MiB groups, so that every pipeline
+slot is reused, frame, unit and file boundaries fall on group edges and a carried content hash has a partial stripe; at the default group size a 1 GiB frame of 4 MB blocks and one of 64 KB blocks,
 20 000 small files in one call and outputs past 2^32 in one buffer; the single-frame files against
 LZ4B200_decompressFrame_host; device memory over repeated calls; four threads beside LZ4B200_decompress_blocks_host;
 and the Python wrappers."""
@@ -164,6 +164,21 @@ def late_corruptions(frame):
     return out
 
 
+SHORT_BLOCKS = [65536 - 1 - k % 15 for k in range(40)]
+
+
+def short_blocks_frames(oracle, data):
+    """a frame with block and content checksums of blocks of SHORT_BLOCKS bytes, three stored raw, so that the group
+    edges inside it fall after content that is not a multiple of 16 bytes; then the same frame with its content
+    checksum flipped"""
+    ends = np.cumsum(SHORT_BLOCKS)
+    pieces = [data[e - n:e] for e, n in zip(ends, SHORT_BLOCKS)]
+    frame = dm.fm.frame_of_blocks(oracle, pieces, 4, raw=(3, 17, 30), block_sum=True, content_sum=True)
+    bad = bytearray(frame)
+    bad[-1] ^= 1
+    return [frame, bytes(bad)]
+
+
 def chunked_files(oracle):
     """the corpus, then files whose frames, units and blocks cross 1 MiB group edges"""
     _, files = golden_files(oracle)
@@ -173,7 +188,7 @@ def chunked_files(oracle):
         dm.fm.compress_frame(oracle, data[:300000], 5, True, 1, 1)
     mixed = b"".join(dm.fm.compress_frame(oracle, data[k * 70000:(k + 1) * 70000 + k], 4 + k % 4, k % 2 == 0, k % 3 == 0,
                                           k % 2 == 1) + dm.skippable(b"s" * k, k % 16) for k in range(40))
-    return files + [big, leg, mixed] + late_corruptions(big) + files[:20]
+    return files + [big, leg, mixed] + late_corruptions(big) + short_blocks_frames(oracle, data) + files[:20]
 
 
 def chunked_results(lib, files):
@@ -211,11 +226,12 @@ def test_one_mib_groups_in_a_child(lib, oracle, tmp_path):
         assert got[k][3] == [sha(b) for b in dbytes]
         assert got[k + 1] == list(device_call(files, caps, skip, size_only=True)[:3])
         k += 2
-        n = len(files) - 20 - 3
+        n = len(files) - 20 - 5
         if not skip:                                      # the late corruptions fail with a checksum error: the
-            sres = got[k - 1][0]                          # block ones in the size-only pass, the content one decoding
+            sres = got[k - 1][0]                          # block ones in the size-only pass, the content ones decoding
             assert dres[n - 3:n] == [40 * MIB, 20 * MIB + 1 + 300000, dres[n - 1]] and dres[n - 1] > 0
             assert sres[n:n + 2] == [ERR_CHECKSUM] * 2 and dres[n + 2] == ERR_CHECKSUM, (sres[n:n + 3], dres[n:n + 3])
+            assert dres[n + 3:n + 5] == [sum(SHORT_BLOCKS), ERR_CHECKSUM], dres[n + 3:n + 5]
 
 
 def gpu_frame(data, bsid):
