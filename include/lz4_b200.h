@@ -776,6 +776,61 @@ LZ4B200_API int LZ4B200_compress_frames_host(const void* h_src, const int64_t* h
 LZ4B200_API int LZ4B200_compress_legacy_host(const void* h_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
                                              void* h_dst, const int64_t* h_dstOff, const int64_t* h_dstCap,
                                              int64_t* h_result, int64_t nFiles, int compressionLevel);
+
+/*
+ * Decode nFiles whole .lz4 files in host memory into device memory: LZ4B200_decompress_files_host with the output in
+ * device memory.  File f is h_src + h_srcOff[f], h_srcSize[f] bytes, and decodes to d_dst + h_dstOff[f] with h_dstCap[f]
+ * bytes of room; d_dst is one device base pointer, the offset, size and capacity arrays are host arrays.
+ *   h_result[f], h_consumed[f], h_prefix[f] (the last two optional): what LZ4B200_decompress_files_host returns for the
+ *   same files and arguments with sizeOnly == 0 -- the same grammar, unit order, verdict order, skipChecksums rule and
+ *   deviations from `lz4 -d`.  There is no size-only mode: LZ4B200_decompress_files_host answers it from the same bytes.
+ * On success [d_dst + h_dstOff[f], + result) holds the host call's bytes; on failure [.., + prefix) does.  Nothing
+ * outside [d_dst + h_dstOff[f], + h_dstCap[f]) is written; destinations are byte-aligned anywhere and must not overlap
+ * one another.  Only compressed bytes cross PCIe, in one direction: each group's output is copied from the pipeline's
+ * buffer to the files in device memory by one scatter kernel per group (DESIGN section 3.19).
+ * Device memory held at most: section 3.17's four slots, plus per slot a run table of 24 bytes x (the group's blocks +
+ * 64 MiB / 256 KiB + 1) in device and pinned memory.
+ * Ordering: the call's device work starts after the work enqueued on `stream` (a cudaStream_t, NULL for the legacy
+ * default stream) before the call, and every write to d_dst is complete when it returns.  Synchronous; one host-buffer
+ * call runs at a time.
+ * Returns LZ4B200_OK, LZ4B200_ERR_ARG (in this order: nFiles < 0; then, with files, a NULL pointer other than h_consumed
+ * and h_prefix; d_dst not device or managed memory of the pipeline's device, or an h_ pointer that is device memory,
+ * which LZ4B200_last_cuda_error() names; host memory for the walk ran out) or LZ4B200_ERR_CUDA (no device included:
+ * there is no CPU fallback).  nFiles == 0 returns LZ4B200_OK without touching the device.
+ */
+LZ4B200_API int LZ4B200_decompress_files_to_device(const void* h_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
+                                                   void* d_dst, const int64_t* h_dstOff, const int64_t* h_dstCap,
+                                                   int64_t* h_result, int64_t* h_consumed, int64_t* h_prefix,
+                                                   int64_t nFiles, int skipChecksums, void* stream);
+
+/*
+ * Write nFiles whole .lz4 files from device memory into host memory: LZ4B200_compress_frames_host and
+ * LZ4B200_compress_legacy_host with the source in device memory.  File f is d_src + h_srcOff[f], h_srcSize[f] bytes (d_src
+ * one device base pointer, the arrays host arrays), written to h_dst + h_dstOff[f] with h_dstCap[f] bytes of room.
+ *   h_result[f] and the bytes: exactly what the host writer returns and writes for the same sources and arguments -- so
+ *   the reference tool's bytes with parallel == 0, the same LZ4B200_ERR_DSTSIZE thresholds and level mappings, never
+ *   LZ4B200_ERR_LIMIT.  Only [dst_f, dst_f + h_result[f]) is written.
+ * The source is read where it lies, so its readable padding is the device calls': the aligned 16-byte granules holding
+ * a byte of a file (LZ4B200_compress_frames_checksummed; with neither checksum, the encoder's rule), and at HC levels
+ * the aligned 4-byte words holding one (LZ4B200_compress_legacy).  Only compressed bytes cross PCIe, in one direction.
+ * Device memory held at most: that of the host writers above without the staged source (2 G + 16 bytes per slot).
+ * Ordering: the call's device work starts after the work enqueued on `stream` before the call.  Synchronous; one
+ * host-buffer call runs at a time.  DESIGN section 3.19.
+ * Returns LZ4B200_OK or, in this order: LZ4B200_ERR_ARG for nFiles < 0; LZ4B200_OK for nFiles == 0 without touching the
+ * device; LZ4B200_ERR_ARG for a NULL pointer, for frames blockSizeID outside {0, 4 .. 7} or parallel with
+ * compressionLevel >= 2, d_src not device or managed memory of the pipeline's device, or an h_ pointer that is device
+ * memory (LZ4B200_last_cuda_error() names it), or host memory for the plan ran out; LZ4B200_ERR_CUDA (no device
+ * included: there is no CPU fallback).
+ */
+LZ4B200_API int LZ4B200_compress_frames_from_device(const void* d_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
+                                                    void* h_dst, const int64_t* h_dstOff, const int64_t* h_dstCap,
+                                                    int64_t* h_result, int64_t nFiles,
+                                                    int blockSizeID, int compressionLevel, int contentSizeFlag, int parallel,
+                                                    int blockChecksumFlag, int contentChecksumFlag, void* stream);
+LZ4B200_API int LZ4B200_compress_legacy_from_device(const void* d_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
+                                                    void* h_dst, const int64_t* h_dstOff, const int64_t* h_dstCap,
+                                                    int64_t* h_result, int64_t nFiles, int compressionLevel, void* stream);
+
 /* The capacity below which LZ4B200_compress_frames_checksummed and LZ4B200_compress_frames_host give a frame of srcSize
  * bytes LZ4B200_ERR_DSTSIZE: LZ4F_compressFrameBound for the checksums at the frame's own block size ID (blockSizeID
  * shrunk as LZ4F_optimalBSID does), 19 + (4 + 4 B) x blocks + srcSize + 4 + 4 C.  LZ4B200_ERR_ARG for srcSize < 0 or

@@ -80,6 +80,10 @@ PROTOTYPES = [
     ("LZ4B200_compress_frames_host", C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, C.c_int, C.c_int, C.c_int,
                                               C.c_int, C.c_int, C.c_int]),
     ("LZ4B200_compress_legacy_host", C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, C.c_int]),
+    ("LZ4B200_decompress_files_to_device", C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, C.c_int, _vp]),
+    ("LZ4B200_compress_frames_from_device", C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, C.c_int, C.c_int, C.c_int,
+                                                      C.c_int, C.c_int, C.c_int, _vp]),
+    ("LZ4B200_compress_legacy_from_device", C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, C.c_int, _vp]),
     ("LZ4B200_compressFrameBound_checksummed", _i64, [_i64, C.c_int, C.c_int, C.c_int]),
     ("LZ4B200_compressFrameBound", _i64, [_i64, C.c_int]),
     ("LZ4B200_compressFrame_host", _i64, [_vp, _i64, _vp, _i64, C.c_int, C.c_int, C.c_int]),

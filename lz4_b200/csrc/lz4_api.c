@@ -109,7 +109,7 @@ typedef struct {
     int64_t pend_cnt;
 } slot_t;
 
-static struct { int ready; slot_t slot[N_PIPE]; } g_ctx;
+static struct { int ready, device; slot_t slot[N_PIPE]; } g_ctx;   /* device: the one the slots' streams belong to */
 
 static int ctx_init(void)
 {
@@ -119,6 +119,7 @@ static int ctx_init(void)
         snprintf(g_cuda_error, sizeof(g_cuda_error), "no CUDA device: liblz4_b200 has no CPU fallback");
         return LZ4B200_ERR_CUDA;
     }
+    CU(cudaGetDevice(&g_ctx.device));
     for (i = 0; i < N_PIPE; i++) CU(cudaStreamCreateWithFlags(&g_ctx.slot[i].stream, cudaStreamNonBlocking));
     g_ctx.ready = 1;
 done:
@@ -1457,13 +1458,15 @@ done:
  * of the groups before it run beside its kernels and the copies up of the groups after it.  Its slot is taken again
  * N_PIPE groups after it: FH_LAG < N_PIPE. */
 #define FH_LAG     (N_PIPE - 1)
-static struct { int ready; cudaEvent_t hashed[N_PIPE]; void* carry; } g_fh;
+/* entered: the caller's stream at the start of a call that reads or writes the caller's device memory */
+static struct { int ready; cudaEvent_t hashed[N_PIPE], entered; void* carry; } g_fh;
 
 static int fh_init(void)
 {
     int rc = LZ4B200_OK, i;
     if (g_fh.ready) return rc;
     for (i = 0; i < N_PIPE; i++) CU(cudaEventCreateWithFlags(&g_fh.hashed[i], cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&g_fh.entered, cudaEventDisableTiming));
     CU(cudaMalloc(&g_fh.carry, FH_CARRIES * sizeof(fc_xxh32_state)));
     g_fh.ready = 1;
 done:
@@ -1471,6 +1474,35 @@ done:
 }
 
 static int64_t up16(int64_t x) { return (x + 15) & ~(int64_t)15; }
+
+/* The checks of a call whose d_ pointers arrive from outside the library (under the host lock, after ctx_init):
+ * LZ4B200_ERR_ARG, with LZ4B200_last_cuda_error() naming the pointer, for a d_ pointer that is not device or managed
+ * memory of the pipeline's device, or an h_ pointer (NULL: not given) that is device memory, which the host would fault
+ * on. */
+static int ptr_check(const char* call, const char* name, const void* p, int device)
+{
+    struct cudaPointerAttributes at;
+    int ok;
+    if (!p) return LZ4B200_OK;
+    if (cudaPointerGetAttributes(&at, p) != cudaSuccess) { cudaGetLastError(); at.type = cudaMemoryTypeUnregistered; }
+    ok = device ? (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) && at.device == g_ctx.device
+                : at.type != cudaMemoryTypeDevice;
+    if (ok) return LZ4B200_OK;
+    snprintf(g_cuda_error, sizeof(g_cuda_error), "%s: %s is %s", call, name,
+             device ? "not device memory of the pipeline's device" : "device memory, which the host cannot reach");
+    return LZ4B200_ERR_ARG;
+}
+
+/* Every slot stream waits for the work enqueued on the caller's stream before the call (the slot streams do not
+ * synchronise with the legacy default stream). */
+static int enter_after(void* stream)
+{
+    int rc = LZ4B200_OK, i;
+    CU(cudaEventRecord(g_fh.entered, (cudaStream_t)stream));
+    for (i = 0; i < N_PIPE; i++) CU(cudaStreamWaitEvent(g_ctx.slot[i].stream, g_fh.entered, 0));
+done:
+    return rc;
+}
 
 /* Source pieces: [hostOff, devOff, bytes] triples in copies (room for one per block).  A block's bytes [lo, hi) join
  * the last piece when they begin in it or at most FH_GAP past its end, while the group's gaps stay within budget. */
@@ -1544,10 +1576,11 @@ static int run_add(slot_t* s, run_t* r, int64_t dev, uint8_t* host, int64_t len)
 
 /* A group's table in its slot (the host copy pinned, the device copy the kernels use), for n blocks and nSegs segments:
  * [srcOff, gatherOff, dstOff: i64 n | segments | srcSize, rawLen, ord, sum: i32 n] go up, [sum, outSize: i32 n |
- * digest: u32 nSegs] come back, [blockSize: i32 n | blockFrom: i64 n | blockOff: i64 n + 1] stay on the device. */
-typedef struct { size_t srcOff, gatherOff, dstOff, segs, srcSize, rawLen, ord, sum, outSize, digest, blockSize, blockFrom, blockOff, bytes; } fh_tab_t;
+ * digest: u32 nSegs] come back, [blockSize: i32 n | blockFrom: i64 n | blockOff: i64 n + 1] stay on the device;
+ * [runs: lz4k_run nRuns] go up at retire when the output goes to device memory. */
+typedef struct { size_t srcOff, gatherOff, dstOff, segs, srcSize, rawLen, ord, sum, outSize, digest, blockSize, blockFrom, blockOff, runs, bytes; } fh_tab_t;
 
-static fh_tab_t fh_tab(int64_t n, int64_t nSegs)
+static fh_tab_t fh_tab(int64_t n, int64_t nSegs, int64_t nRuns)
 {
     fh_tab_t t;
     const size_t w8 = (size_t)n * 8, w4 = (size_t)n * 4;
@@ -1557,17 +1590,20 @@ static fh_tab_t fh_tab(int64_t n, int64_t nSegs)
     t.blockSize = t.digest + (size_t)nSegs * 4;
     t.blockFrom = (t.blockSize + w4 + 7) & ~(size_t)7;
     t.blockOff = t.blockFrom + w8;
-    t.bytes = t.blockOff + w8 + 8;
+    t.runs = t.blockOff + w8 + 8;
+    t.bytes = t.runs + (size_t)nRuns * sizeof(lz4k_run);
     return t;
 }
 
-/* what the host keeps of a group in flight: its blocks and segments (the rest is in its slot's pinned table) */
-typedef struct { int64_t first, end, nSegs; } fh_group_t;
+/* what the host keeps of a group in flight: its blocks, segments and room for runs (the rest is in its slot's pinned
+ * table) */
+typedef struct { int64_t first, end, nSegs, nRuns; } fh_group_t;
 
 /* Issue group gr on slot s (group index g): the table, the source pieces, the decode per class, the block checksums,
- * and unless sizeOnly the assembly and the content hash; then the results back to the pinned table. */
+ * and unless sizeOnly the assembly and the content hash; then the results back to the pinned table.  devDst: the table
+ * keeps room for the runs of the group's output, cut at LZ4K_SCATTER_RUN bytes. */
 static int fh_issue(const fp_plan* p, const uint8_t* src, int64_t g, slot_t* s, fh_group_t* gr, int sizeOnly, int verify,
-                    int64_t* copies)
+                    int devDst, int64_t* copies)
 {
     const int64_t n = gr->end - gr->first;
     const int hash = verify && !sizeOnly;               /* the content checksums (none when the call only sizes) */
@@ -1604,7 +1640,8 @@ static int fh_issue(const fp_plan* p, const uint8_t* src, int64_t g, slot_t* s, 
     at = sizeOnly ? 0 : (slotBytes + 255) & ~(int64_t)255;              /* (the scan alone writes no slot) */
     for (k = 0; k < nCopies; k++) { copies[3 * k + 1] = at; at = up16(at + copies[3 * k + 2]); }
     inBytes = at;
-    t = fh_tab(n, nSegs);
+    gr->nRuns = devDst ? n + slotBytes / LZ4K_SCATTER_RUN + 1 : 0;
+    t = fh_tab(n, nSegs, gr->nRuns);
     if ((rc = slot_take(s, 0, (size_t)inBytes, wsBytes, sizeOnly ? 0 : (size_t)slotBytes, t.bytes)) != LZ4B200_OK)
         return rc;
     h = (uint8_t*)s->h_tab.p;
@@ -1682,22 +1719,24 @@ done:
 }
 
 /* Retire the group gr that ran on slot s: its results into the plan, then (unless sizeOnly) its bytes from the slot's
- * packed output to each file's running position, one copy per run of bytes contiguous on both sides, clipped to the
- * file's room and stopping at the file's first block that failed to decode. */
-static int fh_retire(fp_plan* p, slot_t* s, const fh_group_t* gr, int sizeOnly, uint8_t* dst, const int64_t* dstOff,
-                     const int64_t* dstCap, int64_t* filePos, uint8_t* fileStop)
+ * packed output to the files as fp_place places them.  Into host memory (dst, devDst 0): one copy down per run of bytes
+ * contiguous on both sides.  Into device memory (devDst 1): the runs, cut at LZ4K_SCATTER_RUN bytes, in the slot's
+ * table and one scatter on its stream (the slot is taken again only after this, as FH_LAG < N_PIPE).  runs: room for
+ * the group's blocks. */
+static int fh_retire(fp_plan* p, slot_t* s, const fh_group_t* gr, int sizeOnly, uint8_t* dst, int devDst,
+                     const int64_t* dstOff, const int64_t* dstCap, int64_t* filePos, uint8_t* fileStop, fp_run* runs)
 {
     const int64_t n = gr->end - gr->first;
-    const fh_tab_t t = fh_tab(n, gr->nSegs);
-    int64_t k, pos = 0;
+    const fh_tab_t t = fh_tab(n, gr->nSegs, gr->nRuns);
+    int64_t k, r, nRuns;
     run_t run = {NULL, 0, 0};
-    const uint8_t* h;
+    uint8_t* h;
     const int32_t *ord, *sum, *out;
     const uint32_t* digest;
     const lz4k_seg* seg;
     int rc = slot_wait(s);
     if (rc != LZ4B200_OK) return rc;
-    h = (const uint8_t*)s->h_tab.p;
+    h = (uint8_t*)s->h_tab.p;
     ord = (const int32_t*)(h + t.ord); sum = (const int32_t*)(h + t.sum); out = (const int32_t*)(h + t.outSize);
     digest = (const uint32_t*)(h + t.digest); seg = (const lz4k_seg*)(h + t.segs);
     for (k = 0; k < n; k++) {
@@ -1710,22 +1749,30 @@ static int fh_retire(fp_plan* p, slot_t* s, const fh_group_t* gr, int sizeOnly, 
             p->contentBad[u] = digest[k] != p->units[u].contentSum;
         }
     if (sizeOnly) return rc;
-    for (k = 0; k < n; k++) {
-        const fp_block* b = &p->blocks[gr->first + k];
-        const int64_t f = p->units[b->unit].file;
-        const int64_t sz = b->raw ? b->size : out[ord[k]] > 0 ? out[ord[k]] : 0;
-        if (!fileStop[f]) {
-            if (!b->raw && out[ord[k]] < 0) fileStop[f] = 1;
-            else {
-                const int64_t room = dstCap[f] - filePos[f], w = sz < room ? sz : room > 0 ? room : 0;
-                if (w > 0 && (rc = run_add(s, &run, pos, dst + dstOff[f] + filePos[f], w)) != LZ4B200_OK) return rc;
-                if (w < sz) fileStop[f] = 1;
-                filePos[f] += sz;
-            }
-        }
-        pos += sz;
+    nRuns = fp_place(p, gr->first, gr->end, dstCap, filePos, fileStop, runs);
+    if (!devDst) {
+        for (r = 0; r < nRuns; r++)
+            if ((rc = run_add(s, &run, runs[r].packed, dst + dstOff[runs[r].file] + runs[r].fileOff, runs[r].len)) != LZ4B200_OK)
+                return rc;
+        return run_flush(s, &run);
     }
-    return run_flush(s, &run);
+    {
+        lz4k_run* dr = (lz4k_run*)(h + t.runs);
+        lz4k_scatter_args a;
+        int64_t m = 0, at;
+        for (r = 0; r < nRuns; r++)
+            for (at = 0; at < runs[r].len; at += LZ4K_SCATTER_RUN, m++) {
+                dr[m].src = runs[r].packed + at;
+                dr[m].dst = dstOff[runs[r].file] + runs[r].fileOff + at;
+                dr[m].len = runs[r].len - at < LZ4K_SCATTER_RUN ? runs[r].len - at : LZ4K_SCATTER_RUN;
+            }
+        if (!m) return rc;
+        CU(cudaMemcpyAsync((uint8_t*)s->d_tab.p + t.runs, dr, (size_t)m * sizeof(lz4k_run), cudaMemcpyHostToDevice, s->stream));
+        a.packed = (const uint8_t*)s->pack.p; a.dst = dst; a.runs = (const lz4k_run*)((uint8_t*)s->d_tab.p + t.runs); a.nRuns = m;
+        rc = launched(lz4k_launch_group_scatter(&a, s->stream), "lz4k_launch_group_scatter");
+    }
+done:
+    return rc;
 }
 
 /* LZ4B200_ERR_ARG, with LZ4B200_last_cuda_error() saying that the host's memory ran out (under the host lock) */
@@ -1735,31 +1782,39 @@ static int out_of_host_memory(const char* call)
     return LZ4B200_ERR_ARG;
 }
 
-/* walk (host) -> per group, N_PIPE in flight: issue group g, then retire group g - FH_LAG -> fold (host) */
-int LZ4B200_decompress_files_host(const void* h_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
-                                  void* h_dst, const int64_t* h_dstOff, const int64_t* h_dstCap,
-                                  int64_t* h_result, int64_t* h_consumed, int64_t* h_prefix,
-                                  int64_t nFiles, int skipChecksums, int sizeOnly)
+/* walk (host) -> per group, N_PIPE in flight: issue group g, then retire group g - FH_LAG -> fold (host).  devDst: dst is
+ * the caller's device memory, written after the work on `stream` before the call. */
+static int decompress_files_run(const char* call, const void* h_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
+                                void* dst, int devDst, const int64_t* h_dstOff, const int64_t* h_dstCap, int64_t* h_result,
+                                int64_t* h_consumed, int64_t* h_prefix, int64_t nFiles, int skipChecksums, int sizeOnly,
+                                void* stream)
 {
     const int verify = !skipChecksums;
     fp_plan p;
     fh_group_t grs[N_PIPE];
     int64_t *copies = NULL, *filePos = NULL, first, g, nGroups = 0;
     uint8_t* fileStop = NULL;
+    fp_run* runs = NULL;
     int rc;
-    if (nFiles < 0) return LZ4B200_ERR_ARG;
-    if (nFiles == 0) return LZ4B200_OK;
-    if (!h_src || !h_srcOff || !h_srcSize || !h_result) return LZ4B200_ERR_ARG;
-    if (!sizeOnly && (!h_dst || !h_dstOff || !h_dstCap)) return LZ4B200_ERR_ARG;
     memset(&p, 0, sizeof p);
     if ((rc = host_begin()) != LZ4B200_OK) goto done;
     if ((rc = fh_init()) != LZ4B200_OK) goto done;
+    if (devDst) {
+        const void* hp[8] = {h_src, h_srcOff, h_srcSize, h_dstOff, h_dstCap, h_result, h_consumed, h_prefix};
+        const char* hn[8] = {"h_src", "h_srcOff", "h_srcSize", "h_dstOff", "h_dstCap", "h_result", "h_consumed", "h_prefix"};
+        int i;
+        if ((rc = ptr_check(call, "d_dst", dst, 1)) != LZ4B200_OK) goto done;
+        for (i = 0; i < 8; i++)
+            if ((rc = ptr_check(call, hn[i], hp[i], 0)) != LZ4B200_OK) goto done;
+        if ((rc = enter_after(stream)) != LZ4B200_OK) goto done;
+    }
     if (!fp_build((const uint8_t*)h_src, h_srcOff, h_srcSize, sizeOnly ? NULL : h_dstCap, nFiles,
-                  verify ? FC_SUMS_VERIFY : FC_SUMS_SKIP, &p)) { rc = out_of_host_memory(__func__); goto done; }
+                  verify ? FC_SUMS_VERIFY : FC_SUMS_SKIP, &p)) { rc = out_of_host_memory(call); goto done; }
     copies = (int64_t*)malloc((size_t)(p.nBlocks ? p.nBlocks : 1) * 3 * sizeof(int64_t));
+    runs = (fp_run*)malloc((size_t)(p.nBlocks ? p.nBlocks : 1) * sizeof(fp_run));
     filePos = (int64_t*)calloc((size_t)nFiles, sizeof(int64_t));
     fileStop = (uint8_t*)calloc((size_t)nFiles, 1);
-    if (!copies || !filePos || !fileStop) { rc = out_of_host_memory(__func__); goto done; }
+    if (!copies || !runs || !filePos || !fileStop) { rc = out_of_host_memory(call); goto done; }
     for (first = 0; first < p.nBlocks; nGroups++) first = fp_group_end(&p, first, CHUNK_OUT_BYTES);
     for (g = 0, first = 0; g < nGroups + FH_LAG; g++) {
         if (g < nGroups) {
@@ -1767,21 +1822,47 @@ int LZ4B200_decompress_files_host(const void* h_src, const int64_t* h_srcOff, co
             gr->first = first;
             gr->end = fp_group_end(&p, first, CHUNK_OUT_BYTES);
             first = gr->end;
-            if ((rc = fh_issue(&p, (const uint8_t*)h_src, g, &g_ctx.slot[g % N_PIPE], gr, sizeOnly, verify, copies)) != LZ4B200_OK)
+            if ((rc = fh_issue(&p, (const uint8_t*)h_src, g, &g_ctx.slot[g % N_PIPE], gr, sizeOnly, verify, devDst,
+                               copies)) != LZ4B200_OK)
                 goto done;
         }
         if (g >= FH_LAG && (rc = fh_retire(&p, &g_ctx.slot[(g - FH_LAG) % N_PIPE], &grs[(g - FH_LAG) % N_PIPE], sizeOnly,
-                                           (uint8_t*)h_dst, h_dstOff, h_dstCap, filePos, fileStop)) != LZ4B200_OK)
+                                           (uint8_t*)dst, devDst, h_dstOff, h_dstCap, filePos, fileStop, runs)) != LZ4B200_OK)
             goto done;
     }
-    /* every group has retired: the results are in the plan (the last copies down may still run) */
+    /* every group has retired: the results are in the plan (the last copies down or scatters may still run) */
     if (!fp_fold(&p, h_srcSize, sizeOnly ? NULL : h_dstCap, h_result, h_consumed, h_prefix))
-        rc = out_of_host_memory(__func__);
+        rc = out_of_host_memory(call);
 done:
     rc = host_end(rc);
     fp_free(&p);
-    free(copies); free(filePos); free(fileStop);
+    free(copies); free(runs); free(filePos); free(fileStop);
     return rc;
+}
+
+int LZ4B200_decompress_files_host(const void* h_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
+                                  void* h_dst, const int64_t* h_dstOff, const int64_t* h_dstCap,
+                                  int64_t* h_result, int64_t* h_consumed, int64_t* h_prefix,
+                                  int64_t nFiles, int skipChecksums, int sizeOnly)
+{
+    if (nFiles < 0) return LZ4B200_ERR_ARG;
+    if (nFiles == 0) return LZ4B200_OK;
+    if (!h_src || !h_srcOff || !h_srcSize || !h_result) return LZ4B200_ERR_ARG;
+    if (!sizeOnly && (!h_dst || !h_dstOff || !h_dstCap)) return LZ4B200_ERR_ARG;
+    return decompress_files_run(__func__, h_src, h_srcOff, h_srcSize, h_dst, 0, h_dstOff, h_dstCap, h_result, h_consumed,
+                                h_prefix, nFiles, skipChecksums, sizeOnly, NULL);
+}
+
+int LZ4B200_decompress_files_to_device(const void* h_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
+                                       void* d_dst, const int64_t* h_dstOff, const int64_t* h_dstCap,
+                                       int64_t* h_result, int64_t* h_consumed, int64_t* h_prefix,
+                                       int64_t nFiles, int skipChecksums, void* stream)
+{
+    if (nFiles < 0) return LZ4B200_ERR_ARG;
+    if (nFiles == 0) return LZ4B200_OK;
+    if (!h_src || !h_srcOff || !h_srcSize || !d_dst || !h_dstOff || !h_dstCap || !h_result) return LZ4B200_ERR_ARG;
+    return decompress_files_run(__func__, h_src, h_srcOff, h_srcSize, d_dst, 1, h_dstOff, h_dstCap, h_result, h_consumed,
+                                h_prefix, nFiles, skipChecksums, 0, stream);
 }
 
 /* ------------------------------------------------------------------------------------------ */
@@ -1829,9 +1910,10 @@ static cw_tab_t cw_tab(int64_t n, int64_t nSegs)
 typedef struct { int hcLevel, accel, parallel, sums; } cw_enc_t;
 
 /* Issue group gr on slot s (group index g): the table and the source pieces up, the encode, the body, the block
- * checksums, the content checksums; then the body's offsets and the digests back to the pinned table. */
-static int cw_issue(const cp_plan* p, const uint8_t* src, int64_t g, slot_t* s, fh_group_t* gr, const cw_enc_t* c,
-                    int64_t* copies)
+ * checksums, the content checksums; then the body's offsets and the digests back to the pinned table.  devSrc: src is
+ * the caller's device memory, which every step reads where it lies (no pieces, no input buffer). */
+static int cw_issue(const cp_plan* p, const uint8_t* src, int devSrc, int64_t g, slot_t* s, fh_group_t* gr,
+                    const cw_enc_t* c, int64_t* copies)
 {
     const int64_t n = gr->end - gr->first, G = write_group_bytes();
     const int hash = !p->legacy && (c->sums & FC_CONTENT_SUM);
@@ -1840,13 +1922,14 @@ static int cw_issue(const cp_plan* p, const uint8_t* src, int64_t g, slot_t* s, 
     int rc = LZ4B200_OK;
     cw_tab_t t;
     uint8_t *h, *d;
+    const uint8_t* base;                                  /* where the steps read the source */
     lz4k_seg* seg;
     lz4k_encode_args e;
     lz4k_wgroup_args a;
     lz4k_seg_args sa;
     /* the pieces, with the group's gaps within G, so that the staged bytes stay within 2 G (plus alignment) */
     for (k = gr->first; k < gr->end; k++) {
-        piece_add(copies, &nCopies, &gaps, p->srcOff[k], p->srcOff[k] + p->size[k], G);
+        if (!devSrc) piece_add(copies, &nCopies, &gaps, p->srcOff[k], p->srcOff[k] + p->size[k], G);
         slotBytes += up16(p->cap[k]);
         packBytes += 8 + (p->legacy ? p->cap[k] : p->size[k]);
         if (hash && p->file[k] != f) { nSegs++; f = p->file[k]; }
@@ -1857,6 +1940,7 @@ static int cw_issue(const cp_plan* p, const uint8_t* src, int64_t g, slot_t* s, 
     if ((rc = slot_take(s, (size_t)at, (size_t)slotBytes, hcBytes, (size_t)packBytes, t.bytes)) != LZ4B200_OK) return rc;
     h = (uint8_t*)s->h_tab.p;
     d = (uint8_t*)s->d_tab.p;
+    base = devSrc ? src : (const uint8_t*)s->in.p;
     seg = (lz4k_seg*)(h + t.segs);
     gr->nSegs = 0;
     /* the table: blocks in file order, each frame's blocks one segment */
@@ -1868,7 +1952,7 @@ static int cw_issue(const cp_plan* p, const uint8_t* src, int64_t g, slot_t* s, 
         int64_t piece = 0;
         for (k = gr->first, at = 0, f = -1; k < gr->end; k++) {
             const int64_t i = k - gr->first;
-            srcOff[i] = piece_at(copies, &piece, p->srcOff[k], p->srcOff[k] + p->size[k]);
+            srcOff[i] = devSrc ? p->srcOff[k] : piece_at(copies, &piece, p->srcOff[k], p->srcOff[k] + p->size[k]);
             srcSize[i] = p->size[k];
             cap[i] = p->cap[k];
             slotOff[i] = at;
@@ -1889,18 +1973,18 @@ static int cw_issue(const cp_plan* p, const uint8_t* src, int64_t g, slot_t* s, 
         CU(cudaMemcpyAsync((uint8_t*)s->in.p + copies[3 * k + 1], src + copies[3 * k], (size_t)copies[3 * k + 2],
                            cudaMemcpyHostToDevice, s->stream));
     /* the encode of every block into its slot at its capacity */
-    e = encode_args(s->in.p, 0, (const int32_t*)(d + t.srcSize), 0, s->out.p, 0, 0, c->accel, (int32_t*)(d + t.outSize), n);
+    e = encode_args(base, 0, (const int32_t*)(d + t.srcSize), 0, s->out.p, 0, 0, c->accel, (int32_t*)(d + t.outSize), n);
     e.srcOff = (const int64_t*)(d + t.srcOff); e.dstOff = (const int64_t*)(d + t.slotOff); e.dstCapArr = (const int32_t*)(d + t.cap);
     if ((rc = encode_table(&e, c->hcLevel, c->parallel, s->ws.p, s->ws.cap, s->stream)) != LZ4B200_OK) return rc;
     /* the body, the block checksums, the content checksums */
     memset(&a, 0, sizeof a);
-    a.src = (const uint8_t*)s->in.p; a.slots = (const uint8_t*)s->out.p; a.packed = (uint8_t*)s->pack.p; a.n = n;
+    a.src = base; a.slots = (const uint8_t*)s->out.p; a.packed = (uint8_t*)s->pack.p; a.n = n;
     a.srcOff = e.srcOff; a.srcSize = e.srcSizeArr; a.slotOff = e.dstOff; a.outSize = e.outSize;
     a.bodyOff = (int64_t*)(d + t.bodyOff);
     a.legacy = p->legacy;
     a.blockSums = !p->legacy && (c->sums & FC_BLOCK_SUM);
     if ((rc = launched(lz4k_launch_wgroup_body(&a, s->stream), "lz4k_launch_wgroup_body")) != LZ4B200_OK) return rc;
-    memset(&sa, 0, sizeof sa);                            /* the content hash of the staged source */
+    memset(&sa, 0, sizeof sa);                            /* the content hash of the source */
     sa.base = a.src; sa.off = a.srcOff; sa.size = a.srcSize;
     sa.segs = (const lz4k_seg*)(d + t.segs); sa.nSegs = gr->nSegs; sa.digest = (uint32_t*)(d + t.digest);
     if ((rc = seg_content(s, g, seg, &sa)) != LZ4B200_OK) return rc;
@@ -1949,10 +2033,12 @@ static int cw_retire(const cp_plan* p, slot_t* s, const fh_group_t* gr, uint8_t*
 }
 
 /* plan (host: verdicts, headers, empty files) -> per group, N_PIPE in flight: issue group g, then retire group
- * g - FH_LAG (bodies, EndMarks, digests, results) */
-static int compress_files_host(const char* call, const void* h_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
-                               void* h_dst, const int64_t* h_dstOff, const int64_t* h_dstCap, int64_t* h_result,
-                               int64_t nFiles, int legacy, int bsid, int contentSizeFlag, const cw_enc_t* c)
+ * g - FH_LAG (bodies, EndMarks, digests, results).  devSrc: src is the caller's device memory, read after the work on
+ * `stream` before the call. */
+static int compress_files_host(const char* call, const void* src, int devSrc, const int64_t* h_srcOff,
+                               const int64_t* h_srcSize, void* h_dst, const int64_t* h_dstOff, const int64_t* h_dstCap,
+                               int64_t* h_result, int64_t nFiles, int legacy, int bsid, int contentSizeFlag,
+                               const cw_enc_t* c, void* stream)
 {
     uint8_t* dst = (uint8_t*)h_dst;
     cp_plan p;
@@ -1962,6 +2048,15 @@ static int compress_files_host(const char* call, const void* h_src, const int64_
     memset(&p, 0, sizeof p);
     if ((rc = host_begin()) != LZ4B200_OK) goto done;
     if ((rc = fh_init()) != LZ4B200_OK) goto done;
+    if (devSrc) {
+        const void* hp[6] = {h_srcOff, h_srcSize, h_dst, h_dstOff, h_dstCap, h_result};
+        const char* hn[6] = {"h_srcOff", "h_srcSize", "h_dst", "h_dstOff", "h_dstCap", "h_result"};
+        int i;
+        if ((rc = ptr_check(call, "d_src", src, 1)) != LZ4B200_OK) goto done;
+        for (i = 0; i < 6; i++)
+            if ((rc = ptr_check(call, hn[i], hp[i], 0)) != LZ4B200_OK) goto done;
+        if ((rc = enter_after(stream)) != LZ4B200_OK) goto done;
+    }
     if (!cp_build(h_srcOff, h_srcSize, h_dstCap, nFiles, legacy, bsid, contentSizeFlag, c->sums, &p)) {
         rc = out_of_host_memory(call); goto done;
     }
@@ -1981,7 +2076,8 @@ static int compress_files_host(const char* call, const void* h_src, const int64_
             gr->first = first;
             gr->end = cp_group_end(&p, first, write_group_bytes(), maxBlocks);
             first = gr->end;
-            if ((rc = cw_issue(&p, (const uint8_t*)h_src, g, &g_ctx.slot[g % N_PIPE], gr, c, copies)) != LZ4B200_OK) goto done;
+            if ((rc = cw_issue(&p, (const uint8_t*)src, devSrc, g, &g_ctx.slot[g % N_PIPE], gr, c, copies)) != LZ4B200_OK)
+                goto done;
         }
         if (g >= FH_LAG && (rc = cw_retire(&p, &g_ctx.slot[(g - FH_LAG) % N_PIPE], &grs[(g - FH_LAG) % N_PIPE], dst,
                                            h_dstOff, filePos, h_result)) != LZ4B200_OK)
@@ -1994,6 +2090,20 @@ done:
     return rc;
 }
 
+/* the frame writers' arguments: LZ4B200_ERR_ARG or LZ4B200_OK with *c set; nFiles == 0 is the caller's */
+static int frames_enc(int64_t nFiles, int* blockSizeID, int compressionLevel, int parallel, int blockChecksumFlag,
+                      int contentChecksumFlag, cw_enc_t* c)
+{
+    if (nFiles < 0) return LZ4B200_ERR_ARG;
+    if (*blockSizeID == 0) *blockSizeID = 4;
+    if (*blockSizeID < 4 || *blockSizeID > 7) return LZ4B200_ERR_ARG;
+    if (parallel && compressionLevel >= 2) return LZ4B200_ERR_ARG;
+    frames_levels(compressionLevel, &c->hcLevel, &c->accel);
+    c->parallel = parallel != 0;
+    c->sums = (blockChecksumFlag ? FC_BLOCK_SUM : 0) | (contentChecksumFlag ? FC_CONTENT_SUM : 0);
+    return LZ4B200_OK;
+}
+
 int LZ4B200_compress_frames_host(const void* h_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
                                  void* h_dst, const int64_t* h_dstOff, const int64_t* h_dstCap,
                                  int64_t* h_result, int64_t nFiles,
@@ -2001,17 +2111,28 @@ int LZ4B200_compress_frames_host(const void* h_src, const int64_t* h_srcOff, con
                                  int blockChecksumFlag, int contentChecksumFlag)
 {
     cw_enc_t c;
-    if (nFiles < 0) return LZ4B200_ERR_ARG;
-    if (blockSizeID == 0) blockSizeID = 4;
-    if (blockSizeID < 4 || blockSizeID > 7) return LZ4B200_ERR_ARG;
-    if (parallel && compressionLevel >= 2) return LZ4B200_ERR_ARG;
+    if (frames_enc(nFiles, &blockSizeID, compressionLevel, parallel, blockChecksumFlag, contentChecksumFlag, &c) != LZ4B200_OK)
+        return LZ4B200_ERR_ARG;
     if (nFiles == 0) return LZ4B200_OK;
     if (!h_src || !h_srcOff || !h_srcSize || !h_dst || !h_dstOff || !h_dstCap || !h_result) return LZ4B200_ERR_ARG;
-    frames_levels(compressionLevel, &c.hcLevel, &c.accel);
-    c.parallel = parallel != 0;
-    c.sums = (blockChecksumFlag ? FC_BLOCK_SUM : 0) | (contentChecksumFlag ? FC_CONTENT_SUM : 0);
-    return compress_files_host(__func__, h_src, h_srcOff, h_srcSize, h_dst, h_dstOff, h_dstCap,
-                               h_result, nFiles, 0, blockSizeID, contentSizeFlag, &c);
+    return compress_files_host(__func__, h_src, 0, h_srcOff, h_srcSize, h_dst, h_dstOff, h_dstCap,
+                               h_result, nFiles, 0, blockSizeID, contentSizeFlag, &c, NULL);
+}
+
+int LZ4B200_compress_frames_from_device(const void* d_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
+                                        void* h_dst, const int64_t* h_dstOff, const int64_t* h_dstCap,
+                                        int64_t* h_result, int64_t nFiles,
+                                        int blockSizeID, int compressionLevel, int contentSizeFlag, int parallel,
+                                        int blockChecksumFlag, int contentChecksumFlag, void* stream)
+{
+    cw_enc_t c;
+    if (nFiles < 0) return LZ4B200_ERR_ARG;
+    if (nFiles == 0) return LZ4B200_OK;
+    if (frames_enc(nFiles, &blockSizeID, compressionLevel, parallel, blockChecksumFlag, contentChecksumFlag, &c) != LZ4B200_OK)
+        return LZ4B200_ERR_ARG;
+    if (!d_src || !h_srcOff || !h_srcSize || !h_dst || !h_dstOff || !h_dstCap || !h_result) return LZ4B200_ERR_ARG;
+    return compress_files_host(__func__, d_src, 1, h_srcOff, h_srcSize, h_dst, h_dstOff, h_dstCap,
+                               h_result, nFiles, 0, blockSizeID, contentSizeFlag, &c, stream);
 }
 
 int LZ4B200_compress_legacy_host(const void* h_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
@@ -2025,6 +2146,21 @@ int LZ4B200_compress_legacy_host(const void* h_src, const int64_t* h_srcOff, con
     legacy_levels(compressionLevel, &c.hcLevel, &c.accel);
     c.parallel = 0;
     c.sums = 0;
-    return compress_files_host(__func__, h_src, h_srcOff, h_srcSize, h_dst, h_dstOff, h_dstCap,
-                               h_result, nFiles, 1, 0, 0, &c);
+    return compress_files_host(__func__, h_src, 0, h_srcOff, h_srcSize, h_dst, h_dstOff, h_dstCap,
+                               h_result, nFiles, 1, 0, 0, &c, NULL);
+}
+
+int LZ4B200_compress_legacy_from_device(const void* d_src, const int64_t* h_srcOff, const int64_t* h_srcSize,
+                                        void* h_dst, const int64_t* h_dstOff, const int64_t* h_dstCap,
+                                        int64_t* h_result, int64_t nFiles, int compressionLevel, void* stream)
+{
+    cw_enc_t c;
+    if (nFiles < 0) return LZ4B200_ERR_ARG;
+    if (nFiles == 0) return LZ4B200_OK;
+    if (!d_src || !h_srcOff || !h_srcSize || !h_dst || !h_dstOff || !h_dstCap || !h_result) return LZ4B200_ERR_ARG;
+    legacy_levels(compressionLevel, &c.hcLevel, &c.accel);
+    c.parallel = 0;
+    c.sums = 0;
+    return compress_files_host(__func__, d_src, 1, h_srcOff, h_srcSize, h_dst, h_dstOff, h_dstCap,
+                               h_result, nFiles, 1, 0, 0, &c, stream);
 }

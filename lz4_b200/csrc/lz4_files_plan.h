@@ -1,7 +1,8 @@
 /*
- * lz4_files_plan.h -- the host side of LZ4B200_decompress_files_host: the walk of every file into its units and their
- * blocks with the frame core's own steps (lz4_frame_core.h), the cut of the blocks into groups, and the fold of the
- * per-block results into every file's result, consumed and prefix with the verdicts of LZ4B200_decompress_files.  The
+ * lz4_files_plan.h -- the host side of LZ4B200_decompress_files_host and LZ4B200_decompress_files_to_device: the walk of
+ * every file into its units and their blocks with the frame core's own steps (lz4_frame_core.h), the cut of the blocks
+ * into groups, the placement of each group's output in the files, and the fold of the per-block results into every
+ * file's result, consumed and prefix with the verdicts of LZ4B200_decompress_files.  The
  * call's budget is unlimited, so no unit or block is ever over it.  Host C (C99, and C++ for tests/emul); it allocates
  * and hashes no byte of a file.
  */
@@ -140,7 +141,43 @@ static inline int64_t fp_group_end(const fp_plan* p, int64_t first, int64_t capB
     return end;
 }
 
-/* The fold, once every block's results are in: LZ4B200_decompress_files's totals, then either the results at unlimited
+typedef struct {               /* len bytes of a group's output, from byte `packed` of it, to byte fileOff of file's output */
+    int64_t packed, file, fileOff, len;
+} fp_run;
+
+/* The placement of the output of the group of blocks [first, end), once their results are in the plan (outSize): the
+ * blocks' bytes lie back to back in the group's packed output in file order (a stored-raw block's size, a decoded
+ * block's result, 0 when it failed), and each goes to its file's running position filePos[f], clipped to the room
+ * dstCap[f].  A file takes nothing from its first block that failed to decode or was clipped on (fileStop[f]).  Runs of
+ * one file that are contiguous on both sides are merged.  Returns the number of runs written to runs (at most
+ * end - first). */
+static inline int64_t fp_place(const fp_plan* p, int64_t first, int64_t end, const int64_t* dstCap, int64_t* filePos,
+                               uint8_t* fileStop, fp_run* runs)
+{
+    int64_t k, pos = 0, n = 0;
+    for (k = first; k < end; k++) {
+        const fp_block* b = &p->blocks[k];
+        const int64_t f = p->units[b->unit].file;
+        const int64_t sz = b->raw ? b->size : p->outSize[k] > 0 ? p->outSize[k] : 0;
+        if (!fileStop[f]) {
+            if (!b->raw && p->outSize[k] < 0) fileStop[f] = 1;
+            else {
+                const int64_t room = dstCap[f] - filePos[f], w = sz < room ? sz : room > 0 ? room : 0;
+                if (w > 0) {
+                    fp_run* r = n ? &runs[n - 1] : NULL;
+                    if (r && r->file == f && r->packed + r->len == pos && r->fileOff + r->len == filePos[f]) r->len += w;
+                    else { r = &runs[n++]; r->packed = pos; r->file = f; r->fileOff = filePos[f]; r->len = w; }
+                }
+                if (w < sz) fileStop[f] = 1;
+                filePos[f] += sz;
+            }
+        }
+        pos += sz;
+    }
+    return n;
+}
+
+/* The fold, once every block's results are in:LZ4B200_decompress_files's totals, then either the results at unlimited
  * room (dstCap NULL: the call only sizes) or the place of every file's units (fc_place_file), the verdict on each
  * (fc_verdict_frame) and its content checksum; then fc_fold_file.  consumed and prefix may be NULL.  Returns 0 when
  * memory runs out. */

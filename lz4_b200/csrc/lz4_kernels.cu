@@ -2002,6 +2002,41 @@ __global__ void __launch_bounds__(64) lz4_seg_carry_kernel(lz4k_seg_args a)
     }
 }
 
+/* =============================================================================================
+ * the copy of a file reader group's output to its files in device memory: one CTA per run.  The bytes before the
+ * destination's first whole 16-byte granule and after its last go one at a time; every whole granule in between takes
+ * one 16-byte store, from a 16-byte load when the source shares the destination's place in a granule and otherwise from
+ * five aligned 4-byte loads joined by funnel shifts.  No store reaches past a run's ends.
+ * ============================================================================================= */
+__global__ void __launch_bounds__(256) lz4_group_scatter_kernel(lz4k_scatter_args a)
+{
+    for (int64_t r = blockIdx.x; r < a.nRuns; r += gridDim.x) {
+        const lz4k_run run = a.runs[r];
+        const uint8_t* s = a.packed + run.src;
+        uint8_t* d = a.dst + run.dst;
+        const int64_t len = run.len;
+        const int64_t head = min((int64_t)((16 - ((uintptr_t)d & 15)) & 15), len);
+        const int64_t words = (len - head) >> 4, tail = head + 16 * words;
+        for (int64_t i = threadIdx.x; i < head; i += blockDim.x) d[i] = s[i];
+        for (int64_t i = tail + threadIdx.x; i < len; i += blockDim.x) d[i] = s[i];
+        uint4* d16 = reinterpret_cast<uint4*>(d + head);
+        const uintptr_t from = (uintptr_t)(s + head);
+        if ((from & 15) == 0) {
+            const uint4* s16 = reinterpret_cast<const uint4*>(from);
+            for (int64_t i = threadIdx.x; i < words; i += blockDim.x) d16[i] = s16[i];
+        } else {
+            const uint32_t* s4 = reinterpret_cast<const uint32_t*>(from & ~(uintptr_t)3);
+            const uint32_t sh = (uint32_t)(from & 3) * 8;
+            for (int64_t i = threadIdx.x; i < words; i += blockDim.x) {
+                const uint32_t* w = s4 + 4 * i;
+                const uint32_t w0 = w[0], w1 = w[1], w2 = w[2], w3 = w[3], w4 = w[4];
+                d16[i] = make_uint4(__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh), __funnelshift_r(w2, w3, sh),
+                                    __funnelshift_r(w3, w4, sh));
+            }
+        }
+    }
+}
+
 }  // namespace
 
 /* =============================================================================================
@@ -2146,6 +2181,15 @@ int lz4k_launch_seg_content(const lz4k_seg_args* a, int carry, void* stream)
     lz4_seg_hash_kernel<<<(unsigned)xs_grid(a->nSegs), 32 * kXsWarps, 0, s>>>(*a);
     g_launches++;
     if (carry) { lz4_seg_carry_kernel<<<1, 64, 0, s>>>(*a); g_launches++; }
+    return (int)cudaGetLastError();
+}
+
+int lz4k_launch_group_scatter(const lz4k_scatter_args* a, void* stream)
+{
+    const int64_t cap = (int64_t)device_sms() * 16;
+    if (a->nRuns <= 0) return (int)cudaSuccess;
+    lz4_group_scatter_kernel<<<(unsigned)(a->nRuns < cap ? a->nRuns : cap), 256, 0, (cudaStream_t)stream>>>(*a);
+    g_launches++;
     return (int)cudaGetLastError();
 }
 

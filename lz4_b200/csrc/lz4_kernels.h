@@ -185,6 +185,20 @@ int lz4k_launch_group_block_sums(const lz4k_group_args* a, void* stream);
 /* after the decode: each block's output size and place in file order, their scan (the pack scan), the gather into
  * packed (the pack gather) */
 int lz4k_launch_group_assemble(const lz4k_group_args* a, void* stream);
+/* The copy of one group's output to its files in device memory (LZ4B200_decompress_files_to_device): run r is runs[r].len
+ * bytes from packed + runs[r].src to dst + runs[r].dst, byte-aligned anywhere; nothing outside the runs is written. */
+typedef struct { int64_t src, dst, len; } lz4k_run;
+typedef struct {
+    const uint8_t* packed;     /* the group's output (lz4k_group_args.packed); read up to 4 bytes past a run's end */
+    uint8_t* dst;
+    const lz4k_run* runs;      /* [nRuns] */
+    int64_t nRuns;
+} lz4k_scatter_args;
+
+/* one launch, a CTA per run at a time (runs of at most LZ4K_SCATTER_RUN bytes, which the caller cuts, keep the CTAs'
+ * work alike); none for nRuns == 0 */
+#define LZ4K_SCATTER_RUN (256 << 10)
+int lz4k_launch_group_scatter(const lz4k_scatter_args* a, void* stream);
 /* The steps of one group of LZ4B200_compress_frames_host and LZ4B200_compress_legacy_host after the encode of its blocks
  * (by the caller), in file order. */
 typedef struct {
