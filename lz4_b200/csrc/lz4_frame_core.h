@@ -198,7 +198,8 @@ FC_FN int fc_frame_header_sums(uint8_t* h, int bsid, int64_t contentSize, int su
 FC_FN int fc_frame_header_bytes(uint8_t* h, int bsid, int64_t contentSize) { return fc_frame_header_sums(h, bsid, contentSize, 0); }
 
 typedef struct {
-    int64_t contentSize;       /* the header's content size, -1 without one (a field of 2^63 or more reads negative too) */
+    int64_t contentSize;       /* the header's content size, -1 without one; a field of 2^63 or more reads INT64_MAX, a
+                                  size no frame here decodes to, so the frame fails as lz4frame.c's frameSize_wrong */
     int32_t hdrLen;            /* bytes of the header: the first block header starts here */
     int32_t bsid;              /* block size ID, 4 .. 7 */
     int32_t sums;              /* the checksums the frame carries: FC_BLOCK_SUM | FC_CONTENT_SUM */
@@ -241,7 +242,7 @@ FC_FN int fc_frame_header(const uint8_t* src, int64_t srcSize, int64_t dstCap, i
     if ((flg >> 3) & 1) {
         uint64_t v = 0;
         for (i = 0; i < 8; i++) v |= (uint64_t)src[6 + i] << (8 * i);
-        h->contentSize = (int64_t)v;
+        h->contentSize = v > (uint64_t)INT64_MAX ? INT64_MAX : (int64_t)v;
     }
     h->hdrLen = (int32_t)hdrLen;
     h->bsid = bsid;

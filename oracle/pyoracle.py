@@ -261,8 +261,9 @@ class Reference(_Codec):
         return hasattr(self.lib, "LZ4F_compressFrame")
 
     def compress_frame(self, data, block_size_id=4, level=0, content_size=False, block_mode=1,
-                       content_checksum=0, block_checksum=0):
-        """LZ4F_compressFrame (lz4frame.c:484) with the given preferences; returns the frame bytes."""
+                       content_checksum=0, block_checksum=0, capacity=None):
+        """LZ4F_compressFrame (lz4frame.c:484) with the given preferences into capacity bytes (default: its
+        LZ4F_compressFrameBound); returns the frame bytes, RuntimeError when the call fails."""
         lib = self.lib
         class Prefs(C.Structure):              # LZ4F_preferences_t, lz4frame.h:192-198
             _fields_ = [("frameInfo", Reference._FrameInfo), ("compressionLevel", C.c_int), ("autoFlush", C.c_uint),
@@ -281,8 +282,8 @@ class Reference(_Codec):
         lib.LZ4F_compressFrame.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
         lib.LZ4F_isError.restype = C.c_uint
         lib.LZ4F_isError.argtypes = [C.c_size_t]
-        cap = lib.LZ4F_compressFrameBound(len(src), C.byref(p))
-        dst = np.empty(cap, dtype=np.uint8)
+        cap = lib.LZ4F_compressFrameBound(len(src), C.byref(p)) if capacity is None else int(capacity)
+        dst = np.empty(max(cap, 1), dtype=np.uint8)
         r = lib.LZ4F_compressFrame(dst.ctypes.data, cap, src.ctypes.data if len(src) else None, len(src), C.byref(p))
         if lib.LZ4F_isError(r):
             raise RuntimeError("LZ4F_compressFrame failed")

@@ -132,9 +132,10 @@ def _frame_decode(oracle, fr, room, skip, content):
     if content:
         return fm.decode(oracle, fr, room, skip)[:2]
     r, out, _ = fm.decode(oracle, fr, room, skip)
-    if r != ERR_CHECKSUM or skip:
+    if r != ERR_CHECKSUM or skip or not fm.sums_of(fr)[1]:
         return r, out
-    # a CHECKSUM result may be the content checksum's: decode again with the content checksum field made right
+    # a CHECKSUM result may be the content checksum's (when the frame has one): decode again with the content checksum
+    # field made right
     blocks, consumed = fm.walk(fr)
     r2, out2, _ = fm.decode(oracle, fr, room, True)
     if r2 < 0:

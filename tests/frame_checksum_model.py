@@ -210,7 +210,8 @@ def decode(oracle, frame, cap, skip):
         return fc.ERR_FRAME, b"", 0
     blocks, consumed = w
     bsum, csum = sums_of(frame)
-    csize = struct.unpack_from("<q", frame, 6)[0] if flg & 8 else -1
+    # a content-size field past 2^63 is a size no frame decodes to: the frame fails at its end (frameSize_wrong)
+    csize = min(struct.unpack_from("<Q", frame, 6)[0], (1 << 63) - 1) if flg & 8 else -1
     bs = 1 << (8 + 2 * ((bd >> 4) & 7))
     out = bytearray()
     for o, sz, raw in blocks:

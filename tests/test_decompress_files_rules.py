@@ -209,3 +209,20 @@ def test_argument_errors(lib):
             continue
         assert f(*b, 1, 1, ok, 0, 1, p, need, None) == -1, i
     assert lib.LZ4B200_launch_count() == n0
+
+
+def test_size_only_block_checksum_without_content_checksum(oracle):
+    """a frame with block checksums and no content checksum, one block checksum wrong: the size-only pass verifies block
+    checksums, so the file fails with LZ4B200_ERR_CHECKSUM there too (the model once rewrote the EndMark as a content
+    checksum and said LZ4B200_ERR_FRAME)"""
+    import frame_checksum_model as fm
+    pieces = [oracle.datagen(65536, 0.5, 3).tobytes(), oracle.datagen(1000, 0.5, 4).tobytes()]
+    fr = bytearray(fm.frame_of_blocks(oracle, pieces, 4, block_sum=True, content_size=66536))
+    blocks, _ = fm.walk(bytes(fr))
+    o, sz, _ = blocks[1]
+    fr[o + sz] ^= 1
+    files = [bytes(fr)]
+    for size_only in (False, True):
+        r = dm.decompress_files(oracle, files, [1 << 20], 1, [2, 0, 0, 0, 0], size_only=size_only, content=False)
+        assert r[0][:3] == (dm.ERR_CHECKSUM, 0, 0), size_only
+        _check(oracle, files, [1 << 20], 1, [2, 0, 0, 0, 0], False, size_only)

@@ -320,3 +320,33 @@ def test_side_stream_graph_capture_and_launch_count(lib, oracle, golden):
                                                    res.data_ptr(), None, len(frames), (C.c_int64 * 4)(*mb), 0,
                                                    ws.data_ptr(), ws.numel() - 1, None)
     assert rc == fc.ERR_ARG
+
+
+@pytest.mark.parametrize("skip", [False, True])
+def test_content_size_field_past_2_63(lib, oracle, skip):
+    """a content-size field with bit 63 set (its header checksum right) is a size no frame decodes to: LZ4F_decompress
+    fails it with frameSize_wrong, so the frame calls and the file calls give LZ4B200_ERR_FRAME (the frame calls once
+    read such a field as "no content size" and decoded the frame)"""
+    import struct
+    from lz4_b200 import batch
+    data = oracle.datagen(13, 0.5, 9).tobytes()
+    good = bytearray(fm.compress_frame(oracle, data, 4, True, True, True))
+    bad = bytearray(good)
+    struct.pack_into("<Q", bad, 6, (1 << 63) | len(data))
+    hl = fc.header_len(bytes(bad))
+    bad[hl - 1] = (fm.xxh32(bytes(bad[4:hl - 1])) >> 8) & 0xFF
+    assert fm.decode(oracle, bytes(bad), 64, skip)[0] == fc.ERR_FRAME
+    frames = [bytes(good), bytes(bad)]
+    arena = np.zeros(16 + sum(len(f) + 16 for f in frames), dtype=np.uint8)
+    offs = [16, 32 + len(frames[0])]
+    for o, f in zip(offs, frames):
+        arena[o:o + len(f)] = np.frombuffer(f, dtype=np.uint8)
+    t = lambda a: torch.tensor(a, dtype=torch.int64, device="cuda")      # noqa: E731
+    src = torch.from_numpy(arena).cuda()
+    _, res, _ = batch.decompress_frames_checksummed(src, t(offs), t([len(f) for f in frames]), t([64, 64]), [2, 0, 0, 0],
+                                                    skip_checksums=skip)
+    _, fres, _, _ = batch.decompress_files(src, t(offs), t([len(f) for f in frames]), t([64, 64]), 2, [2, 0, 0, 0, 0],
+                                           skip_checksums=skip)
+    torch.cuda.synchronize()
+    assert res.cpu().tolist() == [len(data), fc.ERR_FRAME]
+    assert fres.cpu().tolist() == [len(data), fc.ERR_FRAME]
